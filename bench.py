@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - keyframe depth maps/s of the CVA-MVSNet hot path (BASELINE.json metric) on N B200s.
+"""bench.py - keyframe depth maps/s of the CVA-MVSNet hot path (BASELINE.json metric) on N H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision mixed16|fp32]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -32,14 +32,14 @@ WORKLOAD = "CVA-MVSNet 640x480, 7 views, 3-stage cascade (48/32/8), view aggrega
 WEIGHTS = "abl03_view_aggregation"
 # identical in both arms (the driver compares the two lines' `config`); per-arm run parameters live under "run"
 CONFIG = {"workload": WORKLOAD,
-          "l2": "no flush needed: each step streams > 1 GB of activations through a 126 MB L2 (GPU arm; the CPU arm has no device cache to flush)"}
+          "l2": "no flush needed: each step streams > 1 GB of activations through a 50 MB L2 (GPU arm; the CPU arm has no device cache to flush)"}
 
 
 def tune_host_malloc():
     """Keep freed result buffers inside the process.  DrMvsnet::GetResult hands every keyframe's four maps (4.9 MB) to the caller
     in freshly allocated memory (dr_mvsnet.h:12-34: four malloc'd arrays per output, ownership transferred).  With glibc's
     defaults such blocks are mmap'd and unmapped every time, and the kernel's page faults + zeroing for them (~0.9 ms per
-    keyframe, measured) cost about as much as the whole forward (1.2 ms).  Raising the mmap / trim thresholds - an
+    keyframe on the host it was measured on) cost about as much as a whole forward.  Raising the mmap / trim thresholds - an
     application-level allocator setting, equivalent to MALLOC_MMAP_THRESHOLD_ / MALLOC_TRIM_THRESHOLD_ in the environment -
     lets malloc recycle them.  Applied to both arms."""
     import ctypes
@@ -71,14 +71,14 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth, not measured)"
 
 
 def measured_tensor_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
-        return float(json.load(open(p)).get("bf16_tflops_sustained", 1374.6))
-    return 1400.0
+        return float(json.load(open(p)).get("bf16_tflops_sustained", 989.0))
+    return 989.0   # H100 SXM data sheet, dense BF16 / FP16 (not measured)
 
 
 class ClockSampler:
@@ -131,8 +131,8 @@ def pick_cpu_threads(run=None):
     headline ratio - moved 2x between driver runs; a full forward per candidate costs ~10 s in total and is stable."""
     import torch
     ncpu = os.cpu_count() or 1
-    # (all hardware threads is only a candidate up to 64: on the 128-thread host of the B200 boxes torch's CPU convolutions take
-    #  53 s per forward with 128 threads against 1.7 s with 16 - measured in round 2, profiles/r02_bench_reference.json)
+    # (all hardware threads is only a candidate up to 64: on 128-thread hosts torch's CPU convolutions can be an order of
+    #  magnitude slower with every thread than with 16)
     cands = sorted({c for c in (16, 32, 64, ncpu if ncpu <= 64 else 64) if c <= ncpu}) or [ncpu]
     if run is None or len(cands) == 1:
         torch.set_num_threads(cands[-1])
@@ -182,7 +182,7 @@ def oracle_forward_fn(win, device=None):
 
 
 def time_gpu_reference(win, local, steps=10, warmup=3):
-    """GPU comparator (VERDICT r01 item 3 / SURVEY 8d iii): the reference graph in eager PyTorch on cuDNN on the same B200,
+    """GPU comparator (VERDICT r01 item 3 / SURVEY 8d iii): the reference graph in eager PyTorch on cuDNN on the same GPU,
     timed with CUDA events outside our arm's timed regions: fp32 with TF32 off (bit-comparable arithmetic) and with TF32 on
     (what torch 1.9, the reference's libtorch, allows cuDNN by default).  Returns a dict for the JSON line."""
     import torch
@@ -326,7 +326,10 @@ def main():
     ap.add_argument("--e2e-inflight", type=int, default=4, choices=[1, 2, 3, 4, 5, 6, 7, 8],
                     help="handles used by the end-to-end leg (the first k of the --inflight handles); measured best at 4: with more, "
                          "the extra host threads and staging buffers cost more than the added overlap gives")
-    ap.add_argument("--tc", type=int, default=-1, help="1/0: force the tcgen05 conv path on/off (default: engine default)")
+    ap.add_argument("--tc", type=int, default=-1, help="1/0: force the tensor-core conv path on/off (default: engine default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the four stage-3 maps the last timed step computed (depth, confidence, "
+                         "depth_dense, confidence_dense: what GetResult returns) as DIR/<name>.npy, float32")
     ap.add_argument("--opt", action="append", default=[], help="engine option key=int for A/B runs, e.g. --opt fork_fpn=0")
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3) if a.impl == "ours" else a.warmup
@@ -412,6 +415,11 @@ def main():
         sampler.start()
     ms_dev, launches = DrMvsnet.run_resident_multi(hs, a.steps)   # K windows, one CUDA-event clock over all streams
     barrier()
+    if a.dump_outputs and rank == 0:
+        last = hs[(a.steps - 1) % len(hs)]                          # the handle that ran the last timed step (round robin)
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        for name in ("depth", "confidence", "depth_dense", "confidence_dense"):
+            np.save(os.path.join(a.dump_outputs, name + ".npy"), last.stage_output(3, name).astype(np.float32))
     ms_single, _ = m.run_resident(max(a.steps // 2, 1))            # one window at a time: the latency of a keyframe
     ms_single /= max(a.steps // 2, 1)
     barrier()
@@ -472,7 +480,7 @@ def main():
         value = world * a.steps / (ms_dev / 1e3)
         e2e = world * a.steps / (ms_e2e / 1e3)
         # roofline, measured live: per-kernel CUDA-event durations of one forward (m.profile()) with each record's
-        # algorithmic bytes / flops.  Reported per FAMILY (tcgen05 convs / cost volume / tail) and for the whole step; the
+        # algorithmic bytes / flops.  Reported per FAMILY (tensor-core convs / cost volume / tail) and for the whole step; the
         # "dominant kernel" entry the contract asks for is the largest single record.
         rows = m.profile()
         tot = sum(r[1] for r in rows)

@@ -1,4 +1,4 @@
-/* tandem_b200 — C ABI of the B200-native replacement for TANDEM's libdr (dense per-frame hot path).
+/* tandem_b200 — C ABI of the H100-native (sm_90a) replacement for TANDEM's libdr (dense per-frame hot path).
  *
  * One opaque handle per object, int return codes (0 = ok, <0 = error, text via tdm_last_error()),
  * no exceptions and no C++/torch types across the boundary, all pointers caller-owned unless stated.
@@ -28,7 +28,7 @@ extern "C" {
 
 /* Thread-local text of the last error raised by any tdm_* call on this thread. */
 const char* tdm_last_error(void);
-/* Library / build identification: "tandem_b200 <version> sm_100a". */
+/* Library / build identification: "tandem_b200 <version> sm_90a". */
 const char* tdm_version(void);
 /* Number of CUDA devices visible (0 on a CPU-only box; never throws). */
 int tdm_device_count(void);
@@ -96,9 +96,9 @@ int tdm_mvsnet_run_resident_multi(tdm_mvsnet* const* hs, int n, int iters_total,
  * a reference pixel (x, y) at depth d lands at rot (x, y, 1)^T d + trans in the source image. K row-major 3x3, poses row-major
  * 4x4 cam->world. */
 int tdm_debug_homography(const float* K3x3, const float* c2w_ref, const float* c2w_src, float* rot9, float* trans3);
-/* Host-only introspection (no GPU needed): the tile plan the tcgen05 convolution planner picks for a layer - cin, N columns of
+/* Host-only introspection (no GPU needed): the tile plan the tensor-core convolution planner picks for a layer - cin, N columns of
  * the MMA (npad, doubled for hi/lo weights), kd (1: 2-D over planes, 3: 3-D, 2: transposed-as-GEMM), the grid D x H x W the
- * tiles live on, pd (D halo), mode (0 stride-1, 1 transposed, 3 up2, 4 input-stationary), shared-memory budget in KB.
+ * tiles live on, pd (D halo), mode (0 stride-1, 1 transposed, 3 up2; +100: tiles span all D planes), shared-memory budget in KB.
  * out12 = {ring slots, tile rows, tile cols, pitch, planes per tile, 128-row chunks per plane, slot positions, tiles_w,
  * tiles_h, tiles_d, grid, shared-memory bytes}. */
 int tdm_debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out12);
@@ -216,9 +216,9 @@ long long tdm_fusion_dump_blocks(tdm_fusion* h, int* coords, void* voxels, size_
 int tdm_fusion_run_resident(tdm_fusion* h, int iters, float* ms_integrate, float* ms_render);
 int tdm_fusion_last_alloc_ms(tdm_fusion* h, float* ms);
 /* A/B switches for measurements (results are bit-identical either way): "alloc_filter" (CTA-level shared-memory filter in
- * front of the hash table during allocation), "raycast_cache8" (8-entry per-ray block cache); both default to 0 - measured
- * on B200 they do not pay (the table probes are L2 hits behind other latency); "raycast_persistent" (warps pull rays from a
- * counter and refill finished lanes; default 0 = one ray per thread, which measured faster: 0.82 vs 0.875 ms), "raycast_shared" (index arithmetic shared between the nine voxel reads of a sample, one block lookup when they sit in one
+ * front of the hash table during allocation), "raycast_cache8" (8-entry per-ray block cache); both default to 0 (the table
+ * probes are L2 hits behind other latency); "raycast_persistent" (warps pull rays from a
+ * counter and refill finished lanes; default 0 = one ray per thread), "raycast_shared" (index arithmetic shared between the nine voxel reads of a sample, one block lookup when they sit in one
  * block; default 1), "integrate_compact" (visibility pass + update of the
  * visible blocks only, default 1; 0 = every CTA scans the whole block list); "raycast_tile" (0: 16x16-pixel CTAs, 1: 8x8
  * (default), 2: 8x4, 3: 16x8); "raycast_dedup" (a sample whose eight corners straddle voxel-block faces looks every distinct

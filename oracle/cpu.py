@@ -206,7 +206,7 @@ class FrontOracle:
 
 class FrontRef:
     """oracle/_ref/libfront_ref.so: the REFERENCE's own makeImages / setCoarseTrackingRef bodies (HessianBlocks.cpp:128-191,
-    CoarseTracker.cpp:655-725) compiled from where they lie by oracle/ref_build.mk (build container only). Pins FrontOracle."""
+    CoarseTracker.cpp:655-725) compiled from where they lie by oracle/ref_build.mk; used by oracle/gen_reference_pins.py."""
 
     PATH = os.path.join(_HERE, "_ref", "libfront_ref.so")
 

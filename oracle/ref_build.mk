@@ -1,9 +1,12 @@
-# Build-container-only recipe: compiles the REFERENCE's own CUDA sources, unmodified and from where they lie under
-# /root/reference, into oracle/_ref/ (git-ignored; travels to the GPU box with the snapshot).  Nothing is copied into
-# the repo.  The reference's CMake build is not used (needs OpenCV/Eigen/Boost, none installed).
-REF := /root/reference/tandem/libdr
+# Compiles the REFERENCE's own sources, unmodified and from where they lie in a checkout of the reference
+# (make -f ref_build.mk REFERENCE=<dir>), into oracle/_ref/ (git-ignored).  Nothing is copied into the repo.  Only
+# oracle/gen_reference_pins.py uses the result.  The reference's CMake build is not used (it needs OpenCV/Eigen/Boost).
+ifndef REFERENCE
+$(error set REFERENCE to the root of a checkout of the reference)
+endif
+REF := $(REFERENCE)/tandem/libdr
 NVCC ?= /usr/local/cuda/bin/nvcc
-ARCH := -gencode arch=compute_100a,code=sm_100a
+ARCH := -gencode arch=compute_90a,code=sm_90a
 OUT := _ref
 FUS := $(REF)/dr_fusion/src
 FUS_SRCS := $(FUS)/tsdfvh/heap.cu $(FUS)/tsdfvh/hash_table.cu $(FUS)/tsdfvh/tsdf_volume.cu $(FUS)/marching_cubes/mesh.cu \
@@ -26,7 +29,7 @@ $(OUT)/libtracker_ref.so: ref_wrap_tracker.cu
 # n1 / n2 pins (SURVEY.md 8f): two function bodies of tandem/src/FullSystem, cut out of the files where they lie (line ranges
 # as cited in oracle/front_oracle.c) into _ref/gen/ (build output, git-ignored - nothing is copied into the repo) and
 # compiled, unmodified, against the stand-in Eigen of tests/cpp/eigen_stub and the harness ref_wrap_front.cpp.  CPU only.
-FS := /root/reference/tandem/src/FullSystem
+FS := $(REFERENCE)/tandem/src/FullSystem
 CXX ?= g++
 all: $(OUT)/libfront_ref.so
 $(OUT)/gen/make_images.inc: $(FS)/HessianBlocks.cpp

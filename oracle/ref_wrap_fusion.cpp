@@ -1,7 +1,7 @@
 // Test infrastructure: C entry points around the REFERENCE's own `class DrFusion`
 // (tandem/libdr/dr_fusion/src/dr_fusion/dr_fusion.h), compiled unmodified from /root/reference by
 // oracle/ref_build.mk into oracle/_ref/libdr_fusion_ref.so.  Used only by tests (-m gpu) to pin our CPU oracle and
-// CUDA path against the reference run on the same B200, and as an on-box GPU baseline in profiles/.
+// CUDA path against the reference (oracle/gen_reference_pins.py) and as a GPU baseline (tools/bench_fusion_tracker.py).
 #include <cstdlib>
 #include <cstring>
 #include <vector>

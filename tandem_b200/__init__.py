@@ -1,4 +1,4 @@
-"""tandem_b200: B200-native (sm_100a) implementation of TANDEM's dense per-frame hot path behind the
+"""tandem_b200: H100-native (sm_90a) implementation of TANDEM's dense per-frame hot path behind the
 libdr call surface (DrMvsnet / DrFusion / CudaCoarseTracker).  Python here is only the host-side mirror
 of those classes over the C ABI in include/tandem_b200.h; all compute is in libtandem_b200.so."""
 from ._lib import TandemError, lib  # noqa: F401

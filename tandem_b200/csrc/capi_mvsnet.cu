@@ -20,7 +20,7 @@ struct tdm_mvsnet {
 extern "C" {
 
 const char* tdm_last_error(void) { return tdm::g_last_error.c_str(); }
-const char* tdm_version(void) { return "tandem_b200 0.1.0 sm_100a"; }
+const char* tdm_version(void) { return "tandem_b200 0.1.0 sm_90a"; }
 int tdm_device_count(void) {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }

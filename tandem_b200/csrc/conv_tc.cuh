@@ -1,26 +1,23 @@
-// Generation-2 convolution: im2col-free implicit GEMM on the 5th-gen tensor cores (tcgen05 / TMEM), fed by 1-D
-// TMA bulk copies.  Replaces cuDNN's per-layer library calls of the reference (module.forward, dr_mvsnet.cpp:294)
-// for every stride-1 3x3(x3) convolution of FeatureNet / CostRegNet (module.py:496-531, 577-600).
+// Tensor-core convolution: im2col-free implicit GEMM on Hopper's warpgroup MMA (wgmma), fed by tiled TMA.  Replaces
+// cuDNN's per-layer library calls of the reference (module.forward, dr_mvsnet.cpp:294) for every stride-1 3x3(x3)
+// convolution of FeatureNet / CostRegNet (module.py:496-531, 577-600).
 //
 // Formulation ("flattened zero-haloed planes"): activations are P8, i.e. [C/8][D+2][H+2][W+2][8] with zero halos
 // (mvsnet_kernels.cuh).  A CTA owns an output tile of R rows x TW columns x DR planes.  For every input plane it
-// needs, (R+2) row segments of TW+2 positions per channel group are copied with cp.async.bulk into a shared-memory
-// tile of pitch P = TW+2 positions.  Flattening (row, col) -> l = row*P + col makes every tap (kh,kw) a CONSTANT
-// shift kh*P + kw of l, so the A operand of tap (kd,kh,kw) for the 128 output positions l0..l0+127 is the same
-// shared-memory tile read through a descriptor whose start address is advanced by (l0 + kh*P + kw)*16 bytes:
-//   K-major, SWIZZLE_NONE canonical layout  ((8,m),(8,2)) : ((16 B, SBO = 128 B), (2 B, LBO))
+// needs, (R+2) row segments of TW+2 positions per channel group are copied by TMA into a shared-memory tile of pitch
+// P = TW+2 positions.  Flattening (row, col) -> l = row*P + col makes every tap (kh,kw) a CONSTANT shift kh*P + kw of
+// l, so the A operand of tap (kd,kh,kw) for the 64 output positions l0..l0+63 is the same shared-memory tile read
+// through a descriptor whose start address is advanced by (l0 + kh*P + kw)*16 bytes:
+//   K-major, no-swizzle canonical layout  ((8,m),(8,2)) : ((16 B, SBO = 128 B), (2 B, LBO))
 //   rows = positions (16 B apart), SBO = 8 positions, LBO = distance between the two 8-channel halves of a K=16 step
 //   (the next channel group's plane for CIN >= 16, the next tap's shift for CIN == 8).
 // Outputs computed for the 2 pad columns of each row are garbage and masked in the epilogue (utilisation TW/(TW+2)).
 // B (weights, all taps) is pre-arranged on the host in the same canonical core-matrix order and stays resident.
-// Accumulators live in TMEM, double-buffered per output plane, so the epilogue (tcgen05.ld -> bias/ReLU/skip ->
-// 16-byte stores) of plane d overlaps the MMAs of plane d+1.
 //
-// Warp roles (256 threads): warp 0 = TMA producer (one lane); warps 1,6,7 = MMA issuers (warp-uniform code, one elected
-// lane issues; chunk c of a plane belongs to issuer c mod 3 - a single issuing thread needs ~60 cycles of descriptor
-// arithmetic per tcgen05.mma, more than the ~36 cycles the tensor core needs to stream the 4.5 KB of operands, so the
-// issue work is spread over three warps); warp 1 also owns the TMEM allocation; warps 2..5 = epilogue (TMEM lane
-// quarter = warp_id % 4).
+// Roles (288 threads): warpgroups 0 and 1 consume, warp 8 produces (one lane issues the TMA copies).  A plane's
+// 64-position sub-chunks alternate between the two consumer warpgroups; each accumulates its sub-chunk in registers
+// (m64nNk16, one instruction per K=16 step) and runs the epilogue (bias / ReLU / skip / store) straight from the
+// accumulator fragment, so one warpgroup's epilogue overlaps the other's MMAs.
 #pragma once
 #include <cuda.h>
 
@@ -33,11 +30,6 @@
 namespace tdm {
 namespace tc {
 
-#ifdef TDM_TIMING_EXPERIMENTS
-#define TDM_DBG_MODE(g) ((g).dbg_aligned)
-#else
-#define TDM_DBG_MODE(g) 0
-#endif
 struct Geom {
   int D, H, W;            // output == input dims (stride 1, pad 1)
   int Hp, Wp;             // H+2, W+2
@@ -45,7 +37,7 @@ struct Geom {
   long long in_gs, out_gs, res_gs;   // channel-group strides in elements
   int R, TW, DR;          // tile: rows, cols, output planes
   int P;                  // TW + 2
-  int nch;                // 128-position chunks per plane = ceil(R*P / 128)
+  int nch;                // 128-position chunks per plane = ceil(R*P / 128), each two 64-position wgmma sub-chunks
   int slot_pos;           // positions per (ring slot, channel group)
   int tiles_w, tiles_h, tiles_d;
   int relu, has_res;
@@ -53,8 +45,6 @@ struct Geom {
   int S;                  // ring slots
   int oHp, oWp, opd;      // padded dims / D halo of the OUTPUT tensor (differs from the input in deconv mode)
   int iDp;                // padded plane count of the input: tensor-map dim 3 = channel_group * iDp + plane
-  int dbg_aligned;        // only read when built with -DTDM_TIMING_EXPERIMENTS (env TDM_DEBUG_ALIGNED_TAPS; WRONG RESULTS, timing only):
-                          // 1 = every tap reads a 128-byte aligned A tile, 2 = a third of the MMA instructions, 3 = no epilogue work, 4 = 2 + 3
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -92,30 +82,75 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  // SmemDescriptor (cute/arch/mma_sm100_desc.hpp): start[0,14) lbo[16,30) sbo[32,46) version[46,48)=1 layout[61,64)=0
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46);
+// wgmma shared-memory matrix descriptor (sm_90): start[0,14) lbo[16,30) sbo[32,46), all in 16-byte units; base offset 0,
+// layout type 0 (no swizzle).  SBO is always 128 B (8 rows of 16 B), so the high word is a constant.
+constexpr uint32_t kDescHi = 128u >> 4;
+__device__ __forceinline__ uint64_t desc(uint32_t start16, uint32_t lbo16) {
+  return ((uint64_t)kDescHi << 32) | (uint64_t)((start16 & 0x3FFFu) | (lbo16 << 16));
 }
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], both operands K-major in shared memory, fp32 accumulators in registers.
+// Fragment: d[4j + 2i + e] is row (warp % 4) * 16 + lane / 4 + 8i, column 8j + 2 * (lane % 4) + e.
+template <int N, typename T> __device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc);
+template <> __device__ __forceinline__ void wgmma<16, __half>(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(acc));
 }
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
+template <> __device__ __forceinline__ void wgmma<16, __nv_bfloat16>(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(acc));
 }
+template <> __device__ __forceinline__ void wgmma<32, __half>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<32, __nv_bfloat16>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<64, __half>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<64, __nv_bfloat16>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<128, __half>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<128, __nv_bfloat16>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
 // Tiled TMA load of one box of a 4-D tensor map (SASS: UTMALDG); out-of-bounds elements are zero-filled.
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* tmap, int x0, int x1, int x2, int x3, uint64_t* bar) {
@@ -126,42 +161,79 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* tmap, 
       : "memory");
 }
 
-
 // Programmatic dependent launch: a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start
-// while its predecessor drains; everything before pdl_wait() (barrier init, TMEM allocation, the weight image load)
-// overlaps the predecessor's tail, everything that touches activations comes after it.
+// while its predecessor drains; everything before pdl_wait() (barrier init, the weight image load) overlaps the
+// predecessor's tail, everything that touches activations comes after it.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-constexpr int kThreads = 384;   // warp 0 TMA, warps 1,6,7 MMA (warp 1 also TMEM alloc), warps 2..5 + 8..11 epilogue
-constexpr int kEpiGroups = 2;   // two epilogue warpgroups alternate over the chunks of a plane (TMEM lane quarter = warp % 4)
-constexpr int kMmaWarps = 3;
+constexpr int kConsumerWG = 2;                       // consumer warpgroups (warps 0..7)
+constexpr int kThreads = 128 * kConsumerWG + 32;     // + the producer warp
+constexpr int kProducerWarp = 4 * kConsumerWG;
+
+// One 64-position sub-chunk of one output plane: every (kd, K=16 step) is one wgmma.  aoff(b) is the A offset of step b
+// inside an input plane's ring slot, alo(b) its LBO (16-byte units); B block (kd, b) starts at b_base16 + (kd*NBLK+b)*N*2.
+template <int N, typename T, int KD, int NBLK, typename AOff, typename ALbo>
+__device__ __forceinline__ void mma_subchunk(float (&acc)[N / 2], const uint32_t (&slot16)[KD], uint32_t sub16, uint32_t b_base16,
+                                             uint32_t b_lbo16, AOff aoff, ALbo alo) {
+  wgmma_fence();
+#pragma unroll
+  for (int kd = 0; kd < KD; ++kd) {
+#pragma unroll
+    for (int b = 0; b < NBLK; ++b) {
+      const uint64_t ad = desc(slot16[kd] + sub16 + aoff(b), alo(b));
+      const uint64_t bd = desc(b_base16 + (uint32_t)((kd * NBLK + b) * N * 2), b_lbo16);
+      wgmma<N, T>(acc, ad, bd, (kd | b) != 0 ? 1u : 0u);
+    }
+  }
+  wgmma_commit();
+  wgmma_wait_all();
+}
+
+// Two consecutive channels of an 8-channel group: one 4-byte store / load.
+template <typename T> __device__ __forceinline__ void store2(T* p, float x0, float x1) {
+  T v[2] = {from_f<T>(x0), from_f<T>(x1)};
+  *reinterpret_cast<uint32_t*>(p) = *reinterpret_cast<const uint32_t*>(v);
+}
+template <typename T> __device__ __forceinline__ void load2(const T* p, float& x0, float& x1) {
+  const uint32_t u = __ldg(reinterpret_cast<const unsigned int*>(p));
+  const T* v = reinterpret_cast<const T*>(&u);
+  x0 = to_f<T>(v[0]); x1 = to_f<T>(v[1]);
+}
+
+// Per-pixel tail of the OUT_PLAIN (prob) instantiation: with tiles that span all D planes (make_plan(full_depth)) the thread
+// that stored a pixel's D logits is the same for every plane, so once the tile's last plane is stored it can finish the
+// pixel (softmax / soft-argmin / confidence, module.py:1116-1133) without another launch.  NoTail = plain convolution.
+struct NoTail {
+  static constexpr bool enabled = false;
+  __device__ __forceinline__ void operator()(const float*, int, int, int, int) const {}
+};
 
 // blocks of B per kd plane: one block = one K=16 MMA step = NPAD x 16 elements in canonical order
 // MODE 0: 3x3 stencil per plane (9 taps).  MODE 1: transposed conv k3 s2 p1 op1 as a GEMM over the INPUT grid: 2x2 taps
 // per plane at offsets {0,1}^2 (stencil positions (1..2,1..2)), 2 planes, N = 8 output parity classes x COUT.
 template <int CIN, int MODE = 0> constexpr int blocks_per_kd() { return MODE == 1 ? 4 * (CIN / 16) : (CIN >= 16 ? 9 * (CIN / 16) : 5); }  // MODE 3 == MODE 0 geometry
 
-// AFMT: 0 = f16, 1 = bf16 (a_format/b_format of the instruction descriptor).  OUT_PLAIN: fp32 [D][H][W] (prob conv).
+// OUT_PLAIN: fp32 [D][H][W] (prob conv).
 // HILO: the B image carries every weight twice, as W_hi = round16(W) in columns [0,NPAD) and W_lo = round16(W - W_hi)
 // in columns [NPAD, 2*NPAD); the MMA runs with N = 2*NPAD and the epilogue adds the two halves, which restores ~fp32
-// weight precision.  It is free here: at N <= 64 the instruction is bound by streaming the 4 KB A operand, not by N.
-template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool OUT_PLAIN, int MODE = 0, bool HILO = false>
+// weight precision at the cost of a wider N.
+template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool OUT_PLAIN, int MODE = 0, bool HILO = false, typename Tail = NoTail>
 __global__ void __launch_bounds__(kThreads, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, groups*planes}, box {8, P, R+2, 1}*/,
           const TIn* __restrict__ bimg /*host-arranged B image*/, const float* __restrict__ bias,
-          const TOut* __restrict__ res, TOut* __restrict__ out, float* __restrict__ plain_out, const __grid_constant__ Geom g) {
+          const TOut* __restrict__ res, TOut* __restrict__ out, float* __restrict__ plain_out, const __grid_constant__ Geom g,
+          const __grid_constant__ Tail tail) {
+  static_assert(!Tail::enabled || OUT_PLAIN, "a per-pixel tail only exists for the single-channel fp32 output");
   constexpr int CG = CIN / 8;
   constexpr int NBLK = blocks_per_kd<CIN, MODE>();
-  constexpr int NMMA = HILO ? 2 * NPAD : NPAD;   // instruction N and TMEM columns per chunk
+  constexpr int NMMA = HILO ? 2 * NPAD : NPAD;   // instruction N
   static_assert(!(HILO && MODE == 1), "hi/lo weights are not wired for the 3-D transposed-conv epilogue");
   // MODE 3: 2-D "conv3x3 of a nearest-x2 up-sampled map" evaluated on the COARSE grid: 9 taps, N = 4 output parity
   // classes x COUT (the 3x3 fine taps collapse onto 2x2 coarse neighbours; weights pre-summed on the host).
   constexpr int B_BYTES = KD * NBLK * NMMA * 32;
   constexpr int PLANE0 = MODE == 1 ? 1 : 0;
   constexpr bool CLASS_EPI = MODE == 1 || MODE == 3;   // deconv reads input planes d and d+1 (padded indices d+1, d+2)
-  constexpr uint32_t AFMT = std::is_same<TIn, __nv_bfloat16>::value ? 1u : 0u;
-  constexpr uint32_t IDESC = (1u << 4) | (AFMT << 7) | (AFMT << 10) | ((uint32_t)(NMMA >> 3) << 17) | ((128u >> 4) << 24);
 
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* sB = smem;
@@ -171,10 +243,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
   uint64_t* bars = reinterpret_cast<uint64_t*>(sA + (size_t)slot_bytes * g.S);
   uint64_t* full = bars;                 // [S]
   uint64_t* empty = bars + 8;            // [S]
-  uint64_t* acc_full = bars + 16;        // [2]
-  uint64_t* acc_empty = bars + 18;       // [2]
-  uint64_t* b_full = bars + 20;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 21);
+  uint64_t* b_full = bars + 16;
 
   // N-slicing (blockIdx.y): wide outputs (CIN = 64 layers, whose full B image would not fit shared memory) are split into
   // slices of NPAD columns, each with its own contiguous B image; slice ns produces output columns [ns*NPAD, (ns+1)*NPAD).
@@ -189,32 +258,21 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
   const int w0 = tw * g.TW, h0 = th * g.R, d0 = td * g.DR;
   const int ndo = min(g.DR, g.D - d0);             // output planes of this tile
   const int nin = ndo + KD - 1;                    // input planes to stream
-  const uint32_t acc_cols = (uint32_t)g.nch * NMMA;  // TMEM columns per accumulator buffer
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < 2 * acc_cols) tmem_cols <<= 1;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < g.S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kMmaWarps); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], kMmaWarps); mbar_init(&acc_empty[b], 4 * kEpiGroups); }
+    for (int s = 0; s < g.S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4 * kConsumerWG); }
     mbar_init(b_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     mbar_expect_tx(b_full, B_BYTES);          // weights do not depend on the previous kernel: fetch them before pdl_wait
     bulk_g2s(sB, bimg, B_BYTES, b_full);
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
   pdl_wait();   // from here on activations written by the previous kernel are read and our outputs are written
   // trigger the dependents only now: a trigger BEFORE the wait lets the whole chain of later kernels become resident early (each
   // one's prologue would trigger the next), and their idle CTAs then hold the shared memory the running kernel's tiles need
   if (threadIdx.x == 0) pdl_launch_dependents();
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       // one tiled TMA per (plane, channel group): box = (R+2) rows x P positions, rows / columns beyond the tensor are
@@ -230,195 +288,117 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
           tma_load_4d(sA + (size_t)slot * slot_bytes + (size_t)cg * cg_bytes, &tmap, 0, w0, h0, cg * g.iDp + pp, &full[slot]);
       }
     }
-  } else if (warp == 1 || warp == 6 || warp == 7) {
-    // ===================== MMA issuers (warp-uniform; one elected lane issues) =====================
-    const int issuer = warp == 1 ? 0 : warp - 5;   // 0,1,2
-    const bool leader = lane == 0;
-    {
-      // Descriptor deltas are loop invariants: a K=16 step b of any plane / chunk reads A at (slot + chunk + a_off[b])
-      // and B at block (kd*NBLK + b).  Everything below is in the descriptor's 16-byte units.
-      uint32_t a_off[NBLK], a_lbo[NBLK];
-#pragma unroll
-      for (int b = 0; b < NBLK; ++b) {
-        if constexpr (MODE == 1) {
-          const int t = b / (CIN / 16), j = b % (CIN / 16);
-          a_off[b] = (uint32_t)(2 * j) * (cg_bytes >> 4) + (uint32_t)((1 + t / 2) * g.P + (1 + t % 2));
-          a_lbo[b] = cg_bytes >> 4;
-        } else if constexpr (CIN >= 16) {
-          const int t = b / (CIN / 16), j = b % (CIN / 16);
-          a_off[b] = (uint32_t)(2 * j) * (cg_bytes >> 4) + (uint32_t)((t / 3) * g.P + (t % 3));
-          a_lbo[b] = cg_bytes >> 4;
-        } else {
-          // taps are paired (0,1)(2,3)(4,5)(6,7)(7*,8): the 5th block re-reads tap 7 against zero weights so that no
-          // K slice ever touches shared memory outside the copied tile
-          const int t0 = b < 4 ? 2 * b : 7, t1 = b < 4 ? 2 * b + 1 : 8;
-          const int o0 = (t0 / 3) * g.P + (t0 % 3), o1 = (t1 / 3) * g.P + (t1 % 3);
-          a_off[b] = (uint32_t)o0;
-          a_lbo[b] = (uint32_t)(o1 - o0);
-        }
-      }
-      const uint32_t desc_hi = (128u >> 4) | (1u << 14);            // SBO = 128 B, version = 1 (bits 46..47 of the desc)
-      const uint32_t sB16 = (smem_u32(sB) & 0x3FFFFu) >> 4, sA16 = (smem_u32(sA) & 0x3FFFFu) >> 4;
-      const uint32_t b_lo_base = sB16 | ((uint32_t)(NMMA * 16 >> 4) << 16);
-      mbar_wait(b_full, 0);
-      int next_wait = 0;
-      for (int od = 0; od < ndo; ++od) {
-        const int buf = od & 1;
-        if (od >= 2) mbar_wait(&acc_empty[buf], ((od >> 1) - 1) & 1);
-        while (next_wait <= od + KD - 1) {
-          mbar_wait(&full[next_wait % g.S], (next_wait / g.S) & 1);
-          ++next_wait;
-        }
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t slot16[KD];
-#pragma unroll
-        for (int kd = 0; kd < KD; ++kd) slot16[kd] = sA16 + (uint32_t)((od + kd) % g.S) * (slot_bytes >> 4);
-        for (int c = issuer; c < g.nch; c += kMmaWarps) {
-          const uint32_t d_tmem = tmem_base + (uint32_t)(buf * acc_cols + c * NMMA);
-#pragma unroll
-          for (int kd = 0; kd < KD; ++kd) {
-            const uint32_t a16 = slot16[kd] + (uint32_t)c * 128u;
-#pragma unroll
-            for (int b = 0; b < NBLK; ++b) {
-              const uint64_t ad = ((uint64_t)desc_hi << 32) | (uint64_t)((a16 + a_off[b]) | (a_lbo[b] << 16));
-              const uint64_t bd = ((uint64_t)desc_hi << 32) | (uint64_t)(b_lo_base + (uint32_t)((kd * NBLK + b) * NMMA * 2));
-              if (leader) mma_f16(d_tmem, ad, bd, IDESC, (kd | b) != 0 ? 1u : 0u);
-            }
-          }
-        }
-        if (leader) {
-          mma_commit(&acc_full[buf]);         // this issuer's share of plane od complete -> epilogue (3 arrivals)
-          mma_commit(&empty[od % g.S]);       // oldest input plane no longer needed by this issuer -> producer may refill
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const int egroup = warp >= 8 ? 1 : 0;
-    for (int od = 0; od < ndo; ++od) {
-      const int buf = od & 1;
-      mbar_wait(&acc_full[buf], (od >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int d = d0 + od;
-      for (int c = egroup; c < g.nch; c += kEpiGroups) {
-        const int l = c * 128 + q * 32 + lane;
-        const int hh = l / g.P, ww = l - hh * g.P;
-        const int h = h0 + hh, w = w0 + ww;
-        const bool valid = hh < g.R && ww < g.TW && h < g.H && w < g.W;
-        const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * acc_cols + c * NMMA);
-        if constexpr (CLASS_EPI) {
-          // N = 8 (MODE 1) or 4 (MODE 3) parity classes x COUT: class (pd,ph,pw) of input position (d,h,w) is output (2d+pd, 2h+ph, 2w+pw)
-          const int COUT = g.cout;
-          // All skip-tensor reads of this row are issued up front (NPAD/8 independent 16-byte loads): with only four
-          // epilogue warps per SM, eight dependent load->add->store round trips per chunk would serialise ~600 clk of
-          // HBM latency each and make the epilogue 20x slower than the MMAs that feed it.
-          uint4 rbuf[NPAD / 8];
-          if (valid && g.has_res) {
-#pragma unroll
-            for (int k = 0; k < NPAD / 8; ++k) {
-              const int n = ns * NPAD + k * 8;
-              const int cls = n / COUT, co = n % COUT;
-              const int od2 = MODE == 1 ? 2 * d + (cls >> 2) : d, oh2 = 2 * h + ((cls >> 1) & 1), ow2 = 2 * w + (cls & 1);
-              const long long pos = ((((long long)(od2 + g.opd)) * g.oHp + (oh2 + 1)) * g.oWp + (ow2 + 1)) * 8;
-              rbuf[k] = __ldg(reinterpret_cast<const uint4*>(res + pos + (co >> 3) * g.res_gs));
-            }
-          }
-#pragma unroll
-          for (int n0 = 0; n0 < NPAD; n0 += 16) {
-            uint32_t v[16];
-            tmem_ld16(t_row + (uint32_t)n0, v);
-            if constexpr (HILO) {
-              uint32_t v2[16];
-              tmem_ld16(t_row + (uint32_t)(NPAD + n0), v2);
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(v2[i]));
-            }
-            if (valid) {
-#pragma unroll
-              for (int k0 = 0; k0 < 16; k0 += 8) {
-                const int n = ns * NPAD + n0 + k0;
-                const int cls = n / COUT, co = n % COUT;
-                const int od2 = MODE == 1 ? 2 * d + (cls >> 2) : d, oh2 = 2 * h + ((cls >> 1) & 1), ow2 = 2 * w + (cls & 1);
-                const long long pos = ((((long long)(od2 + g.opd)) * g.oHp + (oh2 + 1)) * g.oWp + (ow2 + 1)) * 8;
-                float o8[8];
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  float x = __uint_as_float(v[k0 + i]) + (bias ? bias[co + i] : 0.f);
-                  if (g.relu) x = fmaxf(x, 0.f);
-                  o8[i] = x;
-                }
-                if (g.has_res) {
-                  const TOut* rv = reinterpret_cast<const TOut*>(&rbuf[(n0 + k0) / 8]);
-#pragma unroll
-                  for (int i = 0; i < 8; ++i) o8[i] += to_f<TOut>(rv[i]);
-                }
-                store_vec<TOut, 8>(out + pos + (co >> 3) * g.out_gs, o8);
-              }
-            }
-          }
-        } else {
-          uint4 rbuf[NPAD / 8];
-          const long long pos0 = ((((long long)(d + g.pd)) * g.Hp + (h + 1)) * g.Wp + (w + 1)) * 8;
-          if constexpr (!OUT_PLAIN) {
-            if (valid && g.has_res) {   // skip-tensor reads issued before the TMEM loads (latency overlap)
-#pragma unroll
-              for (int k = 0; k < NPAD / 8; ++k)
-                if (ns * NPAD + k * 8 < g.cout)
-                  rbuf[k] = __ldg(reinterpret_cast<const uint4*>(res + pos0 + ((ns * NPAD + k * 8) >> 3) * g.res_gs));
-            }
-          }
-          uint32_t v[16];
-          float acc[NPAD];
-#pragma unroll
-          for (int n0 = 0; n0 < NPAD; n0 += 16) {
-            tmem_ld16(t_row + (uint32_t)n0, v);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) acc[n0 + i] = __uint_as_float(v[i]);
-            if constexpr (HILO) {
-              tmem_ld16(t_row + (uint32_t)(NPAD + n0), v);
-#pragma unroll
-              for (int i = 0; i < 16; ++i) acc[n0 + i] += __uint_as_float(v[i]);
-            }
-          }
-          if (valid) {
-            if constexpr (OUT_PLAIN) {
-              plain_out[((long long)d * g.H + h) * g.W + w] = acc[0] + (bias ? bias[0] : 0.f);
-            } else {
-              const long long pos = ((((long long)(d + g.pd)) * g.Hp + (h + 1)) * g.Wp + (w + 1)) * 8;
-#pragma unroll
-              for (int c0 = 0; c0 < NPAD; c0 += 8) {
-                const int co = ns * NPAD + c0;
-                if (co < g.cout) {
-                  float o8[8];
-#pragma unroll
-                  for (int i = 0; i < 8; ++i) {
-                    float x = acc[c0 + i] + (bias ? bias[co + i] : 0.f);
-                    if (g.relu) x = fmaxf(x, 0.f);
-                    o8[i] = x;
-                  }
-                  if (g.has_res) {
-                    const TOut* rv = reinterpret_cast<const TOut*>(&rbuf[c0 / 8]);
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) o8[i] += to_f<TOut>(rv[i]);
-                  }
-                  store_vec<TOut, 8>(out + pos + (co >> 3) * g.out_gs, o8);
-                }
-              }
-            }
-          }
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
-    }
+    return;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
+  // ===================== consumers: MMA + epilogue =====================
+  const int wg = warp >> 2, wq = warp & 3;
+  const int P = g.P;
+  const uint32_t cgb16 = cg_bytes >> 4;
+  // A offset / LBO of K=16 step b inside a ring slot, in 16-byte units
+  auto aoff = [&](int b) -> uint32_t {
+    if constexpr (MODE == 1) {
+      const int t = b / (CIN / 16), j = b % (CIN / 16);
+      return (uint32_t)(2 * j) * cgb16 + (uint32_t)((1 + t / 2) * P + (1 + t % 2));
+    } else if constexpr (CIN >= 16) {
+      const int t = b / (CIN / 16), j = b % (CIN / 16);
+      return (uint32_t)(2 * j) * cgb16 + (uint32_t)((t / 3) * P + (t % 3));
+    } else {
+      // taps are paired (0,1)(2,3)(4,5)(6,7)(7*,8): the 5th step re-reads tap 7 against zero weights so that no K slice
+      // ever touches shared memory outside the copied tile
+      const int t0 = b < 4 ? 2 * b : 7;
+      return (uint32_t)((t0 / 3) * P + (t0 % 3));
+    }
+  };
+  auto alo = [&](int b) -> uint32_t {
+    if constexpr (MODE == 1 || CIN >= 16) {
+      return cgb16;
+    } else {
+      const int t0 = b < 4 ? 2 * b : 7, t1 = b < 4 ? 2 * b + 1 : 8;
+      return (uint32_t)(((t1 / 3) - (t0 / 3)) * P + (t1 % 3) - (t0 % 3));
+    }
+  };
+  const uint32_t sB16 = smem_u32(sB) >> 4, sA16 = smem_u32(sA) >> 4;
+  const uint32_t b_lbo16 = (uint32_t)(NMMA * 16 >> 4);
+  const int nsub = 2 * g.nch;                      // 64-position sub-chunks per plane
+  mbar_wait(b_full, 0);
+  int next_wait = 0;
+  for (int od = 0; od < ndo; ++od) {
+    while (next_wait <= od + KD - 1) {
+      mbar_wait(&full[next_wait % g.S], (next_wait / g.S) & 1);
+      ++next_wait;
+    }
+    uint32_t slot16[KD];
+#pragma unroll
+    for (int kd = 0; kd < KD; ++kd) slot16[kd] = sA16 + (uint32_t)((od + kd) % g.S) * (slot_bytes >> 4);
+    const int d = d0 + od;
+    for (int sc = wg; sc < nsub; sc += kConsumerWG) {
+      float acc[NMMA / 2];
+      mma_subchunk<NMMA, TIn, KD, NBLK>(acc, slot16, (uint32_t)sc * 64u, sB16, b_lbo16, aoff, alo);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int l = sc * 64 + wq * 16 + (lane >> 2) + 8 * i;
+        const int hh = l / P, ww = l - hh * P;
+        const int h = h0 + hh, w = w0 + ww;
+        if (!(hh < g.R && ww < g.TW && h < g.H && w < g.W)) continue;
+        if constexpr (OUT_PLAIN) {
+          if ((lane & 3) == 0) {
+            float x = acc[2 * i];
+            if constexpr (HILO) x += acc[4 * (NPAD / 8) + 2 * i];
+            plain_out[((long long)d * g.H + h) * g.W + w] = x + (bias ? bias[0] : 0.f);
+          }
+        } else {
+#pragma unroll
+          for (int j = 0; j < NPAD / 8; ++j) {
+            const int n = ns * NPAD + 8 * j + 2 * (lane & 3);
+            float x[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              x[e] = acc[4 * j + 2 * i + e];
+              if constexpr (HILO) x[e] += acc[4 * (j + NPAD / 8) + 2 * i + e];
+            }
+            long long pos;
+            int co;
+            if constexpr (CLASS_EPI) {
+              // N = 8 (MODE 1) or 4 (MODE 3) parity classes x COUT: class (pd,ph,pw) of input position (d,h,w) is output (2d+pd, 2h+ph, 2w+pw)
+              const int cls = n / g.cout;
+              co = n % g.cout;
+              const int od2 = MODE == 1 ? 2 * d + (cls >> 2) : d, oh2 = 2 * h + ((cls >> 1) & 1), ow2 = 2 * w + (cls & 1);
+              pos = ((((long long)(od2 + g.opd)) * g.oHp + (oh2 + 1)) * g.oWp + (ow2 + 1)) * 8;
+            } else {
+              co = n;
+              if (ns * NPAD + 8 * j >= g.cout) continue;
+              pos = ((((long long)(d + g.pd)) * g.Hp + (h + 1)) * g.Wp + (w + 1)) * 8;
+            }
+            const long long e0 = pos + (co >> 3) * g.out_gs + (co & 7);
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              x[e] += bias ? bias[co + e] : 0.f;
+              if (g.relu) x[e] = fmaxf(x[e], 0.f);
+            }
+            if (g.has_res) {
+              float r0, r1;
+              load2<TOut>(res + pos + (co >> 3) * g.res_gs + (co & 7), r0, r1);
+              x[0] += r0; x[1] += r1;
+            }
+            store2<TOut>(out + e0, x[0], x[1]);
+          }
+        }
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[od % g.S]);   // oldest input plane of od no longer read by this warp -> producer may refill
+  }
+  if constexpr (Tail::enabled) {
+    // ndo == D (host-checked): this thread wrote all D logits of its pixels itself (program order makes them visible to it)
+    if ((lane & 3) == 0) {
+      for (int sc = wg; sc < nsub; sc += kConsumerWG)
+        for (int i = 0; i < 2; ++i) {
+          const int l = sc * 64 + wq * 16 + (lane >> 2) + 8 * i;
+          const int hh = l / P, ww = l - hh * P;
+          const int h = h0 + hh, w = w0 + ww;
+          if (hh < g.R && ww < g.TW && h < g.H && w < g.W) tail(plain_out, h * g.W + w, w, h, g.H * g.W);
+        }
+    }
   }
 }
 
@@ -520,13 +500,11 @@ inline Plan make_plan(int cin, int npad, int kd, int D, int H, int W, int pd, in
   const size_t bbytes = (((size_t)kd * nblk * npad * 32) + 127) / 128 * 128;
   // Search (ring depth, tile width, tile rows, planes per tile) for the cheapest feasible tiling.
   // cost = L2 bytes per useful output position (halo re-reads in h, w and d)
-  //        x MMA rows issued per useful position (pad columns, partial last chunk; weighted 1/4: MMA is not the limiter)
-  //        x wave quantisation on 148 SMs (one CTA per SM: time ~ ceil(T/148) tile-times for T tiles)
+  //        x MMA rows issued per useful position (pad columns, partial last chunk)
+  //        x wave quantisation on the 132 SMs of an H100 SXM (one CTA per SM: time ~ ceil(T/132) tile-times for T tiles)
   double best_cost = 1e30;
   int bestR = 0, bestTW = 0, bestS = 0, bestDR = 0;
-  // mode 4 = input-stationary 3-D kernel (conv_tc_is.cuh): an input plane is consumed once -> ring of 3; its TMEM ring
-  // holds 4 plane accumulators per chunk
-  const int s_hi = mode == 4 ? 3 : (kd == 3 ? 4 : 3), s_lo = mode == 4 ? 3 : (kd == 3 ? 3 : 2);   // kd == 2 (deconv): 2 live + 1 prefetch
+  const int s_hi = kd == 3 ? 4 : 3, s_lo = kd == 3 ? 3 : 2;   // kd == 2 (deconv): 2 live + 1 prefetch
   for (int S = s_hi; S >= s_lo; --S) {
     for (int tiles_w = 1; tiles_w <= 20; ++tiles_w) {
       const int TW = (W + tiles_w - 1) / tiles_w;
@@ -538,7 +516,7 @@ inline Plan make_plan(int cin, int npad, int kd, int D, int H, int W, int pd, in
         const int nch = (R * P + 127) / 128;
         const int slot_pos = (std::max((R + 2) * P, nch * 128 + 2 * P + 2) + 8 + 7) / 8 * 8;
         const size_t smem = bbytes + (size_t)S * cg * slot_pos * 16 + 256;
-        if (smem > smem_limit || (mode == 4 ? 4 : 2) * nch * npad > 512) break;
+        if (smem > smem_limit) break;
         const int th_n = (H + R - 1) / R;
         for (int dsplit = 1; dsplit <= (full_depth ? 1 : D); ++dsplit) {
           const int DR = (D + dsplit - 1) / dsplit;
@@ -547,15 +525,11 @@ inline Plan make_plan(int cin, int npad, int kd, int D, int H, int W, int pd, in
           const double T = (double)tw_n * th_n * td_n;
           const double amp = (double)(R + 2) / R * (double)P / TW * (kd == 3 ? (double)(DR + 2) / DR : (kd == 2 ? (double)(DR + 1) / DR : 1.0));
           // estimated kernel time in clocks: waves x (per-CTA fixed cost + instruction stream), inflated by halo re-reads.
-          // Measured on B200: ~55 clk per instruction at N <= 64 (operand streaming), more for wide N; ~8.5 k clk per
-          // CTA for prologue (barriers, TMEM alloc, B image), pipeline fill and the last plane's drain.
-          const double clk_mma = mode == 4 ? 40.0 + 0.35 * 3 * npad : (mode == 1 ? 35.0 + 0.45 * npad : 45.0 + 0.35 * npad);
-          const int planes_in = mode == 4 ? DR + 2 : DR;                       // instruction streams per tile
-          const double per_plane = (double)nch * nblk * (mode == 4 ? 1.25 : (double)kd) * clk_mma;
-          // mode 4 is persistent over tiles (conv_tc_is.cuh): the ~8.5 k clk of prologue / fill / drain are paid once per CTA,
-          // a tile boundary costs ~1.5 k clk (plane-ring turnover)
-          const double tile_clk = (mode == 4 ? 1500.0 : 8500.0) + planes_in * per_plane;
-          const double cost = (std::ceil(T / 148.0) * tile_clk + (mode == 4 ? 8500.0 : 0.0)) * (1.0 + 0.25 * (amp - 1.0)) * (S == s_hi ? 1.0 : 1.05);
+          // The constants are a model (instruction cost growing with N, a fixed per-CTA prologue, fill and drain), not
+          // a measurement; they only rank tilings against each other.
+          const double clk_mma = mode == 1 ? 35.0 + 0.45 * npad : 45.0 + 0.35 * npad;
+          const double tile_clk = 8500.0 + (double)DR * nch * nblk * kd * clk_mma;
+          const double cost = std::ceil(T / 132.0) * tile_clk * (1.0 + 0.25 * (amp - 1.0)) * (S == s_hi ? 1.0 : 1.05);
           if (cost < best_cost - 1e-9) { best_cost = cost; bestR = R; bestTW = TW; bestS = S; bestDR = DR; }
           if (T > 4000) break;
         }

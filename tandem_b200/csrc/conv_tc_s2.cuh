@@ -1,13 +1,13 @@
 // Stride-2 convolutions (3x3x3 s2 p1 of CostRegNet conv1/conv3/conv5, module.py:544-552; 5x5 s2 p2 of FeatureNet
-// conv1.0/conv2.0, module.py:466-474) on tcgen05, fed by TILED TMA with element strides.
+// conv1.0/conv2.0, module.py:466-474) on wgmma, fed by TILED TMA with element strides.
 //
 // A stride-2 conv reads input position 2*o + k + c0 (c0 = 1 - pad in padded coordinates) for output o and tap k.  Along
-// the flattened (contiguous) W axis that is a stride of two positions = 32 B between MMA rows, which no canonical UMMA
+// the flattened (contiguous) W axis that is a stride of two positions = 32 B between MMA rows, which no canonical wgmma
 // layout can express.  The TMA engine de-interleaves instead: a tensor map over the P8 tensor with elementStrides
 // {1,2,2,1} loads every second column / row, so a tile's input plane lands in shared memory as 4 parity sub-tiles
 // (row parity x column parity), each a dense [R + KS/2][TW + KS/2][8] array.  Inside a sub-tile, tap (kh,kw) of output
 // (hh,ww) sits at (hh + kh/2)*P + (ww + kw/2): once more a CONSTANT shift of the flattened index, so everything
-// downstream (descriptors with SBO = 128 B, TMEM accumulators, epilogue) is the stride-1 machinery of conv_tc.cuh.
+// downstream (descriptors with SBO = 128 B, register accumulators, epilogue) is the stride-1 machinery of conv_tc.cuh.
 // Out-of-bounds rows / columns (the 5x5 kernels reach one position beyond the stored halo) are zero-filled by TMA.
 #pragma once
 #include "conv_tc.cuh"
@@ -41,8 +41,6 @@ k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ b
   constexpr int CG = CIN / 8;
   constexpr int NBLK = s2_blocks<CIN, KS>();
   constexpr int B_BYTES = KD * NBLK * NPAD * 32;
-  constexpr uint32_t AFMT = std::is_same<TIn, __nv_bfloat16>::value ? 1u : 0u;
-  constexpr uint32_t IDESC = (1u << 4) | (AFMT << 7) | (AFMT << 10) | ((uint32_t)(NPAD >> 3) << 17) | ((128u >> 4) << 24);
 
   extern __shared__ __align__(128) uint8_t smem[];
   const int ns = blockIdx.y;
@@ -55,10 +53,7 @@ k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ b
   uint64_t* bars = reinterpret_cast<uint64_t*>(sA + (size_t)slot_bytes * g.S);
   uint64_t* full = bars;
   uint64_t* empty = bars + 8;
-  uint64_t* acc_full = bars + 16;
-  uint64_t* acc_empty = bars + 18;
-  uint64_t* b_full = bars + 20;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 21);
+  uint64_t* b_full = bars + 16;
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
@@ -69,32 +64,21 @@ k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ b
   const int w0 = tw * g.TW, h0 = th * g.R, d0 = td * g.DR;
   const int ndo = min(g.DR, g.D - d0);
   const int nin = KD == 3 ? 2 * ndo + 1 : ndo;
-  const uint32_t acc_cols = (uint32_t)g.nch * NPAD;
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < 2 * acc_cols) tmem_cols <<= 1;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < g.S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kMmaWarps); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], kMmaWarps); mbar_init(&acc_empty[b], 4 * kEpiGroups); }
+    for (int s = 0; s < g.S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4 * kConsumerWG); }
     mbar_init(b_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     mbar_expect_tx(b_full, B_BYTES);          // weights do not depend on the previous kernel: fetch them before pdl_wait
     bulk_g2s(sB, bimg, B_BYTES, b_full);
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
   pdl_wait();   // from here on activations written by the previous kernel are read and our outputs are written
   // trigger the dependents only now: a trigger BEFORE the wait lets the whole chain of later kernels become resident early (each
   // one's prologue would trigger the next), and their idle CTAs then hold the shared memory the running kernel's tiles need
   if (threadIdx.x == 0) pdl_launch_dependents();
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===================== TMA producer: 4 parity sub-tiles per channel group per input plane =====================
     if (lane == 0) {
       const uint32_t box_bytes = (uint32_t)g.P * (uint32_t)g.RR * 16u;
@@ -114,115 +98,77 @@ k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ b
         }
       }
     }
-  } else if (warp == 1 || warp == 6 || warp == 7) {
-    // ===================== MMA issuers =====================
-    const int issuer = warp == 1 ? 0 : warp - 5;
-    const bool leader = lane == 0;
-    uint32_t a_off[NBLK], a_lbo[NBLK];
-#pragma unroll
-    for (int b = 0; b < NBLK; ++b) {
-      if constexpr (CIN >= 16) {
-        const int t = b / (CIN / 16), j = b % (CIN / 16);
-        a_off[b] = (uint32_t)(2 * j) * (cg_bytes >> 4) + (uint32_t)g.tap_off[t];
-        a_lbo[b] = cg_bytes >> 4;
-      } else {
-        // taps paired in table (= address) order; an odd last tap is paired with its predecessor against zero weights
-        const int t1 = min(2 * b + 1, g.ntaps - 1), t0 = t1 - 1;
-        a_off[b] = (uint32_t)g.tap_off[t0];
-        a_lbo[b] = (uint32_t)(g.tap_off[t1] - g.tap_off[t0]);
-      }
+    return;
+  }
+  // ===================== consumers: MMA + epilogue =====================
+  const int wg = warp >> 2, wq = warp & 3;
+  const uint32_t cgb16 = cg_bytes >> 4;
+  auto aoff = [&](int b) -> uint32_t {
+    if constexpr (CIN >= 16) {
+      return (uint32_t)(2 * (b % (CIN / 16))) * cgb16 + (uint32_t)g.tap_off[b / (CIN / 16)];
+    } else {
+      // taps paired in table (= address) order; an odd last tap is paired with its predecessor against zero weights
+      const int t1 = min(2 * b + 1, g.ntaps - 1);
+      return (uint32_t)g.tap_off[t1 - 1];
     }
-    const uint32_t desc_hi = (128u >> 4) | (1u << 14);
-    const uint32_t sB16 = (smem_u32(sB) & 0x3FFFFu) >> 4, sA16 = (smem_u32(sA) & 0x3FFFFu) >> 4;
-    const uint32_t b_lo_base = sB16 | ((uint32_t)(NPAD * 16 >> 4) << 16);
-    mbar_wait(b_full, 0);
-    int next_wait = 0;
-    for (int od = 0; od < ndo; ++od) {
-      const int buf = od & 1;
-      if (od >= 2) mbar_wait(&acc_empty[buf], ((od >> 1) - 1) & 1);
-      const int first = KD == 3 ? 2 * od : od;
-      while (next_wait <= first + KD - 1) {
-        mbar_wait(&full[next_wait % g.S], (next_wait / g.S) & 1);
-        ++next_wait;
-      }
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      uint32_t slot16[KD];
-#pragma unroll
-      for (int kd = 0; kd < KD; ++kd) slot16[kd] = sA16 + (uint32_t)((first + kd) % g.S) * (slot_bytes >> 4);
-      for (int c = issuer; c < g.nch; c += kMmaWarps) {
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * acc_cols + c * NPAD);
-#pragma unroll
-        for (int kd = 0; kd < KD; ++kd) {
-          const uint32_t a16 = slot16[kd] + (uint32_t)c * 128u;
-#pragma unroll
-          for (int b = 0; b < NBLK; ++b) {
-            const uint64_t ad = ((uint64_t)desc_hi << 32) | (uint64_t)((a16 + a_off[b]) | (a_lbo[b] << 16));
-            const uint64_t bd = ((uint64_t)desc_hi << 32) | (uint64_t)(b_lo_base + (uint32_t)((kd * NBLK + b) * NPAD * 2));
-            if (leader) mma_f16(d_tmem, ad, bd, IDESC, (kd | b) != 0 ? 1u : 0u);
-          }
-        }
-      }
-      if (leader) {
-        mma_commit(&acc_full[buf]);
-        if (KD == 3) {             // input planes 2*od and 2*od+1 are dead after output plane od
-          mma_commit(&empty[(2 * od) % g.S]);
-          mma_commit(&empty[(2 * od + 1) % g.S]);
-        } else {
-          mma_commit(&empty[od % g.S]);
-        }
-      }
-      __syncwarp();
+  };
+  auto alo = [&](int b) -> uint32_t {
+    if constexpr (CIN >= 16) {
+      return cgb16;
+    } else {
+      const int t1 = min(2 * b + 1, g.ntaps - 1);
+      return (uint32_t)(g.tap_off[t1] - g.tap_off[t1 - 1]);
     }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;
-    const int egroup = warp >= 8 ? 1 : 0;
-    for (int od = 0; od < ndo; ++od) {
-      const int buf = od & 1;
-      mbar_wait(&acc_full[buf], (od >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int d = d0 + od;
-      for (int c = egroup; c < g.nch; c += kEpiGroups) {
-        const int l = c * 128 + q * 32 + lane;
+  };
+  const uint32_t sB16 = smem_u32(sB) >> 4, sA16 = smem_u32(sA) >> 4;
+  const uint32_t b_lbo16 = (uint32_t)(NPAD * 16 >> 4);
+  const int nsub = 2 * g.nch;
+  mbar_wait(b_full, 0);
+  int next_wait = 0;
+  for (int od = 0; od < ndo; ++od) {
+    const int first = KD == 3 ? 2 * od : od;
+    while (next_wait <= first + KD - 1) {
+      mbar_wait(&full[next_wait % g.S], (next_wait / g.S) & 1);
+      ++next_wait;
+    }
+    uint32_t slot16[KD];
+#pragma unroll
+    for (int kd = 0; kd < KD; ++kd) slot16[kd] = sA16 + (uint32_t)((first + kd) % g.S) * (slot_bytes >> 4);
+    const int d = d0 + od;
+    for (int sc = wg; sc < nsub; sc += kConsumerWG) {
+      float acc[NPAD / 2];
+      mma_subchunk<NPAD, TIn, KD, NBLK>(acc, slot16, (uint32_t)sc * 64u, sB16, b_lbo16, aoff, alo);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int l = sc * 64 + wq * 16 + (lane >> 2) + 8 * i;
         const int hh = l / g.P, ww = l - hh * g.P;
         const int h = h0 + hh, w = w0 + ww;
-        const bool valid = hh < g.R && ww < g.TW && h < g.H && w < g.W;
-        const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * acc_cols + c * NPAD);
-        uint32_t v[16];
-        float acc[NPAD];
+        if (!(hh < g.R && ww < g.TW && h < g.H && w < g.W)) continue;
+        const long long pos = ((((long long)(d + g.opd)) * g.oHp + (h + 1)) * g.oWp + (w + 1)) * 8;
 #pragma unroll
-        for (int n0 = 0; n0 < NPAD; n0 += 16) {
-          tmem_ld16(t_row + (uint32_t)n0, v);
+        for (int j = 0; j < NPAD / 8; ++j) {
+          const int co = ns * NPAD + 8 * j;
+          if (co >= g.cout) continue;
+          const int c = co + 2 * (lane & 3);
+          float x[2];
 #pragma unroll
-          for (int i = 0; i < 16; ++i) acc[n0 + i] = __uint_as_float(v[i]);
-        }
-        if (valid) {
-          const long long pos = ((((long long)(d + g.opd)) * g.oHp + (h + 1)) * g.oWp + (w + 1)) * 8;
-#pragma unroll
-          for (int c0 = 0; c0 < NPAD; c0 += 8) {
-            const int co = ns * NPAD + c0;
-            if (co < g.cout) {
-              float o8[8];
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                float x = acc[c0 + i] + (bias ? bias[co + i] : 0.f);
-                if (g.relu) x = fmaxf(x, 0.f);
-                o8[i] = x;
-              }
-              store_vec<TOut, 8>(out + pos + (co >> 3) * g.out_gs, o8);
-            }
+          for (int e = 0; e < 2; ++e) {
+            x[e] = acc[4 * j + 2 * i + e] + (bias ? bias[c + e] : 0.f);
+            if (g.relu) x[e] = fmaxf(x[e], 0.f);
           }
+          store2<TOut>(out + pos + (co >> 3) * g.out_gs + (c & 7), x[0], x[1]);
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
+    __syncwarp();
+    if (lane == 0) {               // input planes no longer read by this warp -> producer may refill
+      if (KD == 3) {               // input planes 2*od and 2*od+1 are dead after output plane od
+        mbar_arrive(&empty[(2 * od) % g.S]);
+        mbar_arrive(&empty[(2 * od + 1) % g.S]);
+      } else {
+        mbar_arrive(&empty[od % g.S]);
+      }
+    }
   }
 }
 
@@ -274,7 +220,7 @@ inline PlanS2 make_plan_s2(int cin, int npad, int kd, int ks, int D, int H, int 
         int sub_pos = std::max(RR * P, nch * 128 + hk * (P + 1)) + 8;
         sub_pos = (sub_pos + 7) / 8 * 8;       // 128-byte aligned TMA destinations
         const size_t smem = bbytes + (size_t)S * cg * 4 * sub_pos * 16 + 256;
-        if (smem > smem_limit || 2 * nch * npad > 512 || sub_pos * 4 > 32000) break;
+        if (smem > smem_limit || sub_pos * 4 > 32000) break;
         const int th_n = (H + R - 1) / R;
         for (int dsplit = 1; dsplit <= D; ++dsplit) {
           const int DR = (D + dsplit - 1) / dsplit;
@@ -284,7 +230,7 @@ inline PlanS2 make_plan_s2(int cin, int npad, int kd, int ks, int D, int H, int 
                              (kd == 3 ? (double)(2 * DR + 1) / (2 * DR) : 1.0);
           // same time model as conv_tc.cuh::make_plan
           const double tile_clk = 8500.0 + (double)DR * nch * nblk * kd * (45.0 + 0.35 * npad);
-          const double cost = std::ceil(T / 148.0) * tile_clk * (1.0 + 0.25 * (amp - 1.0)) * (S == s_hi ? 1.0 : 1.05);
+          const double cost = std::ceil(T / 132.0) * tile_clk * (1.0 + 0.25 * (amp - 1.0)) * (S == s_hi ? 1.0 : 1.05);
           if (cost < best_cost - 1e-9) { best_cost = cost; bR = R; bTW = TW; bS = S; bDR = DR; }
           if (T > 4000) break;
         }

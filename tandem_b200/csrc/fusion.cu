@@ -4,7 +4,7 @@
 //   AllocateFromDepthKernel  tandem/libdr/dr_fusion/src/tsdfvh/tsdf_volume.cu:317-434 (+ hash_table.cu:80-115)
 //   IntegrateScanKernel      tsdf_volume.cu:436-513 (+ :303-315, voxel.h:29-53)
 //   GenerateRgbDepthKernel   tsdf_volume.cu:600-632 (+ GetInterpolatedVoxel :161-289)
-// B200 design (not a port):
+// Design (not a port):
 //   K5 allocate : one thread per depth PIXEL (the reference sizes its grid by the 10 M hash entries), lock-free
 //                 insert with a single 64-bit CAS on the packed block key (no lock state, no duplicate blocks),
 //                 every new block appended to a compact block list.
@@ -838,8 +838,8 @@ k_raycast(FusionDev d, Mat4 T, unsigned char* __restrict__ bgr_out, float* __res
 }
 
 // K7, persistent form.  Rays differ a lot in length (a few steps next to the camera's near surfaces, > 100 through free space),
-// so with one ray per thread a CTA - and every lane of a warp - idles until its slowest ray is done (ncu on B200: 38 % warps
-// active, 22 of 32 lanes executing).  Here a fixed grid of warps pulls rays from a global counter: every trip of the warp's
+// so with one ray per thread a CTA - and every lane of a warp - idles until its slowest ray is done (a profile showed a third of the
+// warps active and two thirds of their lanes executing).  Here a fixed grid of warps pulls rays from a global counter: every trip of the warp's
 // loop first refills the lanes whose ray has finished (one warp-aggregated atomicAdd), then advances every lane's ray by ONE
 // sphere-tracing step.  Rays are numbered in 8x4 pixel tiles so a warp's 32 rays stay neighbours.  Per-ray arithmetic is the
 // same expression sequence as k_raycast, so the output is bit-identical.
@@ -1007,8 +1007,8 @@ class FusionImpl final : public FusionIface {
         return d > 0.f && ex > 40 && ex < 214 && man != 0x7FFFFF;   // 2^-87 < d < 2^87, significand not all ones
       };
       fast_div_ok_ = ok(o.voxel_size) && ok(o.fx) && ok(o.fy);
-      // Measured on the B200 (profiles/r02_fusion_tracker.txt): 0.539 ms with, 0.534 ms without - div.rn.f32's fast path is
-      // already ~8 instructions and the ray-cast is latency-, not issue-bound.  Kept as an A/B option (bit-identical), off by default.
+      // div.rn.f32's fast path is already ~8 instructions and the ray-cast is latency-, not issue-bound.  Kept as an A/B option
+      // (bit-identical), off by default.
       const char* e = getenv("TDM_FAST_DIV");
       fast_div_ = fast_div_ok_ && e && e[0] == '1';
     }
@@ -1369,9 +1369,9 @@ class FusionImpl final : public FusionIface {
     if (integrate_compact_) {
       k_visible<<<cdiv(d_.o.num_blocks, 256), 256, 0, stream_>>>(d_, pose_inv_, d_vis_list_);
       TDM_CUDA(cudaGetLastError());
-      k_integrate_list<<<148 * 8, 256, 0, stream_>>>(d_, d_bgr_in_, d_depth_in_, pose_inv_, d_vis_list_);
+      k_integrate_list<<<132 * 8, 256, 0, stream_>>>(d_, d_bgr_in_, d_depth_in_, pose_inv_, d_vis_list_);
     } else {
-      k_integrate<<<148 * 8, 256, 0, stream_>>>(d_, d_bgr_in_, d_depth_in_, pose_inv_);
+      k_integrate<<<132 * 8, 256, 0, stream_>>>(d_, d_bgr_in_, d_depth_in_, pose_inv_);
     }
     TDM_CUDA(cudaGetLastError());
   }
@@ -1441,7 +1441,7 @@ class FusionImpl final : public FusionIface {
     }
     return B == B && B * (16.f / 8388608.f) < 0.4f * 8.f * o.voxel_size;
   }
-  static constexpr int kMeshGrid = 148 * 8;
+  static constexpr int kMeshGrid = 132 * 8;   // 8 CTAs per SM of an H100 SXM
   // count + scan + emit + total on stream_ (no host sync)
   void launch_mesh_all() {
     TDM_CUDA(cudaEventRecord(ev_mesh0_, stream_));
@@ -1581,16 +1581,16 @@ class FusionImpl final : public FusionIface {
   int n_rendered_ = 0;
   bool have_scan_ = false;
   Next next_ = kIntegrate;
-  bool alloc_filter_ = false, raycast_cache8_ = false;   // tdm_fusion_set_option: measured on B200 (profiles/r01_fusion_tracker.txt), neither pays: 0.071 vs 0.065 ms, 0.87 vs 0.82 ms
+  bool alloc_filter_ = false, raycast_cache8_ = false;   // tdm_fusion_set_option A/B switches (bit-identical), off by default
   bool raycast_shared_ = true;
   int raycast_tile_ = 1;   // 0: 16x16 px CTAs, 1: 8x8, 2: 8x4 (one warp), 3: 16x8
-  bool raycast_persistent_ = false, integrate_compact_ = true;   // measured: persistent 0.875 ms vs 0.820 ms (instruction-bound, not imbalance-bound)
+  bool raycast_persistent_ = false, integrate_compact_ = true;
   bool fast_div_ok_ = false, fast_div_ = false;   // constant-divisor division in the ray-cast (cdiv_): bit-identical, 3 instructions per division
   std::vector<void*> ipc_opened_;   // peers' allocations mapped with cudaIpcOpenMemHandle (closed in the destructor)
   bool slab_clip_ = true;        // Z-slab volumes: rays are only sampled inside the slab's z range (bit-identical, see k_raycast_shared)
   bool raycast_dedup_ = true;    // ray-cast: samples whose corners straddle block faces look every distinct block up once
   bool occ_skip_ = false;        // ray-cast: dilated occupancy bitmap in front of the sampler (bit-identical, see k_raycast_shared OCC).
-                                 // Measured on the B200 (profiles/r02_fusion_tracker.txt): 0.445 ms with, 0.422 ms without - the
+                                 // Off by default: the
                                  // reference's allocation DDA walks every ray from the CAMERA to the surface (tsdf_volume.cu:317-434),
                                  // so the free space a later ray crosses is itself allocated (sdf ~ tau, weight > 0) and every
                                  // sample there must be interpolated; the bitmap only ever skips what the bounding-box clip
@@ -1598,7 +1598,7 @@ class FusionImpl final : public FusionIface {
   bool slab_exchange_ = false;   // Z-slab volumes: the ray-cast emits packed nearest-hit keys for the exchange step, the per-slab
                                  // render is not copied back and GetRenderResult does not wait (tandem_b200.parallel)
   int* d_vis_list_ = nullptr;
-  int raycast_grid_ = 148;
+  int raycast_grid_ = 132;
   cudaEvent_t ev_split_ = nullptr;
   float last_alloc_ms_ = 0.f;
   long long* d_hit_keys_ = nullptr;

@@ -10,7 +10,7 @@
 // with 65 hash probes per surviving cell, appends 72-byte triangles to managed memory through one global atomic and
 // re-packs them on the host one triangle at a time.
 //
-// B200 design (block-sparse, two passes, no global atomics):
+// Design (block-sparse, two passes, no global atomics):
 //   * every quantity a cell needs is SEPARABLE per axis (cell position, the +-s/2 corner coordinates, the two voxel
 //     indices and the trilinear weight of each corner sample, the centre voxel index), so the host evaluates three small
 //     per-axis tables once per call with exactly the reference's fp32 expression sequence;

@@ -26,7 +26,6 @@
 #include "mvsnet_kernels.cuh"
 #include "conv_tc.cuh"
 #include "conv_tc_s2.cuh"
-#include "conv_tc_is.cuh"
 #include "cost_volume_tma.cuh"
 #include "weights.h"
 
@@ -104,15 +103,13 @@ struct DevConv {
   bool transposed = false;
   float* w = nullptr;
   float* bias = nullptr;
-  // tcgen05 path (conv_tc.cuh): weights pre-arranged as the canonical K-major B image in the input's 16-bit type
+  // tensor-core path (conv_tc.cuh): weights pre-arranged as the canonical K-major B image in the input's 16-bit type
   void* bimg = nullptr;
   int npad = 0;
   bool tc_ok = false;
   bool tc_deconv = false;  // transposed conv evaluated as a GEMM over the input grid (N = 8 parity classes x cout)
   int nsplit = 1;          // N slices (blockIdx.y) for the 64-channel layers
   bool hilo = false;       // weights carried as hi + lo 16-bit halves (N doubled), see conv_tc.cuh
-  void* bimg_is = nullptr; // input-stationary B image (3-D stride-1 convs), conv_tc_is.cuh
-  int npad_is = 0;         // its column padding: 8 for the <= 8-channel outputs with hi/lo weights (tight [hi|lo] packing), else npad
   bool tc_up2 = false;     // MODE 3: conv3x3 of a nearest-x2 up-sampled map on the coarse grid (fused FPN tail)
   bool tc_s2 = false;      // stride-2 conv on the tensor-map (strided TMA) kernel, conv_tc_s2.cuh
   void* bimg_s2 = nullptr;
@@ -160,7 +157,7 @@ class MvsnetEngine final : public MvsnetIface {
     if (worker_.joinable()) worker_.join();
     cudaSetDevice(device_);
     free_plan();
-    for (auto& kv : convs_) { cudaFree(kv.second.w); cudaFree(kv.second.bias); cudaFree(kv.second.bimg); cudaFree(kv.second.bimg_s2); cudaFree(kv.second.bimg_is); }
+    for (auto& kv : convs_) { cudaFree(kv.second.w); cudaFree(kv.second.bias); cudaFree(kv.second.bimg); cudaFree(kv.second.bimg_s2); }
     if (d_cv_stats_) {
       unsigned st[2] = {0, 0};
       if (std::getenv("TDM_DEBUG_PLAN") && cudaMemcpy(st, d_cv_stats_, sizeof(st), cudaMemcpyDeviceToHost) == cudaSuccess)
@@ -210,7 +207,6 @@ class MvsnetEngine final : public MvsnetIface {
     }
     else if (key == "keep_intermediates") keep_ = value != 0;
     else if (key == "use_tc") use_tc_ = value != 0;
-    else if (key == "use_is") use_is_ = value != 0;
     else if (key == "fork_fpn") fork_fpn_ = value != 0;
     else if (key == "prob_direct") prob_direct_ = value != 0;
     else if (key == "direct_conv00") direct_conv00_ = value != 0;
@@ -541,15 +537,6 @@ class MvsnetEngine final : public MvsnetIface {
     else tc::build_b_image<TB, 64>(fc.w.data(), fc.cin, fc.cout, dc.npad, fc.kd, img, +cvt, dc.nsplit);
     TDM_CUDA(cudaMalloc(&dc.bimg, img.size() * sizeof(TB)));
     TDM_CUDA(cudaMemcpy(dc.bimg, img.data(), img.size() * sizeof(TB), cudaMemcpyHostToDevice));
-    if (fc.kd == 3 && fc.cin <= 32 && dc.nsplit == 1) {
-      std::vector<TB> im2;
-      dc.npad_is = (dc.hilo && fc.cout <= 8 && is_npad8_) ? 8 : dc.npad;
-      if (fc.cin == 8) tc::build_b_image_is<TB, 8>(fc.w.data(), fc.cin, fc.cout, dc.npad_is, im2, +cvt, dc.hilo, +back);
-      else if (fc.cin == 16) tc::build_b_image_is<TB, 16>(fc.w.data(), fc.cin, fc.cout, dc.npad_is, im2, +cvt, dc.hilo, +back);
-      else tc::build_b_image_is<TB, 32>(fc.w.data(), fc.cin, fc.cout, dc.npad_is, im2, +cvt, dc.hilo, +back);
-      TDM_CUDA(cudaMalloc(&dc.bimg_is, im2.size() * sizeof(TB)));
-      TDM_CUDA(cudaMemcpy(dc.bimg_is, im2.data(), im2.size() * sizeof(TB), cudaMemcpyHostToDevice));
-    }
   }
   template <typename TB> static TB from_host(float v);
   template <typename TB> static float to_host(TB v) { return (float)v; }
@@ -794,7 +781,7 @@ class MvsnetEngine final : public MvsnetIface {
     cfg.gridDim = grid;
     cfg.blockDim = dim3(tc::kThreads);
     // with PDL an early-launched dependent must not stack several CTAs on the few SMs its predecessor left idle (they would
-    // serialise on the 512 TMEM columns): ask for enough shared memory that one CTA fills an SM
+    // compete for those SMs' issue slots while the rest of the GPU waits): ask for enough shared memory that one CTA fills an SM
     cfg.dynamicSmemBytes = use_pdl_ ? std::max(smem, (size_t)pdl_min_smem_kb_ * 1024) : smem;
     cfg.stream = stream_;
     cudaLaunchAttribute attr[1];
@@ -808,13 +795,17 @@ class MvsnetEngine final : public MvsnetIface {
   struct TcCache { tc::Plan plan; CUtensorMap tmap; };
   std::map<std::string, TcCache> tc_cache_;
 
-  template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool PLAIN, int MODE = 0, bool HILO = false>
-  void tc_inst(const std::string& wkey, const DevBuf& in, const DevConv& c, const DevBuf* res, const DevBuf& out, bool relu) {
-    auto it = tc_cache_.find(wkey);
+  template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool PLAIN, int MODE = 0, bool HILO = false, typename Tail = tc::NoTail>
+  void tc_inst(const std::string& wkey, const DevBuf& in, const DevConv& c, const DevBuf* res, const DevBuf& out, bool relu,
+               const Tail& tail = Tail()) {
+    const std::string key = wkey + (Tail::enabled ? "#tail" : "");
+    auto it = tc_cache_.find(key);
     if (it == tc_cache_.end()) {
       TcCache tcx;
-      tcx.plan = tc::make_plan(CIN, HILO ? 2 * NPAD : NPAD, KD, in.D, in.H, in.W, in.pd, MODE, (size_t)tc_smem_kb_ * 1024);   // tiles live on the INPUT grid
+      tcx.plan = tc::make_plan(CIN, HILO ? 2 * NPAD : NPAD, KD, in.D, in.H, in.W, in.pd, MODE, (size_t)tc_smem_kb_ * 1024,   // tiles live on the INPUT grid
+                               Tail::enabled);
       tc::Geom& g = tcx.plan.g;
+      TDM_CHECK(!Tail::enabled || g.tiles_d == 1, "the prob tail needs tiles that span all depth planes");
       g.oHp = out.H + 2; g.oWp = out.W + 2; g.opd = out.pd;
       g.iDp = in.D + 2 * in.pd;
       g.in_gs = p8<const TIn>(in).gs;
@@ -837,7 +828,7 @@ class MvsnetEngine final : public MvsnetIface {
       if (std::getenv("TDM_DEBUG_PLAN"))
         fprintf(stderr, "[plan] %-14s mode %d cin %d N %d kd %d in %dx%dx%d -> R %d TW %d DR %d S %d nch %d tiles %d x nsplit %d smem %zu\n", wkey.c_str(), MODE, CIN,
                 HILO ? 2 * NPAD : NPAD, KD, in.D, in.H, in.W, g.R, g.TW, g.DR, g.S, g.nch, tcx.plan.grid, c.nsplit, tcx.plan.smem);
-      it = tc_cache_.emplace(wkey, tcx).first;
+      it = tc_cache_.emplace(key, tcx).first;
     }
     const tc::Plan& pl = it->second.plan;
     TOut* op = nullptr;
@@ -849,68 +840,13 @@ class MvsnetEngine final : public MvsnetIface {
       op = (TOut*)out.p;
       if (res) rp = (const TOut*)res->p;
     }
-    auto kern = tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO>;
+    auto kern = tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail>;
     static bool attr_set = false;
     if (!attr_set) {
       TDM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       attr_set = true;
     }
-    launch_pdl(kern, dim3(pl.grid, c.nsplit), pl.smem, it->second.tmap, (const TIn*)c.bimg, (const float*)c.bias, rp, op, plain, pl.g);
-  }
-
-  template <typename TIn, typename TOut, int CIN, int NPAD, bool PLAIN, bool HILO, typename Tail = tc::NoTail>
-  void tc_is_inst(const std::string& wkey, const DevBuf& in, const DevConv& c, const DevBuf* res, const DevBuf& out, bool relu,
-                  const Tail& tail = Tail()) {
-    const std::string key = wkey + (Tail::enabled ? "#is+tail" : "#is");
-    auto it = tc_cache_.find(key);
-    if (it == tc_cache_.end()) {
-      TcCache tcx;
-      tcx.plan = tc::make_plan(CIN, HILO ? 2 * NPAD : NPAD, 3, in.D, in.H, in.W, in.pd, 4, (size_t)tc_smem_kb_ * 1024, Tail::enabled);
-      tc::Geom& g = tcx.plan.g;
-      TDM_CHECK(!Tail::enabled || g.tiles_d == 1, "the prob tail needs tiles that span all depth planes");
-#ifdef TDM_TIMING_EXPERIMENTS
-      g.dbg_aligned = std::getenv("TDM_DEBUG_ALIGNED_TAPS") ? std::atoi(std::getenv("TDM_DEBUG_ALIGNED_TAPS")) : 0;
-#else
-      g.dbg_aligned = 0;
-#endif
-      g.oHp = out.H + 2; g.oWp = out.W + 2; g.opd = out.pd;
-      g.iDp = in.D + 2 * in.pd;
-      g.in_gs = p8<const TIn>(in).gs;
-      g.relu = relu ? 1 : 0;
-      g.has_res = res ? 1 : 0;
-      g.cout = c.cout;
-      if constexpr (!PLAIN) {
-        g.out_gs = p8<TOut>(out).gs;
-        if (res) g.res_gs = p8<const TOut>(*res).gs;
-      }
-      const cuuint64_t dims[4] = {8, (cuuint64_t)(in.W + 2), (cuuint64_t)(in.H + 2), (cuuint64_t)g.iDp * (CIN / 8)};
-      const cuuint64_t strides[3] = {16, (cuuint64_t)(in.W + 2) * 16, (cuuint64_t)(in.W + 2) * (in.H + 2) * 16};
-      const cuuint32_t box[4] = {8, (cuuint32_t)g.P, (cuuint32_t)(g.R + 2), 1};
-      const cuuint32_t estr[4] = {1, 1, 1, 1};
-      const CUtensorMapDataType dt = std::is_same<TIn, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-      const CUresult r = tc::encode_tiled_fn()(&tcx.tmap, dt, 4, in.p, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      TDM_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed for " + key);
-      if (std::getenv("TDM_DEBUG_PLAN"))
-        fprintf(stderr, "[plan] %-14s IS cin %d N 3x%d in %dx%dx%d -> R %d TW %d DR %d S %d nch %d tiles %d smem %zu\n", key.c_str(), CIN, HILO ? 2 * NPAD : NPAD,
-                in.D, in.H, in.W, g.R, g.TW, g.DR, g.S, g.nch, tcx.plan.grid, tcx.plan.smem);
-      it = tc_cache_.emplace(key, tcx).first;
-    }
-    const tc::Plan& pl = it->second.plan;
-    auto kern = tc::k_conv_tc_is<TIn, TOut, CIN, NPAD, PLAIN, HILO, Tail>;
-    static bool attr_set = false;
-    if (!attr_set) {
-      TDM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      attr_set = true;
-    }
-    // persistent over tiles: every CTA takes ceil(tiles / SMs) tiles, the grid is what that needs (<= one CTA per SM)
-    static const bool persist = !(std::getenv("TDM_IS_PERSIST") && std::getenv("TDM_IS_PERSIST")[0] == '0');   // A/B: 0 = one tile per CTA
-    const int tpc = persist ? (pl.grid + kNumSm - 1) / kNumSm : 1;
-    const int gx = (pl.grid + tpc - 1) / tpc;
-    launch_pdl(kern, dim3(gx, 1), pl.smem, it->second.tmap, (const TIn*)c.bimg_is, (const float*)c.bias,
-               (const TOut*)(PLAIN ? nullptr : (res ? res->p : nullptr)), (TOut*)(PLAIN ? nullptr : out.p),
-               (float*)(PLAIN ? out.p : nullptr), pl.g, tail);
+    launch_pdl(kern, dim3(pl.grid, c.nsplit), pl.smem, it->second.tmap, (const TIn*)c.bimg, (const float*)c.bias, rp, op, plain, pl.g, tail);
   }
 
   struct S2Cache { tc::PlanS2 plan; CUtensorMap tmap; };
@@ -970,7 +906,7 @@ class MvsnetEngine final : public MvsnetIface {
     }
   }
 
-  // returns true if the tcgen05 kernel was launched
+  // returns true if the tensor-core kernel was launched
   bool conv_tc_dispatch(const std::string& wkey, const DevBuf& bi, const DevConv& c, const DevBuf* rp, const DevBuf& bo, bool relu) {
     if constexpr (sizeof(TA) != 2) {
       return false;
@@ -984,46 +920,27 @@ class MvsnetEngine final : public MvsnetIface {
         if (c.cin == 64) { tc_inst<TA, TA, 64, 64, 2, false, 1>(wkey, bi, c, rp, bo, relu); return true; }
         return false;
       }
-      if (use_is_ && c.bimg_is && c.kd == 3) {
-        if (bo.f32) {
-          if (c.cin == 8 && c.cout == 1 && bi.kind == 1 && c.hilo) {
-            if (tail_req_.stage && c.npad_is == 8 && fused_regress_) {
-              // a8 inside the prob convolution's epilogue (round 2): the thread that stored a pixel's D logits finishes the pixel
-              const TailReq& t = tail_req_;
-#define TDM_TAIL(MAXD)                                                                                           \
-  tc_is_inst<TA, TA, 8, 8, true, true, RegressTail<MAXD>>(wkey, bi, c, nullptr, bo, false,                        \
-                                                          RegressTail<MAXD>{t.dsrc, t.depth, t.conf, t.hyp, t.half_range})
-              if (t.D <= 8) TDM_TAIL(8); else if (t.D <= 32) TDM_TAIL(32); else if (t.D <= 48) TDM_TAIL(48); else TDM_TAIL(64);
-#undef TDM_TAIL
-              tail_req_.done = true;
-            }
-            else if (c.npad_is == 8) tc_is_inst<TA, TA, 8, 8, true, true>(wkey, bi, c, nullptr, bo, false);
-            else tc_is_inst<TA, TA, 8, 16, true, true>(wkey, bi, c, nullptr, bo, false);
-            return true;
-          }
-          return false;
-        }
-#define TDM_IS(TI, CI, NP, HL)                                                             \
-  if (c.cin == CI && c.npad_is == NP && c.hilo == HL) {                                    \
-    tc_is_inst<TI, TA, CI, NP, false, HL>(wkey, bi, c, rp, bo, relu);                      \
-    return true;                                                                           \
-  }
-        if (bi.kind == 2) {
-          TDM_IS(TV, 32, 8, true) TDM_IS(TV, 16, 8, true) TDM_IS(TV, 8, 8, true)
-          TDM_IS(TV, 32, 16, true) TDM_IS(TV, 16, 16, true) TDM_IS(TV, 8, 16, true)
-        } else {
-          TDM_IS(TA, 16, 16, true) TDM_IS(TA, 32, 32, false)
-        }
-#undef TDM_IS
-      }
 #define TDM_TC(TI, CI, NP, KDV, HL)                                                        \
   if (c.cin == CI && c.npad == NP && c.kd == KDV && c.hilo == HL) {                        \
     tc_inst<TI, TA, CI, NP, KDV, false, 0, HL>(wkey, bi, c, rp, bo, relu);                       \
     return true;                                                                           \
   }
       if (bo.f32) {
-        if (c.cin == 8 && c.cout == 1 && c.kd == 3 && bi.kind == 1 && c.hilo) { tc_inst<TA, TA, 8, 16, 3, true, 0, true>(wkey, bi, c, nullptr, bo, false); return true; }
-        return false;
+        if (!(c.cin == 8 && c.cout == 1 && c.kd == 3 && bi.kind == 1 && c.hilo)) return false;
+        if (tail_req_.stage && fused_regress_) {
+          // softmax / soft-argmin / confidence inside the prob convolution's epilogue: the thread that stored a pixel's D logits
+          // finishes the pixel
+          const TailReq& t = tail_req_;
+#define TDM_TAIL(MAXD)                                                                                           \
+  tc_inst<TA, TA, 8, 16, 3, true, 0, true, RegressTail<MAXD>>(wkey, bi, c, nullptr, bo, false,                   \
+                                                            RegressTail<MAXD>{t.dsrc, t.depth, t.conf, t.hyp, t.half_range})
+          if (t.D <= 8) TDM_TAIL(8); else if (t.D <= 32) TDM_TAIL(32); else if (t.D <= 48) TDM_TAIL(48); else TDM_TAIL(64);
+#undef TDM_TAIL
+          tail_req_.done = true;
+        } else {
+          tc_inst<TA, TA, 8, 16, 3, true, 0, true>(wkey, bi, c, nullptr, bo, false);
+        }
+        return true;
       }
       if (bi.kind == 2) {
         TDM_TC(TV, 32, 16, 3, true) TDM_TC(TV, 16, 16, 3, true) TDM_TC(TV, 8, 16, 3, true)
@@ -1274,7 +1191,7 @@ class MvsnetEngine final : public MvsnetIface {
       rec_end();
       rec_begin(k + "percentile", 8.0 * n, 0);
       for (int pass = 1; pass <= 2; ++pass)
-        launch_k(k_select_pass, dim3(std::min(cdiv(n, 256 * 8), 296)), dim3(256), fbuf(k + "edge"), n, select2_, pass, fbuf("thr") + (s - 1));
+        launch_k(k_select_pass, dim3(std::min(cdiv(n, 256 * 8), 2 * kNumSm)), dim3(256), fbuf(k + "edge"), n, select2_, pass, fbuf("thr") + (s - 1));
       launch_count_ += 1;
       rec_end();
     } else {
@@ -1507,9 +1424,9 @@ class MvsnetEngine final : public MvsnetIface {
 
   struct Gate { int C = 0; float w1[64]; float b1 = 0, w2 = 0, b2 = 0; };
   // mixed16: the cost volume is fp16 too, stored x 2^-5 (values reach ~1e4 and fp16 ends at 65504; bf16 has the range but only 8
-  // significant bits - the CPU study (profiles/r02_precision_study.md) attributes 1 % of mask IoU to that alone)
+  // significant bits, which a CPU study found to cost about 1 % of mask IoU on its own)
   static constexpr float kVolScale = (std::is_same<TA, __half>::value && std::is_same<TV, __half>::value) ? 0.03125f : 1.f;
-  static constexpr int kNumSm = 148;   // B200 (sm_100a only build)
+  static constexpr int kNumSm = 132;   // H100 SXM (sm_90a only build)
   static constexpr bool kRawInput = sizeof(TA) == 2;   // 16-bit engines: exact u8/256 input, 256/255 folded into f.conv0.0
 
   int device_ = 0;
@@ -1524,9 +1441,8 @@ class MvsnetEngine final : public MvsnetIface {
   SelectState2* select2_ = nullptr;
   bool inline_dmin_ = true;    // adaptive range's d_min computed where it is consumed (dmin_px) instead of by k_adaptive_dmin (A/B: 0)
   // softmax / soft-argmin / confidence in the epilogue of the tensor-core prob convolution (set_option("fused_regress", 1)):
-  // bit-identical to k_regress and three launches fewer, but measured SLOWER (forward 1.368 vs 1.337 ms, 875 vs 904 keyframes/s
-  // with eight windows in flight; profiles/r02_bench_ab.txt): the 256 epilogue threads of a CTA finish their pixels after the
-  // last plane with nothing left to overlap, where the stand-alone kernel spreads the same work over 2048 threads per SM. Off.
+  // bit-identical to k_regress and three launches fewer, but the consumer threads of a CTA finish their pixels after the last
+  // plane with nothing left to overlap, where the stand-alone kernel spreads the same work over 2048 threads per SM. Off.
   bool fused_regress_ = false;
   struct TailReq { int stage; int D; DminSrc dsrc; float* depth; float* conf; const HypSpec* hyp; const float* half_range; bool done; };
   TailReq tail_req_{};
@@ -1551,27 +1467,21 @@ class MvsnetEngine final : public MvsnetIface {
   bool cv_tmap_ok_ = false;
   unsigned* d_cv_stats_ = nullptr;
   int cv_variant_ = 3;   // 0: generic cost-volume kernel; 1-4: k_cost_volume_va16 (ND 2/2/4 | 4/4/4, fp32 | fp16 accumulate)
-  // Programmatic dependent launch of the tensor-core kernels (round 2: ON). Round 1 measured it slower (1.86 vs 1.73 ms) for two
-  // reasons found in round 2: (1) the trigger sat BEFORE griddepcontrol.wait, so every kernel's prologue triggered the next and the
-  // whole chain became resident early; (2) early CTAs of the small-footprint kernels stacked 2-5 deep on the few SMs the predecessor
-  // left idle and then serialised on the 512 TMEM columns. With the trigger after the wait and pdl_min_smem_kb_ = 120 (one
-  // tensor-core CTA per SM) it wins at every concurrency: 1.339 / 1.157 / 1.100 / 1.084 ms per window with 1 / 2 / 4 / 8 windows
-  // in flight against 1.352 / 1.204 / 1.128 / 1.117 without (tools/pdl_sweep.py, profiles/r02_bench_ab.txt).
+  // Programmatic dependent launch of the tensor-core kernels: the trigger sits after griddepcontrol.wait (a trigger before it
+  // lets the whole chain of later kernels become resident early), and pdl_min_smem_kb_ = 120 keeps one tensor-core CTA per SM.
   bool warmed_ = false, use_graph_ = true;
   int use_pdl_ = 1;   // 2: the FMA-pipe kernels (cost volume, soft-argmin, edge filter ...) are launched with the attribute as well
   int slot_ = 0;           // index into c_call_params
   int tc_smem_kb_ = 225;   // shared-memory budget of the tile planner (<= 113 lets two CTAs share an SM)
-  bool use_is_ = true;   // input-stationary kernel for the 3-D stride-1 convs
-  bool is_npad8_ = std::getenv("TDM_IS_NPAD8") ? std::getenv("TDM_IS_NPAD8")[0] != '0' : true;   // tight [hi|lo] packing of <= 8 output channels (A/B: TDM_IS_NPAD8=0)
   bool fused_fpn_ = false;
-  bool prob_direct_ = false;  // `prob` (8 -> 1 channels) on the FMA pipes (k_prob_direct): measured SLOWER than the 1/16-utilised tensor-core tile (0.181 vs 0.143 ms over the three stages, 812 vs 850 keyframes/s); kept as an A/B option
+  bool prob_direct_ = false;  // `prob` (8 -> 1 channels) on the FMA pipes (k_prob_direct) instead of the tensor-core tile; an A/B option and an independent check
   bool have_prob_w_ = false;
   ProbWeights prob_w_[3] = {};
   bool direct_conv00_ = true; // 16-bit engines: pre-processing + conv0.0 fused on the FMA pipes (k_conv00_u8); 0 = preprocess + tensor-core conv
   bool fork_fpn_ = true;      // FPN tail on a second stream / graph branch (A/B: set_option("fork_fpn", 0))
   cudaStream_t side_stream_ = nullptr;
   cudaEvent_t ev_fork_ = nullptr, ev_join_ = nullptr;
-  bool filter_all_ = false, keep_ = true, use_tc_ = (sizeof(TA) == 2);  // tcgen05 convs are the default on 16-bit engines
+  bool filter_all_ = false, keep_ = true, use_tc_ = (sizeof(TA) == 2);  // tensor-core convs are the default on 16-bit engines
   bool profiling_ = false;
   int launch_count_ = 0, launches_per_forward_ = 0;
   std::vector<LaunchRec> recs_;
@@ -1611,7 +1521,7 @@ void debug_homography(const float* K3x3, const float* c2w_ref, const float* c2w_
   }
 }
 
-// host-only view of the tcgen05 tile planner (no GPU involved; used by the CPU test-suite): out12 = {S, R, TW, P, DR, nch,
+// host-only view of the tensor-core tile planner (no GPU involved; used by the CPU test-suite): out12 = {S, R, TW, P, DR, nch,
 // slot_pos, tiles_w, tiles_h, tiles_d, grid, smem_bytes}
 void debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out12) {
   // mode + 100 = the same mode with tiles that span all D planes (the prob layer with the soft-argmin tail)

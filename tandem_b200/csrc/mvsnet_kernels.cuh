@@ -1,9 +1,9 @@
 // CVA-MVSNet device kernels, generation 1 ("direct" path): fp32 accumulation, one thread per output
-// position.  These kernels are the parity baseline for every layer; the tcgen05 implicit-GEMM
+// position.  These kernels are the parity baseline for every layer; the wgmma implicit-GEMM
 // kernels (conv_tc.cuh) replace the convolutions layer by layer and are validated against these and
 // against the CPU oracle.
 //
-// Activation layout "P8" (shared with the tcgen05 path): channel-group-planar with zero halos,
+// Activation layout "P8" (shared with the tensor-core path): channel-group-planar with zero halos,
 //     [C/8][D+2*pd][H+2][W+2][8]          (pd = 1 for volumes, 0 for the view axis of 2-D maps)
 // so one position of one channel group is a 16-byte (16-bit types) vector, a row segment of a group
 // is contiguous (1-D TMA bulk copies), and every 3x3x3 tap is a constant address shift inside a
@@ -27,7 +27,7 @@ namespace tdm {
 // cudaLaunchAttributeProgrammaticStreamSerialization the grid may become resident while its predecessor still runs; it must not touch
 // memory before griddepcontrol.wait (= predecessor complete and visible).  The trigger right behind the wait lets the NEXT kernel's
 // launch latency / prologue overlap this grid (one kernel of look-ahead).  Launched normally, both instructions are no-ops apart from
-// the trigger, which still lets a tensor-core successor set up its barriers, TMEM and weight image early.
+// the trigger, which still lets a tensor-core successor set up its barriers and weight image early.
 __device__ __forceinline__ void grid_dep_sync() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -149,7 +149,7 @@ struct ConvGeom {
 };
 
 // COUT_T output channels per thread (COUT_T == COUT: one thread owns a position; COUT_T == 8: blockIdx.y selects the
-// 8-channel group, used for the small low-resolution layers where positions alone cannot fill 148 SMs).
+// 8-channel group, used for the small low-resolution layers where positions alone cannot fill 132 SMs).
 template <typename TIn, typename TOut, int CIN, int COUT, int COUT_T = COUT>
 __global__ void __launch_bounds__(128)
 k_conv_direct(const P8<const TIn> in, const float* __restrict__ wgt /*[taps][CIN][COUT]*/,
@@ -266,9 +266,8 @@ k_conv_direct(const P8<const TIn> in, const float* __restrict__ wgt /*[taps][CIN
 // (8 fp16 channels = 16 B each) of each of the 9 (kd, kh) rows once with 128-bit loads (zero halos: no bounds tests), and
 // multiplies them with weights that arrive as a __grid_constant__ kernel parameter, i.e. as constant-bank operands of the
 // FFMAs (no weight loads at all).  fp32 accumulation with the fp32 BN-free weights of the checkpoint.
-// MEASURED on B200 (round 1): 0.035 / 0.072 / 0.074 ms for the three stages against 0.027 / 0.052 / 0.064 ms of the tcgen05
-// kernel, logits equal to 8e-5 (scale 1e2) - the 864 FFMA + 432 conversions per thread do not beat the tensor-core tile even
-// at 1/16 utilisation, so this kernel is OFF by default (set_option("prob_direct", 1)) and serves as an independent check.
+// The 864 FFMA + 432 conversions per thread are expected to lose to the tensor-core tile even at 1/16 utilisation, so this
+// kernel is OFF by default (set_option("prob_direct", 1)) and serves as an independent check.
 // ------------------------------------------------------------------------------------------------
 struct ProbWeights {
   float w[27 * 8];   // [kd][kh][kw][cin]
@@ -425,7 +424,7 @@ struct CallParams {
 
 // One slot per engine instance (several DrMvsnet handles may be in flight on a device); refreshed stream-ordered with
 // cudaMemcpyToSymbolAsync before each forward.  Constant memory keeps the homographies as uniform operands of the inner
-// loops (measured: reading them through a global pointer or shared memory costs the cost-volume kernel 10-15 %).
+// loops (reading them through a global pointer or shared memory would add loads to the cost-volume kernel's inner loop).
 constexpr int kMaxEngines = 8;
 __constant__ CallParams c_call_params[kMaxEngines];
 
@@ -621,16 +620,8 @@ __device__ __forceinline__ float rcp_approx(float x) {
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
   return r;
 }
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  unsigned long long ra, rb, rc, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rc) : "f"(c.x), "f"(c.y));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
-}
+// two independent correctly rounded FMAs (Hopper has no paired fp32 FMA instruction)
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
 template <typename TV, int C /*channels of one thread*/, int CSPLIT, int ND, bool ACC16>
 __global__ void __launch_bounds__(128)

@@ -5,7 +5,7 @@
 //   calcResKernelNew<128>  cuda_coarse_tracker_private.cu:41-214   7 x cub::BlockReduce + 7 float atomics / block
 //   calcGKernel<128,float> cuda_coarse_tracker_private.cu:261-394  45 serialized block reductions, <1 wave
 //   host wrapper           cuda_coarse_tracker.cpp:195-356          memset + H2D + kernel + sync + D2H per call
-// B200 design: K8 = ONE kernel template for calcRes, calcG and the fused calcRes+calcG.  296 persistent CTAs
+// Design: K8 = ONE kernel template for calcRes, calcG and the fused calcRes+calcG.  264 persistent CTAs
 // (2 per SM) grid-stride over the points, per-thread fp32 partials are widened to double, reduced with warp
 // shuffles and one shared-memory pass, each CTA writes its partial vector, and the last CTA to finish (atomic
 // ticket) adds the partials in a fixed order and writes the result straight into mapped pinned host memory:
@@ -21,7 +21,7 @@ namespace tdm {
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kBlocks = 296;  // 2 x 148 SMs
+constexpr int kBlocks = 264;  // 2 x 132 SMs (H100 SXM)
 constexpr int kRes = 7;       // E, numTermsInE, numTermsInWarped, numSaturated, shiftT, shiftRT, shiftNum
 constexpr int kG = 45;
 constexpr int kOut = kRes + kG;

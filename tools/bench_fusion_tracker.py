@@ -1,6 +1,6 @@
 """Secondary measurements (SURVEY.md §8d configs 3/4): TSDF integrate + ray-cast at the initDr map size with a stream
 of synthetic 640x480 depth maps, the level-0 tracker evaluation, and - when oracle/_ref is present - the REFERENCE's own
-dr_fusion (compiled unmodified for sm_100a) on the same inputs on the same GPU.
+dr_fusion (compiled unmodified for sm_90a) on the same inputs on the same GPU.
     python tools/bench_fusion_tracker.py [n_frames]
 Prints one JSON line per measurement."""
 import ctypes
@@ -90,7 +90,7 @@ if os.path.exists(ref_lib):
     t0 = time.perf_counter()
     nm = l.ref_fusion_get_mesh(r, lo.ctypes.data_as(_fp), up.ctypes.data_as(_fp), None, None, ctypes.c_longlong(0))
     tm = (time.perf_counter() - t0) * 1e3
-    print(json.dumps({"what": "tsdf reference dr_fusion (unmodified, sm_100a)", "frames": nref,
+    print(json.dumps({"what": "tsdf reference dr_fusion (unmodified, sm_90a)", "frames": nref,
                       "integrate_ms_per_frame(wall)": ti * 1e3 / nref, "render_ms_per_frame(wall)": tr * 1e3 / nref,
                       "GetMesh_wall_ms(10 m box)": tm, "mesh_triangles": nm // 3}))
     l.ref_fusion_destroy(r)
@@ -154,7 +154,7 @@ if os.path.exists(trk_lib):
                                       c["pc_idepth"].ctypes.data_as(_fp), c["pc_color"].ctypes.data_as(_fp),
                                       np.ascontiguousarray(c["dInew"]).ctypes.data_as(_fp), o7.ctypes.data_as(_fp),
                                       o45.ctypes.data_as(_fp), None, 200, ctypes.byref(mr), ctypes.byref(mg))
-        print(json.dumps({"what": "tracker reference kernels (calcResKernelNew + calcGKernel<float>, unmodified, sm_100a) on this GPU",
+        print(json.dumps({"what": "tracker reference kernels (calcResKernelNew + calcGKernel<float>, unmodified, sm_90a) on this GPU",
                           "rc": rc, "n_points": c["n"], "calcRes_kernel_us(device)": mr.value * 1e3, "calcG_kernel_us(device)": mg.value * 1e3,
                           "pair_us(device)": (mr.value + mg.value) * 1e3, "ours_fused_kernel_us(device)": ms / 200 * 1e3,
                           "ours_speedup": (mr.value + mg.value) * 1e3 / (ms / 200 * 1e3),
