@@ -67,6 +67,25 @@ public:
   TrackResult track(Eigen::Matrix<double, 4, 4> const &refToNew, Eigen::Vector2d const &aff_g2l, float new_exposure,
                     float coarseCutoffTH, int maxIterations, float lambdaExtrapolationLimit, bool fix_a, bool fix_b);
 
+  // Extension: the body of CoarseTracker::trackNewestCoarse (CoarseTracker.cpp:750-936) in one call, every level on the device
+  // with one host wait.  levels[l] is the tracker of pyramid level l (levels.size() - 1 = coarsestLvl), each with setK, a
+  // reference and a new image.  affineOptModeA/B = setting_affineOptModeA/B.  Throws std::runtime_error on invalid input.
+  struct PyramidTrackResult {
+    bool ok;                                       // trackNewestCoarse's return value
+    Eigen::Matrix<double, 4, 4> refToNew;          // lastToNew_out (the input when the loop aborted)
+    Eigen::Vector2d aff_g2l;                       // aff_g2l_out
+    Eigen::Matrix<double, 5, 1> lastResiduals;
+    Eigen::Matrix<double, 3, 1> lastFlowIndicators;
+    int abortedLevel, repeatedLevel;               // -1: none
+    int iterations[5], evaluations[5];
+    float levelCutoffRepeat[5];
+  };
+  static PyramidTrackResult trackPyramid(std::vector<CudaCoarseTracker *> const &levels,
+                                         Eigen::Matrix<double, 4, 4> const &refToNew, Eigen::Vector2d const &aff_g2l,
+                                         float new_exposure, float coarseCutoffTH, const int maxIterations[5],
+                                         float lambdaExtrapolationLimit, float affineOptModeA, float affineOptModeB,
+                                         Eigen::Matrix<double, 5, 1> const &minResForAbort);
+
   void synchronize();
 
   void startTiming();

@@ -308,6 +308,33 @@ int tdm_tracker_track(tdm_tracker* t, const double refToNew[16], const double af
                       float coarse_cutoff_th, int max_iterations, float lambda_extrapolation_limit, int fix_a, int fix_b,
                       tdm_track_result* out);
 
+/* n5  CoarseTracker::trackNewestCoarse (CoarseTracker.cpp:750-936) for one motion hypothesis, all levels on the device
+ *     with one host wait: levels[l] is the tracker of pyramid level l, (w0>>l) x (h0>>l), each with setK, a reference and a
+ *     new image (setNewFromPyramid); the loop runs on levels[0]'s stream after the pending work of every level's stream.
+ *     Per level coarsest_level..0: lambda = 0.01, cutoff doubling while > 60 % of the residuals saturate, the LM iterations
+ *     of tdm_tracker_track (max_iterations[l]), lastResiduals[l] = sqrtf(E / numTermsInE), abort (ok = 0, pose unchanged)
+ *     when it exceeds 1.5 * min_res_for_abort[l] (NaN never aborts), and one repeat of the first level whose cutoff had to
+ *     be raised.  Then the affine checks of :923-931 with setting_affineOptModeA/B (< 0: that parameter is fixed and, if
+ *     ok, reported as 0).  Levels > 0 are evaluated with the GPU definitions of calcRes / calcG (DESIGN.md, n5).
+ *     Blocking.  Invalid input (missing setK / reference / new image, wrong level sizes, different devices,
+ *     coarsest_level outside 0..4, max_iterations outside 0..200) is an error and launches nothing. */
+typedef struct tdm_track_pyramid_result {
+  double ref_to_new[16];        /* lastToNew_out (row-major); unchanged from the input when the loop aborted */
+  double aff_g2l[2];            /* aff_g2l_out, after the "mode < 0 -> 0" rule of :934-935 */
+  double last_residuals[5];     /* CoarseTracker::lastResiduals, NaN for levels not reached */
+  double last_flow_indicators[3];
+  int ok;                       /* trackNewestCoarse's return value */
+  int aborted_level;            /* level whose residual exceeded 1.5 * min_res_for_abort, else -1 */
+  int repeated_level;           /* level run twice by the repeat rule (:911-915), else -1 */
+  int iterations[5], evaluations[5];   /* per level, summed over both passes of a repeated level */
+  float cutoff_repeat[5];       /* largest levelCutoffRepeat of each level's passes */
+  float device_ms;
+} tdm_track_pyramid_result;
+int tdm_tracker_track_pyramid(tdm_tracker* const* levels, int coarsest_level, const double refToNew[16], const double aff_g2l[2],
+                              float new_exposure, float coarse_cutoff_th, const int max_iterations[5],
+                              float lambda_extrapolation_limit, float affine_opt_mode_a, float affine_opt_mode_b,
+                              const double min_res_for_abort[5], tdm_track_pyramid_result* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -140,6 +140,34 @@ CudaCoarseTracker::TrackResult CudaCoarseTracker::track(Eigen::Matrix<double, 4,
   return out;
 }
 
+CudaCoarseTracker::PyramidTrackResult CudaCoarseTracker::trackPyramid(
+    std::vector<CudaCoarseTracker*> const& levels, Eigen::Matrix<double, 4, 4> const& refToNew, Eigen::Vector2d const& aff,
+    float new_exposure, float coarseCutoffTH, const int maxIterations[5], float lambdaExtrapolationLimit, float affineOptModeA,
+    float affineOptModeB, Eigen::Matrix<double, 5, 1> const& minResForAbort) {
+  std::vector<tdm_tracker*> h;
+  for (CudaCoarseTracker* t : levels) h.push_back(t ? t->handle_ : nullptr);
+  double T[16], minRes[5];
+  to_row_major(refToNew, T);
+  const double a[2] = {aff(0), aff(1)};
+  for (int i = 0; i < 5; ++i) minRes[i] = minResForAbort(i);
+  tdm_track_pyramid_result r;
+  chk(tdm_tracker_track_pyramid(h.data(), (int)h.size() - 1, T, a, new_exposure, coarseCutoffTH, maxIterations, lambdaExtrapolationLimit,
+                                affineOptModeA, affineOptModeB, minRes, &r),
+      "CudaCoarseTracker::trackPyramid");
+  PyramidTrackResult out;
+  out.ok = r.ok != 0;
+  for (int rr = 0; rr < 4; ++rr)
+    for (int c = 0; c < 4; ++c) out.refToNew(rr, c) = r.ref_to_new[4 * rr + c];
+  out.aff_g2l = Eigen::Vector2d(r.aff_g2l[0], r.aff_g2l[1]);
+  for (int i = 0; i < 5; ++i) {
+    out.lastResiduals(i) = r.last_residuals[i];
+    out.iterations[i] = r.iterations[i]; out.evaluations[i] = r.evaluations[i]; out.levelCutoffRepeat[i] = r.cutoff_repeat[i];
+  }
+  for (int i = 0; i < 3; ++i) out.lastFlowIndicators(i) = r.last_flow_indicators[i];
+  out.abortedLevel = r.aborted_level; out.repeatedLevel = r.repeated_level;
+  return out;
+}
+
 void CudaCoarseTracker::synchronize() { chk(tdm_tracker_synchronize(handle_), "CudaCoarseTracker::synchronize"); }
 
 void CudaCoarseTracker::startTiming() {

@@ -61,6 +61,14 @@ class TrackResult(ctypes.Structure):
                 ("iterations", ctypes.c_int), ("evaluations", ctypes.c_int), ("cutoff_repeat", ctypes.c_float), ("device_ms", ctypes.c_float)]
 
 
+class TrackPyramidResult(ctypes.Structure):
+    """tdm_track_pyramid_result (include/tandem_b200.h)."""
+    _fields_ = [("ref_to_new", ctypes.c_double * 16), ("aff_g2l", ctypes.c_double * 2), ("last_residuals", ctypes.c_double * 5),
+                ("last_flow_indicators", ctypes.c_double * 3), ("ok", ctypes.c_int), ("aborted_level", ctypes.c_int),
+                ("repeated_level", ctypes.c_int), ("iterations", ctypes.c_int * 5), ("evaluations", ctypes.c_int * 5),
+                ("cutoff_repeat", ctypes.c_float * 5), ("device_ms", ctypes.c_float)]
+
+
 def _declare(l):
     c = ctypes
     P = c.POINTER
@@ -130,6 +138,7 @@ def _declare(l):
         "tdm_tracker_set_reference_dense": (i, [vp, fp, vp, i, dp, i, i, i, fp, fp, fp, fp, fp, fp, vp, f, dp, ip]),
         "tdm_tracker_get_reference": (i, [vp, i, fp, fp, fp, fp]),
         "tdm_tracker_track": (i, [vp, dp, dp, f, f, i, f, i, i, P(TrackResult)]),
+        "tdm_tracker_track_pyramid": (i, [P(vp), i, dp, dp, f, f, ip, f, f, f, dp, P(TrackPyramidResult)]),
     }
     missing = []
     for name, (res, args) in sigs.items():

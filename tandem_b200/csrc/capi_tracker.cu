@@ -200,4 +200,35 @@ int tdm_tracker_track(tdm_tracker* t, const double refToNew[16], const double af
   TDM_API_END
 }
 
+/* ---- SURVEY 8(f) n5: CoarseTracker::trackNewestCoarse over all pyramid levels on the device ---- */
+int tdm_tracker_track_pyramid(tdm_tracker* const* levels, int coarsest_level, const double refToNew[16], const double aff_g2l[2],
+                              float new_exposure, float coarse_cutoff_th, const int max_iterations[5],
+                              float lambda_extrapolation_limit, float affine_opt_mode_a, float affine_opt_mode_b,
+                              const double min_res_for_abort[5], tdm_track_pyramid_result* out) {
+  TDM_API_BEGIN
+  TDM_CHECK(levels && refToNew && aff_g2l && max_iterations && min_res_for_abort && out, "null argument");
+  TDM_CHECK(coarsest_level >= 0 && coarsest_level <= 4, "coarsest_level must be in 0..4");
+  tdm::TrackerIface* impl[5] = {};
+  for (int l = 0; l <= coarsest_level; ++l) {
+    TDM_CHECK(levels[l], "track_pyramid level " + std::to_string(l) + ": null tracker");
+    impl[l] = levels[l]->impl;
+  }
+  tdm::TrackerIface::PyramidArgs a;
+  a.refToNew = refToNew; a.aff = aff_g2l; a.new_exposure = new_exposure; a.coarse_cutoff = coarse_cutoff_th;
+  a.max_iterations = max_iterations; a.lambda_extrapolation_limit = lambda_extrapolation_limit;
+  a.affine_mode_a = affine_opt_mode_a; a.affine_mode_b = affine_opt_mode_b; a.min_res_for_abort = min_res_for_abort;
+  tdm::TrackerIface::PyramidResult r;
+  impl[0]->track_pyramid(impl, coarsest_level, a, &r);
+  for (int i = 0; i < 16; ++i) out->ref_to_new[i] = r.refToNew[i];
+  out->aff_g2l[0] = r.aff[0]; out->aff_g2l[1] = r.aff[1];
+  for (int l = 0; l < 5; ++l) {
+    out->last_residuals[l] = r.last_residuals[l];
+    out->iterations[l] = r.iterations[l]; out->evaluations[l] = r.evaluations[l]; out->cutoff_repeat[l] = r.cutoff_repeat[l];
+  }
+  for (int i = 0; i < 3; ++i) out->last_flow_indicators[i] = r.last_flow_indicators[i];
+  out->ok = r.ok; out->aborted_level = r.aborted_level; out->repeated_level = r.repeated_level; out->device_ms = r.device_ms;
+  return TDM_OK;
+  TDM_API_END
+}
+
 }  // extern "C"

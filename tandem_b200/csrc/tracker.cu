@@ -44,7 +44,7 @@ struct TrkPose {
 
 struct LmCtx;
 struct TrkBufs {
-  LmCtx* lm;            // device LM loop (tdm_tracker_track): pose in, LM step out; nullptr for the plain calls
+  LmCtx* lm;            // device LM loop (tdm_tracker_track / _track_pyramid): level, pose in, LM step out; nullptr for the plain calls
   const float *pc_u, *pc_v, *pc_idepth, *pc_color, *dInew;
   float* warped;        // 7 x n_max: u, v, dx, dy, idepth, residual, weight
   long long n_max;
@@ -55,8 +55,61 @@ struct TrkBufs {
                         // then arrays indexed by blockIdx.y
 };
 
-__device__ bool lm_done(const LmCtx* c);
-__device__ const TrkPose* lm_pose(const LmCtx* c);
+// ---- device LM loop (n3 one level, n5 coarse-to-fine), see the n3 / n5 section below ----
+constexpr int kMaxLevels = 5;   // CoarseTracker::trackNewestCoarse: coarsestLvl < 5
+struct LmConfig {
+  float Ki[9];
+  float ref_exposure, new_exposure;
+  double ref_aff[2];
+  float huber, coarse_cutoff;
+  int max_iter;
+  float lambda_limit;
+  int fix_a, fix_b;
+};
+struct LmLevel {             // one pyramid level: its tracker's parameters and buffers, as the host hands them over
+  TrkParams p;               // pose-dependent fields are taken from LmCtx::pose
+  const float *pc_u, *pc_v, *pc_idepth, *pc_color, *dInew;
+  LmConfig cfg;
+};
+struct LmIn {                // uploaded once per call
+  LmLevel lv[kMaxLevels];    // lv[l] = pyramid level l
+  double T0[16], aff0[2];
+  double min_res[kMaxLevels];   // minResForAbort (pyramid mode)
+  float mode_a, mode_b;         // setting_affineOptModeA/B (pyramid mode; < 0 = fixed)
+  int coarsest;
+  int pyramid;               // 0: one level (tdm_tracker_track), 1: the coarse-to-fine rules of trackNewestCoarse
+  int max_evals;             // bound on the evaluations of the whole call (the rules never exceed it)
+};
+struct LmState {
+  double T[16], aff[2];      // accepted
+  double Tn[16], affn[2];    // candidate under evaluation
+  double res_old[6], H[64], b[8];
+  double lambda, inc_norm;
+  float repeat;
+  int phase, iter, evals;    // of the current pass over the current level
+};
+struct LmResult {            // mapped pinned host memory (device copy in LmCtx::r)
+  double T[16], aff[2];
+  double res[kMaxLevels][6];       // resOld of each level's last pass
+  double last_res[kMaxLevels];     // lastResiduals, NaN for levels not reached (pyramid mode)
+  double flow[3];                  // lastFlowIndicators (pyramid mode)
+  int iterations[kMaxLevels], evaluations[kMaxLevels];   // summed over the passes of a level
+  float repeat[kMaxLevels];        // largest levelCutoffRepeat of each level's passes
+  int num_warped;
+  int ok, aborted_level, repeated_level;
+  int done;                        // written last: 1 = finished, 2 = evaluation bound exceeded (internal error)
+};
+struct LmCtx {               // device memory, one per tracker
+  LmIn in;
+  LmState s;
+  TrkPose pose;
+  int lvl;                   // level under evaluation
+  int have_repeated, total_evals;
+  LmResult r;
+  LmResult* out;             // mapped pinned host memory
+  cudaGraphConditionalHandle loop;   // the WHILE node around the evaluation kernel
+};
+
 __device__ __noinline__ void lm_step(LmCtx* c, const double* o);
 
 __device__ __forceinline__ float3 bilinear33(const float* __restrict__ mat, float x, float y, int width) {  // cu:22-38
@@ -92,16 +145,23 @@ __device__ __forceinline__ void accumulate_g(float* g, float dxI, float dyI, flo
 }
 
 // MODE 0: calcRes (stats + warped buffers)   1: calcG from warped buffers   2: fused (stats + G, no buffers)
+// MODE 4: MODE 2 inside the device LM loop: the level's parameters, buffers and pose come from b.lm, the LM step runs in the
+//         last CTA.  Same arithmetic as MODE 2; a template of its own so that the plain MODE 2 keeps its registers.
 // MODE 3: calcRes statistics of blockIdx.y = 0..n_hyp-1 independent poses in one launch (no buffers): the motion hypotheses
 //         DSO tries one after the other (FullSystem.cpp:437-530) evaluated as a batch - SURVEY 8(e)'s only parallel axis of the
 //         tracker.  Same per-thread point striding and the same fixed-order reduction as MODE 0 -> identical numbers.
 template <int MODE>
 __global__ void __launch_bounds__(kThreads)
 k_tracker(const __grid_constant__ TrkParams p_in, TrkBufs b) {
+  constexpr bool FUSED = MODE == 2 || MODE == 4;
   TrkParams p = p_in;
-  if (MODE == 2 && b.lm) {
-    if (lm_done(b.lm)) return;                   // uniform over the grid: nobody touches the ticket
-    const TrkPose* q = lm_pose(b.lm);
+  const float* Ki = p.Ki;
+  if (MODE == 4) {                       // the current level's parameters and buffers, the LM step's candidate pose
+    const LmLevel& L = b.lm->in.lv[b.lm->lvl];
+    p = L.p;
+    Ki = L.p.Ki;                         // read where the flow statistics need it: keeps 9 registers free
+    b.pc_u = L.pc_u; b.pc_v = L.pc_v; b.pc_idepth = L.pc_idepth; b.pc_color = L.pc_color; b.dInew = L.dInew;
+    const TrkPose* q = &b.lm->pose;
 #pragma unroll
     for (int i = 0; i < 9; ++i) p.RKi[i] = q->RKi[i];
 #pragma unroll
@@ -124,8 +184,8 @@ k_tracker(const __grid_constant__ TrkParams p_in, TrkBufs b) {
   float acc[NV];
 #pragma unroll
   for (int k = 0; k < NV; ++k) acc[k] = 0.f;
-  float* st = acc;                               // stats (MODE 0, 2)
-  float* g = acc + (MODE == 2 ? kRes : 0);       // 45 products (MODE 1, 2)
+  float* st = acc;                               // stats (MODE 0, 2, 4)
+  float* g = acc + (FUSED ? kRes : 0);           // 45 products (MODE 1, 2, 4)
   const long long nm = b.n_max;
 
   for (int i = blockIdx.x * kThreads + threadIdx.x; i < p.n; i += kBlocks * kThreads) {
@@ -150,7 +210,7 @@ k_tracker(const __grid_constant__ TrkParams p_in, TrkBufs b) {
       float ptK[3], a[3], c[3], d[3];
 #pragma unroll
       for (int r = 0; r < 3; ++r) {
-        ptK[r] = mad3(p.Ki + 3 * r, x, y);
+        ptK[r] = mad3(Ki + 3 * r, x, y);
         const float tid = __fmul_rn(p.t[r], id);
         a[r] = __fadd_rn(ptK[r], tid); c[r] = __fsub_rn(ptK[r], tid); d[r] = __fsub_rn(pt[r], tid);
       }
@@ -174,7 +234,7 @@ k_tracker(const __grid_constant__ TrkParams p_in, TrkBufs b) {
         } else {
           st[0] += hw * res * res * (2.f - hw); st[1] += 1.f; st[2] += 1.f;
           wu = u; wv = v; wdx = hit.y; wdy = hit.z; wid = nid; wres = res; whw = hw;
-          if (MODE == 2) accumulate_g(g, hit.y, hit.z, u, v, nid, refc, res, hw, p);
+          if (FUSED) accumulate_g(g, hit.y, hit.z, u, v, nid, refc, res, hw, p);
         }
       }
     }
@@ -214,7 +274,7 @@ k_tracker(const __grid_constant__ TrkParams p_in, TrkBufs b) {
       b.out[OFF + threadIdx.x] = s;
     }
     if (threadIdx.x == 0) *b.ticket = 0;
-    if (MODE == 2 && b.lm) {                     // n3: the LM step rides on the evaluation's last CTA - no extra launch
+    if (MODE == 4) {                             // n3 / n5: the LM step rides on the evaluation's last CTA - no extra launch
       __threadfence();
       __syncthreads();
       if (threadIdx.x == 0) lm_step(b.lm, b.out);
@@ -342,44 +402,12 @@ __global__ void __launch_bounds__(256) k_dense_emit(const unsigned* __restrict__
 
 // ================================================================================================
 // n3 (SURVEY 8f): the level's Levenberg-Marquardt loop of CoarseTracker::trackNewestCoarse (CoarseTracker.cpp:761-916)
-// as a chain of (k_tracker<2>, k_lm_step) launches with NO host round trip: k_lm_step (one thread, double) turns the
-// evaluation's 52 sums into the accept/reject decision, the damped 8x8 solve, the SE3 update and the next candidate's
-// TrkPose; a `done` flag turns the remaining enqueued launches into no-ops.
+// and n5: the coarse-to-fine loop around it (CoarseTracker.cpp:750-936), with ONE host wait per call.  A CUDA graph
+// runs k_lm_init and then a conditional WHILE node around k_tracker<4>; the evaluation's last CTA runs lm_step (one
+// thread, double), which turns the 52 sums into the accept/reject decision, the damped 8x8 solve, the SE3 update and the
+// next candidate's TrkPose, moves on to the next level (or repeats one) and ends the WHILE loop when the call is done.
+// Every level runs through the same kernel: it reads its parameters and buffers from LmCtx::in.lv[lvl].
 // ================================================================================================
-struct LmConfig {
-  float Ki[9];
-  float ref_exposure, new_exposure;
-  double ref_aff[2];
-  float huber, coarse_cutoff;
-  int max_iter;
-  float lambda_limit;
-  int fix_a, fix_b;
-};
-struct LmState {
-  double T[16], aff[2];      // accepted
-  double Tn[16], affn[2];    // candidate under evaluation
-  double res_old[6], H[64], b[8];
-  double lambda, inc_norm;
-  float repeat;
-  int phase, iter, evals;
-};
-struct LmResult {            // mapped pinned host memory
-  double T[16], aff[2], res[6];
-  int iterations, evaluations;
-  float repeat;
-  int num_warped;
-};
-
-struct LmCtx {               // device memory, one per tracker
-  LmConfig cfg;
-  LmState s;
-  TrkPose pose;
-  int done;
-  LmResult* out;             // mapped pinned host memory
-};
-__device__ bool lm_done(const LmCtx* c) { return c->done != 0; }
-__device__ const TrkPose* lm_pose(const LmCtx* c) { return &c->pose; }
-
 __device__ void lm_pose_from(const LmConfig& c, const double* T, const double* aff, float cutoff, TrkPose* o) {
   float R[9];
   for (int r = 0; r < 3; ++r) {
@@ -477,27 +505,85 @@ __device__ void lm_take_g(const double* o, int num_warped, LmState* s) {   // fi
   }
 }
 
-__global__ void k_lm_init(LmCtx* c, LmConfig cfg, LmResult* out, const double* T0 /*16 + 2 aff, device*/) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  c->cfg = cfg;
-  c->out = out;
+__device__ void lm_begin_level(LmCtx* c, int lvl) {   // CoarseTracker.cpp:764,798: levelCutoffRepeat = 1, lambda = 0.01
   LmState* s = &c->s;
-  for (int i = 0; i < 16; ++i) s->T[i] = s->Tn[i] = T0[i];
-  s->aff[0] = s->affn[0] = T0[16];
-  s->aff[1] = s->affn[1] = T0[17];
+  const LmConfig& cfg = c->in.lv[lvl].cfg;
+  c->lvl = lvl;
+  for (int i = 0; i < 16; ++i) s->Tn[i] = s->T[i];
+  s->affn[0] = s->aff[0]; s->affn[1] = s->aff[1];
   s->lambda = 0.01; s->inc_norm = 0; s->repeat = 1.f; s->phase = 0; s->iter = 0; s->evals = 0;
-  c->done = 0;
   lm_pose_from(cfg, s->T, s->aff, cfg.coarse_cutoff, &c->pose);
 }
 
+__global__ void k_lm_init(LmCtx* c, LmResult* out, cudaGraphConditionalHandle loop) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  c->out = out;
+  c->loop = loop;
+  LmState* s = &c->s;
+  for (int i = 0; i < 16; ++i) s->T[i] = c->in.T0[i];
+  s->aff[0] = c->in.aff0[0]; s->aff[1] = c->in.aff0[1];
+  LmResult* r = &c->r;
+  for (int l = 0; l < kMaxLevels; ++l) {
+    for (int i = 0; i < 6; ++i) r->res[l][i] = 0;
+    r->last_res[l] = __longlong_as_double(0x7ff8000000000000ll);   // lastResiduals.setConstant(NAN)  (:746)
+    r->iterations[l] = 0; r->evaluations[l] = 0; r->repeat[l] = 1.f;
+  }
+  for (int i = 0; i < 3; ++i) r->flow[i] = 1000;                    // lastFlowIndicators.setConstant(1000)  (:747)
+  r->num_warped = 0; r->ok = 0; r->aborted_level = -1; r->repeated_level = -1; r->done = 0;
+  c->have_repeated = 0; c->total_evals = 0;
+  lm_begin_level(c, c->in.coarsest);
+}
+
+// Publishes the result and ends the WHILE loop.  `pose_out` = the loop reached the end (lastToNew_out / aff_g2l_out are
+// written, :919-920); otherwise the input pose is returned.
+__device__ void lm_finish(LmCtx* ctx, int ok, bool pose_out, int done) {
+  LmResult* r = &ctx->r;
+  const LmState* s = &ctx->s;
+  for (int i = 0; i < 16; ++i) r->T[i] = pose_out ? s->T[i] : ctx->in.T0[i];
+  r->aff[0] = pose_out ? s->aff[0] : ctx->in.aff0[0];
+  r->aff[1] = pose_out ? s->aff[1] : ctx->in.aff0[1];
+  r->ok = ok;
+  LmResult* out = ctx->out;
+  const int* src = reinterpret_cast<const int*>(r);
+  int* dst = reinterpret_cast<int*>(out);
+  for (int i = 0; i < (int)(offsetof(LmResult, done) / sizeof(int)); ++i) dst[i] = src[i];
+  __threadfence_system();
+  out->done = done;                                  // written last: the host checks it after its one wait
+  __threadfence_system();
+  cudaGraphSetConditional(ctx->loop, 0);
+}
+
+// :918-935, after the level loop: the affine sanity checks with the float modes, then fixed parameters reported as 0
+__device__ void lm_finish_pyramid(LmCtx* ctx) {
+  LmState* s = &ctx->s;
+  const float ma = ctx->in.mode_a, mb = ctx->in.mode_b;
+  const double a = s->aff[0], b = s->aff[1];
+  bool ok = !((ma != 0 && fabsf((float)a) > 1.2) || (mb != 0 && fabsf((float)b) > 200));
+  if (ok) {
+    const LmConfig& c0 = ctx->in.lv[0].cfg;        // AffLight::fromToVecExposure(lastRef, newFrame, ...).cast<float>()
+    float eF = c0.ref_exposure, eT = c0.new_exposure;
+    if (eF == 0 || eT == 0) eT = eF = 1;
+    const double ra = exp(a - c0.ref_aff[0]) * eT / eF;
+    const double rb = b - ra * c0.ref_aff[1];
+    const float rel0 = (float)ra, rel1 = (float)rb;
+    ok = !((ma == 0 && fabsf(logf(rel0)) > 1.5) || (mb == 0 && fabsf(rel1) > 200));
+  }
+  if (ok) {
+    if (ma < 0) s->aff[0] = 0;
+    if (mb < 0) s->aff[1] = 0;
+  }
+  lm_finish(ctx, ok ? 1 : 0, true, 1);
+}
+
 __device__ __noinline__ void lm_step(LmCtx* ctx, const double* o /*kOut sums of the evaluation just finished*/) {
-  const LmConfig& c = ctx->cfg;
+  const int lvl = ctx->lvl;
+  const LmConfig& c = ctx->in.lv[lvl].cfg;
   LmState* s = &ctx->s;
   TrkPose* pose = &ctx->pose;
-  LmResult* out = ctx->out;
   double res[6] = {o[0], o[1], o[4] / o[6], 0.0, o[5] / o[6], o[3] / o[1]};   // finish_res, cuda_coarse_tracker.cpp:264-272
   const int num_warped = (int)o[2];
   s->evals++;
+  if (++ctx->total_evals > ctx->in.max_evals) { lm_finish(ctx, 0, false, 2); return; }
   bool finished = false;
   if (s->phase == 0) {
     if (res[5] > 0.6 && s->repeat < 50.f) {              // CoarseTracker.cpp:779-790: too many saturated residuals
@@ -524,18 +610,32 @@ __device__ __noinline__ void lm_step(LmCtx* ctx, const double* o /*kOut sums of 
     s->iter++;
     if (!(s->inc_norm > 1e-3) || s->iter >= c.max_iter) finished = true;
   }
-  if (finished) {
-    for (int i = 0; i < 16; ++i) out->T[i] = s->T[i];
-    out->aff[0] = s->aff[0]; out->aff[1] = s->aff[1];
-    for (int i = 0; i < 6; ++i) out->res[i] = s->res_old[i];
-    out->evaluations = s->evals; out->repeat = s->repeat; out->num_warped = num_warped;
-    __threadfence_system();
-    out->iterations = s->iter;                       // written last: the host polls it (>= 0 means finished)
-    __threadfence_system();
-    ctx->done = 1;
+  if (!finished) {
+    lm_next_candidate(c, s, pose);
     return;
   }
-  lm_next_candidate(c, s, pose);
+  LmResult* r = &ctx->r;
+  for (int i = 0; i < 6; ++i) r->res[lvl][i] = s->res_old[i];
+  r->iterations[lvl] += s->iter; r->evaluations[lvl] += s->evals; r->num_warped = num_warped;
+  r->repeat[lvl] = fmaxf(r->repeat[lvl], s->repeat);
+  if (!ctx->in.pyramid) { lm_finish(ctx, 1, true, 1); return; }
+  // :906-915 - lastResiduals / lastFlowIndicators, the abort test, the one-time repeat of a level whose cutoff was raised
+  const float last_res = sqrtf((float)(s->res_old[0] / s->res_old[1]));
+  r->last_res[lvl] = last_res;
+  for (int i = 0; i < 3; ++i) r->flow[i] = s->res_old[2 + i];
+  if (last_res > 1.5 * ctx->in.min_res[lvl]) {      // NaN never aborts
+    r->aborted_level = lvl;
+    lm_finish(ctx, 0, false, 1);
+    return;
+  }
+  if (s->repeat > 1 && !ctx->have_repeated) {
+    ctx->have_repeated = 1;
+    r->repeated_level = lvl;
+    lm_begin_level(ctx, lvl);
+    return;
+  }
+  if (lvl > 0) { lm_begin_level(ctx, lvl - 1); return; }
+  lm_finish_pyramid(ctx);
 }
 
 }  // namespace
@@ -573,7 +673,10 @@ class TrackerImpl final : public TrackerIface {
     cudaFreeHost(h_pc_); cudaFreeHost(h_dI_); cudaFreeHost(h_out_);
     if (d_batch_) { cudaFree(d_batch_); cudaFreeHost(h_batch_); cudaFree(d_batch_partials_); cudaFree(d_batch_ticket_); cudaFreeHost(h_batch_out_); }
     cudaFree(d_proj_); cudaFree(d_depth_); cudaFree(d_idepth0_); cudaFree(d_gray_); cudaFree(d_rowcnt_); cudaFree(d_rowoff_);
-    cudaFree(d_total_); cudaFree(d_lm_ctx_); cudaFree(d_lm_out_); cudaFree(d_lm_in_);
+    cudaFree(d_total_); cudaFree(d_lm_ctx_); cudaFree(d_lm_out_);
+    if (lm_exec_) cudaGraphExecDestroy(lm_exec_);
+    for (cudaEvent_t e : {lm_in_free_, lm_e0_, lm_e1_, ready_})
+      if (e) cudaEventDestroy(e);
     if (h_front_) cudaFreeHost(h_front_);
     if (h_total_) cudaFreeHost(h_total_);
     if (h_lm_in_) cudaFreeHost(h_lm_in_);
@@ -605,6 +708,7 @@ class TrackerImpl final : public TrackerIface {
       TDM_CUDA(cudaMemcpyAsync(d_pc_ + a * nm, h_pc_ + a * nm, 4 * (size_t)n, cudaMemcpyHostToDevice, stream_));
     ref_exposure_ = ref_exposure;
     ref_aff_[0] = ref_aff[0]; ref_aff_[1] = ref_aff[1];
+    have_ref_ = true;
     have_params_ = false;   // a calcG now needs a calcRes against the new reference first
   }
 
@@ -728,6 +832,7 @@ class TrackerImpl final : public TrackerIface {
     n_ = a.n_sparse + total;      // the pre-increment quirk: the last appended point is not counted
     ref_exposure_ = a.ref_exposure;
     ref_aff_[0] = a.ref_aff[0]; ref_aff_[1] = a.ref_aff[1];
+    have_ref_ = true;
     have_params_ = false;
     return n_;
   }
@@ -756,49 +861,59 @@ class TrackerImpl final : public TrackerIface {
     TDM_CHECK(have_k_, "track before setK");
     TDM_CHECK(have_new_, "track before setNew");
     TDM_CHECK(a.refToNew && a.aff && r, "null argument");
-    TDM_CHECK(a.max_iterations >= 0 && a.max_iterations <= 200, "max_iterations out of range");
+    TDM_CHECK(a.max_iterations >= 0 && a.max_iterations <= kMaxIterations, "max_iterations out of range");
     TDM_CUDA(cudaSetDevice(device_));
-    ensure_lm_buffers();
-    p_.w = w_; p_.h = h_; p_.n = n_;
-    p_.fx = fx_; p_.fy = fy_; p_.cx = cx_; p_.cy = cy_;
-    for (int i = 0; i < 9; ++i) p_.Ki[i] = Ki_[i];
-    p_.huber = huber_; p_.ref_b = (float)ref_aff_[1];
-    LmConfig c;
-    for (int i = 0; i < 9; ++i) c.Ki[i] = Ki_[i];
-    c.ref_exposure = ref_exposure_; c.new_exposure = a.new_exposure;
-    c.ref_aff[0] = ref_aff_[0]; c.ref_aff[1] = ref_aff_[1];
-    c.huber = huber_; c.coarse_cutoff = a.coarse_cutoff; c.max_iter = a.max_iterations;
-    c.lambda_limit = a.lambda_extrapolation_limit; c.fix_a = a.fix_a; c.fix_b = a.fix_b;
-    TDM_CUDA(cudaStreamSynchronize(stream_));      // h_lm_in_ may still be read by a previous call
-    for (int i = 0; i < 16; ++i) h_lm_in_[i] = a.refToNew[i];
-    h_lm_in_[16] = a.aff[0]; h_lm_in_[17] = a.aff[1];
-    h_lm_res_->iterations = -1;
-    cudaEvent_t e0, e1;
-    TDM_CUDA(cudaEventCreate(&e0)); TDM_CUDA(cudaEventCreate(&e1));
-    TDM_CUDA(cudaEventRecord(e0, stream_));
-    TDM_CUDA(cudaMemcpyAsync(d_lm_in_, h_lm_in_, 18 * 8, cudaMemcpyHostToDevice, stream_));
-    k_lm_init<<<1, 32, 0, stream_>>>(d_lm_ctx_, c, d_lm_res_, d_lm_in_);
-    // Evaluations are enqueued in batches of kBatch with no host involvement inside a batch (the LM step runs in the
-    // evaluation kernel's last CTA; a converged loop turns the rest of a batch into empty launches).  Between batches
-    // the host looks at the mapped result once.  Worst case: initial + 6 cutoff doublings (2^6 > 50) + one per iteration.
-    constexpr int kBatch = 4;
-    const int max_evals = 1 + 6 + a.max_iterations;
-    const volatile LmResult* o = h_lm_res_;
-    for (int e = 0; e < max_evals && o->iterations < 0; e += kBatch) {
-      for (int k = 0; k < kBatch && e + k < max_evals; ++k) launch(2, true);
-      TDM_CUDA(cudaStreamSynchronize(stream_));
-    }
-    TDM_CUDA(cudaEventRecord(e1, stream_));
-    TDM_CUDA(cudaGetLastError());
-    TDM_CUDA(cudaEventSynchronize(e1));
-    TDM_CUDA(cudaEventElapsedTime(&r->device_ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    if (o->iterations < 0) throw Error("track: the device loop did not finish (internal error)");
+    LmIn& in = lm_in();
+    fill_level(&in.lv[0], a.new_exposure, a.coarse_cutoff, a.max_iterations, a.lambda_extrapolation_limit, a.fix_a, a.fix_b);
+    in.coarsest = 0;
+    in.pyramid = 0;
+    in.max_evals = 1 + 6 + a.max_iterations;   // initial + 6 cutoff doublings (2^6 > 50) + one per iteration
+    const LmResult* o = run_lm(a.refToNew, a.aff, &r->device_ms);
     for (int i = 0; i < 16; ++i) r->refToNew[i] = o->T[i];
     r->aff[0] = o->aff[0]; r->aff[1] = o->aff[1];
-    for (int i = 0; i < 6; ++i) r->res[i] = o->res[i];
-    r->iterations = o->iterations; r->evaluations = o->evaluations; r->cutoff_repeat = o->repeat;
+    for (int i = 0; i < 6; ++i) r->res[i] = o->res[0][i];
+    r->iterations = o->iterations[0]; r->evaluations = o->evaluations[0]; r->cutoff_repeat = o->repeat[0];
     num_warped_ = o->num_warped;
+  }
+  // ---------------------------------------------------------------------------------------------- n5
+  void track_pyramid(TrackerIface* const* levels, int coarsest, const PyramidArgs& a, PyramidResult* r) override {
+    TDM_CHECK(levels && a.refToNew && a.aff && a.max_iterations && a.min_res_for_abort && r, "null argument");
+    TDM_CHECK(coarsest >= 0 && coarsest < kMaxLevels, "coarsest_level must be in 0..4");
+    TrackerImpl* lv[kMaxLevels] = {};
+    for (int l = 0; l <= coarsest; ++l) {
+      const std::string at = "track_pyramid level " + std::to_string(l) + ": ";
+      TDM_CHECK(levels[l], at + "null tracker");
+      lv[l] = dynamic_cast<TrackerImpl*>(levels[l]);
+      TDM_CHECK(lv[l], at + "not a tracker of this library");
+      TDM_CHECK(lv[l]->w_ == (w_ >> l) && lv[l]->h_ == (h_ >> l), at + "size must be level 0's size >> level");
+      TDM_CHECK(lv[l]->device_ == device_, at + "trackers live on different devices");
+      TDM_CHECK(lv[l]->have_k_, at + "setK missing");
+      TDM_CHECK(lv[l]->have_ref_, at + "no reference set");
+      TDM_CHECK(lv[l]->have_new_, at + "no new image set");
+      TDM_CHECK(a.max_iterations[l] >= 0 && a.max_iterations[l] <= kMaxIterations, at + "max_iterations out of range");
+    }
+    TDM_CUDA(cudaSetDevice(device_));
+    LmIn& in = lm_in();
+    in.max_evals = 0;
+    for (int l = 0; l <= coarsest; ++l) {
+      lv[l]->fill_level(&in.lv[l], a.new_exposure, a.coarse_cutoff, a.max_iterations[l], a.lambda_extrapolation_limit,
+                        a.affine_mode_a < 0, a.affine_mode_b < 0);
+      in.max_evals += 2 * (1 + 6 + a.max_iterations[l]);   // a level may run twice (the repeat rule)
+      in.min_res[l] = a.min_res_for_abort[l];
+      if (l > 0) lv[l]->order_before(stream_);           // reference upload, setNewFromPyramid copy of that tracker
+    }
+    in.mode_a = a.affine_mode_a; in.mode_b = a.affine_mode_b;
+    in.coarsest = coarsest;
+    in.pyramid = 1;
+    const LmResult* o = run_lm(a.refToNew, a.aff, &r->device_ms);
+    for (int i = 0; i < 16; ++i) r->refToNew[i] = o->T[i];
+    r->aff[0] = o->aff[0]; r->aff[1] = o->aff[1];
+    for (int l = 0; l < kMaxLevels; ++l) {
+      r->last_residuals[l] = o->last_res[l];
+      r->iterations[l] = o->iterations[l]; r->evaluations[l] = o->evaluations[l]; r->cutoff_repeat[l] = o->repeat[l];
+    }
+    for (int i = 0; i < 3; ++i) r->last_flow_indicators[i] = o->flow[i];
+    r->ok = o->ok; r->aborted_level = o->aborted_level; r->repeated_level = o->repeated_level;
   }
   void synchronize() override {
     TDM_CUDA(cudaSetDevice(device_));
@@ -831,14 +946,98 @@ class TrackerImpl final : public TrackerIface {
     TDM_CUDA(cudaMallocHost(&h_front_, 3 * 4 * npx));
     TDM_CUDA(cudaMallocHost(&h_total_, 4));
   }
+  // The device LM loop as a graph, built once per tracker: k_lm_init, then WHILE (handle, default 1) { k_tracker<4> }.
+  // Every parameter that changes between calls (levels, sizes, buffers, pose) travels in LmCtx::in, so the graph never
+  // needs an update.
   void ensure_lm_buffers() {
-    if (d_lm_ctx_) return;
+    if (lm_exec_) return;
     TDM_CUDA(cudaMalloc(&d_lm_ctx_, sizeof(LmCtx)));
     TDM_CUDA(cudaMalloc(&d_lm_out_, kOut * 8));
-    TDM_CUDA(cudaMalloc(&d_lm_in_, 18 * 8));
-    TDM_CUDA(cudaMallocHost(&h_lm_in_, 18 * 8));
+    TDM_CUDA(cudaMallocHost(&h_lm_in_, sizeof(LmIn)));
     TDM_CUDA(cudaHostAlloc(&h_lm_res_, sizeof(LmResult), cudaHostAllocMapped));
     TDM_CUDA(cudaHostGetDevicePointer(&d_lm_res_, h_lm_res_, 0));
+    TDM_CUDA(cudaEventCreateWithFlags(&lm_in_free_, cudaEventDisableTiming));
+    TDM_CUDA(cudaEventCreate(&lm_e0_));
+    TDM_CUDA(cudaEventCreate(&lm_e1_));
+    cudaGraph_t g = nullptr;
+    TDM_CUDA(cudaGraphCreate(&g, 0));
+    try {
+      cudaGraphConditionalHandle loop;
+      TDM_CUDA(cudaGraphConditionalHandleCreate(&loop, g, 1, cudaGraphCondAssignDefault));
+      cudaKernelNodeParams kp = {};
+      void* init_args[] = {&d_lm_ctx_, &d_lm_res_, &loop};
+      kp.func = (void*)k_lm_init;
+      kp.gridDim = dim3(1); kp.blockDim = dim3(32);
+      kp.kernelParams = init_args;
+      cudaGraphNode_t init;
+      TDM_CUDA(cudaGraphAddKernelNode(&init, g, nullptr, 0, &kp));
+      cudaGraphNodeParams cp = {};
+      cp.type = cudaGraphNodeTypeConditional;
+      cp.conditional.handle = loop;
+      cp.conditional.type = cudaGraphCondTypeWhile;
+      cp.conditional.size = 1;
+      cudaGraphNode_t while_node;
+      TDM_CUDA(cudaGraphAddNode(&while_node, g, &init, 1, &cp));
+      TrkParams p{};                                 // unused: the kernel reads the level's parameters from LmCtx
+      TrkBufs b{};
+      b.lm = d_lm_ctx_; b.partials = d_partials_; b.ticket = d_ticket_; b.out = d_lm_out_;
+      void* eval_args[] = {&p, &b};
+      kp.func = (void*)k_tracker<4>;
+      kp.gridDim = dim3(kBlocks); kp.blockDim = dim3(kThreads);
+      kp.kernelParams = eval_args;
+      cudaGraphNode_t eval;
+      TDM_CUDA(cudaGraphAddKernelNode(&eval, cp.conditional.phGraph_out[0], nullptr, 0, &kp));
+      TDM_CUDA(cudaGraphInstantiate(&lm_exec_, g, 0));
+    } catch (...) {
+      cudaGraphDestroy(g);
+      throw;
+    }
+    cudaGraphDestroy(g);
+  }
+  // the staging of LmCtx::in; free once the previous call's upload has completed (normally long since)
+  LmIn& lm_in() {
+    ensure_lm_buffers();
+    TDM_CUDA(cudaEventSynchronize(lm_in_free_));
+    return *h_lm_in_;
+  }
+  // this tracker's parameters and buffers as one level of the device LM loop
+  void fill_level(LmLevel* L, float new_exposure, float coarse_cutoff, int max_iter, float lambda_limit, int fix_a, int fix_b) const {
+    L->p = TrkParams{};
+    L->p.w = w_; L->p.h = h_; L->p.n = n_;
+    L->p.fx = fx_; L->p.fy = fy_; L->p.cx = cx_; L->p.cy = cy_;
+    for (int i = 0; i < 9; ++i) L->p.Ki[i] = Ki_[i];
+    L->p.huber = huber_; L->p.ref_b = (float)ref_aff_[1];
+    const size_t nm = (size_t)n_max_;
+    L->pc_u = d_pc_; L->pc_v = d_pc_ + nm; L->pc_idepth = d_pc_ + 2 * nm; L->pc_color = d_pc_ + 3 * nm; L->dInew = d_dI_;
+    LmConfig& c = L->cfg;
+    for (int i = 0; i < 9; ++i) c.Ki[i] = Ki_[i];
+    c.ref_exposure = ref_exposure_; c.new_exposure = new_exposure;
+    c.ref_aff[0] = ref_aff_[0]; c.ref_aff[1] = ref_aff_[1];
+    c.huber = huber_; c.coarse_cutoff = coarse_cutoff; c.max_iter = max_iter;
+    c.lambda_limit = lambda_limit; c.fix_a = fix_a; c.fix_b = fix_b;
+  }
+  // orders this tracker's pending stream work before work enqueued later on `other`
+  void order_before(cudaStream_t other) {
+    if (!ready_) TDM_CUDA(cudaEventCreateWithFlags(&ready_, cudaEventDisableTiming));
+    TDM_CUDA(cudaEventRecord(ready_, stream_));
+    TDM_CUDA(cudaStreamWaitEvent(other, ready_, 0));
+  }
+  // Runs the graph on h_lm_in_ (filled by the caller) with one host wait; returns the mapped result.
+  const LmResult* run_lm(const double* T0, const double* aff0, float* device_ms) {
+    LmIn& in = *h_lm_in_;
+    for (int i = 0; i < 16; ++i) in.T0[i] = T0[i];
+    in.aff0[0] = aff0[0]; in.aff0[1] = aff0[1];
+    h_lm_res_->done = 0;
+    TDM_CUDA(cudaEventRecord(lm_e0_, stream_));
+    TDM_CUDA(cudaMemcpyAsync(&d_lm_ctx_->in, h_lm_in_, sizeof(LmIn), cudaMemcpyHostToDevice, stream_));
+    TDM_CUDA(cudaEventRecord(lm_in_free_, stream_));
+    TDM_CUDA(cudaGraphLaunch(lm_exec_, stream_));
+    TDM_CUDA(cudaEventRecord(lm_e1_, stream_));
+    TDM_CUDA(cudaEventSynchronize(lm_e1_));
+    TDM_CUDA(cudaEventElapsedTime(device_ms, lm_e0_, lm_e1_));
+    const volatile LmResult* o = h_lm_res_;
+    if (o->done != 1) throw Error("track: the device loop did not finish (internal error)");
+    return h_lm_res_;
   }
   void set_aff(float new_exposure, const double aff[2]) {  // AffLight::fromToVecExposure, cpp:42-52
     float eF = ref_exposure_, eT = new_exposure;
@@ -870,14 +1069,14 @@ class TrackerImpl final : public TrackerIface {
     p_.maxEnergy = 2 * huber_ * cutoffTH - huber_ * huber_;
     have_params_ = true;
   }
-  void launch(int mode, bool dev_loop = false) {
+  void launch(int mode) {
     TDM_CUDA(cudaSetDevice(device_));   // another handle of this thread may have switched the current device
     TrkBufs b;
     const size_t nm = (size_t)n_max_;
-    b.lm = dev_loop ? d_lm_ctx_ : nullptr;
+    b.lm = nullptr;
     b.pc_u = d_pc_; b.pc_v = d_pc_ + nm; b.pc_idepth = d_pc_ + 2 * nm; b.pc_color = d_pc_ + 3 * nm;
     b.dInew = d_dI_; b.warped = d_warped_; b.n_max = n_max_;
-    b.partials = d_partials_; b.ticket = d_ticket_; b.out = dev_loop ? d_lm_out_ : d_out_; b.batch = nullptr;
+    b.partials = d_partials_; b.ticket = d_ticket_; b.out = d_out_; b.batch = nullptr;
     if (mode == 0) k_tracker<0><<<kBlocks, kThreads, 0, stream_>>>(p_, b);
     else if (mode == 1) k_tracker<1><<<kBlocks, kThreads, 0, stream_>>>(p_, b);
     else k_tracker<2><<<kBlocks, kThreads, 0, stream_>>>(p_, b);
@@ -953,7 +1152,8 @@ class TrackerImpl final : public TrackerIface {
   int device_;
   int n_max_ = 0, n_ = 0;
   float fx_ = 0, fy_ = 0, cx_ = 0, cy_ = 0, Ki_[9];
-  bool have_k_ = false, have_new_ = false, have_params_ = false;
+  bool have_k_ = false, have_ref_ = false, have_new_ = false, have_params_ = false;
+  static constexpr int kMaxIterations = 200;
   float ref_exposure_ = 1.f;
   double ref_aff_[2] = {0, 0};
   cudaStream_t stream_ = nullptr;
@@ -972,8 +1172,12 @@ class TrackerImpl final : public TrackerIface {
   int *d_rowcnt_ = nullptr, *d_rowoff_ = nullptr, *d_total_ = nullptr, *h_total_ = nullptr;
   // n3 buffers
   LmCtx* d_lm_ctx_ = nullptr;
-  double *d_lm_out_ = nullptr, *d_lm_in_ = nullptr, *h_lm_in_ = nullptr;
+  double* d_lm_out_ = nullptr;
+  LmIn* h_lm_in_ = nullptr;
   LmResult *h_lm_res_ = nullptr, *d_lm_res_ = nullptr;
+  cudaGraphExec_t lm_exec_ = nullptr;
+  cudaEvent_t lm_in_free_ = nullptr, lm_e0_ = nullptr, lm_e1_ = nullptr;
+  cudaEvent_t ready_ = nullptr;   // order_before
 };
 
 

@@ -61,6 +61,25 @@ class TrackerIface {
     float device_ms;
   };
   virtual void track(const TrackArgs& a, TrackResult* r) = 0;
+  // n5: CoarseTracker::trackNewestCoarse over levels[0..coarsest] (called on levels[0], which runs the loop on its stream)
+  struct PyramidArgs {
+    const double* refToNew = nullptr;
+    const double* aff = nullptr;
+    float new_exposure = 1.f, coarse_cutoff = 20.f;
+    const int* max_iterations = nullptr;          // [5]
+    float lambda_extrapolation_limit = 0.001f;
+    float affine_mode_a = 0.f, affine_mode_b = 0.f;
+    const double* min_res_for_abort = nullptr;    // [5]
+  };
+  struct PyramidResult {
+    double refToNew[16], aff[2];
+    double last_residuals[5], last_flow_indicators[3];
+    int ok, aborted_level, repeated_level;
+    int iterations[5], evaluations[5];
+    float cutoff_repeat[5];
+    float device_ms;
+  };
+  virtual void track_pyramid(TrackerIface* const* levels, int coarsest, const PyramidArgs& a, PyramidResult* r) = 0;
 };
 
 // FrameHessian::makeImages on the device (n2): all pyramid levels of (I, dx, dy) + absSquaredGrad.

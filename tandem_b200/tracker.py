@@ -5,7 +5,7 @@ import ctypes
 
 import numpy as np
 
-from ._lib import TrackResult, check, lib
+from ._lib import TrackPyramidResult, TrackResult, check, lib
 
 _fp = ctypes.POINTER(ctypes.c_float)
 _dp = ctypes.POINTER(ctypes.c_double)
@@ -177,3 +177,31 @@ class CudaCoarseTracker:
         ms = ctypes.c_float()
         check(lib().tdm_tracker_run_resident(self._h, iters, ctypes.byref(ms)))
         return ms.value
+
+
+def track_pyramid(trackers, refToNew, aff_g2l, new_exposure, coarse_cutoff=20.0, max_iterations=(10, 20, 50, 50, 50),
+                  lambda_extrapolation_limit=0.001, affine_opt_mode_a=0.0, affine_opt_mode_b=0.0, min_res_for_abort=None):
+    """CoarseTracker::trackNewestCoarse (CoarseTracker.cpp:750-936) for one motion hypothesis, every level on the device with
+    one host wait.  trackers[l] is the CudaCoarseTracker of pyramid level l ((w >> l) x (h >> l)), each with setK, a reference and
+    a new image; len(trackers) - 1 is the coarsest level.  affine_opt_mode_a/b are setting_affineOptModeA/B (< 0: fixed).
+    min_res_for_abort: 5 values, NaN (the default) never aborts.  Returns a dict like CudaCoarseTracker.track plus the
+    coarse-to-fine outcome (ok, aborted_level, repeated_level, per-level last_residuals / iterations / evaluations /
+    cutoff_repeat, last_flow_indicators)."""
+    n = len(trackers)
+    hs = (ctypes.c_void_p * max(n, 1))(*[t._h for t in trackers])
+    T = np.ascontiguousarray(refToNew, np.float64)
+    aff = np.ascontiguousarray(aff_g2l, np.float64)
+    its = np.zeros(5, np.int32)
+    its[:min(len(max_iterations), 5)] = np.asarray(max_iterations, np.int32)[:5]
+    mr = np.full(5, np.nan) if min_res_for_abort is None else np.ascontiguousarray(min_res_for_abort, np.float64)
+    assert T.size == 16 and aff.size == 2 and mr.size == 5
+    r = TrackPyramidResult()
+    check(lib().tdm_tracker_track_pyramid(hs, n - 1, T.ctypes.data_as(_dp), aff.ctypes.data_as(_dp), float(new_exposure),
+                                          float(coarse_cutoff), its.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+                                          float(lambda_extrapolation_limit), float(affine_opt_mode_a), float(affine_opt_mode_b),
+                                          mr.ctypes.data_as(_dp), ctypes.byref(r)))
+    return dict(refToNew=np.array(r.ref_to_new, np.float64).reshape(4, 4), aff=np.array(r.aff_g2l, np.float64), ok=bool(r.ok),
+                aborted_level=r.aborted_level, repeated_level=r.repeated_level,
+                last_residuals=np.array(r.last_residuals, np.float64), last_flow_indicators=np.array(r.last_flow_indicators, np.float64),
+                iterations=np.array(r.iterations[:], np.int32), evaluations=np.array(r.evaluations[:], np.int32),
+                cutoff_repeat=np.array(r.cutoff_repeat[:], np.float32), device_ms=r.device_ms)

@@ -1,11 +1,13 @@
 """Secondary measurements (SURVEY.md §8d configs 3/4): TSDF integrate + ray-cast at the initDr map size with a stream
-of synthetic 640x480 depth maps, the level-0 tracker evaluation, and - when oracle/_ref is present - the REFERENCE's own
+of synthetic 640x480 depth maps, the level-0 tracker evaluation, the coarse-to-fine track of a frame (host-driven chain of
+per-level tdm_tracker_track calls vs one tdm_tracker_track_pyramid), and - when oracle/_ref is present - the REFERENCE's own
 dr_fusion (compiled unmodified for sm_90a) on the same inputs on the same GPU.
-    python tools/bench_fusion_tracker.py [n_frames]
+    python tools/bench_fusion_tracker.py [n_frames] [--pyramid-only]
 Prints one JSON line per measurement."""
 import ctypes
 import json
 import os
+import subprocess
 import sys
 import time
 
@@ -13,11 +15,88 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from tandem_b200 import CudaCoarseTracker, DrFusion, DrFusionOptions  # noqa: E402
-from tandem_b200.synthetic import RoomScene, circle_trajectory, tracker_case  # noqa: E402
+from tandem_b200 import CudaCoarseTracker, DrFusion, DrFusionOptions, ImagePyramid, track_pyramid  # noqa: E402
+from tandem_b200.synthetic import RoomScene, circle_trajectory, look_at_pose, tracker_case  # noqa: E402
 
 _fp = ctypes.POINTER(ctypes.c_float)
-n_frames = int(sys.argv[1]) if len(sys.argv) > 1 else 40
+args = [a for a in sys.argv[1:] if not a.startswith("--")]
+n_frames = int(args[0]) if args else 40
+
+
+def gpu_name_and_power_limit():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
+
+
+def coarse_to_fine_leg(n=200, warmup=20, levels=4, H=480, W=640):
+    """Per-frame coarse-to-fine track at 640x480 over 4 levels, set up as tandem_b200/loop.py does (device pyramid of the new
+    frame, dense reference per level): (a) tdm_tracker_track level by level from the host, (b) one tdm_tracker_track_pyramid.
+    The two alternate frame by frame in the same run; the frames cycle through small camera motions around the reference."""
+    fx = 320.0
+    K = (fx, fx, 319.5, 239.5)
+    scene = RoomScene()
+    ref_pose = look_at_pose((0.3, 0.0, -0.2), (2.5, 0.2, 0.5))
+    bgr_r, depth_r = scene.render(ref_pose, H, W, *K)
+    gw = np.array([0.114, 0.587, 0.299], np.float32)
+    pyr_ref = ImagePyramid(W, H, levels)
+    pyr_ref.build(bgr_r.astype(np.float32) @ gw)
+    trk = []
+    for l in range(levels):
+        t = CudaCoarseTracker(W >> l, H >> l)
+        t.init()
+        t.setK(W >> l, H >> l, fx / 2 ** l, fx / 2 ** l, (K[2] + 0.5) / 2 ** l - 0.5, (K[3] + 0.5) / 2 ** l - 0.5)
+        t.setReferenceDense(np.eye(4), 1.0, np.zeros(2), depth=np.ascontiguousarray(depth_r[::2 ** l, ::2 ** l]), dense_only=True,
+                            ref_gray=np.ascontiguousarray(pyr_ref.level(l)[0][..., 0]))
+        trk.append(t)
+    grays = []
+    for k in range(8):
+        a = 2 * np.pi * k / 8
+        pose = look_at_pose((0.3 + 0.03 * np.cos(a), 0.01 * np.sin(a), -0.2 + 0.02 * np.sin(a)), (2.5, 0.2 + 0.02 * np.cos(a), 0.5))
+        grays.append(scene.render(pose, H, W, *K)[0].astype(np.float32) @ gw)
+    pyr = ImagePyramid(W, H, levels)
+    its = (10, 20, 50, 50)
+    modes = dict(affine_opt_mode_a=1e12, affine_opt_mode_b=1e8)
+
+    def chain():
+        T, aff, dev = np.eye(4), np.zeros(2), 0.0
+        for l in range(levels - 1, -1, -1):
+            r = trk[l].track(T, aff, 1.0, max_iterations=its[l])
+            T, aff, dev = r["refToNew"], r["aff"], dev + r["device_ms"]
+        return dev
+
+    def pyramid():
+        return track_pyramid(trk, np.eye(4), np.zeros(2), 1.0, max_iterations=its, **modes)["device_ms"]
+
+    wall = {"chain": [], "pyramid": []}
+    dev = {"chain": [], "pyramid": []}
+    evals = []
+    for f in range(warmup + n):
+        pyr.build(grays[f % len(grays)])
+        for l in range(levels):
+            trk[l].setNewFromPyramid(pyr, l)
+        for name, fn in (("chain", chain), ("pyramid", pyramid)) if f % 2 == 0 else (("pyramid", pyramid), ("chain", chain)):
+            t0 = time.perf_counter()
+            d = fn()
+            if f >= warmup:
+                wall[name].append((time.perf_counter() - t0) * 1e3)
+                dev[name].append(d)
+        if f >= warmup:
+            evals.append(int(track_pyramid(trk, np.eye(4), np.zeros(2), 1.0, max_iterations=its, **modes)["evaluations"].sum()))
+    med = {k: float(np.median(v)) for k, v in wall.items()}
+    print(json.dumps({"what": "coarse-to-fine track of one frame, 640x480, 4 levels (median over frames)", "frames": n, "warmup": warmup,
+                      "gpu(name, power limit)": gpu_name_and_power_limit(),
+                      "chain_wall_ms(track per level from the host)": med["chain"],
+                      "pyramid_wall_ms(one track_pyramid)": med["pyramid"],
+                      "chain_device_ms(sum of per-level event times)": float(np.median(dev["chain"])),
+                      "pyramid_device_ms": float(np.median(dev["pyramid"])),
+                      "host_waits_per_frame": {"chain": levels, "pyramid": 1},
+                      "evaluations_per_frame(median)": float(np.median(evals)),
+                      "wall_speedup": med["chain"] / med["pyramid"]}))
+
+
+if "--pyramid-only" in sys.argv:
+    coarse_to_fine_leg()
+    sys.exit(0)
 H, W = 480, 640
 intr = dict(fx=320.0, fy=320.0, cx=319.5, cy=239.5)
 scene = RoomScene()
@@ -159,3 +238,5 @@ if os.path.exists(trk_lib):
                           "pair_us(device)": (mr.value + mg.value) * 1e3, "ours_fused_kernel_us(device)": ms / 200 * 1e3,
                           "ours_speedup": (mr.value + mg.value) * 1e3 / (ms / 200 * 1e3),
                           "note": "device time of the kernels + the per-call output memsets only; the reference's host wrapper adds a blocking sync and D2H per call (cuda_coarse_tracker.cpp:195-356)"}))
+
+coarse_to_fine_leg()
