@@ -86,6 +86,25 @@ public:
                                          float lambdaExtrapolationLimit, float affineOptModeA, float affineOptModeB,
                                          Eigen::Matrix<double, 5, 1> const &minResForAbort);
 
+  // Extension: FullSystem::trackNewCoarse's loop over the motion hypotheses (FullSystem.cpp:538-617, monocular path) in one
+  // call: every try is a trackPyramid run from tries[i] and aff_last_2_l with minResForAbort = achievedRes, the winner, takeover
+  // and break rules run on the device after each try, and the host waits once.  1..64 tries; reTrackThreshold =
+  // setting_reTrackThreshold.  Throws std::runtime_error on invalid input (an empty try list included).
+  struct NewCoarseResult {
+    Eigen::Matrix<double, 4, 4> lastF_2_fh;
+    Eigen::Vector2d aff_g2l;
+    Eigen::Matrix<double, 3, 1> flowVecs;
+    Eigen::Matrix<double, 5, 1> achievedRes;       // the caller's new lastCoarseRMSE
+    bool haveOneGood;
+    int tryIterations;
+    int winner;                                    // index of the last winning try, -1: none
+  };
+  static NewCoarseResult trackNewCoarse(std::vector<CudaCoarseTracker *> const &levels,
+                                        std::vector<Eigen::Matrix<double, 4, 4>> const &tries, Eigen::Vector2d const &aff_last_2_l,
+                                        float new_exposure, float coarseCutoffTH, const int maxIterations[5],
+                                        float lambdaExtrapolationLimit, float affineOptModeA, float affineOptModeB,
+                                        Eigen::Matrix<double, 5, 1> const &lastCoarseRMSE, float reTrackThreshold);
+
   void synchronize();
 
   void startTiming();

@@ -335,6 +335,38 @@ int tdm_tracker_track_pyramid(tdm_tracker* const* levels, int coarsest_level, co
                               float lambda_extrapolation_limit, float affine_opt_mode_a, float affine_opt_mode_b,
                               const double min_res_for_abort[5], tdm_track_pyramid_result* out);
 
+/* n6  FullSystem::trackNewCoarse (tandem/src/FullSystem/FullSystem.cpp:538-617), monocular path: the loop over the motion
+ *     hypotheses the caller built (lastF_2_fh_tries, :420-536), every try an n5 run, all on the device with one host wait.
+ *     Try i starts from tries[i] (n_tries x 16, row-major) and aff_last_2_l with min_res_for_abort = achievedRes as it stands
+ *     (all NaN for the first try).  After each try, statement for statement: a winner (ok, lastResiduals[0] finite as a float
+ *     and not >= achievedRes[0]) gives the pose, aff and lastFlowIndicators; once one has won, every level of achievedRes takes
+ *     over the try's lastResiduals where it is not finite (as a float) or larger; the loop stops when
+ *     achievedRes[0] < last_coarse_rmse[0] * retrack_threshold (setting_reTrackThreshold).  Without a winner the pose is
+ *     tries[0], the aff aff_last_2_l and the flow (0, 0, 0).  The other arguments and the level requirements are those of
+ *     tdm_tracker_track_pyramid.  Blocking.  Invalid input (everything tdm_tracker_track_pyramid rejects, n_tries outside 1..64,
+ *     null arrays) is an error and launches nothing.  tries_out, when not NULL, receives `tries` records. */
+typedef struct tdm_track_try {
+  double last_residuals[5];     /* lastResiduals after the try, NaN for levels it did not reach */
+  int ok;                       /* trackNewestCoarse's return value */
+  int aborted_level, repeated_level;   /* as in tdm_track_pyramid_result, -1: none */
+  int evaluations[5];
+} tdm_track_try;
+typedef struct tdm_track_new_coarse_result {
+  double ref_to_new[16];        /* lastF_2_fh (row-major) */
+  double aff_g2l[2];            /* aff_g2l */
+  double achieved_res[5];       /* achievedRes: the caller's new lastCoarseRMSE (:617) */
+  double flow_vecs[3];          /* flowVecs */
+  int have_one_good;
+  int tries;                    /* tryIterations: tries run */
+  int winner;                   /* index of the last winning try, -1: none (not in the reference) */
+  float device_ms;
+} tdm_track_new_coarse_result;
+int tdm_tracker_track_new_coarse(tdm_tracker* const* levels, int coarsest_level, const double* tries, int n_tries,
+                                 const double aff_last_2_l[2], float new_exposure, float coarse_cutoff_th, const int max_iterations[5],
+                                 float lambda_extrapolation_limit, float affine_opt_mode_a, float affine_opt_mode_b,
+                                 const double last_coarse_rmse[5], float retrack_threshold, tdm_track_new_coarse_result* out,
+                                 tdm_track_try* tries_out);
+
 #ifdef __cplusplus
 }
 #endif

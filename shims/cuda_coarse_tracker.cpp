@@ -168,6 +168,34 @@ CudaCoarseTracker::PyramidTrackResult CudaCoarseTracker::trackPyramid(
   return out;
 }
 
+CudaCoarseTracker::NewCoarseResult CudaCoarseTracker::trackNewCoarse(
+    std::vector<CudaCoarseTracker*> const& levels, std::vector<Eigen::Matrix<double, 4, 4>> const& tries,
+    Eigen::Vector2d const& aff_last_2_l, float new_exposure, float coarseCutoffTH, const int maxIterations[5],
+    float lambdaExtrapolationLimit, float affineOptModeA, float affineOptModeB, Eigen::Matrix<double, 5, 1> const& lastCoarseRMSE,
+    float reTrackThreshold) {
+  std::vector<tdm_tracker*> h;
+  for (CudaCoarseTracker* t : levels) h.push_back(t ? t->handle_ : nullptr);
+  std::vector<double> T(16 * tries.size() + 1);
+  for (size_t k = 0; k < tries.size(); ++k) to_row_major(tries[k], &T[16 * k]);
+  const double a[2] = {aff_last_2_l(0), aff_last_2_l(1)};
+  double rmse[5];
+  for (int i = 0; i < 5; ++i) rmse[i] = lastCoarseRMSE(i);
+  tdm_track_new_coarse_result r;
+  chk(tdm_tracker_track_new_coarse(h.data(), (int)h.size() - 1, T.data(), (int)tries.size(), a, new_exposure, coarseCutoffTH, maxIterations,
+                                   lambdaExtrapolationLimit, affineOptModeA, affineOptModeB, rmse, reTrackThreshold, &r, nullptr),
+      "CudaCoarseTracker::trackNewCoarse");
+  NewCoarseResult out;
+  for (int rr = 0; rr < 4; ++rr)
+    for (int c = 0; c < 4; ++c) out.lastF_2_fh(rr, c) = r.ref_to_new[4 * rr + c];
+  out.aff_g2l = Eigen::Vector2d(r.aff_g2l[0], r.aff_g2l[1]);
+  for (int i = 0; i < 3; ++i) out.flowVecs(i) = r.flow_vecs[i];
+  for (int i = 0; i < 5; ++i) out.achievedRes(i) = r.achieved_res[i];
+  out.haveOneGood = r.have_one_good != 0;
+  out.tryIterations = r.tries;
+  out.winner = r.winner;
+  return out;
+}
+
 void CudaCoarseTracker::synchronize() { chk(tdm_tracker_synchronize(handle_), "CudaCoarseTracker::synchronize"); }
 
 void CudaCoarseTracker::startTiming() {

@@ -69,6 +69,19 @@ class TrackPyramidResult(ctypes.Structure):
                 ("cutoff_repeat", ctypes.c_float * 5), ("device_ms", ctypes.c_float)]
 
 
+class TrackTry(ctypes.Structure):
+    """tdm_track_try (include/tandem_b200.h)."""
+    _fields_ = [("last_residuals", ctypes.c_double * 5), ("ok", ctypes.c_int), ("aborted_level", ctypes.c_int),
+                ("repeated_level", ctypes.c_int), ("evaluations", ctypes.c_int * 5)]
+
+
+class TrackNewCoarseResult(ctypes.Structure):
+    """tdm_track_new_coarse_result (include/tandem_b200.h)."""
+    _fields_ = [("ref_to_new", ctypes.c_double * 16), ("aff_g2l", ctypes.c_double * 2), ("achieved_res", ctypes.c_double * 5),
+                ("flow_vecs", ctypes.c_double * 3), ("have_one_good", ctypes.c_int), ("tries", ctypes.c_int), ("winner", ctypes.c_int),
+                ("device_ms", ctypes.c_float)]
+
+
 def _declare(l):
     c = ctypes
     P = c.POINTER
@@ -139,6 +152,7 @@ def _declare(l):
         "tdm_tracker_get_reference": (i, [vp, i, fp, fp, fp, fp]),
         "tdm_tracker_track": (i, [vp, dp, dp, f, f, i, f, i, i, P(TrackResult)]),
         "tdm_tracker_track_pyramid": (i, [P(vp), i, dp, dp, f, f, ip, f, f, f, dp, P(TrackPyramidResult)]),
+        "tdm_tracker_track_new_coarse": (i, [P(vp), i, dp, i, dp, f, f, ip, f, f, f, dp, f, P(TrackNewCoarseResult), P(TrackTry)]),
     }
     missing = []
     for name, (res, args) in sigs.items():

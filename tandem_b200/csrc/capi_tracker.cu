@@ -231,4 +231,40 @@ int tdm_tracker_track_pyramid(tdm_tracker* const* levels, int coarsest_level, co
   TDM_API_END
 }
 
+/* ---- SURVEY 8(f) n6: FullSystem::trackNewCoarse's motion-hypothesis loop on the device ---- */
+int tdm_tracker_track_new_coarse(tdm_tracker* const* levels, int coarsest_level, const double* tries, int n_tries,
+                                 const double aff_last_2_l[2], float new_exposure, float coarse_cutoff_th, const int max_iterations[5],
+                                 float lambda_extrapolation_limit, float affine_opt_mode_a, float affine_opt_mode_b,
+                                 const double last_coarse_rmse[5], float retrack_threshold, tdm_track_new_coarse_result* out,
+                                 tdm_track_try* tries_out) {
+  TDM_API_BEGIN
+  TDM_CHECK(levels && tries && aff_last_2_l && max_iterations && last_coarse_rmse && out, "null argument");
+  TDM_CHECK(n_tries >= 1 && n_tries <= 64, "n_tries must be in 1..64");
+  TDM_CHECK(coarsest_level >= 0 && coarsest_level <= 4, "coarsest_level must be in 0..4");
+  tdm::TrackerIface* impl[5] = {};
+  for (int l = 0; l <= coarsest_level; ++l) {
+    TDM_CHECK(levels[l], "track_pyramid level " + std::to_string(l) + ": null tracker");
+    impl[l] = levels[l]->impl;
+  }
+  tdm::TrackerIface::NewCoarseArgs a;
+  a.tries = tries; a.n_tries = n_tries; a.aff_last_2_l = aff_last_2_l; a.new_exposure = new_exposure;
+  a.coarse_cutoff = coarse_cutoff_th; a.max_iterations = max_iterations; a.lambda_extrapolation_limit = lambda_extrapolation_limit;
+  a.affine_mode_a = affine_opt_mode_a; a.affine_mode_b = affine_opt_mode_b; a.last_coarse_rmse = last_coarse_rmse;
+  a.retrack_threshold = retrack_threshold;
+  tdm::TrackerIface::NewCoarseResult r;
+  tdm::TrackerIface::TryResult rec[64];
+  impl[0]->track_new_coarse(impl, coarsest_level, a, &r, tries_out ? rec : nullptr);
+  for (int i = 0; i < 16; ++i) out->ref_to_new[i] = r.refToNew[i];
+  out->aff_g2l[0] = r.aff[0]; out->aff_g2l[1] = r.aff[1];
+  for (int l = 0; l < 5; ++l) out->achieved_res[l] = r.achieved_res[l];
+  for (int i = 0; i < 3; ++i) out->flow_vecs[i] = r.flow_vecs[i];
+  out->have_one_good = r.have_one_good; out->tries = r.tries; out->winner = r.winner; out->device_ms = r.device_ms;
+  for (int k = 0; tries_out && k < r.tries; ++k) {
+    for (int l = 0; l < 5; ++l) { tries_out[k].last_residuals[l] = rec[k].last_residuals[l]; tries_out[k].evaluations[l] = rec[k].evaluations[l]; }
+    tries_out[k].ok = rec[k].ok; tries_out[k].aborted_level = rec[k].aborted_level; tries_out[k].repeated_level = rec[k].repeated_level;
+  }
+  return TDM_OK;
+  TDM_API_END
+}
+
 }  // extern "C"

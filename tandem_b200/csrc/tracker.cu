@@ -77,7 +77,8 @@ struct LmIn {                // uploaded once per call
   double min_res[kMaxLevels];   // minResForAbort (pyramid mode)
   float mode_a, mode_b;         // setting_affineOptModeA/B (pyramid mode; < 0 = fixed)
   int coarsest;
-  int pyramid;               // 0: one level (tdm_tracker_track), 1: the coarse-to-fine rules of trackNewestCoarse
+  int pyramid;               // 0: one level (tdm_tracker_track), 1: the coarse-to-fine rules of trackNewestCoarse,
+                             // 2: those rules once per motion hypothesis of trackNewCoarse (LmCtx::rin)
   int max_evals;             // bound on the evaluations of the whole call (the rules never exceed it)
 };
 struct LmState {
@@ -99,6 +100,30 @@ struct LmResult {            // mapped pinned host memory (device copy in LmCtx:
   int ok, aborted_level, repeated_level;
   int done;                        // written last: 1 = finished, 2 = evaluation bound exceeded (internal error)
 };
+// ---- n6: the motion-hypothesis loop of FullSystem::trackNewCoarse around n5 (pyramid mode 2), see the n6 section below ----
+constexpr int kMaxTries = 64;     // as calc_res_batch; the reference builds at most 31
+struct TryRec {              // one try's outcome (tdm_track_try)
+  double last_res[kMaxLevels];
+  int ok, aborted_level, repeated_level;
+  int evaluations[kMaxLevels];
+};
+struct RetrackOut {          // mapped pinned host memory of tdm_tracker_track_new_coarse, written only in mode 2
+  double T[16], aff[2], achieved[kMaxLevels], flow[3];   // lastF_2_fh, aff_g2l, achievedRes, flowVecs
+  int have_one_good, tries, winner;
+  int done;                  // written after everything else: 1 = finished, 2 = evaluation bound exceeded (internal error)
+  TryRec rec[kMaxTries];
+};
+struct RetrackIn {           // uploaded by tdm_tracker_track_new_coarse only: this header + n_tries poses
+  RetrackOut* out;           // device pointer of the mapped result
+  double last_rmse0;         // lastCoarseRMSE[0]
+  float threshold;           // setting_reTrackThreshold
+  int n_tries;
+  double tries[kMaxTries][16];   // lastF_2_fh_tries, row-major
+};
+struct RetrackState {
+  double achieved[kMaxLevels], T[16], aff[2], flow[3];   // achievedRes; pose, aff and flow of the last winner
+  int have_one_good, cur, winner;                       // cur = the try under way
+};
 struct LmCtx {               // device memory, one per tracker
   LmIn in;
   LmState s;
@@ -108,6 +133,8 @@ struct LmCtx {               // device memory, one per tracker
   LmResult r;
   LmResult* out;             // mapped pinned host memory
   cudaGraphConditionalHandle loop;   // the WHILE node around the evaluation kernel
+  RetrackIn rin;             // n6 only
+  RetrackState rs;
 };
 
 __device__ __noinline__ void lm_step(LmCtx* c, const double* o);
@@ -515,12 +542,10 @@ __device__ void lm_begin_level(LmCtx* c, int lvl) {   // CoarseTracker.cpp:764,7
   lm_pose_from(cfg, s->T, s->aff, cfg.coarse_cutoff, &c->pose);
 }
 
-__global__ void k_lm_init(LmCtx* c, LmResult* out, cudaGraphConditionalHandle loop) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  c->out = out;
-  c->loop = loop;
+// the per-call state of trackNewestCoarse (:746-747), starting from T0 and in.aff0 on the coarsest level
+__device__ void lm_start(LmCtx* c, const double* T0) {
   LmState* s = &c->s;
-  for (int i = 0; i < 16; ++i) s->T[i] = c->in.T0[i];
+  for (int i = 0; i < 16; ++i) s->T[i] = T0[i];
   s->aff[0] = c->in.aff0[0]; s->aff[1] = c->in.aff0[1];
   LmResult* r = &c->r;
   for (int l = 0; l < kMaxLevels; ++l) {
@@ -530,13 +555,30 @@ __global__ void k_lm_init(LmCtx* c, LmResult* out, cudaGraphConditionalHandle lo
   }
   for (int i = 0; i < 3; ++i) r->flow[i] = 1000;                    // lastFlowIndicators.setConstant(1000)  (:747)
   r->num_warped = 0; r->ok = 0; r->aborted_level = -1; r->repeated_level = -1; r->done = 0;
-  c->have_repeated = 0; c->total_evals = 0;
+  c->have_repeated = 0;
   lm_begin_level(c, c->in.coarsest);
 }
+
+__global__ void k_lm_init(LmCtx* c, LmResult* out, cudaGraphConditionalHandle loop) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  c->out = out;
+  c->loop = loop;
+  c->total_evals = 0;
+  if (c->in.pyramid == 2) {                           // FullSystem.cpp:549-551: achievedRes = NaN, no winner yet
+    RetrackState* q = &c->rs;
+    for (int l = 0; l < kMaxLevels; ++l) q->achieved[l] = __longlong_as_double(0x7ff8000000000000ll);
+    q->have_one_good = 0; q->cur = 0; q->winner = -1;
+  }
+  lm_start(c, c->in.T0);
+}
+
+__device__ void rt_publish(LmCtx* ctx, int done);
+__device__ void rt_end_try(LmCtx* ctx, int ok);
 
 // Publishes the result and ends the WHILE loop.  `pose_out` = the loop reached the end (lastToNew_out / aff_g2l_out are
 // written, :919-920); otherwise the input pose is returned.
 __device__ void lm_finish(LmCtx* ctx, int ok, bool pose_out, int done) {
+  if (ctx->in.pyramid == 2) { rt_publish(ctx, done); return; }   // n6 reaches this only past the evaluation bound
   LmResult* r = &ctx->r;
   const LmState* s = &ctx->s;
   for (int i = 0; i < 16; ++i) r->T[i] = pose_out ? s->T[i] : ctx->in.T0[i];
@@ -572,7 +614,56 @@ __device__ void lm_finish_pyramid(LmCtx* ctx) {
     if (ma < 0) s->aff[0] = 0;
     if (mb < 0) s->aff[1] = 0;
   }
+  if (ctx->in.pyramid == 2) { rt_end_try(ctx, ok ? 1 : 0); return; }
   lm_finish(ctx, ok ? 1 : 0, true, 1);
+}
+
+// ================================================================================================
+// n6: FullSystem::trackNewCoarse's loop over the motion hypotheses (FullSystem.cpp:538-617, rgbd_flag == false) on the same
+// graph.  In mode 2 the points where n5 ends the call end a try instead: the try's outcome is recorded, the winner test, the
+// achievedRes takeover and the break test run statement for statement, and either the next try starts on the coarsest level
+// (without a launch: the WHILE loop simply goes on) or the result is published and the loop ends.
+// ================================================================================================
+__device__ void rt_publish(LmCtx* ctx, int done) {
+  const RetrackState* q = &ctx->rs;
+  RetrackOut* o = ctx->rin.out;
+  const bool good = q->have_one_good != 0;            // :610-615: no winner -> tries[0], aff_last_2_l, flow 0
+  for (int i = 0; i < 16; ++i) o->T[i] = good ? q->T[i] : ctx->rin.tries[0][i];
+  for (int i = 0; i < 2; ++i) o->aff[i] = good ? q->aff[i] : ctx->in.aff0[i];
+  for (int i = 0; i < 3; ++i) o->flow[i] = good ? q->flow[i] : 0.0;
+  for (int l = 0; l < kMaxLevels; ++l) o->achieved[l] = q->achieved[l];
+  o->have_one_good = q->have_one_good; o->tries = q->cur; o->winner = q->winner;
+  __threadfence_system();
+  o->done = done;                                     // written last: the host checks it after its one wait
+  __threadfence_system();
+  cudaGraphSetConditional(ctx->loop, 0);
+}
+
+__device__ void rt_end_try(LmCtx* ctx, int ok) {
+  RetrackState* q = &ctx->rs;
+  const LmResult* r = &ctx->r;
+  const double* lr = r->last_res;
+  const int i = q->cur;
+  TryRec* rec = &ctx->rin.out->rec[i];
+  for (int l = 0; l < kMaxLevels; ++l) { rec->last_res[l] = lr[l]; rec->evaluations[l] = r->evaluations[l]; }
+  rec->ok = ok; rec->aborted_level = r->aborted_level; rec->repeated_level = r->repeated_level;
+  if (ok && isfinite((float)lr[0]) && !(lr[0] >= q->achieved[0])) {   // :586-592 a new winner (ok: the pose was written)
+    for (int k = 0; k < 16; ++k) q->T[k] = ctx->s.T[k];
+    q->aff[0] = ctx->s.aff[0]; q->aff[1] = ctx->s.aff[1];
+    for (int k = 0; k < 3; ++k) q->flow[k] = r->flow[k];
+    q->have_one_good = 1;
+    q->winner = i;
+  }
+  if (q->have_one_good)                               // :595-602 take over achievedRes (always; NaN where never reached)
+    for (int l = 0; l < kMaxLevels; ++l)
+      if (!isfinite((float)q->achieved[l]) || q->achieved[l] > lr[l]) q->achieved[l] = lr[l];
+  q->cur = i + 1;
+  if ((q->have_one_good && q->achieved[0] < ctx->rin.last_rmse0 * (double)ctx->rin.threshold) || q->cur == ctx->rin.n_tries) {
+    rt_publish(ctx, 1);                               // :605 break, or the last try
+    return;
+  }
+  for (int l = 0; l < kMaxLevels; ++l) ctx->in.min_res[l] = q->achieved[l];   // :553-559 the next try
+  lm_start(ctx, ctx->rin.tries[q->cur]);
 }
 
 __device__ __noinline__ void lm_step(LmCtx* ctx, const double* o /*kOut sums of the evaluation just finished*/) {
@@ -625,6 +716,7 @@ __device__ __noinline__ void lm_step(LmCtx* ctx, const double* o /*kOut sums of 
   for (int i = 0; i < 3; ++i) r->flow[i] = s->res_old[2 + i];
   if (last_res > 1.5 * ctx->in.min_res[lvl]) {      // NaN never aborts
     r->aborted_level = lvl;
+    if (ctx->in.pyramid == 2) { rt_end_try(ctx, 0); return; }
     lm_finish(ctx, 0, false, 1);
     return;
   }
@@ -681,6 +773,8 @@ class TrackerImpl final : public TrackerIface {
     if (h_total_) cudaFreeHost(h_total_);
     if (h_lm_in_) cudaFreeHost(h_lm_in_);
     if (h_lm_res_) cudaFreeHost(h_lm_res_);
+    if (h_rt_in_) cudaFreeHost(h_rt_in_);
+    if (h_rt_out_) cudaFreeHost(h_rt_out_);
     cudaStreamDestroy(stream_);
   }
 
@@ -878,32 +972,9 @@ class TrackerImpl final : public TrackerIface {
   // ---------------------------------------------------------------------------------------------- n5
   void track_pyramid(TrackerIface* const* levels, int coarsest, const PyramidArgs& a, PyramidResult* r) override {
     TDM_CHECK(levels && a.refToNew && a.aff && a.max_iterations && a.min_res_for_abort && r, "null argument");
-    TDM_CHECK(coarsest >= 0 && coarsest < kMaxLevels, "coarsest_level must be in 0..4");
-    TrackerImpl* lv[kMaxLevels] = {};
-    for (int l = 0; l <= coarsest; ++l) {
-      const std::string at = "track_pyramid level " + std::to_string(l) + ": ";
-      TDM_CHECK(levels[l], at + "null tracker");
-      lv[l] = dynamic_cast<TrackerImpl*>(levels[l]);
-      TDM_CHECK(lv[l], at + "not a tracker of this library");
-      TDM_CHECK(lv[l]->w_ == (w_ >> l) && lv[l]->h_ == (h_ >> l), at + "size must be level 0's size >> level");
-      TDM_CHECK(lv[l]->device_ == device_, at + "trackers live on different devices");
-      TDM_CHECK(lv[l]->have_k_, at + "setK missing");
-      TDM_CHECK(lv[l]->have_ref_, at + "no reference set");
-      TDM_CHECK(lv[l]->have_new_, at + "no new image set");
-      TDM_CHECK(a.max_iterations[l] >= 0 && a.max_iterations[l] <= kMaxIterations, at + "max_iterations out of range");
-    }
-    TDM_CUDA(cudaSetDevice(device_));
-    LmIn& in = lm_in();
-    in.max_evals = 0;
-    for (int l = 0; l <= coarsest; ++l) {
-      lv[l]->fill_level(&in.lv[l], a.new_exposure, a.coarse_cutoff, a.max_iterations[l], a.lambda_extrapolation_limit,
-                        a.affine_mode_a < 0, a.affine_mode_b < 0);
-      in.max_evals += 2 * (1 + 6 + a.max_iterations[l]);   // a level may run twice (the repeat rule)
-      in.min_res[l] = a.min_res_for_abort[l];
-      if (l > 0) lv[l]->order_before(stream_);           // reference upload, setNewFromPyramid copy of that tracker
-    }
-    in.mode_a = a.affine_mode_a; in.mode_b = a.affine_mode_b;
-    in.coarsest = coarsest;
+    LmIn& in = pyramid_in(levels, coarsest, a.new_exposure, a.coarse_cutoff, a.max_iterations, a.lambda_extrapolation_limit,
+                          a.affine_mode_a, a.affine_mode_b);
+    for (int l = 0; l <= coarsest; ++l) in.min_res[l] = a.min_res_for_abort[l];
     in.pyramid = 1;
     const LmResult* o = run_lm(a.refToNew, a.aff, &r->device_ms);
     for (int i = 0; i < 16; ++i) r->refToNew[i] = o->T[i];
@@ -914,6 +985,36 @@ class TrackerImpl final : public TrackerIface {
     }
     for (int i = 0; i < 3; ++i) r->last_flow_indicators[i] = o->flow[i];
     r->ok = o->ok; r->aborted_level = o->aborted_level; r->repeated_level = o->repeated_level;
+  }
+  // ---------------------------------------------------------------------------------------------- n6
+  void track_new_coarse(TrackerIface* const* levels, int coarsest, const NewCoarseArgs& a, NewCoarseResult* r, TryResult* tries) override {
+    TDM_CHECK(levels && a.tries && a.aff_last_2_l && a.max_iterations && a.last_coarse_rmse && r, "null argument");
+    TDM_CHECK(a.n_tries >= 1 && a.n_tries <= kMaxTries, "n_tries must be in 1..64");
+    LmIn& in = pyramid_in(levels, coarsest, a.new_exposure, a.coarse_cutoff, a.max_iterations, a.lambda_extrapolation_limit,
+                          a.affine_mode_a, a.affine_mode_b);
+    in.max_evals *= a.n_tries;                       // the n5 bound of every try
+    for (int l = 0; l < kMaxLevels; ++l) in.min_res[l] = std::nan("");   // achievedRes of the first try (FullSystem.cpp:549)
+    in.pyramid = 2;
+    ensure_rt_buffers();
+    RetrackIn& q = *h_rt_in_;                        // free: lm_in() waited for the previous upload
+    q.out = d_rt_out_;
+    q.last_rmse0 = a.last_coarse_rmse[0];
+    q.threshold = a.retrack_threshold;
+    q.n_tries = a.n_tries;
+    std::memcpy(q.tries, a.tries, (size_t)a.n_tries * 16 * sizeof(double));
+    run_lm(a.tries, a.aff_last_2_l, &r->device_ms, &h_rt_out_->done, offsetof(RetrackIn, tries) + (size_t)a.n_tries * 16 * sizeof(double));
+    const volatile RetrackOut* o = h_rt_out_;
+    for (int i = 0; i < 16; ++i) r->refToNew[i] = o->T[i];
+    for (int i = 0; i < 2; ++i) r->aff[i] = o->aff[i];
+    for (int l = 0; l < kMaxLevels; ++l) r->achieved_res[l] = o->achieved[l];
+    for (int i = 0; i < 3; ++i) r->flow_vecs[i] = o->flow[i];
+    r->have_one_good = o->have_one_good; r->tries = o->tries; r->winner = o->winner;
+    if (tries)
+      for (int k = 0; k < o->tries; ++k) {
+        const volatile TryRec& t = o->rec[k];
+        for (int l = 0; l < kMaxLevels; ++l) { tries[k].last_residuals[l] = t.last_res[l]; tries[k].evaluations[l] = t.evaluations[l]; }
+        tries[k].ok = t.ok; tries[k].aborted_level = t.aborted_level; tries[k].repeated_level = t.repeated_level;
+      }
   }
   void synchronize() override {
     TDM_CUDA(cudaSetDevice(device_));
@@ -1000,6 +1101,36 @@ class TrackerImpl final : public TrackerIface {
     TDM_CUDA(cudaEventSynchronize(lm_in_free_));
     return *h_lm_in_;
   }
+  // Checks the levels of an n5 / n6 call and fills LmCtx::in's staging with them (everything but min_res and the mode); an
+  // invalid call throws before anything is touched.
+  LmIn& pyramid_in(TrackerIface* const* levels, int coarsest, float new_exposure, float coarse_cutoff, const int* max_iterations,
+                   float lambda_limit, float mode_a, float mode_b) {
+    TDM_CHECK(coarsest >= 0 && coarsest < kMaxLevels, "coarsest_level must be in 0..4");
+    TrackerImpl* lv[kMaxLevels] = {};
+    for (int l = 0; l <= coarsest; ++l) {
+      const std::string at = "track_pyramid level " + std::to_string(l) + ": ";
+      TDM_CHECK(levels[l], at + "null tracker");
+      lv[l] = dynamic_cast<TrackerImpl*>(levels[l]);
+      TDM_CHECK(lv[l], at + "not a tracker of this library");
+      TDM_CHECK(lv[l]->w_ == (w_ >> l) && lv[l]->h_ == (h_ >> l), at + "size must be level 0's size >> level");
+      TDM_CHECK(lv[l]->device_ == device_, at + "trackers live on different devices");
+      TDM_CHECK(lv[l]->have_k_, at + "setK missing");
+      TDM_CHECK(lv[l]->have_ref_, at + "no reference set");
+      TDM_CHECK(lv[l]->have_new_, at + "no new image set");
+      TDM_CHECK(max_iterations[l] >= 0 && max_iterations[l] <= kMaxIterations, at + "max_iterations out of range");
+    }
+    TDM_CUDA(cudaSetDevice(device_));
+    LmIn& in = lm_in();
+    in.max_evals = 0;
+    for (int l = 0; l <= coarsest; ++l) {
+      lv[l]->fill_level(&in.lv[l], new_exposure, coarse_cutoff, max_iterations[l], lambda_limit, mode_a < 0, mode_b < 0);
+      in.max_evals += 2 * (1 + 6 + max_iterations[l]);   // a level may run twice (the repeat rule)
+      if (l > 0) lv[l]->order_before(stream_);           // reference upload, setNewFromPyramid copy of that tracker
+    }
+    in.mode_a = mode_a; in.mode_b = mode_b;
+    in.coarsest = coarsest;
+    return in;
+  }
   // this tracker's parameters and buffers as one level of the device LM loop
   void fill_level(LmLevel* L, float new_exposure, float coarse_cutoff, int max_iter, float lambda_limit, int fix_a, int fix_b) const {
     L->p = TrkParams{};
@@ -1022,22 +1153,31 @@ class TrackerImpl final : public TrackerIface {
     TDM_CUDA(cudaEventRecord(ready_, stream_));
     TDM_CUDA(cudaStreamWaitEvent(other, ready_, 0));
   }
-  // Runs the graph on h_lm_in_ (filled by the caller) with one host wait; returns the mapped result.
-  const LmResult* run_lm(const double* T0, const double* aff0, float* device_ms) {
+  // Runs the graph on h_lm_in_ (filled by the caller) with one host wait; returns the mapped result.  n6 passes its own mapped
+  // completion flag and the first rt_bytes of h_rt_in_ to upload next to LmIn.
+  const LmResult* run_lm(const double* T0, const double* aff0, float* device_ms, volatile int* done = nullptr, size_t rt_bytes = 0) {
     LmIn& in = *h_lm_in_;
     for (int i = 0; i < 16; ++i) in.T0[i] = T0[i];
     in.aff0[0] = aff0[0]; in.aff0[1] = aff0[1];
-    h_lm_res_->done = 0;
+    if (!done) done = &h_lm_res_->done;
+    *done = 0;
     TDM_CUDA(cudaEventRecord(lm_e0_, stream_));
     TDM_CUDA(cudaMemcpyAsync(&d_lm_ctx_->in, h_lm_in_, sizeof(LmIn), cudaMemcpyHostToDevice, stream_));
+    if (rt_bytes) TDM_CUDA(cudaMemcpyAsync(&d_lm_ctx_->rin, h_rt_in_, rt_bytes, cudaMemcpyHostToDevice, stream_));
     TDM_CUDA(cudaEventRecord(lm_in_free_, stream_));
     TDM_CUDA(cudaGraphLaunch(lm_exec_, stream_));
     TDM_CUDA(cudaEventRecord(lm_e1_, stream_));
     TDM_CUDA(cudaEventSynchronize(lm_e1_));
     TDM_CUDA(cudaEventElapsedTime(device_ms, lm_e0_, lm_e1_));
-    const volatile LmResult* o = h_lm_res_;
-    if (o->done != 1) throw Error("track: the device loop did not finish (internal error)");
+    if (*done != 1) throw Error("track: the device loop did not finish (internal error)");
     return h_lm_res_;
+  }
+  // n6: the try list's pinned staging (guarded like LmCtx::in's, by lm_in_free_) and the mapped result with the per-try records
+  void ensure_rt_buffers() {
+    if (h_rt_in_) return;
+    TDM_CUDA(cudaMallocHost(&h_rt_in_, sizeof(RetrackIn)));
+    TDM_CUDA(cudaHostAlloc(&h_rt_out_, sizeof(RetrackOut), cudaHostAllocMapped));
+    TDM_CUDA(cudaHostGetDevicePointer(&d_rt_out_, h_rt_out_, 0));
   }
   void set_aff(float new_exposure, const double aff[2]) {  // AffLight::fromToVecExposure, cpp:42-52
     float eF = ref_exposure_, eT = new_exposure;
@@ -1178,6 +1318,9 @@ class TrackerImpl final : public TrackerIface {
   cudaGraphExec_t lm_exec_ = nullptr;
   cudaEvent_t lm_in_free_ = nullptr, lm_e0_ = nullptr, lm_e1_ = nullptr;
   cudaEvent_t ready_ = nullptr;   // order_before
+  // n6 buffers
+  RetrackIn* h_rt_in_ = nullptr;
+  RetrackOut *h_rt_out_ = nullptr, *d_rt_out_ = nullptr;
 };
 
 

@@ -80,6 +80,30 @@ class TrackerIface {
     float device_ms;
   };
   virtual void track_pyramid(TrackerIface* const* levels, int coarsest, const PyramidArgs& a, PyramidResult* r) = 0;
+  // n6: FullSystem::trackNewCoarse's loop over the motion hypotheses (one n5 run per try) in one call on levels[0]
+  struct NewCoarseArgs {
+    const double* tries = nullptr;                // n_tries x 16, row-major lastF_2_fh_tries
+    int n_tries = 0;
+    const double* aff_last_2_l = nullptr;         // [2]
+    float new_exposure = 1.f, coarse_cutoff = 20.f;
+    const int* max_iterations = nullptr;          // [5]
+    float lambda_extrapolation_limit = 0.001f;
+    float affine_mode_a = 0.f, affine_mode_b = 0.f;
+    const double* last_coarse_rmse = nullptr;     // [5]
+    float retrack_threshold = 1.5f;
+  };
+  struct TryResult {
+    double last_residuals[5];
+    int ok, aborted_level, repeated_level;
+    int evaluations[5];
+  };
+  struct NewCoarseResult {
+    double refToNew[16], aff[2], achieved_res[5], flow_vecs[3];
+    int have_one_good, tries, winner;
+    float device_ms;
+  };
+  virtual void track_new_coarse(TrackerIface* const* levels, int coarsest, const NewCoarseArgs& a, NewCoarseResult* r,
+                                TryResult* tries /* r->tries entries, may be null */) = 0;
 };
 
 // FrameHessian::makeImages on the device (n2): all pyramid levels of (I, dx, dy) + absSquaredGrad.

@@ -5,7 +5,7 @@ import ctypes
 
 import numpy as np
 
-from ._lib import TrackPyramidResult, TrackResult, check, lib
+from ._lib import TrackNewCoarseResult, TrackPyramidResult, TrackResult, TrackTry, check, lib
 
 _fp = ctypes.POINTER(ctypes.c_float)
 _dp = ctypes.POINTER(ctypes.c_double)
@@ -205,3 +205,34 @@ def track_pyramid(trackers, refToNew, aff_g2l, new_exposure, coarse_cutoff=20.0,
                 last_residuals=np.array(r.last_residuals, np.float64), last_flow_indicators=np.array(r.last_flow_indicators, np.float64),
                 iterations=np.array(r.iterations[:], np.int32), evaluations=np.array(r.evaluations[:], np.int32),
                 cutoff_repeat=np.array(r.cutoff_repeat[:], np.float32), device_ms=r.device_ms)
+
+
+def track_new_coarse(trackers, tries, aff_last_2_l, new_exposure, last_coarse_rmse, retrack_threshold=1.5, coarse_cutoff=20.0,
+                     max_iterations=(10, 20, 50, 50, 50), lambda_extrapolation_limit=0.001, affine_opt_mode_a=0.0,
+                     affine_opt_mode_b=0.0):
+    """FullSystem::trackNewCoarse's loop over the motion hypotheses (FullSystem.cpp:538-617, monocular): every try is a
+    track_pyramid run from tries[i] (n x 4 x 4, 1 <= n <= 64) and aff_last_2_l with min_res_for_abort = achievedRes, the winner /
+    takeover / break rules run after each try, all on the device with one host wait.  trackers as for track_pyramid;
+    retrack_threshold is setting_reTrackThreshold.  Returns dict(refToNew (lastF_2_fh), aff (aff_g2l), flow_vecs,
+    achieved_res (the new lastCoarseRMSE), have_one_good, tries (tryIterations), winner (last winning try, -1: none), device_ms,
+    per_try: a list of dict(ok, aborted_level, repeated_level, last_residuals, evaluations) for the tries run)."""
+    n = len(trackers)
+    hs = (ctypes.c_void_p * max(n, 1))(*[t._h for t in trackers])
+    T = np.ascontiguousarray(tries, np.float64).reshape(-1, 16)
+    aff = np.ascontiguousarray(aff_last_2_l, np.float64)
+    its = np.zeros(5, np.int32)
+    its[:min(len(max_iterations), 5)] = np.asarray(max_iterations, np.int32)[:5]
+    rmse = np.ascontiguousarray(last_coarse_rmse, np.float64)
+    assert aff.size == 2 and rmse.size == 5
+    r = TrackNewCoarseResult()
+    recs = (TrackTry * max(T.shape[0], 1))()
+    check(lib().tdm_tracker_track_new_coarse(hs, n - 1, T.ctypes.data_as(_dp), T.shape[0], aff.ctypes.data_as(_dp), float(new_exposure),
+                                             float(coarse_cutoff), its.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+                                             float(lambda_extrapolation_limit), float(affine_opt_mode_a), float(affine_opt_mode_b),
+                                             rmse.ctypes.data_as(_dp), float(retrack_threshold), ctypes.byref(r), recs))
+    per_try = [dict(ok=bool(t.ok), aborted_level=t.aborted_level, repeated_level=t.repeated_level,
+                    last_residuals=np.array(t.last_residuals, np.float64), evaluations=np.array(t.evaluations[:], np.int32))
+               for t in recs[:r.tries]]
+    return dict(refToNew=np.array(r.ref_to_new, np.float64).reshape(4, 4), aff=np.array(r.aff_g2l, np.float64),
+                flow_vecs=np.array(r.flow_vecs, np.float64), achieved_res=np.array(r.achieved_res, np.float64),
+                have_one_good=bool(r.have_one_good), tries=r.tries, winner=r.winner, device_ms=r.device_ms, per_try=per_try)

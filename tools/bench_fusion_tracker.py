@@ -1,8 +1,9 @@
 """Secondary measurements (SURVEY.md §8d configs 3/4): TSDF integrate + ray-cast at the initDr map size with a stream
 of synthetic 640x480 depth maps, the level-0 tracker evaluation, the coarse-to-fine track of a frame (host-driven chain of
 per-level tdm_tracker_track calls vs one tdm_tracker_track_pyramid), and - when oracle/_ref is present - the REFERENCE's own
-dr_fusion (compiled unmodified for sm_90a) on the same inputs on the same GPU.
-    python tools/bench_fusion_tracker.py [n_frames] [--pyramid-only]
+dr_fusion (compiled unmodified for sm_90a) on the same inputs on the same GPU.  --retrack times the motion-hypothesis loop of
+FullSystem::trackNewCoarse (host loop over tdm_tracker_track_pyramid vs one tdm_tracker_track_new_coarse).
+    python tools/bench_fusion_tracker.py [n_frames] [--pyramid-only | --retrack]
 Prints one JSON line per measurement."""
 import ctypes
 import json
@@ -94,8 +95,96 @@ def coarse_to_fine_leg(n=200, warmup=20, levels=4, H=480, W=640):
                       "wall_speedup": med["chain"] / med["pyramid"]}))
 
 
+def retrack_leg(n=200, warmup=20, levels=4, H=480, W=640):
+    """Per-frame motion-hypothesis loop (FullSystem::trackNewCoarse) at 640x480 over 4 levels with the full 31-try list of
+    FullSystem.cpp:437-530 around a last motion far larger than the true one (oracle/pins_retrack.py): (a) the loop on the host
+    over track_pyramid (one host wait per try), (b) one track_new_coarse call.  Two lastCoarseRMSE settings: 0 (no try is good
+    enough: all 31 run, most abort on the coarsest level) and 2 (the first try that reaches the true pose stops the loop).
+    The two ways alternate frame by frame in the same run."""
+    from oracle import pins_retrack as R
+    from oracle.retrack_driver import track_new_coarse as host_loop
+    from tandem_b200 import track_new_coarse
+    fx = 320.0
+    K = (fx, fx, 319.5, 239.5)
+    scene = RoomScene()
+    ref_pose = look_at_pose((0.3, 0.0, -0.2), (2.5, 0.2, 0.5))
+    bgr_r, depth_r = scene.render(ref_pose, H, W, *K)
+    gw = np.array([0.114, 0.587, 0.299], np.float32)
+    pyr_ref = ImagePyramid(W, H, levels)
+    pyr_ref.build(bgr_r.astype(np.float32) @ gw)
+    trk = []
+    for l in range(levels):
+        t = CudaCoarseTracker(W >> l, H >> l)
+        t.init()
+        t.setK(W >> l, H >> l, fx / 2 ** l, fx / 2 ** l, (K[2] + 0.5) / 2 ** l - 0.5, (K[3] + 0.5) / 2 ** l - 0.5)
+        t.setReferenceDense(np.eye(4), 1.0, np.zeros(2), depth=np.ascontiguousarray(depth_r[::2 ** l, ::2 ** l]), dense_only=True,
+                            ref_gray=np.ascontiguousarray(pyr_ref.level(l)[0][..., 0]))
+        trk.append(t)
+    grays, tries = [], []
+    for k in range(8):
+        a = 2 * np.pi * k / 8
+        pose = look_at_pose((0.3 + 0.03 * np.cos(a), 0.01 * np.sin(a), -0.2 + 0.02 * np.sin(a)), (2.5, 0.2 + 0.02 * np.cos(a), 0.5))
+        grays.append(scene.render(pose, H, W, *K)[0].astype(np.float32) @ gw)
+        tries.append(R.motion_tries(R.FAR, np.linalg.inv(pose.astype(np.float64)) @ ref_pose.astype(np.float64)))
+    pyr = ImagePyramid(W, H, levels)
+    its = (10, 20, 50, 50)
+    modes = dict(affine_opt_mode_a=1e12, affine_opt_mode_b=1e8)
+    aff0 = np.zeros(2)
+    for rmse0 in (0.0, 2.0):
+        rmse = np.full(5, rmse0)
+        waits = [0]
+
+        def host(tr):
+            dev = [0.0]
+
+            def tp(T, aff, min_res):
+                r = track_pyramid(trk, T, aff, 1.0, max_iterations=its, min_res_for_abort=min_res, **modes)
+                dev[0] += r["device_ms"]
+                waits[0] += 1
+                return r
+            r = host_loop(tp, tr, aff0, rmse)
+            return r, dev[0]
+
+        def device(tr):
+            r = track_new_coarse(trk, tr, aff0, 1.0, rmse, max_iterations=its, **modes)
+            return r, r["device_ms"]
+
+        wall = {"host": [], "device": []}
+        dev = {"host": [], "device": []}
+        n_tries, n_evals, n_waits = [], [], []
+        for f in range(warmup + n):
+            pyr.build(grays[f % len(grays)])
+            for l in range(levels):
+                trk[l].setNewFromPyramid(pyr, l)
+            tr = tries[f % len(tries)]
+            for name, fn in (("host", host), ("device", device)) if f % 2 == 0 else (("device", device), ("host", host)):
+                waits[0] = 0
+                t0 = time.perf_counter()
+                r, d = fn(tr)
+                if f >= warmup:
+                    wall[name].append((time.perf_counter() - t0) * 1e3)
+                    dev[name].append(d)
+                    if name == "host":
+                        n_waits.append(waits[0])
+                    else:
+                        n_tries.append(r["tries"])
+                        n_evals.append(sum(int(t["evaluations"].sum()) for t in r["per_try"]))
+        med = {k: float(np.median(v)) for k, v in wall.items()}
+        print(json.dumps({"what": "motion-hypothesis loop of one frame, 640x480, 4 levels, 31 tries (median over frames)",
+                          "last_coarse_rmse": rmse0, "frames": n, "warmup": warmup, "gpu(name, power limit)": gpu_name_and_power_limit(),
+                          "host_loop_wall_ms(track_pyramid per try)": med["host"], "track_new_coarse_wall_ms": med["device"],
+                          "host_loop_device_ms(sum of per-try event times)": float(np.median(dev["host"])),
+                          "track_new_coarse_device_ms": float(np.median(dev["device"])),
+                          "host_waits_per_frame": {"host_loop": float(np.median(n_waits)), "track_new_coarse": 1},
+                          "tries_per_frame(median)": float(np.median(n_tries)), "evaluations_per_frame(median)": float(np.median(n_evals)),
+                          "wall_speedup": med["host"] / med["device"]}))
+
+
 if "--pyramid-only" in sys.argv:
     coarse_to_fine_leg()
+    sys.exit(0)
+if "--retrack" in sys.argv:
+    retrack_leg()
     sys.exit(0)
 H, W = 480, 640
 intr = dict(fx=320.0, fy=320.0, cx=319.5, cy=239.5)

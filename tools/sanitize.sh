@@ -15,5 +15,7 @@ leg() {  # name, timeout, tool, pytest selection...
 leg mem $T1 memcheck tests/test_fusion_gpu.py tests/test_tracker_gpu.py tests/test_front_gpu.py tests/test_mvsnet_gpu.py \
   -k "integrate_and_render or negative_coordinates or mesh_matches_oracle_bit_exact or roundtrip or bucket_overflow or (calc_res and size0) or cutoff or (pyramid and not size0) or (dense_reference_matches and not True) or (lm_loop and size0) or (config1 and mixed16) or interleaved or pixel_partitioned or mesh_state_machine or batched_hypotheses or (tma_staged and small)"
 leg race $T2 racecheck tests/test_fusion_gpu.py tests/test_mvsnet_gpu.py -k "mesh_call_order or negative_coordinates or (tma_staged and small)"
-leg pyramid_mem $T1 memcheck tests/test_track_pyramid_gpu.py -k "not shim and not 480"
-leg pyramid_race $T2 racecheck tests/test_track_pyramid_gpu.py -k "equals_host and 240"
+leg pyramid_mem $T1 memcheck tests/test_track_pyramid_gpu.py -k "not shim and not size1"
+leg pyramid_race $T2 racecheck tests/test_track_pyramid_gpu.py -k "equals_host and size0"
+leg new_coarse_mem $T1 memcheck tests/test_track_new_coarse_gpu.py -k "not shim and not size1"
+leg new_coarse_race $T2 racecheck tests/test_track_new_coarse_gpu.py -k "host_loop and size0 and retrack"
