@@ -148,9 +148,44 @@ template <> __device__ __forceinline__ void wgmma<128, __nv_bfloat16>(float (&d)
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(a), "l"(b), "r"(acc));
 }
+// N = 24 / 48: the input-stationary kernel's three 8- / 16-column kd blocks (conv_tc_is.cuh)
+template <> __device__ __forceinline__ void wgmma<24, __half>(float (&d)[12], uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %14, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n24k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, %12, %13, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
+      : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<24, __nv_bfloat16>(float (&d)[12], uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %14, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n24k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, %12, %13, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
+      : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<48, __half>(float (&d)[24], uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<48, __nv_bfloat16>(float (&d)[24], uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(a), "l"(b), "r"(acc));
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Orders an accumulator fragment against the asynchronous wgmma that writes it: the compiler may not move a read of d
+// above the wait_group that precedes this fence, nor a write below the wgmma issue that follows it.
+template <int NR> __device__ __forceinline__ void fence_frag(float (&d)[NR]) {
+#pragma unroll
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
 // Tiled TMA load of one box of a 4-D tensor map (SASS: UTMALDG); out-of-bounds elements are zero-filled.
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* tmap, int x0, int x1, int x2, int x3, uint64_t* bar) {
@@ -213,6 +248,27 @@ struct NoTail {
 // MODE 0: 3x3 stencil per plane (9 taps).  MODE 1: transposed conv k3 s2 p1 op1 as a GEMM over the INPUT grid: 2x2 taps
 // per plane at offsets {0,1}^2 (stencil positions (1..2,1..2)), 2 planes, N = 8 output parity classes x COUT.
 template <int CIN, int MODE = 0> constexpr int blocks_per_kd() { return MODE == 1 ? 4 * (CIN / 16) : (CIN >= 16 ? 9 * (CIN / 16) : 5); }  // MODE 3 == MODE 0 geometry
+
+// A offset / LBO (16-byte units) of K=16 step b of the 3x3 stencil (MODE 0 / 3) inside a ring slot of pitch P
+template <int CIN> __device__ __forceinline__ uint32_t stencil_aoff(int b, int P, uint32_t cgb16) {
+  if constexpr (CIN >= 16) {
+    const int t = b / (CIN / 16), j = b % (CIN / 16);
+    return (uint32_t)(2 * j) * cgb16 + (uint32_t)((t / 3) * P + (t % 3));
+  } else {
+    // taps are paired (0,1)(2,3)(4,5)(6,7)(7*,8): the 5th step re-reads tap 7 against zero weights so that no K slice
+    // ever touches shared memory outside the copied tile
+    const int t0 = b < 4 ? 2 * b : 7;
+    return (uint32_t)((t0 / 3) * P + (t0 % 3));
+  }
+}
+template <int CIN> __device__ __forceinline__ uint32_t stencil_alo(int b, int P, uint32_t cgb16) {
+  if constexpr (CIN >= 16) {
+    return cgb16;
+  } else {
+    const int t0 = b < 4 ? 2 * b : 7, t1 = b < 4 ? 2 * b + 1 : 8;
+    return (uint32_t)(((t1 / 3) - (t0 / 3)) * P + (t1 % 3) - (t0 % 3));
+  }
+}
 
 // OUT_PLAIN: fp32 [D][H][W] (prob conv).
 // HILO: the B image carries every weight twice, as W_hi = round16(W) in columns [0,NPAD) and W_lo = round16(W - W_hi)
@@ -299,23 +355,13 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
     if constexpr (MODE == 1) {
       const int t = b / (CIN / 16), j = b % (CIN / 16);
       return (uint32_t)(2 * j) * cgb16 + (uint32_t)((1 + t / 2) * P + (1 + t % 2));
-    } else if constexpr (CIN >= 16) {
-      const int t = b / (CIN / 16), j = b % (CIN / 16);
-      return (uint32_t)(2 * j) * cgb16 + (uint32_t)((t / 3) * P + (t % 3));
     } else {
-      // taps are paired (0,1)(2,3)(4,5)(6,7)(7*,8): the 5th step re-reads tap 7 against zero weights so that no K slice
-      // ever touches shared memory outside the copied tile
-      const int t0 = b < 4 ? 2 * b : 7;
-      return (uint32_t)((t0 / 3) * P + (t0 % 3));
+      return stencil_aoff<CIN>(b, P, cgb16);
     }
   };
   auto alo = [&](int b) -> uint32_t {
-    if constexpr (MODE == 1 || CIN >= 16) {
-      return cgb16;
-    } else {
-      const int t0 = b < 4 ? 2 * b : 7, t1 = b < 4 ? 2 * b + 1 : 8;
-      return (uint32_t)(((t1 / 3) - (t0 / 3)) * P + (t1 % 3) - (t0 % 3));
-    }
+    if constexpr (MODE == 1) return cgb16;
+    else return stencil_alo<CIN>(b, P, cgb16);
   };
   const uint32_t sB16 = smem_u32(sB) >> 4, sA16 = smem_u32(sA) >> 4;
   const uint32_t b_lbo16 = (uint32_t)(NMMA * 16 >> 4);

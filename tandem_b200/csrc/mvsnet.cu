@@ -25,6 +25,7 @@
 #include "mvsnet.h"
 #include "mvsnet_kernels.cuh"
 #include "conv_tc.cuh"
+#include "conv_tc_is.cuh"
 #include "conv_tc_s2.cuh"
 #include "cost_volume_tma.cuh"
 #include "weights.h"
@@ -114,6 +115,7 @@ struct DevConv {
   bool tc_s2 = false;      // stride-2 conv on the tensor-map (strided TMA) kernel, conv_tc_s2.cuh
   void* bimg_s2 = nullptr;
   int npad_s2 = 0, nsplit_s2 = 1;
+  void* bimg_is = nullptr;  // input-stationary B image (conv_tc_is.cuh): 3x3x3 layers with 1 or 8 output channels
 };
 
 struct LaunchRec {
@@ -157,7 +159,7 @@ class MvsnetEngine final : public MvsnetIface {
     if (worker_.joinable()) worker_.join();
     cudaSetDevice(device_);
     free_plan();
-    for (auto& kv : convs_) { cudaFree(kv.second.w); cudaFree(kv.second.bias); cudaFree(kv.second.bimg); cudaFree(kv.second.bimg_s2); }
+    for (auto& kv : convs_) { cudaFree(kv.second.w); cudaFree(kv.second.bias); cudaFree(kv.second.bimg); cudaFree(kv.second.bimg_s2); cudaFree(kv.second.bimg_is); }
     if (d_cv_stats_) {
       unsigned st[2] = {0, 0};
       if (std::getenv("TDM_DEBUG_PLAN") && cudaMemcpy(st, d_cv_stats_, sizeof(st), cudaMemcpyDeviceToHost) == cudaSuccess)
@@ -207,6 +209,7 @@ class MvsnetEngine final : public MvsnetIface {
     }
     else if (key == "keep_intermediates") keep_ = value != 0;
     else if (key == "use_tc") use_tc_ = value != 0;
+    else if (key == "use_is") use_is_ = value != 0;
     else if (key == "fork_fpn") fork_fpn_ = value != 0;
     else if (key == "prob_direct") prob_direct_ = value != 0;
     else if (key == "direct_conv00") direct_conv00_ = value != 0;
@@ -445,6 +448,9 @@ class MvsnetEngine final : public MvsnetIface {
         dc.hilo = dc.npad <= 32 && fc.cin <= 32 && !(fc.kd == 3 && fc.cin == 32 && fc.cout == 32);
         dc.tc_ok = true;
         if (vol_in) upload_bimg<TV>(fc, dc); else upload_bimg<TA>(fc, dc);
+        if (fc.kd == 3 && (fc.cout == 1 || fc.cout == 8)) {
+          if (vol_in) upload_bimg_is<TV>(fc, dc); else upload_bimg_is<TA>(fc, dc);
+        }
       }
       const bool deconv_ok = fc.transposed && fc.kd == 3 && fc.kh == 3 && fc.kw == 3 &&
                              ((fc.cin == 16 && fc.cout == 8) || (fc.cin == 32 && fc.cout == 16) || (fc.cin == 64 && fc.cout == 32));
@@ -537,6 +543,17 @@ class MvsnetEngine final : public MvsnetIface {
     else tc::build_b_image<TB, 64>(fc.w.data(), fc.cin, fc.cout, dc.npad, fc.kd, img, +cvt, dc.nsplit);
     TDM_CUDA(cudaMalloc(&dc.bimg, img.size() * sizeof(TB)));
     TDM_CUDA(cudaMemcpy(dc.bimg, img.data(), img.size() * sizeof(TB), cudaMemcpyHostToDevice));
+  }
+  template <typename TB>
+  void upload_bimg_is(const FoldedConv& fc, DevConv& dc) {
+    std::vector<TB> img;
+    auto cvt = [](float v) -> TB { return from_host<TB>(v); };
+    auto back = [](TB v) -> float { return to_host<TB>(v); };
+    if (fc.cin == 8) tc::build_b_image_is<TB, 8>(fc.w.data(), fc.cin, fc.cout, img, +cvt, +back);
+    else if (fc.cin == 16) tc::build_b_image_is<TB, 16>(fc.w.data(), fc.cin, fc.cout, img, +cvt, +back);
+    else tc::build_b_image_is<TB, 32>(fc.w.data(), fc.cin, fc.cout, img, +cvt, +back);
+    TDM_CUDA(cudaMalloc(&dc.bimg_is, img.size() * sizeof(TB)));
+    TDM_CUDA(cudaMemcpy(dc.bimg_is, img.data(), img.size() * sizeof(TB), cudaMemcpyHostToDevice));
   }
   template <typename TB> static TB from_host(float v);
   template <typename TB> static float to_host(TB v) { return (float)v; }
@@ -795,6 +812,53 @@ class MvsnetEngine final : public MvsnetIface {
   struct TcCache { tc::Plan plan; CUtensorMap tmap; };
   std::map<std::string, TcCache> tc_cache_;
 
+  // tensor map over a P8 input: {8 channels, Wp, Hp, channel group * padded planes}, box = one (R+2) x P tile of a plane
+  template <typename TIn, int CIN>
+  CUtensorMap tile_tmap(const std::string& wkey, const DevBuf& in, const tc::Geom& g) {
+    CUtensorMap tmap;
+    const cuuint64_t dims[4] = {8, (cuuint64_t)(in.W + 2), (cuuint64_t)(in.H + 2), (cuuint64_t)g.iDp * (CIN / 8)};
+    const cuuint64_t strides[3] = {16, (cuuint64_t)(in.W + 2) * 16, (cuuint64_t)(in.W + 2) * (in.H + 2) * 16};
+    const cuuint32_t box[4] = {8, (cuuint32_t)g.P, (cuuint32_t)(g.R + 2), 1};
+    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    const CUtensorMapDataType dt = std::is_same<TIn, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    const CUresult r = tc::encode_tiled_fn()(&tmap, dt, 4, in.p, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    TDM_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed for " + wkey + " (" + std::to_string((int)r) + ")");
+    return tmap;
+  }
+
+  // input-stationary 3x3x3 stride-1 conv (conv_tc_is.cuh) of a layer with 8 (CPK 16) or 1 (CPK 8, fp32 plain output) channels
+  template <typename TIn, int CIN, int CPK, bool PLAIN, typename Tail = tc::NoTail>
+  void tc_is_inst(const std::string& wkey, const DevBuf& in, const DevConv& c, const DevBuf& out, bool relu, const Tail& tail = Tail()) {
+    const std::string key = wkey + (Tail::enabled ? "#is#tail" : "#is");
+    auto it = tc_cache_.find(key);
+    if (it == tc_cache_.end()) {
+      TcCache tcx;
+      tcx.plan = tc::make_plan_is(CIN, CPK, in.D, in.H, in.W, (size_t)tc_smem_kb_ * 1024, Tail::enabled);
+      tc::Geom& g = tcx.plan.g;
+      TDM_CHECK(!Tail::enabled || g.tiles_d == 1, "the prob tail needs tiles that span all depth planes");
+      g.iDp = in.D + 2;
+      g.relu = relu ? 1 : 0;
+      g.cout = c.cout;
+      tcx.tmap = tile_tmap<TIn, CIN>(wkey, in, g);
+      if (std::getenv("TDM_DEBUG_PLAN"))
+        fprintf(stderr, "[plan] %-14s IS cin %d N %d in %dx%dx%d -> R %d TW %d DR %d S %d nch %d tiles %d smem %zu\n", wkey.c_str(), CIN,
+                3 * CPK, in.D, in.H, in.W, g.R, g.TW, g.DR, g.S, g.nch, tcx.plan.grid, tcx.plan.smem);
+      it = tc_cache_.emplace(key, tcx).first;
+    }
+    const tc::Plan& pl = it->second.plan;
+    if (profiling_) recs_.back().name = wkey + "[tc-is]";   // the record conv() opened as "[tc]"
+    auto kern = tc::k_conv_tc_is<TIn, TA, CIN, CPK, PLAIN, Tail>;
+    static bool attr_set = false;
+    if (!attr_set) {
+      TDM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      attr_set = true;
+    }
+    launch_pdl(kern, dim3(pl.grid), pl.smem, it->second.tmap, (const TIn*)c.bimg_is, (const float*)c.bias,
+               PLAIN ? (TA*)nullptr : (TA*)out.p, PLAIN ? (float*)out.p : (float*)nullptr, pl.g, tail);
+  }
+
   template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool PLAIN, int MODE = 0, bool HILO = false, typename Tail = tc::NoTail>
   void tc_inst(const std::string& wkey, const DevBuf& in, const DevConv& c, const DevBuf* res, const DevBuf& out, bool relu,
                const Tail& tail = Tail()) {
@@ -816,15 +880,7 @@ class MvsnetEngine final : public MvsnetIface {
         g.out_gs = p8<TOut>(out).gs;
         if (res) g.res_gs = p8<const TOut>(*res).gs;
       }
-      const cuuint64_t dims[4] = {8, (cuuint64_t)(in.W + 2), (cuuint64_t)(in.H + 2), (cuuint64_t)g.iDp * (CIN / 8)};
-      const cuuint64_t strides[3] = {16, (cuuint64_t)(in.W + 2) * 16, (cuuint64_t)(in.W + 2) * (in.H + 2) * 16};
-      const cuuint32_t box[4] = {8, (cuuint32_t)g.P, (cuuint32_t)(g.R + 2), 1};
-      const cuuint32_t estr[4] = {1, 1, 1, 1};
-      const CUtensorMapDataType dt = std::is_same<TIn, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-      const CUresult r = tc::encode_tiled_fn()(&tcx.tmap, dt, 4, in.p, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      TDM_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed for " + wkey + " (" + std::to_string((int)r) + ")");
+      tcx.tmap = tile_tmap<TIn, CIN>(wkey, in, g);
       if (std::getenv("TDM_DEBUG_PLAN"))
         fprintf(stderr, "[plan] %-14s mode %d cin %d N %d kd %d in %dx%dx%d -> R %d TW %d DR %d S %d nch %d tiles %d x nsplit %d smem %zu\n", wkey.c_str(), MODE, CIN,
                 HILO ? 2 * NPAD : NPAD, KD, in.D, in.H, in.W, g.R, g.TW, g.DR, g.S, g.nch, tcx.plan.grid, c.nsplit, tcx.plan.smem);
@@ -925,6 +981,27 @@ class MvsnetEngine final : public MvsnetIface {
     tc_inst<TI, TA, CI, NP, KDV, false, 0, HL>(wkey, bi, c, rp, bo, relu);                       \
     return true;                                                                           \
   }
+      if (use_is_ && c.bimg_is && !rp) {
+        // input-stationary kernel: the stages' conv0 (cost volume in) and prob (fp32 logits out, with fused_regress the
+        // softmax / soft-argmin / confidence tail)
+        if (bo.f32 && bi.kind == 1 && c.cin == 8 && c.cout == 1) {
+          if (tail_req_.stage && fused_regress_) {
+            const TailReq& t = tail_req_;
+#define TDM_TAIL(MAXD) tc_is_inst<TA, 8, 8, true, RegressTail<MAXD>>(wkey, bi, c, bo, false, RegressTail<MAXD>{t.dsrc, t.depth, t.conf, t.hyp, t.half_range})
+            if (t.D <= 8) TDM_TAIL(8); else if (t.D <= 32) TDM_TAIL(32); else if (t.D <= 48) TDM_TAIL(48); else TDM_TAIL(64);
+#undef TDM_TAIL
+            tail_req_.done = true;
+          } else {
+            tc_is_inst<TA, 8, 8, true>(wkey, bi, c, bo, false);
+          }
+          return true;
+        }
+        if (!bo.f32 && bi.kind == 2 && c.cout == 8) {
+          if (c.cin == 32) { tc_is_inst<TV, 32, 16, false>(wkey, bi, c, bo, relu); return true; }
+          if (c.cin == 16) { tc_is_inst<TV, 16, 16, false>(wkey, bi, c, bo, relu); return true; }
+          if (c.cin == 8) { tc_is_inst<TV, 8, 16, false>(wkey, bi, c, bo, relu); return true; }
+        }
+      }
       if (bo.f32) {
         if (!(c.cin == 8 && c.cout == 1 && c.kd == 3 && bi.kind == 1 && c.hilo)) return false;
         if (tail_req_.stage && fused_regress_) {
@@ -1444,6 +1521,9 @@ class MvsnetEngine final : public MvsnetIface {
   // bit-identical to k_regress and three launches fewer, but the consumer threads of a CTA finish their pixels after the last
   // plane with nothing left to overlap, where the stand-alone kernel spreads the same work over 2048 threads per SM. Off.
   bool fused_regress_ = false;
+  // the stages' conv0 and prob on the input-stationary kernel (conv_tc_is.cuh); 0: the output-stationary k_conv_tc.
+  // Measured on an H100 80GB HBM3 at 400 W (DESIGN.md section 5): the six launches 0.81 -> 0.58 ms, bench value +9 %
+  bool use_is_ = true;
   struct TailReq { int stage; int D; DminSrc dsrc; float* depth; float* conf; const HypSpec* hyp; const float* half_range; bool done; };
   TailReq tail_req_{};
   int pdl_min_smem_kb_ = 120;
@@ -1524,8 +1604,11 @@ void debug_homography(const float* K3x3, const float* c2w_ref, const float* c2w_
 // host-only view of the tensor-core tile planner (no GPU involved; used by the CPU test-suite): out12 = {S, R, TW, P, DR, nch,
 // slot_pos, tiles_w, tiles_h, tiles_d, grid, smem_bytes}
 void debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out12) {
-  // mode + 100 = the same mode with tiles that span all D planes (the prob layer with the soft-argmin tail)
-  const tc::Plan p = tc::make_plan(cin, npad, kd, D, H, W, pd, mode % 100, (size_t)smem_kb * 1024, mode >= 100);
+  // mode + 100 = the same mode with tiles that span all D planes (the prob layer with the soft-argmin tail);
+  // mode 200 = the input-stationary planner (make_plan_is) with npad = columns per kd block (kd and pd are implied: 3, 1),
+  // mode 300 = the same with tiles that span all D planes
+  const tc::Plan p = mode >= 200 ? tc::make_plan_is(cin, npad, D, H, W, (size_t)smem_kb * 1024, mode == 300)
+                                 : tc::make_plan(cin, npad, kd, D, H, W, pd, mode % 100, (size_t)smem_kb * 1024, mode >= 100);
   const tc::Geom& g = p.g;
   const long long v[12] = {g.S, g.R, g.TW, g.P, g.DR, g.nch, g.slot_pos, g.tiles_w, g.tiles_h, g.tiles_d, p.grid, (long long)p.smem};
   for (int i = 0; i < 12; ++i) out12[i] = v[i];

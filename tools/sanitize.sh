@@ -19,3 +19,4 @@ leg pyramid_mem $T1 memcheck tests/test_track_pyramid_gpu.py -k "not shim and no
 leg pyramid_race $T2 racecheck tests/test_track_pyramid_gpu.py -k "equals_host and size0"
 leg new_coarse_mem $T1 memcheck tests/test_track_new_coarse_gpu.py -k "not shim and not size1"
 leg new_coarse_race $T2 racecheck tests/test_track_new_coarse_gpu.py -k "host_loop and size0 and retrack"
+leg conv_is_mem $T1 memcheck tests/test_conv_is_gpu.py -k "abl04"
