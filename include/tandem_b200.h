@@ -98,7 +98,10 @@ int tdm_mvsnet_run_resident_multi(tdm_mvsnet* const* hs, int n, int iters_total,
 int tdm_debug_homography(const float* K3x3, const float* c2w_ref, const float* c2w_src, float* rot9, float* trans3);
 /* Host-only introspection (no GPU needed): the tile plan the tensor-core convolution planner picks for a layer - cin, N columns of
  * the MMA (npad, doubled for hi/lo weights), kd (1: 2-D over planes, 3: 3-D, 2: transposed-as-GEMM), the grid D x H x W the
- * tiles live on, pd (D halo), mode (0 stride-1, 1 transposed, 3 up2; +100: tiles span all D planes), shared-memory budget in KB.
+ * tiles live on, pd (D halo), mode (0 stride-1, 1 transposed, 3 up2; +100: tiles span all D planes; 200: input-stationary 3x3x3
+ * planner with npad = columns per kd block, 300: the same with tiles that span all D planes), shared-memory budget in KB.
+ * Mode 400 is the stride-2 planner: kd is 1 or 3, D x H x W is the OUTPUT grid and pd carries the kernel size (3 or 5); its
+ * "slot positions" are the positions of one of the four parity sub-tiles.
  * out12 = {ring slots, tile rows, tile cols, pitch, planes per tile, 128-row chunks per plane, slot positions, tiles_w,
  * tiles_h, tiles_d, grid, shared-memory bytes}. */
 int tdm_debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out12);

@@ -1606,7 +1606,16 @@ void debug_homography(const float* K3x3, const float* c2w_ref, const float* c2w_
 void debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out12) {
   // mode + 100 = the same mode with tiles that span all D planes (the prob layer with the soft-argmin tail);
   // mode 200 = the input-stationary planner (make_plan_is) with npad = columns per kd block (kd and pd are implied: 3, 1),
-  // mode 300 = the same with tiles that span all D planes
+  // mode 300 = the same with tiles that span all D planes,
+  // mode 400 = the stride-2 planner (make_plan_s2): D, H, W are the OUTPUT dims, pd carries the kernel size (3 or 5)
+  if (mode == 400) {
+    TDM_CHECK((kd == 1 || kd == 3) && (pd == 3 || pd == 5), "mode 400: kd must be 1 or 3 and pd the kernel size 3 or 5");
+    const tc::PlanS2 p = tc::make_plan_s2(cin, npad, kd, pd, D, H, W, (size_t)smem_kb * 1024);
+    const tc::GeomS2& g = p.g;
+    const long long v[12] = {g.S, g.R, g.TW, g.P, g.DR, g.nch, g.sub_pos, g.tiles_w, g.tiles_h, g.tiles_d, p.grid, (long long)p.smem};
+    for (int i = 0; i < 12; ++i) out12[i] = v[i];
+    return;
+  }
   const tc::Plan p = mode >= 200 ? tc::make_plan_is(cin, npad, D, H, W, (size_t)smem_kb * 1024, mode == 300)
                                  : tc::make_plan(cin, npad, kd, D, H, W, pd, mode % 100, (size_t)smem_kb * 1024, mode >= 100);
   const tc::Geom& g = p.g;
