@@ -225,13 +225,13 @@ __device__ __forceinline__ void mma_subchunk(float (&acc)[N / 2], const uint32_t
   wgmma_wait_all();
 }
 
-// Two consecutive channels of an 8-channel group: one 4-byte store / load.
+// Two consecutive channels of an 8-channel group: one 4-byte store / load (the load is split into its issue, a plain
+// 4-byte __ldg, and unpack2, so that it can be issued early).
 template <typename T> __device__ __forceinline__ void store2(T* p, float x0, float x1) {
   T v[2] = {from_f<T>(x0), from_f<T>(x1)};
   *reinterpret_cast<uint32_t*>(p) = *reinterpret_cast<const uint32_t*>(v);
 }
-template <typename T> __device__ __forceinline__ void load2(const T* p, float& x0, float& x1) {
-  const uint32_t u = __ldg(reinterpret_cast<const unsigned int*>(p));
+template <typename T> __device__ __forceinline__ void unpack2(uint32_t u, float& x0, float& x1) {
   const T* v = reinterpret_cast<const T*>(&u);
   x0 = to_f<T>(v[0]); x1 = to_f<T>(v[1]);
 }
@@ -367,6 +367,29 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
   const uint32_t b_lbo16 = (uint32_t)(NMMA * 16 >> 4);
   const int nsub = 2 * g.nch;                      // 64-position sub-chunks per plane
   mbar_wait(b_full, 0);
+  // output pixel (h, w) of row half i of sub-chunk sc; false for the pad columns and positions beyond the tensor
+  auto pixel = [&](int sc, int i, int& h, int& w) -> bool {
+    const int l = sc * 64 + wq * 16 + (lane >> 2) + 8 * i;
+    const int hh = l / P, ww = l - hh * P;
+    h = h0 + hh; w = w0 + ww;
+    return hh < g.R && ww < g.TW && h < g.H && w < g.W;
+  };
+  // P8 position and first channel of column block j of pixel (d, h, w); false for blocks beyond COUT
+  auto out_at = [&](int d, int h, int w, int j, long long& pos, int& co) -> bool {
+    const int n = ns * NPAD + 8 * j + 2 * (lane & 3);
+    if constexpr (CLASS_EPI) {
+      // N = 8 (MODE 1) or 4 (MODE 3) parity classes x COUT: class (pd,ph,pw) of input position (d,h,w) is output (2d+pd, 2h+ph, 2w+pw)
+      const int cls = n / g.cout;
+      co = n % g.cout;
+      const int od2 = MODE == 1 ? 2 * d + (cls >> 2) : d, oh2 = 2 * h + ((cls >> 1) & 1), ow2 = 2 * w + (cls & 1);
+      pos = ((((long long)(od2 + g.opd)) * g.oHp + (oh2 + 1)) * g.oWp + (ow2 + 1)) * 8;
+    } else {
+      co = n;
+      if (ns * NPAD + 8 * j >= g.cout) return false;
+      pos = ((((long long)(d + g.pd)) * g.Hp + (h + 1)) * g.Wp + (w + 1)) * 8;
+    }
+    return true;
+  };
   int next_wait = 0;
   for (int od = 0; od < ndo; ++od) {
     while (next_wait <= od + KD - 1) {
@@ -378,14 +401,32 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
     for (int kd = 0; kd < KD; ++kd) slot16[kd] = sA16 + (uint32_t)((od + kd) % g.S) * (slot_bytes >> 4);
     const int d = d0 + od;
     for (int sc = wg; sc < nsub; sc += kConsumerWG) {
+      // the skip operand is fetched before the MMA chain, so that its load latency overlaps the chain (except for N = 128,
+      // whose accumulators leave no room for it)
+      constexpr bool RES_EARLY = !OUT_PLAIN && NPAD <= 64;
+      uint32_t rv[2][RES_EARLY ? NPAD / 8 : 1];
+      if constexpr (RES_EARLY) {
+        if (g.has_res) {
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            int h, w;
+            const bool in = pixel(sc, i, h, w);
+#pragma unroll
+            for (int j = 0; j < NPAD / 8; ++j) {
+              long long pos;
+              int co;
+              rv[i][j] = in && out_at(d, h, w, j, pos, co)
+                             ? __ldg(reinterpret_cast<const unsigned int*>(res + pos + (co >> 3) * g.res_gs + (co & 7))) : 0u;
+            }
+          }
+        }
+      }
       float acc[NMMA / 2];
       mma_subchunk<NMMA, TIn, KD, NBLK>(acc, slot16, (uint32_t)sc * 64u, sB16, b_lbo16, aoff, alo);
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        const int l = sc * 64 + wq * 16 + (lane >> 2) + 8 * i;
-        const int hh = l / P, ww = l - hh * P;
-        const int h = h0 + hh, w = w0 + ww;
-        if (!(hh < g.R && ww < g.TW && h < g.H && w < g.W)) continue;
+        int h, w;
+        if (!pixel(sc, i, h, w)) continue;
         if constexpr (OUT_PLAIN) {
           if ((lane & 3) == 0) {
             float x = acc[2 * i];
@@ -395,25 +436,14 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
         } else {
 #pragma unroll
           for (int j = 0; j < NPAD / 8; ++j) {
-            const int n = ns * NPAD + 8 * j + 2 * (lane & 3);
+            long long pos;
+            int co;
+            if (!out_at(d, h, w, j, pos, co)) continue;
             float x[2];
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               x[e] = acc[4 * j + 2 * i + e];
               if constexpr (HILO) x[e] += acc[4 * (j + NPAD / 8) + 2 * i + e];
-            }
-            long long pos;
-            int co;
-            if constexpr (CLASS_EPI) {
-              // N = 8 (MODE 1) or 4 (MODE 3) parity classes x COUT: class (pd,ph,pw) of input position (d,h,w) is output (2d+pd, 2h+ph, 2w+pw)
-              const int cls = n / g.cout;
-              co = n % g.cout;
-              const int od2 = MODE == 1 ? 2 * d + (cls >> 2) : d, oh2 = 2 * h + ((cls >> 1) & 1), ow2 = 2 * w + (cls & 1);
-              pos = ((((long long)(od2 + g.opd)) * g.oHp + (oh2 + 1)) * g.oWp + (ow2 + 1)) * 8;
-            } else {
-              co = n;
-              if (ns * NPAD + 8 * j >= g.cout) continue;
-              pos = ((((long long)(d + g.pd)) * g.Hp + (h + 1)) * g.Wp + (w + 1)) * 8;
             }
             const long long e0 = pos + (co >> 3) * g.out_gs + (co & 7);
 #pragma unroll
@@ -422,8 +452,11 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
               if (g.relu) x[e] = fmaxf(x[e], 0.f);
             }
             if (g.has_res) {
+              uint32_t r;
+              if constexpr (RES_EARLY) r = rv[i][j];
+              else r = __ldg(reinterpret_cast<const unsigned int*>(res + pos + (co >> 3) * g.res_gs + (co & 7)));
               float r0, r1;
-              load2<TOut>(res + pos + (co >> 3) * g.res_gs + (co & 7), r0, r1);
+              unpack2<TOut>(r, r0, r1);
               x[0] += r0; x[1] += r1;
             }
             store2<TOut>(out + e0, x[0], x[1]);
@@ -439,10 +472,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
     if ((lane & 3) == 0) {
       for (int sc = wg; sc < nsub; sc += kConsumerWG)
         for (int i = 0; i < 2; ++i) {
-          const int l = sc * 64 + wq * 16 + (lane >> 2) + 8 * i;
-          const int hh = l / P, ww = l - hh * P;
-          const int h = h0 + hh, w = w0 + ww;
-          if (hh < g.R && ww < g.TW && h < g.H && w < g.W) tail(plain_out, h * g.W + w, w, h, g.H * g.W);
+          int h, w;
+          if (pixel(sc, i, h, w)) tail(plain_out, h * g.W + w, w, h, g.H * g.W);
         }
     }
   }
