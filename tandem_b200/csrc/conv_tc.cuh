@@ -369,8 +369,12 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
   mbar_wait(b_full, 0);
   // output pixel (h, w) of row half i of sub-chunk sc; false for the pad columns and positions beyond the tensor
   auto pixel = [&](int sc, int i, int& h, int& w) -> bool {
-    const int l = sc * 64 + wq * 16 + (lane >> 2) + 8 * i;
-    const int hh = l / P, ww = l - hh * P;
+    const int l = sc * 64 + wq * 16 + (lane >> 2);
+    int hh = l / P, ww = l - hh * P;   // row half 1 is 8 positions on: one division serves both halves
+    if (i) {
+      ww += 8;
+      while (ww >= P) { ww -= P; ++hh; }
+    }
     h = h0 + hh; w = w0 + ww;
     return hh < g.R && ww < g.TW && h < g.H && w < g.W;
   };
@@ -390,6 +394,22 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
     }
     return true;
   };
+  // this thread's bias values, loaded once per CTA: bv[j][e] is added to column 8j + 2 * (lane % 4) + e of the fragment
+  // (except for N = 128, whose 32 more registers would spill: it loads them in the epilogue)
+  constexpr bool BIAS_REG = NPAD <= 64;
+  float bv[OUT_PLAIN || !BIAS_REG ? 1 : NPAD / 8][2];
+  if constexpr (OUT_PLAIN) {
+    bv[0][0] = bias ? bias[0] : 0.f;
+  } else if constexpr (BIAS_REG) {
+#pragma unroll
+    for (int j = 0; j < NPAD / 8; ++j) {
+      const int n = ns * NPAD + 8 * j + 2 * (lane & 3);
+      const int co = CLASS_EPI ? n % g.cout : n;
+      const bool live = bias && (CLASS_EPI || ns * NPAD + 8 * j < g.cout);
+#pragma unroll
+      for (int e = 0; e < 2; ++e) bv[j][e] = live ? bias[co + e] : 0.f;
+    }
+  }
   int next_wait = 0;
   for (int od = 0; od < ndo; ++od) {
     while (next_wait <= od + KD - 1) {
@@ -431,7 +451,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
           if ((lane & 3) == 0) {
             float x = acc[2 * i];
             if constexpr (HILO) x += acc[4 * (NPAD / 8) + 2 * i];
-            plain_out[((long long)d * g.H + h) * g.W + w] = x + (bias ? bias[0] : 0.f);
+            plain_out[((long long)d * g.H + h) * g.W + w] = x + bv[0][0];
           }
         } else {
 #pragma unroll
@@ -448,7 +468,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
             const long long e0 = pos + (co >> 3) * g.out_gs + (co & 7);
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              x[e] += bias ? bias[co + e] : 0.f;
+              if constexpr (BIAS_REG) x[e] += bv[j][e];
+              else x[e] += bias ? bias[co + e] : 0.f;
               if (g.relu) x[e] = fmaxf(x[e], 0.f);
             }
             if (g.has_res) {

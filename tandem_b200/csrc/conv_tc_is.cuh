@@ -96,6 +96,10 @@ k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/
 #pragma unroll
     for (int q = 0; q < PN; ++q) pa[k][q] = pb[k][q] = 0.f;
   float fr[N / 2];
+  // this thread's bias values, loaded once per CTA (channels 2 * (lane % 4) + e, or the single prob channel)
+  float bv[2];
+#pragma unroll
+  for (int e = 0; e < 2; ++e) bv[e] = bias ? bias[OUT_PLAIN ? 0 : 2 * (lane & 3) + e] : 0.f;
 
   // value q of column block s (0: kd=2, 1: kd=1, 2: kd=0) of fragment f, hi + lo
   auto blk = [&](const float (&f)[N / 2], int s, int q) -> float {
@@ -114,18 +118,22 @@ k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/
     const int d = d0 + rp - 2;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      const int l = (2 * k + wg) * 64 + wq * 16 + (lane >> 2) + 8 * i;
-      const int hh = l / P, ww = l - hh * P;
+      const int l = (2 * k + wg) * 64 + wq * 16 + (lane >> 2);
+      int hh = l / P, ww = l - hh * P;   // row half 1 is 8 positions on: one division serves both halves
+      if (i) {
+        ww += 8;
+        while (ww >= P) { ww -= P; ++hh; }
+      }
       const int h = h0 + hh, w = w0 + ww;
       if (!(hh < g.R && ww < g.TW && h < g.H && w < g.W)) continue;
       if constexpr (OUT_PLAIN) {
-        if ((lane & 3) == 0) plain_out[((long long)d * g.H + h) * g.W + w] = o[i] + (bias ? bias[0] : 0.f);
+        if ((lane & 3) == 0) plain_out[((long long)d * g.H + h) * g.W + w] = o[i] + bv[0];
       } else {
         const int co = 2 * (lane & 3);
         float x[2];
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          x[e] = o[2 * i + e] + (bias ? bias[co + e] : 0.f);
+          x[e] = o[2 * i + e] + bv[e];
           if (g.relu) x[e] = fmaxf(x[e], 0.f);
         }
         const long long pos = ((((long long)(d + 1)) * g.Hp + (h + 1)) * g.Wp + (w + 1)) * 8;

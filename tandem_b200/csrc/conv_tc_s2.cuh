@@ -124,6 +124,15 @@ k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ b
   const uint32_t b_lbo16 = (uint32_t)(NPAD * 16 >> 4);
   const int nsub = 2 * g.nch;
   mbar_wait(b_full, 0);
+  // this thread's bias values, loaded once per CTA: bv[j][e] is added to column 8j + 2 * (lane % 4) + e of the fragment
+  float bv[NPAD / 8][2];
+#pragma unroll
+  for (int j = 0; j < NPAD / 8; ++j) {
+    const int c = ns * NPAD + 8 * j + 2 * (lane & 3);
+    const bool live = bias && ns * NPAD + 8 * j < g.cout;
+#pragma unroll
+    for (int e = 0; e < 2; ++e) bv[j][e] = live ? bias[c + e] : 0.f;
+  }
   int next_wait = 0;
   for (int od = 0; od < ndo; ++od) {
     const int first = KD == 3 ? 2 * od : od;
@@ -140,8 +149,12 @@ k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ b
       mma_subchunk<NPAD, TIn, KD, NBLK>(acc, slot16, (uint32_t)sc * 64u, sB16, b_lbo16, aoff, alo);
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        const int l = sc * 64 + wq * 16 + (lane >> 2) + 8 * i;
-        const int hh = l / g.P, ww = l - hh * g.P;
+        const int l = sc * 64 + wq * 16 + (lane >> 2);
+        int hh = l / g.P, ww = l - hh * g.P;   // row half 1 is 8 positions on: one division serves both halves
+        if (i) {
+          ww += 8;
+          while (ww >= g.P) { ww -= g.P; ++hh; }
+        }
         const int h = h0 + hh, w = w0 + ww;
         if (!(hh < g.R && ww < g.TW && h < g.H && w < g.W)) continue;
         const long long pos = ((((long long)(d + g.opd)) * g.oHp + (h + 1)) * g.oWp + (w + 1)) * 8;
@@ -153,7 +166,7 @@ k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ b
           float x[2];
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            x[e] = acc[4 * j + 2 * i + e] + (bias ? bias[c + e] : 0.f);
+            x[e] = acc[4 * j + 2 * i + e] + bv[j][e];
             if (g.relu) x[e] = fmaxf(x[e], 0.f);
           }
           store2<TOut>(out + pos + (co >> 3) * g.out_gs + (c & 7), x[0], x[1]);
