@@ -18,9 +18,14 @@
 // 64-position sub-chunks alternate between the two consumer warpgroups; each accumulates its sub-chunk in registers
 // (m64nNk16, one instruction per K=16 step) and runs the epilogue (bias / ReLU / skip / store) straight from the
 // accumulator fragment, so one warpgroup's epilogue overlaps the other's MMAs.
+//
+// This file also holds what the stride-2 (conv_tc_s2.cuh) and input-stationary (conv_tc_is.cuh) kernels share with
+// k_conv_tc: the TMA ring and its prologue, the tile decode, the fragment-row -> pixel map, the bias registers, the
+// per-pixel tail loop, the wgmma wrappers, the K-step pairing of taps, the B-image index and the tile search.
 #pragma once
 #include <cuda.h>
 
+#include <climits>
 #include <cmath>
 #include <vector>
 
@@ -30,19 +35,25 @@
 namespace tdm {
 namespace tc {
 
-struct Geom {
-  int D, H, W;            // output == input dims (stride 1, pad 1)
+// A tiling of a D x H x W grid of positions (the output grid; for the transposed / up-2 modes of k_conv_tc the input
+// grid) into tiles of R rows x TW columns x DR planes, and the TMA ring that feeds them.
+struct Tile {
+  int D, H, W;
+  int S;                  // ring slots (input planes in flight)
+  int R, TW, DR;          // tile: rows, cols, planes
+  int P;                  // row pitch of a TMA box in shared memory, TW + halo
+  int nch;                // 128-position chunks per plane = ceil(R*P / 128), each two 64-position wgmma sub-chunks
+  int slot_pos;           // positions per TMA box destination in a slot: a channel group's plane, or one of its 4 parity
+                          // sub-tiles in the stride-2 kernel
+  int tiles_w, tiles_h, tiles_d;
+};
+
+struct Geom : Tile {
   int Hp, Wp;             // H+2, W+2
   int pd;                 // 1: 3-D conv (KD = 3, halo planes exist), 0: 2-D conv over independent planes (KD = 1)
   long long in_gs, out_gs, res_gs;   // channel-group strides in elements
-  int R, TW, DR;          // tile: rows, cols, output planes
-  int P;                  // TW + 2
-  int nch;                // 128-position chunks per plane = ceil(R*P / 128), each two 64-position wgmma sub-chunks
-  int slot_pos;           // positions per (ring slot, channel group)
-  int tiles_w, tiles_h, tiles_d;
   int relu, has_res;
   int cout;               // real output channels (<= NPAD)
-  int S;                  // ring slots
   int oHp, oWp, opd;      // padded dims / D halo of the OUTPUT tensor (differs from the input in deconv mode)
   int iDp;                // padded plane count of the input: tensor-map dim 3 = channel_group * iDp + plane
 };
@@ -91,92 +102,37 @@ __device__ __forceinline__ uint64_t desc(uint32_t start16, uint32_t lbo16) {
 
 // D[64 x N] (+)= A[64 x 16] * B[16 x N], both operands K-major in shared memory, fp32 accumulators in registers.
 // Fragment: d[4j + 2i + e] is row (warp % 4) * 16 + lane / 4 + 8i, column 8j + 2 * (lane % 4) + e.
+// One asm body per N: TY is the PTX type of the 16-bit operands ("f16" / "bf16"), IA / IB / IP the operand numbers of
+// the two descriptors and of the accumulate flag.
 template <int N, typename T> __device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc);
-template <> __device__ __forceinline__ void wgmma<16, __half>(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(a), "l"(b), "r"(acc));
-}
-template <> __device__ __forceinline__ void wgmma<16, __nv_bfloat16>(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(a), "l"(b), "r"(acc));
-}
-template <> __device__ __forceinline__ void wgmma<32, __half>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(a), "l"(b), "r"(acc));
-}
-template <> __device__ __forceinline__ void wgmma<32, __nv_bfloat16>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(a), "l"(b), "r"(acc));
-}
-template <> __device__ __forceinline__ void wgmma<64, __half>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(a), "l"(b), "r"(acc));
-}
-template <> __device__ __forceinline__ void wgmma<64, __nv_bfloat16>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(a), "l"(b), "r"(acc));
-}
-template <> __device__ __forceinline__ void wgmma<128, __half>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(a), "l"(b), "r"(acc));
-}
-template <> __device__ __forceinline__ void wgmma<128, __nv_bfloat16>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(a), "l"(b), "r"(acc));
-}
+#define TDM_WGMMA_ASM(N, TY, REGS, IA, IB, IP, ...)                                                                       \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #IP ", 0;\n\t"                                                    \
+               "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." TY "." TY " {" REGS "}, %" #IA ", %" #IB                 \
+               ", p, 1, 1, 0, 0;\n\t}"                                                                                   \
+               : __VA_ARGS__                                                                                             \
+               : "l"(a), "l"(b), "r"(acc))
+#define TDM_WGMMA(N, REGS, IA, IB, IP, ...)                                                                                  \
+  template <> __device__ __forceinline__ void wgmma<N, __half>(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc) {        \
+    TDM_WGMMA_ASM(N, "f16", REGS, IA, IB, IP, __VA_ARGS__);                                                                  \
+  }                                                                                                                         \
+  template <> __device__ __forceinline__ void wgmma<N, __nv_bfloat16>(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc) { \
+    TDM_WGMMA_ASM(N, "bf16", REGS, IA, IB, IP, __VA_ARGS__);                                                                 \
+  }
+TDM_WGMMA(16, "%0,%1,%2,%3,%4,%5,%6,%7", 8, 9, 10,
+          "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]))
+TDM_WGMMA(32, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15", 16, 17, 18,
+          "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]))
+TDM_WGMMA(64, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31", 32, 33, 34,
+          "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]))
+TDM_WGMMA(128, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63", 64, 65, 66,
+          "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]))
 // N = 24 / 48: the input-stationary kernel's three 8- / 16-column kd blocks (conv_tc_is.cuh)
-template <> __device__ __forceinline__ void wgmma<24, __half>(float (&d)[12], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %14, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n24k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, %12, %13, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
-      : "l"(a), "l"(b), "r"(acc));
-}
-template <> __device__ __forceinline__ void wgmma<24, __nv_bfloat16>(float (&d)[12], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %14, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n24k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, %12, %13, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
-      : "l"(a), "l"(b), "r"(acc));
-}
-template <> __device__ __forceinline__ void wgmma<48, __half>(float (&d)[24], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-      : "l"(a), "l"(b), "r"(acc));
-}
-template <> __device__ __forceinline__ void wgmma<48, __nv_bfloat16>(float (&d)[24], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-      : "l"(a), "l"(b), "r"(acc));
-}
+TDM_WGMMA(24, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11", 12, 13, 14,
+          "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]))
+TDM_WGMMA(48, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23", 24, 25, 26,
+          "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]))
+#undef TDM_WGMMA
+#undef TDM_WGMMA_ASM
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
@@ -197,14 +153,157 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* tmap, 
 }
 
 // Programmatic dependent launch: a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start
-// while its predecessor drains; everything before pdl_wait() (barrier init, the weight image load) overlaps the
-// predecessor's tail, everything that touches activations comes after it.
+// while its predecessor drains (see Ring::start for what runs before pdl_wait()).
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 constexpr int kConsumerWG = 2;                       // consumer warpgroups (warps 0..7)
 constexpr int kThreads = 128 * kConsumerWG + 32;     // + the producer warp
 constexpr int kProducerWarp = 4 * kConsumerWG;
+
+// ---------------------------------------------------------------------------------------------------------------
+// K-step pairing of taps, shared by the kernels' A descriptors and the host B images
+// ---------------------------------------------------------------------------------------------------------------
+// One K=16 MMA step covers two 8-channel K halves.  CIN >= 16: step b reads tap b / (CIN/16) in both halves, channels
+// (b % (CIN/16)) * 16 + 8 * half.  CIN == 8: half h of step b reads tap 2b + h, so taps pair as (0,1)(2,3)...; an odd
+// last tap is paired with its predecessor, whose half carries zero weights, so that no K slice ever reads shared memory
+// outside the copied tile.  ntaps = taps per input plane (9: 3x3 stencil, 4: transposed conv, KS*KS: stride 2).
+__host__ __device__ constexpr int ksteps(int cin, int ntaps) { return cin >= 16 ? ntaps * (cin / 16) : (ntaps + 1) / 2; }
+__host__ __device__ constexpr int kstep_tap(int cin, int ntaps, int b, int half) {
+  return cin >= 16 ? b / (cin / 16) : (2 * b + 1 < ntaps ? 2 * b + half : ntaps - 2 + half);
+}
+__host__ __device__ constexpr int kstep_ch(int cin, int b, int half) { return cin >= 16 ? (b % (cin / 16)) * 16 + 8 * half : 0; }
+// false for the zero-weight half of an odd last pair
+__host__ __device__ constexpr bool kstep_live(int cin, int ntaps, int b, int half) { return cin >= 16 || half == 1 || 2 * b + 1 < ntaps; }
+
+// A offset / LBO (16-byte units) of K=16 step b inside a ring slot; off(t) is tap t's position offset, cgb16 the
+// distance between two channel groups
+template <int CIN, int NTAPS, typename TapOff>
+__device__ __forceinline__ uint32_t kstep_aoff(int b, uint32_t cgb16, TapOff off) {
+  return (uint32_t)(kstep_ch(CIN, b, 0) / 8) * cgb16 + (uint32_t)off(kstep_tap(CIN, NTAPS, b, 0));
+}
+template <int CIN, int NTAPS, typename TapOff>
+__device__ __forceinline__ uint32_t kstep_alo(int b, uint32_t cgb16, TapOff off) {
+  if constexpr (CIN >= 16) return cgb16;
+  else return (uint32_t)(off(kstep_tap(CIN, NTAPS, b, 1)) - off(kstep_tap(CIN, NTAPS, b, 0)));
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The TMA ring
+// ---------------------------------------------------------------------------------------------------------------
+// Shared memory: [B image, 128-byte aligned][S slots of slot_bytes][full[S] at +0, empty[S] at +8, b_full at +16 (8-byte
+// barriers, S <= 8)].  Input plane rp goes to slot rp % S; full[s] counts its TMA bytes, empty[s] the 8 consumer warps'
+// releases of it.
+struct Ring {
+  uint8_t* a;             // slot 0
+  uint32_t slot_bytes;
+  int S;
+  uint64_t* bars;
+  int waited;             // consumer: planes 0 .. waited-1 have landed
+
+  // Carves shared memory and runs the prologue: barrier init, then the weight image fetch, then pdl_wait(), then the
+  // trigger.  The weights do not depend on the previous kernel, so their copy overlaps its tail; from pdl_wait() on,
+  // activations written by the previous kernel are read and outputs are written.  The dependents are triggered only
+  // after the wait: a trigger BEFORE it lets the whole chain of later kernels become resident early (each one's
+  // prologue would trigger the next), and their idle CTAs then hold the shared memory the running kernel's tiles need.
+  __device__ __forceinline__ static Ring start(uint8_t* smem, uint32_t b_bytes, const void* bimg, uint32_t slot_bytes, int S) {
+    Ring r{smem + (b_bytes + 127) / 128 * 128, slot_bytes, S, nullptr, 0};
+    r.bars = reinterpret_cast<uint64_t*>(r.a + (size_t)slot_bytes * S);
+    if (threadIdx.x == 0) {
+      for (int s = 0; s < S; ++s) { mbar_init(r.full(s), 1); mbar_init(r.empty(s), 4 * kConsumerWG); }
+      mbar_init(r.bars + 16, 1);
+      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+      mbar_expect_tx(r.bars + 16, b_bytes);
+      bulk_g2s(smem, bimg, b_bytes, r.bars + 16);
+    }
+    __syncthreads();
+    pdl_wait();
+    if (threadIdx.x == 0) pdl_launch_dependents();
+    return r;
+  }
+  __device__ __forceinline__ uint64_t* full(int s) const { return bars + s; }
+  __device__ __forceinline__ uint64_t* empty(int s) const { return bars + 8 + s; }
+
+  // Producer (one lane): input planes 0 .. nin-1, each into its slot once the consumers released the slot's previous
+  // plane; boxes(dst, rp, bar) issues plane rp's TMA boxes into dst, tx_bytes in all.
+  template <typename Boxes> __device__ __forceinline__ void produce(int nin, uint32_t tx_bytes, Boxes boxes) const {
+    for (int rp = 0; rp < nin; ++rp) {
+      const int slot = rp % S;
+      if (rp >= S) mbar_wait(empty(slot), ((rp / S) - 1) & 1);
+      mbar_expect_tx(full(slot), tx_bytes);
+      boxes(a + (size_t)slot * slot_bytes, rp, full(slot));
+    }
+  }
+
+  // Consumers: the weight image, every input plane up to `plane`, the shared address (16-byte units) of a plane's slot,
+  // and the release of a plane this warp no longer reads (the producer may refill its slot once all 8 warps released it).
+  __device__ __forceinline__ void wait_weights() const { mbar_wait(bars + 16, 0); }
+  __device__ __forceinline__ void wait(int plane) {
+    for (; waited <= plane; ++waited) mbar_wait(full(waited % S), (waited / S) & 1);
+  }
+  __device__ __forceinline__ uint32_t slot16(int plane) const { return (smem_u32(a) >> 4) + (uint32_t)(plane % S) * (slot_bytes >> 4); }
+  __device__ __forceinline__ void release(int plane) const {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(empty(plane % S));
+  }
+};
+
+// First output position (w0, h0, d0) and plane count of this CTA's tile
+struct TileOrigin { int w0, h0, d0, ndo; };
+__device__ __forceinline__ TileOrigin tile_origin(const Tile& t) {
+  int tile = blockIdx.x;
+  const int tw = tile % t.tiles_w; tile /= t.tiles_w;
+  const int th = tile % t.tiles_h; tile /= t.tiles_h;
+  return {tw * t.TW, th * t.R, tile * t.DR, min(t.DR, t.D - tile * t.DR)};
+}
+
+// Pixel (h, w) of fragment row half i, i.e. of tile position l + 8i, where l = sub-chunk * 64 + (warp % 4) * 16 + lane / 4;
+// false for the pad columns and positions beyond the grid
+__device__ __forceinline__ bool frag_pixel(const Tile& t, const TileOrigin& o, int l, int i, int& h, int& w) {
+  int hh = l / t.P, ww = l - hh * t.P;   // row half 1 is 8 positions on: one division serves both halves
+  if (i) {
+    ww += 8;
+    while (ww >= t.P) { ww -= t.P; ++hh; }
+  }
+  h = o.h0 + hh; w = o.w0 + ww;
+  return hh < t.R && ww < t.TW && h < t.H && w < t.W;
+}
+
+// This thread's bias values, loaded once per CTA: bv[j][e] is added to fragment column 8j + 2 * (lane % 4) + e, i.e.
+// output column n0 + 8j + 2 * (lane % 4) + e (for CLASS, parity class x cout + channel); zero beyond cout
+template <bool CLASS, int NB>
+__device__ __forceinline__ void load_bias(float (&bv)[NB][2], const float* bias, int n0, int cout, int lane) {
+#pragma unroll
+  for (int j = 0; j < NB; ++j) {
+    const int n = n0 + 8 * j + 2 * (lane & 3);
+    const int co = CLASS ? n % cout : n;
+    const bool live = bias && (CLASS || n0 + 8 * j < cout);
+#pragma unroll
+    for (int e = 0; e < 2; ++e) bv[j][e] = live ? bias[co + e] : 0.f;
+  }
+}
+
+// Per-pixel tail of the single-channel fp32 (prob) convolution: with tiles that span all D planes the thread that stored a
+// pixel's D logits is the same for every plane, so once the tile's last plane is stored it can finish the pixel
+// (softmax / soft-argmin / confidence, module.py:1116-1133) without another launch.  NoTail = plain convolution.
+struct NoTail {
+  static constexpr bool enabled = false;
+  __device__ __forceinline__ void operator()(const float*, int, int, int, int) const {}
+};
+// Runs the tail over this thread's pixels once the tile is stored.  ndo == D (host-checked): the thread wrote all D
+// logits of its pixels itself (program order makes them visible to it).
+template <typename Tail>
+__device__ __forceinline__ void run_tail(const Tail& tail, float* plain_out, const Tile& t, const TileOrigin& o, int wg, int wq, int lane) {
+  if ((lane & 3) == 0) {
+    for (int sc = wg; sc < 2 * t.nch; sc += kConsumerWG)
+      for (int i = 0; i < 2; ++i) {
+        // each row half decoded on its own: carried over from half 0, its pixel would stay live across the tail call, and
+        // RegressTail<64> already sits at the register cap
+        int h, w;
+        if (frag_pixel(t, o, sc * 64 + wq * 16 + (lane >> 2) + 8 * i, 0, h, w)) tail(plain_out, h * t.W + w, w, h, t.H * t.W);
+      }
+  }
+}
 
 // One 64-position sub-chunk of one output plane: every (kd, K=16 step) is one wgmma.  aoff(b) is the A offset of step b
 // inside an input plane's ring slot, alo(b) its LBO (16-byte units); B block (kd, b) starts at b_base16 + (kd*NBLK+b)*N*2.
@@ -236,44 +335,17 @@ template <typename T> __device__ __forceinline__ void unpack2(uint32_t u, float&
   x0 = to_f<T>(v[0]); x1 = to_f<T>(v[1]);
 }
 
-// Per-pixel tail of the OUT_PLAIN (prob) instantiation: with tiles that span all D planes (make_plan(full_depth)) the thread
-// that stored a pixel's D logits is the same for every plane, so once the tile's last plane is stored it can finish the
-// pixel (softmax / soft-argmin / confidence, module.py:1116-1133) without another launch.  NoTail = plain convolution.
-struct NoTail {
-  static constexpr bool enabled = false;
-  __device__ __forceinline__ void operator()(const float*, int, int, int, int) const {}
-};
-
-// blocks of B per kd plane: one block = one K=16 MMA step = NPAD x 16 elements in canonical order
-// MODE 0: 3x3 stencil per plane (9 taps).  MODE 1: transposed conv k3 s2 p1 op1 as a GEMM over the INPUT grid: 2x2 taps
-// per plane at offsets {0,1}^2 (stencil positions (1..2,1..2)), 2 planes, N = 8 output parity classes x COUT.
-template <int CIN, int MODE = 0> constexpr int blocks_per_kd() { return MODE == 1 ? 4 * (CIN / 16) : (CIN >= 16 ? 9 * (CIN / 16) : 5); }  // MODE 3 == MODE 0 geometry
-
-// A offset / LBO (16-byte units) of K=16 step b of the 3x3 stencil (MODE 0 / 3) inside a ring slot of pitch P
-template <int CIN> __device__ __forceinline__ uint32_t stencil_aoff(int b, int P, uint32_t cgb16) {
-  if constexpr (CIN >= 16) {
-    const int t = b / (CIN / 16), j = b % (CIN / 16);
-    return (uint32_t)(2 * j) * cgb16 + (uint32_t)((t / 3) * P + (t % 3));
-  } else {
-    // taps are paired (0,1)(2,3)(4,5)(6,7)(7*,8): the 5th step re-reads tap 7 against zero weights so that no K slice
-    // ever touches shared memory outside the copied tile
-    const int t0 = b < 4 ? 2 * b : 7;
-    return (uint32_t)((t0 / 3) * P + (t0 % 3));
-  }
-}
-template <int CIN> __device__ __forceinline__ uint32_t stencil_alo(int b, int P, uint32_t cgb16) {
-  if constexpr (CIN >= 16) {
-    return cgb16;
-  } else {
-    const int t0 = b < 4 ? 2 * b : 7, t1 = b < 4 ? 2 * b + 1 : 8;
-    return (uint32_t)(((t1 / 3) - (t0 / 3)) * P + (t1 % 3) - (t0 % 3));
-  }
-}
+// Tap t of the 3x3 stencil (MODE 0 / 3): position offset inside a ring slot of pitch P
+__device__ __forceinline__ int stencil_off(int t, int P) { return (t / 3) * P + (t % 3); }
 
 // OUT_PLAIN: fp32 [D][H][W] (prob conv).
 // HILO: the B image carries every weight twice, as W_hi = round16(W) in columns [0,NPAD) and W_lo = round16(W - W_hi)
 // in columns [NPAD, 2*NPAD); the MMA runs with N = 2*NPAD and the epilogue adds the two halves, which restores ~fp32
 // weight precision at the cost of a wider N.
+// MODE 0: 3x3 stencil per plane (9 taps).  MODE 1: transposed conv k3 s2 p1 op1 as a GEMM over the INPUT grid: 2x2 taps
+// per plane at offsets {0,1}^2 (stencil positions (1..2,1..2)), 2 planes, N = 8 output parity classes x COUT.
+// MODE 3: 2-D "conv3x3 of a nearest-x2 up-sampled map" evaluated on the COARSE grid: 9 taps, N = 4 output parity
+// classes x COUT (the 3x3 fine taps collapse onto 2x2 coarse neighbours; weights pre-summed on the host).
 template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool OUT_PLAIN, int MODE = 0, bool HILO = false, typename Tail = NoTail>
 __global__ void __launch_bounds__(kThreads, 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, groups*planes}, box {8, P, R+2, 1}*/,
@@ -282,51 +354,24 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
           const __grid_constant__ Tail tail) {
   static_assert(!Tail::enabled || OUT_PLAIN, "a per-pixel tail only exists for the single-channel fp32 output");
   constexpr int CG = CIN / 8;
-  constexpr int NBLK = blocks_per_kd<CIN, MODE>();
+  constexpr int NTAPS = MODE == 1 ? 4 : 9;
+  constexpr int NBLK = ksteps(CIN, NTAPS);
   constexpr int NMMA = HILO ? 2 * NPAD : NPAD;   // instruction N
   static_assert(!(HILO && MODE == 1), "hi/lo weights are not wired for the 3-D transposed-conv epilogue");
-  // MODE 3: 2-D "conv3x3 of a nearest-x2 up-sampled map" evaluated on the COARSE grid: 9 taps, N = 4 output parity
-  // classes x COUT (the 3x3 fine taps collapse onto 2x2 coarse neighbours; weights pre-summed on the host).
   constexpr int B_BYTES = KD * NBLK * NMMA * 32;
   constexpr int PLANE0 = MODE == 1 ? 1 : 0;
   constexpr bool CLASS_EPI = MODE == 1 || MODE == 3;   // deconv reads input planes d and d+1 (padded indices d+1, d+2)
 
   extern __shared__ __align__(128) uint8_t smem[];
-  uint8_t* sB = smem;
-  uint8_t* sA = smem + ((B_BYTES + 127) / 128) * 128;
   const uint32_t cg_bytes = (uint32_t)g.slot_pos * 16u;
-  const uint32_t slot_bytes = cg_bytes * CG;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sA + (size_t)slot_bytes * g.S);
-  uint64_t* full = bars;                 // [S]
-  uint64_t* empty = bars + 8;            // [S]
-  uint64_t* b_full = bars + 16;
-
   // N-slicing (blockIdx.y): wide outputs (CIN = 64 layers, whose full B image would not fit shared memory) are split into
   // slices of NPAD columns, each with its own contiguous B image; slice ns produces output columns [ns*NPAD, (ns+1)*NPAD).
   const int ns = blockIdx.y;
-  bimg += (size_t)ns * (B_BYTES / sizeof(TIn));
+  Ring ring = Ring::start(smem, B_BYTES, bimg + (size_t)ns * (B_BYTES / sizeof(TIn)), cg_bytes * CG, g.S);
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // provably warp-uniform (uniform datapath)
   const int lane = threadIdx.x & 31;
-  int tile = blockIdx.x;
-  const int tw = tile % g.tiles_w; tile /= g.tiles_w;
-  const int th = tile % g.tiles_h; tile /= g.tiles_h;
-  const int td = tile;
-  const int w0 = tw * g.TW, h0 = th * g.R, d0 = td * g.DR;
-  const int ndo = min(g.DR, g.D - d0);             // output planes of this tile
-  const int nin = ndo + KD - 1;                    // input planes to stream
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < g.S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4 * kConsumerWG); }
-    mbar_init(b_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    mbar_expect_tx(b_full, B_BYTES);          // weights do not depend on the previous kernel: fetch them before pdl_wait
-    bulk_g2s(sB, bimg, B_BYTES, b_full);
-  }
-  __syncthreads();
-  pdl_wait();   // from here on activations written by the previous kernel are read and our outputs are written
-  // trigger the dependents only now: a trigger BEFORE the wait lets the whole chain of later kernels become resident early (each
-  // one's prologue would trigger the next), and their idle CTAs then hold the shared memory the running kernel's tiles need
-  if (threadIdx.x == 0) pdl_launch_dependents();
+  const TileOrigin o = tile_origin(g);
+  const int nin = o.ndo + KD - 1;                  // input planes to stream
 
   if (warp == kProducerWarp) {
     // ===================== TMA producer =====================
@@ -334,15 +379,11 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
       // one tiled TMA per (plane, channel group): box = (R+2) rows x P positions, rows / columns beyond the tensor are
       // zero-filled by the TMA engine, so partial tiles need no special casing
       const uint32_t box_bytes = (uint32_t)g.P * (uint32_t)(g.R + 2) * 16u;
-      for (int rp = 0; rp < nin; ++rp) {
-        const int slot = rp % g.S;
-        if (rp >= g.S) mbar_wait(&empty[slot], ((rp / g.S) - 1) & 1);
-        mbar_expect_tx(&full[slot], box_bytes * CG);
-        const int pp = d0 + rp + PLANE0;  // padded plane index (pd == 1: plane d-1+kd+1; pd == 0: plane d)
+      ring.produce(nin, box_bytes * CG, [&](uint8_t* dst, int rp, uint64_t* bar) {
+        const int pp = o.d0 + rp + PLANE0;  // padded plane index (pd == 1: plane d-1+kd+1; pd == 0: plane d)
 #pragma unroll 1
-        for (int cg = 0; cg < CG; ++cg)
-          tma_load_4d(sA + (size_t)slot * slot_bytes + (size_t)cg * cg_bytes, &tmap, 0, w0, h0, cg * g.iDp + pp, &full[slot]);
-      }
+        for (int cg = 0; cg < CG; ++cg) tma_load_4d(dst + (size_t)cg * cg_bytes, &tmap, 0, o.w0, o.h0, cg * g.iDp + pp, bar);
+      });
     }
     return;
   }
@@ -350,34 +391,16 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
   const int wg = warp >> 2, wq = warp & 3;
   const int P = g.P;
   const uint32_t cgb16 = cg_bytes >> 4;
-  // A offset / LBO of K=16 step b inside a ring slot, in 16-byte units
-  auto aoff = [&](int b) -> uint32_t {
-    if constexpr (MODE == 1) {
-      const int t = b / (CIN / 16), j = b % (CIN / 16);
-      return (uint32_t)(2 * j) * cgb16 + (uint32_t)((1 + t / 2) * P + (1 + t % 2));
-    } else {
-      return stencil_aoff<CIN>(b, P, cgb16);
-    }
+  auto tap_off = [&](int t) -> int {
+    if constexpr (MODE == 1) return (1 + t / 2) * P + (1 + t % 2);
+    else return stencil_off(t, P);
   };
-  auto alo = [&](int b) -> uint32_t {
-    if constexpr (MODE == 1) return cgb16;
-    else return stencil_alo<CIN>(b, P, cgb16);
-  };
-  const uint32_t sB16 = smem_u32(sB) >> 4, sA16 = smem_u32(sA) >> 4;
+  auto aoff = [&](int b) -> uint32_t { return kstep_aoff<CIN, NTAPS>(b, cgb16, tap_off); };
+  auto alo = [&](int b) -> uint32_t { return kstep_alo<CIN, NTAPS>(b, cgb16, tap_off); };
+  const uint32_t sB16 = smem_u32(smem) >> 4;
   const uint32_t b_lbo16 = (uint32_t)(NMMA * 16 >> 4);
   const int nsub = 2 * g.nch;                      // 64-position sub-chunks per plane
-  mbar_wait(b_full, 0);
-  // output pixel (h, w) of row half i of sub-chunk sc; false for the pad columns and positions beyond the tensor
-  auto pixel = [&](int sc, int i, int& h, int& w) -> bool {
-    const int l = sc * 64 + wq * 16 + (lane >> 2);
-    int hh = l / P, ww = l - hh * P;   // row half 1 is 8 positions on: one division serves both halves
-    if (i) {
-      ww += 8;
-      while (ww >= P) { ww -= P; ++hh; }
-    }
-    h = h0 + hh; w = w0 + ww;
-    return hh < g.R && ww < g.TW && h < g.H && w < g.W;
-  };
+  ring.wait_weights();
   // P8 position and first channel of column block j of pixel (d, h, w); false for blocks beyond COUT
   auto out_at = [&](int d, int h, int w, int j, long long& pos, int& co) -> bool {
     const int n = ns * NPAD + 8 * j + 2 * (lane & 3);
@@ -394,33 +417,19 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
     }
     return true;
   };
-  // this thread's bias values, loaded once per CTA: bv[j][e] is added to column 8j + 2 * (lane % 4) + e of the fragment
-  // (except for N = 128, whose 32 more registers would spill: it loads them in the epilogue)
+  // bias in registers, except for N = 128, whose 32 more registers would spill: it loads them in the epilogue
   constexpr bool BIAS_REG = NPAD <= 64;
   float bv[OUT_PLAIN || !BIAS_REG ? 1 : NPAD / 8][2];
-  if constexpr (OUT_PLAIN) {
-    bv[0][0] = bias ? bias[0] : 0.f;
-  } else if constexpr (BIAS_REG) {
-#pragma unroll
-    for (int j = 0; j < NPAD / 8; ++j) {
-      const int n = ns * NPAD + 8 * j + 2 * (lane & 3);
-      const int co = CLASS_EPI ? n % g.cout : n;
-      const bool live = bias && (CLASS_EPI || ns * NPAD + 8 * j < g.cout);
-#pragma unroll
-      for (int e = 0; e < 2; ++e) bv[j][e] = live ? bias[co + e] : 0.f;
-    }
-  }
-  int next_wait = 0;
-  for (int od = 0; od < ndo; ++od) {
-    while (next_wait <= od + KD - 1) {
-      mbar_wait(&full[next_wait % g.S], (next_wait / g.S) & 1);
-      ++next_wait;
-    }
+  if constexpr (OUT_PLAIN) bv[0][0] = bias ? bias[0] : 0.f;
+  else if constexpr (BIAS_REG) load_bias<CLASS_EPI>(bv, bias, ns * NPAD, g.cout, lane);
+  for (int od = 0; od < o.ndo; ++od) {
+    ring.wait(od + KD - 1);
     uint32_t slot16[KD];
 #pragma unroll
-    for (int kd = 0; kd < KD; ++kd) slot16[kd] = sA16 + (uint32_t)((od + kd) % g.S) * (slot_bytes >> 4);
-    const int d = d0 + od;
+    for (int kd = 0; kd < KD; ++kd) slot16[kd] = ring.slot16(od + kd);
+    const int d = o.d0 + od;
     for (int sc = wg; sc < nsub; sc += kConsumerWG) {
+      const int l = sc * 64 + wq * 16 + (lane >> 2);
       // the skip operand is fetched before the MMA chain, so that its load latency overlaps the chain (except for N = 128,
       // whose accumulators leave no room for it)
       constexpr bool RES_EARLY = !OUT_PLAIN && NPAD <= 64;
@@ -430,7 +439,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
 #pragma unroll
           for (int i = 0; i < 2; ++i) {
             int h, w;
-            const bool in = pixel(sc, i, h, w);
+            const bool in = frag_pixel(g, o, l, i, h, w);
 #pragma unroll
             for (int j = 0; j < NPAD / 8; ++j) {
               long long pos;
@@ -446,7 +455,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         int h, w;
-        if (!pixel(sc, i, h, w)) continue;
+        if (!frag_pixel(g, o, l, i, h, w)) continue;
         if constexpr (OUT_PLAIN) {
           if ((lane & 3) == 0) {
             float x = acc[2 * i];
@@ -485,84 +494,69 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
         }
       }
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[od % g.S]);   // oldest input plane of od no longer read by this warp -> producer may refill
+    ring.release(od);   // oldest input plane of od
   }
-  if constexpr (Tail::enabled) {
-    // ndo == D (host-checked): this thread wrote all D logits of its pixels itself (program order makes them visible to it)
-    if ((lane & 3) == 0) {
-      for (int sc = wg; sc < nsub; sc += kConsumerWG)
-        for (int i = 0; i < 2; ++i) {
-          int h, w;
-          if (pixel(sc, i, h, w)) tail(plain_out, h * g.W + w, w, h, g.H * g.W);
-        }
-    }
-  }
+  if constexpr (Tail::enabled) run_tail(tail, plain_out, g, o, wg, wq, lane);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------
-template <int CIN> inline size_t b_image_elems(int npad, int kd) { return (size_t)kd * blocks_per_kd<CIN>() * npad * 16; }
+// Canonical K-major no-swizzle index of B element (K half, column n, k element e) of K=16 block blk, in an image of
+// ncols columns: block = [k half (2)][n/8][n%8][8 k-elements]
+inline size_t b_index(int blk, int half, int n, int e, int ncols) {
+  return (((size_t)blk * 2 + half) * (ncols / 8) + n / 8) * 64 + (n % 8) * 8 + e;
+}
 
-// w: folded fp32 weights [tap][cin][cout] (tap = (kd*3+kh)*3+kw).  Writes the canonical K-major no-swizzle image:
-// block(kd,b) = [k half (2)][n/8][n%8][8 k-elements]
+// w: folded fp32 weights [tap][cin][cout] (tap = (kd*3+kh)*3+kw).  Writes the canonical K-major no-swizzle image.
 // nsplit > 1: the image holds nsplit consecutive slice images, slice s covering output channels [s*npad, (s+1)*npad).
-template <typename T, int CIN>
+template <typename T>
 inline void build_b_image(const float* w, int cin, int cout, int npad, int kd_n, std::vector<T>& img, T (*cvt)(float),
                           int nsplit = 1, bool hilo = false, float (*back)(T) = nullptr) {
-  constexpr int NBLK = blocks_per_kd<CIN>();
+  const int nblk = ksteps(cin, 9);
   const int nmma = hilo ? 2 * npad : npad;
-  const size_t slice = (size_t)kd_n * NBLK * nmma * 16;
+  const size_t slice = (size_t)kd_n * nblk * nmma * 16;
   img.assign(slice * nsplit, cvt(0.f));
   for (int kd = 0; kd < kd_n; ++kd)
-    for (int b = 0; b < NBLK; ++b)
+    for (int b = 0; b < nblk; ++b)
       for (int half = 0; half < 2; ++half)
         for (int nn = 0; nn < cout; ++nn)
           for (int e = 0; e < 8; ++e) {
             const int n = nn % npad;
             T* simg = img.data() + slice * (nn / npad);
-            int tap9, ci;
-            if (CIN >= 16) { tap9 = b / (CIN / 16); ci = (b % (CIN / 16)) * 16 + half * 8 + e; }
-            else { tap9 = b < 4 ? 2 * b + half : (half == 0 ? -1 : 8); ci = e; }  // block 4 = (zero, tap 8)
-            if (tap9 < 0 || tap9 >= 9 || ci >= cin) continue;
-            const int tap = kd * 9 + tap9;
-            const float val = w[((size_t)tap * cin + ci) * cout + nn];
-            T* blk = simg + ((size_t)(kd * NBLK + b) * 2 + half) * (nmma / 8) * 64;
+            const int tap9 = kstep_tap(cin, 9, b, half), ci = kstep_ch(cin, b, half) + e;
+            if (!kstep_live(cin, 9, b, half) || ci >= cin) continue;
+            const float val = w[((size_t)(kd * 9 + tap9) * cin + ci) * cout + nn];
             const T hi = cvt(val);
-            blk[(n / 8) * 64 + (n % 8) * 8 + e] = hi;
-            if (hilo) {
-              const int n2 = npad + n;
-              blk[(n2 / 8) * 64 + (n2 % 8) * 8 + e] = cvt(val - back(hi));
-            }
+            simg[b_index(kd * nblk + b, half, n, e, nmma)] = hi;
+            if (hilo) simg[b_index(kd * nblk + b, half, npad + n, e, nmma)] = cvt(val - back(hi));
           }
 }
 
 // Transposed conv (k3 s2 p1 op1) B image: w is the gather-form folded weight [tap27][cin][cout] (tap index = kernel index
 // of the ConvTranspose3d).  Per axis, output parity p and input offset t (0 = same index, 1 = next index) select the
 // kernel index: p=0:t=0 -> k=1 ; p=1:t=0 -> k=2, t=1 -> k=0 ; (p=0,t=1) contributes nothing.
-template <typename T, int CIN>
+template <typename T>
 inline void build_b_image_deconv(const float* w, int cin, int cout, std::vector<T>& img, T (*cvt)(float), int nsplit = 1) {
-  constexpr int NBLK = blocks_per_kd<CIN, 1>();
+  const int nblk = ksteps(cin, 4);
   const int npad = 8 * cout / nsplit;
-  const size_t slice = (size_t)2 * NBLK * npad * 16;
+  const size_t slice = (size_t)2 * nblk * npad * 16;
   img.assign(slice * nsplit, cvt(0.f));
   auto kidx = [](int p, int t) { return p == 0 ? (t == 0 ? 1 : -1) : (t == 0 ? 2 : 0); };
   for (int td = 0; td < 2; ++td)
-    for (int b = 0; b < NBLK; ++b)
+    for (int b = 0; b < nblk; ++b)
       for (int half = 0; half < 2; ++half)
         for (int cls = 0; cls < 8; ++cls)
           for (int co = 0; co < cout; ++co)
             for (int e = 0; e < 8; ++e) {
-              const int t = b / (CIN / 16), j = b % (CIN / 16);
-              const int ci = j * 16 + half * 8 + e;
+              const int t = kstep_tap(cin, 4, b, half), ci = kstep_ch(cin, b, half) + e;
               const int th = t / 2, tw = t % 2;
               const int kd = kidx(cls >> 2, td), kh = kidx((cls >> 1) & 1, th), kw = kidx(cls & 1, tw);
               if (kd < 0 || kh < 0 || kw < 0 || ci >= cin) continue;
               const int nfull = cls * cout + co, n = nfull % npad;
               T* simg = img.data() + slice * (nfull / npad);
               const float val = w[((size_t)((kd * 3 + kh) * 3 + kw) * cin + ci) * cout + co];
-              simg[(((size_t)(td * NBLK + b) * 2 + half) * (npad / 8) + n / 8) * 64 + (n % 8) * 8 + e] = cvt(val);
+              simg[b_index(td * nblk + b, half, n, e, npad)] = cvt(val);
             }
 }
 
@@ -582,69 +576,103 @@ inline EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
+// Positions a TMA box of R + halo rows of pitch P occupies in a ring slot: the box itself, and at least as far as the
+// A reads of the last 128-position chunk reach (its taps start up to halo * (P + 1) positions on), plus 8, rounded up
+// to 8 (128-byte aligned TMA destinations).
+inline int box_positions(int R, int P, int halo) {
+  const int nch = (R * P + 127) / 128;
+  return (std::max((R + halo) * P, nch * 128 + halo * (P + 1)) + 8 + 7) / 8 * 8;
+}
+
+// What the tile search of one kernel depends on, apart from its halo amplification and clocks per tile
+struct TileLimits {
+  int s_hi, s_lo;         // ring depth range; the deepest that fits is preferred
+  int halo;               // a tile reads R + halo rows of P = TW + halo positions per input plane
+  int boxes;              // TMA boxes per channel group and plane
+  int p_max;              // TMA box limit on P
+  int tw_min;             // narrowest tile width when W is split
+  int nch_max;            // most 128-position chunks per plane
+  int dr_min;             // fewest planes per tile (when D >= 2)
+  bool full_depth;        // tiles span all D planes (the prob layer's soft-argmin tail needs a pixel's D logits in one CTA)
+};
+
 struct Plan {
   Geom g;
   int grid;
   size_t smem;
 };
 
-inline Plan make_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode = 0, size_t smem_limit = 225 * 1024,
-                      bool full_depth = false /* tiles span all D planes (the prob layer's soft-argmin tail needs a pixel's D logits in one CTA) */) {
-  Plan p{};
-  Geom& g = p.g;
-  g.D = D; g.H = H; g.W = W; g.Hp = H + 2; g.Wp = W + 2; g.pd = pd;
-  const int cg = cin / 8;
-  const int nblk = mode == 1 ? 4 * (cin / 16) : (cin >= 16 ? 9 * (cin / 16) : 5);
-  const size_t bbytes = (((size_t)kd * nblk * npad * 32) + 127) / 128 * 128;
-  // Search (ring depth, tile width, tile rows, planes per tile) for the cheapest feasible tiling.
-  // cost = L2 bytes per useful output position (halo re-reads in h, w and d)
-  //        x MMA rows issued per useful position (pad columns, partial last chunk)
-  //        x wave quantisation on the 132 SMs of an H100 SXM (one CTA per SM: time ~ ceil(T/132) tile-times for T tiles)
+// Searches (ring depth, tile width, tile rows, planes per tile) for the cheapest tiling whose B image (b_bytes), ring
+// slots and barriers fit smem_limit.
+// cost = L2 bytes per useful output position (halo re-reads in h, w and d: amp(R, TW, P, DR))
+//        x MMA rows issued per useful position (pad columns, partial last chunk)
+//        x wave quantisation on the 132 SMs of an H100 SXM (one CTA per SM: time ~ ceil(T/132) tile-times for T tiles)
+// tile_clk(DR, nch) is the estimated time of one tile in clocks: a per-CTA fixed cost + the instruction stream.  Its
+// constants are a model (instruction cost growing with N, a fixed per-CTA prologue, fill and drain), not a measurement;
+// they only rank tilings against each other.  A limit below 225 KB is soft: if nothing fits it, 225 KB is searched.
+template <typename Amp, typename Clk>
+inline Tile plan_tiles(int D, int H, int W, int cg, size_t b_bytes, size_t smem_limit, const TileLimits& lim, Amp amp, Clk tile_clk,
+                       size_t& smem_out) {
+  auto smem_of = [&](int S, int R, int P) { return b_bytes + (size_t)S * cg * lim.boxes * box_positions(R, P, lim.halo) * 16 + 256; };
   double best_cost = 1e30;
   int bestR = 0, bestTW = 0, bestS = 0, bestDR = 0;
-  const int s_hi = kd == 3 ? 4 : 3, s_lo = kd == 3 ? 3 : 2;   // kd == 2 (deconv): 2 live + 1 prefetch
-  for (int S = s_hi; S >= s_lo; --S) {
+  for (int S = lim.s_hi; S >= lim.s_lo; --S) {
     for (int tiles_w = 1; tiles_w <= 20; ++tiles_w) {
       const int TW = (W + tiles_w - 1) / tiles_w;
-      if (TW + 2 > 256) continue;               // TMA box dims <= 256
-      if (tiles_w > 1 && TW < 30) break;
+      if (TW + lim.halo > lim.p_max) continue;
+      if (tiles_w > 1 && TW < lim.tw_min) break;
       const int tw_n = (W + TW - 1) / TW;
-      const int P = TW + 2;
+      const int P = TW + lim.halo;
       for (int R = 1; R <= 32 && R <= H; ++R) {
         const int nch = (R * P + 127) / 128;
-        const int slot_pos = (std::max((R + 2) * P, nch * 128 + 2 * P + 2) + 8 + 7) / 8 * 8;
-        const size_t smem = bbytes + (size_t)S * cg * slot_pos * 16 + 256;
-        if (smem > smem_limit) break;
+        if (nch > lim.nch_max) break;
+        if (smem_of(S, R, P) > smem_limit) break;
         const int th_n = (H + R - 1) / R;
-        for (int dsplit = 1; dsplit <= (full_depth ? 1 : D); ++dsplit) {
+        for (int dsplit = 1; dsplit <= (lim.full_depth ? 1 : D); ++dsplit) {
           const int DR = (D + dsplit - 1) / dsplit;
-          if (kd >= 2 && DR < 2 && D >= 2) break;
+          if (DR < lim.dr_min && D >= 2) break;
           const int td_n = (D + DR - 1) / DR;
           const double T = (double)tw_n * th_n * td_n;
-          const double amp = (double)(R + 2) / R * (double)P / TW * (kd == 3 ? (double)(DR + 2) / DR : (kd == 2 ? (double)(DR + 1) / DR : 1.0));
-          // estimated kernel time in clocks: waves x (per-CTA fixed cost + instruction stream), inflated by halo re-reads.
-          // The constants are a model (instruction cost growing with N, a fixed per-CTA prologue, fill and drain), not
-          // a measurement; they only rank tilings against each other.
-          const double clk_mma = mode == 1 ? 35.0 + 0.45 * npad : 45.0 + 0.35 * npad;
-          const double tile_clk = 8500.0 + (double)DR * nch * nblk * kd * clk_mma;
-          const double cost = std::ceil(T / 132.0) * tile_clk * (1.0 + 0.25 * (amp - 1.0)) * (S == s_hi ? 1.0 : 1.05);
+          const double cost = std::ceil(T / 132.0) * tile_clk(DR, nch) * (1.0 + 0.25 * (amp(R, TW, P, DR) - 1.0)) * (S == lim.s_hi ? 1.0 : 1.05);
           if (cost < best_cost - 1e-9) { best_cost = cost; bestR = R; bestTW = TW; bestS = S; bestDR = DR; }
           if (T > 4000) break;
         }
       }
     }
-    if (bestR > 0 && S == s_hi) break;
+    if (bestR > 0 && S == lim.s_hi) break;
   }
-  if (bestR == 0 && smem_limit < 225 * 1024) return make_plan(cin, npad, kd, D, H, W, pd, mode, 225 * 1024, full_depth);   // soft limit
+  if (bestR == 0 && smem_limit < 225 * 1024) return plan_tiles(D, H, W, cg, b_bytes, 225 * 1024, lim, amp, tile_clk, smem_out);
   TDM_CHECK(bestR > 0, "conv_tc: no tile fits shared memory");
-  g.S = bestS; g.R = bestR; g.TW = bestTW; g.P = bestTW + 2; g.DR = bestDR;
-  g.nch = (g.R * g.P + 127) / 128;
-  g.slot_pos = (std::max((g.R + 2) * g.P, g.nch * 128 + 2 * g.P + 2) + 8 + 7) / 8 * 8;   // 128-byte aligned TMA destinations
-  g.tiles_w = (W + g.TW - 1) / g.TW;
-  g.tiles_h = (H + g.R - 1) / g.R;
-  g.tiles_d = (D + g.DR - 1) / g.DR;
-  p.grid = g.tiles_w * g.tiles_h * g.tiles_d;
-  p.smem = bbytes + (size_t)g.S * cg * g.slot_pos * 16 + 256;
+  Tile t{};
+  t.D = D; t.H = H; t.W = W;
+  t.S = bestS; t.R = bestR; t.TW = bestTW; t.P = bestTW + lim.halo; t.DR = bestDR;
+  t.nch = (t.R * t.P + 127) / 128;
+  t.slot_pos = box_positions(t.R, t.P, lim.halo);
+  t.tiles_w = (W + t.TW - 1) / t.TW;
+  t.tiles_h = (H + t.R - 1) / t.R;
+  t.tiles_d = (D + t.DR - 1) / t.DR;
+  smem_out = smem_of(t.S, t.R, t.P);
+  return t;
+}
+
+inline size_t b_image_bytes(int kd, int nblk, int ncols) { return (((size_t)kd * nblk * ncols * 32) + 127) / 128 * 128; }
+
+inline Plan make_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode = 0, size_t smem_limit = 225 * 1024,
+                      bool full_depth = false /* tiles span all D planes (the prob layer's soft-argmin tail) */) {
+  Plan p{};
+  const int nblk = ksteps(cin, mode == 1 ? 4 : 9);
+  const int s_hi = kd == 3 ? 4 : 3, s_lo = kd == 3 ? 3 : 2;   // kd == 2 (deconv): 2 live + 1 prefetch
+  const TileLimits lim{s_hi, s_lo, 2, 1, 256, 30, INT_MAX, kd >= 2 ? 2 : 1, full_depth};
+  auto amp = [&](int R, int TW, int P, int DR) {
+    return (double)(R + 2) / R * (double)P / TW * (kd == 3 ? (double)(DR + 2) / DR : (kd == 2 ? (double)(DR + 1) / DR : 1.0));
+  };
+  auto tile_clk = [&](int DR, int nch) {
+    const double clk_mma = mode == 1 ? 35.0 + 0.45 * npad : 45.0 + 0.35 * npad;
+    return 8500.0 + (double)DR * nch * nblk * kd * clk_mma;
+  };
+  static_cast<Tile&>(p.g) = plan_tiles(D, H, W, cin / 8, b_image_bytes(kd, nblk, npad), smem_limit, lim, amp, tile_clk, p.smem);
+  p.g.Hp = H + 2; p.g.Wp = W + 2; p.g.pd = pd;
+  p.grid = p.g.tiles_w * p.g.tiles_h * p.g.tiles_d;
   return p;
 }
 

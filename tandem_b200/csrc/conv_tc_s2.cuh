@@ -17,146 +17,80 @@ namespace tc {
 
 constexpr int kMaxTaps = 25;
 
-struct GeomS2 {
-  int D, H, W;             // OUTPUT dims
+struct GeomS2 : Tile {     // Tile: OUTPUT grid; P = TW + KS/2, slot_pos = one parity sub-tile
   int oHp, oWp, opd;       // output padded dims / D halo
   long long out_gs;
   int iDp;                 // input padded plane count (D_in + 2*pd_in): tensor-map dim 3 = cg * iDp + plane
-  int ipd;                 // input D halo (1: 3-D, 0: 2-D over views)
   int c0;                  // 1 - pad (0 for 3x3 p1, -1 for 5x5 p2): padded input coordinate = 2*o + k + c0
-  int R, TW, DR, P, RR;    // tile rows / cols / planes (output coords); sub-tile pitch P = TW + KS/2, rows RR = R + KS/2
-  int nch, sub_pos, S;
-  int tiles_w, tiles_h, tiles_d;
+  int RR;                  // sub-tile rows, R + KS/2
   int relu, cout;
-  int ntaps;               // KS*KS
   short tap_off[kMaxTaps + 1];   // position offset of tap t inside a channel group's 4 sub-tiles (table order)
 };
-
-template <int CIN, int KS> constexpr int s2_blocks() { return CIN >= 16 ? KS * KS * (CIN / 16) : (KS * KS + 1) / 2; }
 
 template <typename TIn, typename TOut, int CIN, int NPAD, int KD, int KS>
 __global__ void __launch_bounds__(kThreads, 1)
 k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ bimg, const float* __restrict__ bias,
              TOut* __restrict__ out, const __grid_constant__ GeomS2 g) {
   constexpr int CG = CIN / 8;
-  constexpr int NBLK = s2_blocks<CIN, KS>();
+  constexpr int NTAPS = KS * KS;
+  constexpr int NBLK = ksteps(CIN, NTAPS);
   constexpr int B_BYTES = KD * NBLK * NPAD * 32;
 
   extern __shared__ __align__(128) uint8_t smem[];
   const int ns = blockIdx.y;
-  bimg += (size_t)ns * (B_BYTES / sizeof(TIn));
-  uint8_t* sB = smem;
-  uint8_t* sA = smem + ((B_BYTES + 127) / 128) * 128;
-  const uint32_t sub_bytes = (uint32_t)g.sub_pos * 16u;
+  const uint32_t sub_bytes = (uint32_t)g.slot_pos * 16u;
   const uint32_t cg_bytes = sub_bytes * 4u;
-  const uint32_t slot_bytes = cg_bytes * CG;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sA + (size_t)slot_bytes * g.S);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + 8;
-  uint64_t* b_full = bars + 16;
-
+  Ring ring = Ring::start(smem, B_BYTES, bimg + (size_t)ns * (B_BYTES / sizeof(TIn)), cg_bytes * CG, g.S);
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
-  int tile = blockIdx.x;
-  const int tw = tile % g.tiles_w; tile /= g.tiles_w;
-  const int th = tile % g.tiles_h; tile /= g.tiles_h;
-  const int td = tile;
-  const int w0 = tw * g.TW, h0 = th * g.R, d0 = td * g.DR;
-  const int ndo = min(g.DR, g.D - d0);
-  const int nin = KD == 3 ? 2 * ndo + 1 : ndo;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < g.S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4 * kConsumerWG); }
-    mbar_init(b_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    mbar_expect_tx(b_full, B_BYTES);          // weights do not depend on the previous kernel: fetch them before pdl_wait
-    bulk_g2s(sB, bimg, B_BYTES, b_full);
-  }
-  __syncthreads();
-  pdl_wait();   // from here on activations written by the previous kernel are read and our outputs are written
-  // trigger the dependents only now: a trigger BEFORE the wait lets the whole chain of later kernels become resident early (each
-  // one's prologue would trigger the next), and their idle CTAs then hold the shared memory the running kernel's tiles need
-  if (threadIdx.x == 0) pdl_launch_dependents();
+  const TileOrigin o = tile_origin(g);
+  const int nin = KD == 3 ? 2 * o.ndo + 1 : o.ndo;
 
   if (warp == kProducerWarp) {
     // ===================== TMA producer: 4 parity sub-tiles per channel group per input plane =====================
     if (lane == 0) {
       const uint32_t box_bytes = (uint32_t)g.P * (uint32_t)g.RR * 16u;
-      const int col0 = 2 * w0 + g.c0, row0 = 2 * h0 + g.c0;
-      for (int rp = 0; rp < nin; ++rp) {
-        const int slot = rp % g.S;
-        if (rp >= g.S) mbar_wait(&empty[slot], ((rp / g.S) - 1) & 1);
-        mbar_expect_tx(&full[slot], box_bytes * 4u * CG);
+      const int col0 = 2 * o.w0 + g.c0, row0 = 2 * o.h0 + g.c0;
+      ring.produce(nin, box_bytes * 4u * CG, [&](uint8_t* dst, int rp, uint64_t* bar) {
         // padded input plane: 3-D: 2*(d0+od) + kd + c0 (+1 halo, -pad) -> 2*d0 + rp ; 2-D: the view index itself
-        const int pp = KD == 3 ? 2 * d0 + rp + g.c0 : d0 + rp;
+        const int pp = KD == 3 ? 2 * o.d0 + rp + g.c0 : o.d0 + rp;
 #pragma unroll 1
         for (int cg = 0; cg < CG; ++cg) {
-          uint8_t* dst = sA + (size_t)slot * slot_bytes + (size_t)cg * cg_bytes;
 #pragma unroll
           for (int sub = 0; sub < 4; ++sub)
-            tma_load_4d(dst + (size_t)sub * sub_bytes, &tmap, 0, col0 + (sub & 1), row0 + (sub >> 1), cg * g.iDp + pp, &full[slot]);
+            tma_load_4d(dst + (size_t)cg * cg_bytes + (size_t)sub * sub_bytes, &tmap, 0, col0 + (sub & 1), row0 + (sub >> 1),
+                        cg * g.iDp + pp, bar);
         }
-      }
+      });
     }
     return;
   }
   // ===================== consumers: MMA + epilogue =====================
   const int wg = warp >> 2, wq = warp & 3;
   const uint32_t cgb16 = cg_bytes >> 4;
-  auto aoff = [&](int b) -> uint32_t {
-    if constexpr (CIN >= 16) {
-      return (uint32_t)(2 * (b % (CIN / 16))) * cgb16 + (uint32_t)g.tap_off[b / (CIN / 16)];
-    } else {
-      // taps paired in table (= address) order; an odd last tap is paired with its predecessor against zero weights
-      const int t1 = min(2 * b + 1, g.ntaps - 1);
-      return (uint32_t)g.tap_off[t1 - 1];
-    }
-  };
-  auto alo = [&](int b) -> uint32_t {
-    if constexpr (CIN >= 16) {
-      return cgb16;
-    } else {
-      const int t1 = min(2 * b + 1, g.ntaps - 1);
-      return (uint32_t)(g.tap_off[t1] - g.tap_off[t1 - 1]);
-    }
-  };
-  const uint32_t sB16 = smem_u32(sB) >> 4, sA16 = smem_u32(sA) >> 4;
+  auto tap_off = [&](int t) -> int { return g.tap_off[t]; };
+  auto aoff = [&](int b) -> uint32_t { return kstep_aoff<CIN, NTAPS>(b, cgb16, tap_off); };
+  auto alo = [&](int b) -> uint32_t { return kstep_alo<CIN, NTAPS>(b, cgb16, tap_off); };
+  const uint32_t sB16 = smem_u32(smem) >> 4;
   const uint32_t b_lbo16 = (uint32_t)(NPAD * 16 >> 4);
   const int nsub = 2 * g.nch;
-  mbar_wait(b_full, 0);
-  // this thread's bias values, loaded once per CTA: bv[j][e] is added to column 8j + 2 * (lane % 4) + e of the fragment
+  ring.wait_weights();
   float bv[NPAD / 8][2];
-#pragma unroll
-  for (int j = 0; j < NPAD / 8; ++j) {
-    const int c = ns * NPAD + 8 * j + 2 * (lane & 3);
-    const bool live = bias && ns * NPAD + 8 * j < g.cout;
-#pragma unroll
-    for (int e = 0; e < 2; ++e) bv[j][e] = live ? bias[c + e] : 0.f;
-  }
-  int next_wait = 0;
-  for (int od = 0; od < ndo; ++od) {
+  load_bias<false>(bv, bias, ns * NPAD, g.cout, lane);
+  for (int od = 0; od < o.ndo; ++od) {
     const int first = KD == 3 ? 2 * od : od;
-    while (next_wait <= first + KD - 1) {
-      mbar_wait(&full[next_wait % g.S], (next_wait / g.S) & 1);
-      ++next_wait;
-    }
+    ring.wait(first + KD - 1);
     uint32_t slot16[KD];
 #pragma unroll
-    for (int kd = 0; kd < KD; ++kd) slot16[kd] = sA16 + (uint32_t)((first + kd) % g.S) * (slot_bytes >> 4);
-    const int d = d0 + od;
+    for (int kd = 0; kd < KD; ++kd) slot16[kd] = ring.slot16(first + kd);
+    const int d = o.d0 + od;
     for (int sc = wg; sc < nsub; sc += kConsumerWG) {
       float acc[NPAD / 2];
       mma_subchunk<NPAD, TIn, KD, NBLK>(acc, slot16, (uint32_t)sc * 64u, sB16, b_lbo16, aoff, alo);
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        const int l = sc * 64 + wq * 16 + (lane >> 2);
-        int hh = l / g.P, ww = l - hh * g.P;   // row half 1 is 8 positions on: one division serves both halves
-        if (i) {
-          ww += 8;
-          while (ww >= g.P) { ww -= g.P; ++hh; }
-        }
-        const int h = h0 + hh, w = w0 + ww;
-        if (!(hh < g.R && ww < g.TW && h < g.H && w < g.W)) continue;
+        int h, w;
+        if (!frag_pixel(g, o, sc * 64 + wq * 16 + (lane >> 2), i, h, w)) continue;
         const long long pos = ((((long long)(d + g.opd)) * g.oHp + (h + 1)) * g.oWp + (w + 1)) * 8;
 #pragma unroll
         for (int j = 0; j < NPAD / 8; ++j) {
@@ -173,15 +107,8 @@ k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ b
         }
       }
     }
-    __syncwarp();
-    if (lane == 0) {               // input planes no longer read by this warp -> producer may refill
-      if (KD == 3) {               // input planes 2*od and 2*od+1 are dead after output plane od
-        mbar_arrive(&empty[(2 * od) % g.S]);
-        mbar_arrive(&empty[(2 * od + 1) % g.S]);
-      } else {
-        mbar_arrive(&empty[od % g.S]);
-      }
-    }
+    ring.release(first);                   // KD = 3: input planes 2*od and 2*od+1 are dead after output plane od
+    if (KD == 3) ring.release(first + 1);
   }
 }
 
@@ -210,59 +137,18 @@ struct PlanS2 {
 // D,H,W: OUTPUT dims.  kd in {1,3}.
 inline PlanS2 make_plan_s2(int cin, int npad, int kd, int ks, int D, int H, int W, size_t smem_limit = 225 * 1024) {
   PlanS2 p{};
-  GeomS2& g = p.g;
-  g.D = D; g.H = H; g.W = W;
-  const int cg = cin / 8;
-  const int nblk = cin >= 16 ? ks * ks * (cin / 16) : (ks * ks + 1) / 2;
-  const size_t bbytes = (((size_t)kd * nblk * npad * 32) + 127) / 128 * 128;
+  const int nblk = ksteps(cin, ks * ks);
   const int hk = ks / 2;
-  double best_cost = 1e30;
-  int bR = 0, bTW = 0, bS = 0, bDR = 0;
-  const int s_hi = kd == 3 ? 5 : 3, s_lo = kd == 3 ? 4 : 2;
-  for (int S = s_hi; S >= s_lo; --S) {
-    for (int tiles_w = 1; tiles_w <= 20; ++tiles_w) {
-      const int TW = (W + tiles_w - 1) / tiles_w;
-      if (TW + hk > 128) continue;             // TMA box dim 2*P <= 256
-      if (tiles_w > 1 && TW < 16) break;
-      const int tw_n = (W + TW - 1) / TW;
-      const int P = TW + hk;
-      for (int R = 1; R <= 32 && R <= H; ++R) {
-        const int RR = R + hk;
-        if (2 * RR > 256) break;
-        const int nch = (R * P + 127) / 128;
-        int sub_pos = std::max(RR * P, nch * 128 + hk * (P + 1)) + 8;
-        sub_pos = (sub_pos + 7) / 8 * 8;       // 128-byte aligned TMA destinations
-        const size_t smem = bbytes + (size_t)S * cg * 4 * sub_pos * 16 + 256;
-        if (smem > smem_limit || sub_pos * 4 > 32000) break;
-        const int th_n = (H + R - 1) / R;
-        for (int dsplit = 1; dsplit <= D; ++dsplit) {
-          const int DR = (D + dsplit - 1) / dsplit;
-          const int td_n = (D + DR - 1) / DR;
-          const double T = (double)tw_n * th_n * td_n;
-          const double amp = (double)(2 * R + ks - 2) / (2 * R) * (double)(2 * TW + ks - 2) / (2 * TW) *
-                             (kd == 3 ? (double)(2 * DR + 1) / (2 * DR) : 1.0);
-          // same time model as conv_tc.cuh::make_plan
-          const double tile_clk = 8500.0 + (double)DR * nch * nblk * kd * (45.0 + 0.35 * npad);
-          const double cost = std::ceil(T / 132.0) * tile_clk * (1.0 + 0.25 * (amp - 1.0)) * (S == s_hi ? 1.0 : 1.05);
-          if (cost < best_cost - 1e-9) { best_cost = cost; bR = R; bTW = TW; bS = S; bDR = DR; }
-          if (T > 4000) break;
-        }
-      }
-    }
-    if (bR > 0 && S == s_hi) break;
-  }
-  if (bR == 0 && smem_limit < 225 * 1024) return make_plan_s2(cin, npad, kd, ks, D, H, W, 225 * 1024);   // soft limit
-  TDM_CHECK(bR > 0, "conv_tc_s2: no tile fits shared memory");
-  g.S = bS; g.R = bR; g.TW = bTW; g.DR = bDR;
-  g.P = bTW + hk; g.RR = bR + hk;
-  g.nch = (g.R * g.P + 127) / 128;
-  g.sub_pos = (std::max(g.RR * g.P, g.nch * 128 + hk * (g.P + 1)) + 8 + 7) / 8 * 8;
-  g.tiles_w = (W + g.TW - 1) / g.TW;
-  g.tiles_h = (H + g.R - 1) / g.R;
-  g.tiles_d = (D + g.DR - 1) / g.DR;
-  g.ntaps = ks * ks;
-  p.grid = g.tiles_w * g.tiles_h * g.tiles_d;
-  p.smem = bbytes + (size_t)g.S * cg * 4 * g.sub_pos * 16 + 256;
+  // a TMA box reads 2 * P columns (every second one): P <= 128
+  const TileLimits lim{kd == 3 ? 5 : 3, kd == 3 ? 4 : 2, hk, 4, 128, 16, INT_MAX, 1, false};
+  auto amp = [&](int R, int TW, int, int DR) {
+    return (double)(2 * R + ks - 2) / (2 * R) * (double)(2 * TW + ks - 2) / (2 * TW) * (kd == 3 ? (double)(2 * DR + 1) / (2 * DR) : 1.0);
+  };
+  auto tile_clk = [&](int DR, int nch) { return 8500.0 + (double)DR * nch * nblk * kd * (45.0 + 0.35 * npad); };
+  static_cast<Tile&>(p.g) = plan_tiles(D, H, W, cin / 8, b_image_bytes(kd, nblk, npad), smem_limit, lim, amp, tile_clk, p.smem);
+  TDM_CHECK(4 * p.g.slot_pos <= SHRT_MAX, "conv_tc_s2: tap offsets overflow");
+  p.g.RR = p.g.R + hk;
+  p.grid = p.g.tiles_w * p.g.tiles_h * p.g.tiles_d;
   return p;
 }
 
@@ -271,7 +157,7 @@ template <typename T>
 inline void build_b_image_s2(const float* w, int cin, int cout, int npad, int kd_n, int ks,
                              const std::vector<std::pair<int, int>>& taps, std::vector<T>& img, T (*cvt)(float), int nsplit = 1) {
   const int ntaps = (int)taps.size();
-  const int nblk = cin >= 16 ? ntaps * (cin / 16) : (ntaps + 1) / 2;
+  const int nblk = ksteps(cin, ntaps);
   const size_t slice = (size_t)kd_n * nblk * npad * 16;
   img.assign(slice * nsplit, cvt(0.f));
   for (int kd = 0; kd < kd_n; ++kd)
@@ -279,20 +165,12 @@ inline void build_b_image_s2(const float* w, int cin, int cout, int npad, int kd
       for (int half = 0; half < 2; ++half)
         for (int nn = 0; nn < cout; ++nn)
           for (int e = 0; e < 8; ++e) {
-            int t, ci;
-            if (cin >= 16) { t = b / (cin / 16); ci = (b % (cin / 16)) * 16 + half * 8 + e; }
-            else {
-              const int t1 = std::min(2 * b + 1, ntaps - 1), t0 = t1 - 1;
-              t = half == 0 ? t0 : t1;
-              if (half == 0 && 2 * b + 1 > ntaps - 1) t = -1;   // odd last block: first half re-reads the previous tap x 0
-              ci = e;
-            }
-            if (t < 0 || ci >= cin) continue;
+            const int t = kstep_tap(cin, ntaps, b, half), ci = kstep_ch(cin, b, half) + e;
+            if (!kstep_live(cin, ntaps, b, half) || ci >= cin) continue;
             const int tap = (kd * ks + taps[t].first) * ks + taps[t].second;
             const int n = nn % npad;
             T* simg = img.data() + slice * (nn / npad);
-            simg[(((size_t)(kd * nblk + b) * 2 + half) * (npad / 8) + n / 8) * 64 + (n % 8) * 8 + e] =
-                cvt(w[((size_t)tap * cin + ci) * cout + nn]);
+            simg[b_index(kd * nblk + b, half, n, e, npad)] = cvt(w[((size_t)tap * cin + ci) * cout + nn]);
           }
 }
 

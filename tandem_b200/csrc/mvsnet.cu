@@ -195,7 +195,7 @@ class MvsnetEngine final : public MvsnetIface {
     else if (key == "use_pdl") { TDM_CHECK(value >= 0 && value <= 2, "use_pdl: 0 off, 1 tensor-core kernels, 2 every kernel of the forward"); use_pdl_ = value; }
     else if (key == "pdl_min_smem_kb") { TDM_CHECK(value >= 0 && value <= 225, "pdl_min_smem_kb out of range"); pdl_min_smem_kb_ = value; }
     else if (key == "cv_variant") { TDM_CHECK(value >= 0 && value <= 5, "cv_variant out of range"); cv_variant_ = value; }
-    else if (key == "tc_smem_kb") { TDM_CHECK(value >= 48 && value <= 225, "tc_smem_kb out of range"); tc_smem_kb_ = value; tc_cache_.clear(); s2_cache_.clear(); }
+    else if (key == "tc_smem_kb") { TDM_CHECK(value >= 48 && value <= 225, "tc_smem_kb out of range"); tc_smem_kb_ = value; tc_cache_.clear(); }
     else if (key.rfind("depth_num_stage", 0) == 0 && key.size() == 16 && key[15] >= '1' && key[15] <= '3') {
       // override the checkpoint's MODEL.DEPTH_NUM for one stage (BASELINE.json configs[0] uses 32 stage-1 hypotheses;
       // CostRegNet is fully convolutional in D).  Forces a re-plan.
@@ -447,10 +447,7 @@ class MvsnetEngine final : public MvsnetIface {
         dc.nsplit = fc.cin == 64 ? 2 : 1;
         dc.hilo = dc.npad <= 32 && fc.cin <= 32 && !(fc.kd == 3 && fc.cin == 32 && fc.cout == 32);
         dc.tc_ok = true;
-        if (vol_in) upload_bimg<TV>(fc, dc); else upload_bimg<TA>(fc, dc);
-        if (fc.kd == 3 && (fc.cout == 1 || fc.cout == 8)) {
-          if (vol_in) upload_bimg_is<TV>(fc, dc); else upload_bimg_is<TA>(fc, dc);
-        }
+        if (vol_in) upload_bimgs<TV>(fc, dc); else upload_bimgs<TA>(fc, dc);
       }
       const bool deconv_ok = fc.transposed && fc.kd == 3 && fc.kh == 3 && fc.kw == 3 &&
                              ((fc.cin == 16 && fc.cout == 8) || (fc.cin == 32 && fc.cout == 16) || (fc.cin == 64 && fc.cout == 32));
@@ -459,12 +456,8 @@ class MvsnetEngine final : public MvsnetIface {
         dc.npad = 8 * fc.cout / dc.nsplit;
         dc.tc_ok = dc.tc_deconv = true;
         std::vector<TA> img;
-        auto cvt = [](float v) -> TA { return from_host<TA>(v); };
-        if (fc.cin == 16) tc::build_b_image_deconv<TA, 16>(fc.w.data(), fc.cin, fc.cout, img, +cvt);
-        else if (fc.cin == 32) tc::build_b_image_deconv<TA, 32>(fc.w.data(), fc.cin, fc.cout, img, +cvt);
-        else tc::build_b_image_deconv<TA, 64>(fc.w.data(), fc.cin, fc.cout, img, +cvt, dc.nsplit);
-        TDM_CUDA(cudaMalloc(&dc.bimg, img.size() * sizeof(TA)));
-        TDM_CUDA(cudaMemcpy(dc.bimg, img.data(), img.size() * sizeof(TA), cudaMemcpyHostToDevice));
+        tc::build_b_image_deconv<TA>(fc.w.data(), fc.cin, fc.cout, img, +from_host<TA>, dc.nsplit);
+        dc.bimg = upload(img);
       }
     }
     if constexpr (sizeof(TA) == 2) {
@@ -481,10 +474,8 @@ class MvsnetEngine final : public MvsnetIface {
         short off[tc::kMaxTaps + 1];
         tc::s2_tap_table(fc.kh, 64, 4096, taps, off);   // only the ORDER matters for the B image
         std::vector<TA> img;
-        auto cvt = [](float v) -> TA { return from_host<TA>(v); };
-        tc::build_b_image_s2<TA>(fc.w.data(), fc.cin, fc.cout, dc.npad_s2, fc.kd, fc.kh, taps, img, +cvt, dc.nsplit_s2);
-        TDM_CUDA(cudaMalloc(&dc.bimg_s2, img.size() * sizeof(TA)));
-        TDM_CUDA(cudaMemcpy(dc.bimg_s2, img.data(), img.size() * sizeof(TA), cudaMemcpyHostToDevice));
+        tc::build_b_image_s2<TA>(fc.w.data(), fc.cin, fc.cout, dc.npad_s2, fc.kd, fc.kh, taps, img, +from_host<TA>, dc.nsplit_s2);
+        dc.bimg_s2 = upload(img);
       }
     }
     convs_[key] = dc;
@@ -532,28 +523,23 @@ class MvsnetEngine final : public MvsnetIface {
     fused_fpn_ = true;
   }
 
-  template <typename TB>
-  void upload_bimg(const FoldedConv& fc, DevConv& dc) {
-    std::vector<TB> img;
-    auto cvt = [](float v) -> TB { return from_host<TB>(v); };
-    auto back = [](TB v) -> float { return to_host<TB>(v); };
-    if (fc.cin == 8) tc::build_b_image<TB, 8>(fc.w.data(), fc.cin, fc.cout, dc.npad, fc.kd, img, +cvt, 1, dc.hilo, +back);
-    else if (fc.cin == 16) tc::build_b_image<TB, 16>(fc.w.data(), fc.cin, fc.cout, dc.npad, fc.kd, img, +cvt, 1, dc.hilo, +back);
-    else if (fc.cin == 32) tc::build_b_image<TB, 32>(fc.w.data(), fc.cin, fc.cout, dc.npad, fc.kd, img, +cvt, 1, dc.hilo, +back);
-    else tc::build_b_image<TB, 64>(fc.w.data(), fc.cin, fc.cout, dc.npad, fc.kd, img, +cvt, dc.nsplit);
-    TDM_CUDA(cudaMalloc(&dc.bimg, img.size() * sizeof(TB)));
-    TDM_CUDA(cudaMemcpy(dc.bimg, img.data(), img.size() * sizeof(TB), cudaMemcpyHostToDevice));
+  template <typename T>
+  static void* upload(const std::vector<T>& img) {
+    void* p = nullptr;
+    TDM_CUDA(cudaMalloc(&p, img.size() * sizeof(T)));
+    TDM_CUDA(cudaMemcpy(p, img.data(), img.size() * sizeof(T), cudaMemcpyHostToDevice));
+    return p;
   }
+  // B images of the stride-1 kernel and, for the 3x3x3 layers with 1 or 8 output channels, of the input-stationary one
   template <typename TB>
-  void upload_bimg_is(const FoldedConv& fc, DevConv& dc) {
+  void upload_bimgs(const FoldedConv& fc, DevConv& dc) {
     std::vector<TB> img;
-    auto cvt = [](float v) -> TB { return from_host<TB>(v); };
-    auto back = [](TB v) -> float { return to_host<TB>(v); };
-    if (fc.cin == 8) tc::build_b_image_is<TB, 8>(fc.w.data(), fc.cin, fc.cout, img, +cvt, +back);
-    else if (fc.cin == 16) tc::build_b_image_is<TB, 16>(fc.w.data(), fc.cin, fc.cout, img, +cvt, +back);
-    else tc::build_b_image_is<TB, 32>(fc.w.data(), fc.cin, fc.cout, img, +cvt, +back);
-    TDM_CUDA(cudaMalloc(&dc.bimg_is, img.size() * sizeof(TB)));
-    TDM_CUDA(cudaMemcpy(dc.bimg_is, img.data(), img.size() * sizeof(TB), cudaMemcpyHostToDevice));
+    tc::build_b_image<TB>(fc.w.data(), fc.cin, fc.cout, dc.npad, fc.kd, img, +from_host<TB>, dc.nsplit, dc.hilo, +to_host<TB>);
+    dc.bimg = upload(img);
+    if (fc.kd == 3 && (fc.cout == 1 || fc.cout == 8)) {
+      tc::build_b_image_is<TB>(fc.w.data(), fc.cin, fc.cout, img, +from_host<TB>, +to_host<TB>);
+      dc.bimg_is = upload(img);
+    }
   }
   template <typename TB> static TB from_host(float v);
   template <typename TB> static float to_host(TB v) { return (float)v; }
@@ -662,7 +648,6 @@ class MvsnetEngine final : public MvsnetIface {
   void free_plan() {
     drop_graph();
     cv_tmap_ok_ = false;
-    s2_cache_.clear();
     tc_cache_.clear();
     for (auto& kv : bufs_) cudaFree(kv.second.p);
     bufs_.clear();
@@ -790,10 +775,16 @@ class MvsnetEngine final : public MvsnetIface {
     TDM_CUDA(cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...));
   }
 
-  // tensor-core kernels are launched with programmatic stream serialization (PDL): their prologue and weight-image
-  // load overlap the tail of the previous kernel (see pdl_wait() in conv_tc.cuh)
-  template <typename Kern, typename... Args>
-  void launch_pdl(Kern kern, dim3 grid, size_t smem, Args... args) {
+  // Tensor-core kernels are launched with programmatic stream serialization (PDL): their prologue and weight-image
+  // load overlap the tail of the previous kernel (see Ring::start in conv_tc.cuh).  Each kernel's shared-memory limit
+  // is raised once, on its first launch.
+  template <auto Kern, typename... Args>
+  void launch_tc(dim3 grid, size_t smem, Args... args) {
+    static bool attr_set = false;
+    if (!attr_set) {
+      TDM_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      attr_set = true;
+    }
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid;
     cfg.blockDim = dim3(tc::kThreads);
@@ -806,22 +797,38 @@ class MvsnetEngine final : public MvsnetIface {
     attr[0].val.programmaticStreamSerializationAllowed = use_pdl_ ? 1 : 0;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    TDM_CUDA(cudaLaunchKernelEx(&cfg, kern, args...));
+    TDM_CUDA(cudaLaunchKernelEx(&cfg, Kern, args...));
   }
 
-  struct TcCache { tc::Plan plan; CUtensorMap tmap; };
+  // Tile plan and input tensor map of one layer's tensor-core launch, made on first use.  Keys: the layer, + "#tail" (prob
+  // with the soft-argmin tail), "#is" / "#is#tail" (input-stationary kernel), "#s2" (stride-2 kernel).
+  struct TcCache { tc::Plan plan; tc::PlanS2 plan_s2; CUtensorMap tmap; };
   std::map<std::string, TcCache> tc_cache_;
 
-  // tensor map over a P8 input: {8 channels, Wp, Hp, channel group * padded planes}, box = one (R+2) x P tile of a plane
-  template <typename TIn, int CIN>
-  CUtensorMap tile_tmap(const std::string& wkey, const DevBuf& in, const tc::Geom& g) {
+  template <typename Make>
+  const TcCache& tc_cached(const std::string& key, Make make) {
+    auto it = tc_cache_.find(key);
+    if (it == tc_cache_.end()) it = tc_cache_.emplace(key, make()).first;
+    return it->second;
+  }
+
+  static void debug_plan(const std::string& wkey, const std::string& what, const tc::Tile& t, int grid, int nsplit, size_t smem) {
+    if (std::getenv("TDM_DEBUG_PLAN"))
+      fprintf(stderr, "[plan] %-14s %s %dx%dx%d -> R %d TW %d DR %d S %d nch %d tiles %d x nsplit %d smem %zu\n", wkey.c_str(), what.c_str(),
+              t.D, t.H, t.W, t.R, t.TW, t.DR, t.S, t.nch, grid, nsplit, smem);
+  }
+
+  // tensor map over a P8 input {8 channels, Wp, Hp, channel group * padded planes}; a box is box_w x box_h positions of
+  // one plane, every estr-th column / row
+  template <typename TIn>
+  CUtensorMap p8_tmap(const std::string& wkey, const DevBuf& in, int cg, int iDp, int box_w, int box_h, int estr) {
     CUtensorMap tmap;
-    const cuuint64_t dims[4] = {8, (cuuint64_t)(in.W + 2), (cuuint64_t)(in.H + 2), (cuuint64_t)g.iDp * (CIN / 8)};
+    const cuuint64_t dims[4] = {8, (cuuint64_t)(in.W + 2), (cuuint64_t)(in.H + 2), (cuuint64_t)iDp * cg};
     const cuuint64_t strides[3] = {16, (cuuint64_t)(in.W + 2) * 16, (cuuint64_t)(in.W + 2) * (in.H + 2) * 16};
-    const cuuint32_t box[4] = {8, (cuuint32_t)g.P, (cuuint32_t)(g.R + 2), 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    const cuuint32_t box[4] = {8, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+    const cuuint32_t es[4] = {1, (cuuint32_t)estr, (cuuint32_t)estr, 1};
     const CUtensorMapDataType dt = std::is_same<TIn, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-    const CUresult r = tc::encode_tiled_fn()(&tmap, dt, 4, in.p, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    const CUresult r = tc::encode_tiled_fn()(&tmap, dt, 4, in.p, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     TDM_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed for " + wkey + " (" + std::to_string((int)r) + ")");
@@ -831,44 +838,32 @@ class MvsnetEngine final : public MvsnetIface {
   // input-stationary 3x3x3 stride-1 conv (conv_tc_is.cuh) of a layer with 8 (CPK 16) or 1 (CPK 8, fp32 plain output) channels
   template <typename TIn, int CIN, int CPK, bool PLAIN, typename Tail = tc::NoTail>
   void tc_is_inst(const std::string& wkey, const DevBuf& in, const DevConv& c, const DevBuf& out, bool relu, const Tail& tail = Tail()) {
-    const std::string key = wkey + (Tail::enabled ? "#is#tail" : "#is");
-    auto it = tc_cache_.find(key);
-    if (it == tc_cache_.end()) {
-      TcCache tcx;
-      tcx.plan = tc::make_plan_is(CIN, CPK, in.D, in.H, in.W, (size_t)tc_smem_kb_ * 1024, Tail::enabled);
-      tc::Geom& g = tcx.plan.g;
+    const TcCache& tcx = tc_cached(wkey + (Tail::enabled ? "#is#tail" : "#is"), [&] {
+      TcCache x{};
+      x.plan = tc::make_plan_is(CIN, CPK, in.D, in.H, in.W, (size_t)tc_smem_kb_ * 1024, Tail::enabled);
+      tc::Geom& g = x.plan.g;
       TDM_CHECK(!Tail::enabled || g.tiles_d == 1, "the prob tail needs tiles that span all depth planes");
       g.iDp = in.D + 2;
       g.relu = relu ? 1 : 0;
       g.cout = c.cout;
-      tcx.tmap = tile_tmap<TIn, CIN>(wkey, in, g);
-      if (std::getenv("TDM_DEBUG_PLAN"))
-        fprintf(stderr, "[plan] %-14s IS cin %d N %d in %dx%dx%d -> R %d TW %d DR %d S %d nch %d tiles %d smem %zu\n", wkey.c_str(), CIN,
-                3 * CPK, in.D, in.H, in.W, g.R, g.TW, g.DR, g.S, g.nch, tcx.plan.grid, tcx.plan.smem);
-      it = tc_cache_.emplace(key, tcx).first;
-    }
-    const tc::Plan& pl = it->second.plan;
+      x.tmap = p8_tmap<TIn>(wkey, in, CIN / 8, g.iDp, g.P, g.R + 2, 1);
+      debug_plan(wkey, "IS cin " + std::to_string(CIN) + " N " + std::to_string(3 * CPK) + " in", g, x.plan.grid, 1, x.plan.smem);
+      return x;
+    });
+    const tc::Plan& pl = tcx.plan;
     if (profiling_) recs_.back().name = wkey + "[tc-is]";   // the record conv() opened as "[tc]"
-    auto kern = tc::k_conv_tc_is<TIn, TA, CIN, CPK, PLAIN, Tail>;
-    static bool attr_set = false;
-    if (!attr_set) {
-      TDM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      attr_set = true;
-    }
-    launch_pdl(kern, dim3(pl.grid), pl.smem, it->second.tmap, (const TIn*)c.bimg_is, (const float*)c.bias,
-               PLAIN ? (TA*)nullptr : (TA*)out.p, PLAIN ? (float*)out.p : (float*)nullptr, pl.g, tail);
+    launch_tc<tc::k_conv_tc_is<TIn, TA, CIN, CPK, PLAIN, Tail>>(dim3(pl.grid), pl.smem, tcx.tmap, (const TIn*)c.bimg_is, (const float*)c.bias,
+                                                               PLAIN ? (TA*)nullptr : (TA*)out.p, PLAIN ? (float*)out.p : (float*)nullptr, pl.g, tail);
   }
 
   template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool PLAIN, int MODE = 0, bool HILO = false, typename Tail = tc::NoTail>
   void tc_inst(const std::string& wkey, const DevBuf& in, const DevConv& c, const DevBuf* res, const DevBuf& out, bool relu,
                const Tail& tail = Tail()) {
-    const std::string key = wkey + (Tail::enabled ? "#tail" : "");
-    auto it = tc_cache_.find(key);
-    if (it == tc_cache_.end()) {
-      TcCache tcx;
-      tcx.plan = tc::make_plan(CIN, HILO ? 2 * NPAD : NPAD, KD, in.D, in.H, in.W, in.pd, MODE, (size_t)tc_smem_kb_ * 1024,   // tiles live on the INPUT grid
-                               Tail::enabled);
-      tc::Geom& g = tcx.plan.g;
+    const TcCache& tcx = tc_cached(wkey + (Tail::enabled ? "#tail" : ""), [&] {
+      TcCache x{};
+      x.plan = tc::make_plan(CIN, HILO ? 2 * NPAD : NPAD, KD, in.D, in.H, in.W, in.pd, MODE, (size_t)tc_smem_kb_ * 1024,   // tiles live on the INPUT grid
+                             Tail::enabled);
+      tc::Geom& g = x.plan.g;
       TDM_CHECK(!Tail::enabled || g.tiles_d == 1, "the prob tail needs tiles that span all depth planes");
       g.oHp = out.H + 2; g.oWp = out.W + 2; g.opd = out.pd;
       g.iDp = in.D + 2 * in.pd;
@@ -880,13 +875,12 @@ class MvsnetEngine final : public MvsnetIface {
         g.out_gs = p8<TOut>(out).gs;
         if (res) g.res_gs = p8<const TOut>(*res).gs;
       }
-      tcx.tmap = tile_tmap<TIn, CIN>(wkey, in, g);
-      if (std::getenv("TDM_DEBUG_PLAN"))
-        fprintf(stderr, "[plan] %-14s mode %d cin %d N %d kd %d in %dx%dx%d -> R %d TW %d DR %d S %d nch %d tiles %d x nsplit %d smem %zu\n", wkey.c_str(), MODE, CIN,
-                HILO ? 2 * NPAD : NPAD, KD, in.D, in.H, in.W, g.R, g.TW, g.DR, g.S, g.nch, tcx.plan.grid, c.nsplit, tcx.plan.smem);
-      it = tc_cache_.emplace(key, tcx).first;
-    }
-    const tc::Plan& pl = it->second.plan;
+      x.tmap = p8_tmap<TIn>(wkey, in, CIN / 8, g.iDp, g.P, g.R + 2, 1);
+      debug_plan(wkey, "mode " + std::to_string(MODE) + " cin " + std::to_string(CIN) + " N " + std::to_string(HILO ? 2 * NPAD : NPAD) +
+                 " kd " + std::to_string(KD) + " in", g, x.plan.grid, c.nsplit, x.plan.smem);
+      return x;
+    });
+    const tc::Plan& pl = tcx.plan;
     TOut* op = nullptr;
     float* plain = nullptr;
     const TOut* rp = nullptr;
@@ -896,56 +890,31 @@ class MvsnetEngine final : public MvsnetIface {
       op = (TOut*)out.p;
       if (res) rp = (const TOut*)res->p;
     }
-    auto kern = tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail>;
-    static bool attr_set = false;
-    if (!attr_set) {
-      TDM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      attr_set = true;
-    }
-    launch_pdl(kern, dim3(pl.grid, c.nsplit), pl.smem, it->second.tmap, (const TIn*)c.bimg, (const float*)c.bias, rp, op, plain, pl.g, tail);
+    launch_tc<tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail>>(dim3(pl.grid, c.nsplit), pl.smem, tcx.tmap, (const TIn*)c.bimg,
+                                                                              (const float*)c.bias, rp, op, plain, pl.g, tail);
   }
-
-  struct S2Cache { tc::PlanS2 plan; CUtensorMap tmap; };
-  std::map<std::string, S2Cache> s2_cache_;
 
   template <int CIN, int NPAD, int KD, int KS>
   void tc_s2_inst(const std::string& wkey, const DevBuf& in, const DevConv& c, const DevBuf& out, bool relu) {
-    auto it = s2_cache_.find(wkey);
-    if (it == s2_cache_.end()) {
-      S2Cache sc;
-      sc.plan = tc::make_plan_s2(CIN, NPAD, KD, KS, out.D, out.H, out.W, (size_t)tc_smem_kb_ * 1024);
-      tc::GeomS2& g = sc.plan.g;
-      const P8<TA> po = p8<TA>(out);
-      g.oHp = out.H + 2; g.oWp = out.W + 2; g.opd = out.pd; g.out_gs = po.gs;
-      g.ipd = in.pd; g.iDp = in.D + 2 * in.pd;
+    const TcCache& tcx = tc_cached(wkey + "#s2", [&] {
+      TcCache x{};
+      x.plan_s2 = tc::make_plan_s2(CIN, NPAD, KD, KS, out.D, out.H, out.W, (size_t)tc_smem_kb_ * 1024);
+      tc::GeomS2& g = x.plan_s2.g;
+      g.oHp = out.H + 2; g.oWp = out.W + 2; g.opd = out.pd; g.out_gs = p8<TA>(out).gs;
+      g.iDp = in.D + 2 * in.pd;
       g.c0 = 1 - KS / 2;
       g.relu = relu ? 1 : 0;
       g.cout = c.cout;
       std::vector<std::pair<int, int>> taps;
-      tc::s2_tap_table(KS, g.P, g.sub_pos, taps, g.tap_off);
-      // tensor map over the P8 input: dims {8 ch, Wp, Hp, groups*planes}, every second column / row per box
-      const cuuint64_t dims[4] = {8, (cuuint64_t)(in.W + 2), (cuuint64_t)(in.H + 2), (cuuint64_t)g.iDp * (CIN / 8)};
-      const cuuint64_t strides[3] = {16, (cuuint64_t)(in.W + 2) * 16, (cuuint64_t)(in.W + 2) * (in.H + 2) * 16};
-      const cuuint32_t box[4] = {8, (cuuint32_t)(2 * g.P), (cuuint32_t)(2 * g.RR), 1};
-      const cuuint32_t estr[4] = {1, 2, 2, 1};
-      const CUtensorMapDataType dt = std::is_same<TA, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-      const CUresult r = tc::encode_tiled_fn()(&sc.tmap, dt, 4, in.p, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      TDM_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed for " + wkey + " (" + std::to_string((int)r) + ")");
-      if (std::getenv("TDM_DEBUG_PLAN"))
-        fprintf(stderr, "[plan] %-14s S2 cin %d N %d kd %d ks %d out %dx%dx%d -> R %d TW %d DR %d S %d nch %d tiles %d x nsplit %d smem %zu\n", wkey.c_str(), CIN, NPAD, KD, KS,
-                out.D, out.H, out.W, g.R, g.TW, g.DR, g.S, g.nch, sc.plan.grid, c.nsplit_s2, sc.plan.smem);
-      it = s2_cache_.emplace(wkey, sc).first;
-    }
-    auto kern = tc::k_conv_tc_s2<TA, TA, CIN, NPAD, KD, KS>;
-    static bool attr_set = false;
-    if (!attr_set) {
-      TDM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      attr_set = true;
-    }
-    const tc::PlanS2& pl = it->second.plan;
-    launch_pdl(kern, dim3(pl.grid, c.nsplit_s2), pl.smem, it->second.tmap, (const TA*)c.bimg_s2, (const float*)c.bias, (TA*)out.p, pl.g);
+      tc::s2_tap_table(KS, g.P, g.slot_pos, taps, g.tap_off);
+      x.tmap = p8_tmap<TA>(wkey, in, CIN / 8, g.iDp, 2 * g.P, 2 * g.RR, 2);   // every second column / row per box
+      debug_plan(wkey, "S2 cin " + std::to_string(CIN) + " N " + std::to_string(NPAD) + " kd " + std::to_string(KD) + " ks " + std::to_string(KS) + " out",
+                 g, x.plan_s2.grid, c.nsplit_s2, x.plan_s2.smem);
+      return x;
+    });
+    const tc::PlanS2& pl = tcx.plan_s2;
+    launch_tc<tc::k_conv_tc_s2<TA, TA, CIN, NPAD, KD, KS>>(dim3(pl.grid, c.nsplit_s2), pl.smem, tcx.tmap, (const TA*)c.bimg_s2,
+                                                          (const float*)c.bias, (TA*)out.p, pl.g);
   }
 
   bool conv_tc_s2_dispatch(const std::string& wkey, const DevBuf& bi, const DevConv& c, const DevBuf& bo, bool relu) {
@@ -1612,7 +1581,7 @@ void debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int
     TDM_CHECK((kd == 1 || kd == 3) && (pd == 3 || pd == 5), "mode 400: kd must be 1 or 3 and pd the kernel size 3 or 5");
     const tc::PlanS2 p = tc::make_plan_s2(cin, npad, kd, pd, D, H, W, (size_t)smem_kb * 1024);
     const tc::GeomS2& g = p.g;
-    const long long v[12] = {g.S, g.R, g.TW, g.P, g.DR, g.nch, g.sub_pos, g.tiles_w, g.tiles_h, g.tiles_d, p.grid, (long long)p.smem};
+    const long long v[12] = {g.S, g.R, g.TW, g.P, g.DR, g.nch, g.slot_pos, g.tiles_w, g.tiles_h, g.tiles_d, p.grid, (long long)p.smem};
     for (int i = 0; i < 12; ++i) out12[i] = v[i];
     return;
   }

@@ -104,10 +104,11 @@ def test_mesh_axis_tables_match_a_float32_restatement():
         assert covered == n
 
 
-def test_tcgen05_tile_planner_invariants():
-    """Host logic of the tensor-core convolutions (no GPU): for every layer shape of the benchmark config (640x480, 7 views,
+def test_wgmma_tile_planner_invariants():
+    """Host logic of the wgmma convolutions (no GPU): for every layer shape of the benchmark config (640x480, 7 views,
     (48,32,8)) and of the small config-1 windows the planner returns a tiling that covers the grid, fits 225 KB of shared
-    memory, the wgmma N limit and the TMA box limit."""
+    memory, the wgmma N limit and the TMA box limit.  Stride-2 plans (mode 400) read sub-tiles of pitch P = TW + KS/2,
+    whose TMA boxes span 2 * P columns."""
     l = lib()
     out = (ctypes.c_longlong * 12)()
     shapes = []
@@ -115,6 +116,10 @@ def test_tcgen05_tile_planner_invariants():
         # FeatureNet: 2-D convs over V planes (kd = 1, pd = 0)
         for cin, npad, sc in [(8, 32, 1), (16, 32, 2), (32, 64, 4), (32, 32, 2), (32, 32, 1)]:
             shapes.append((cin, npad, 1, V, H // sc, W // sc, 0, 0))
+        shapes.append((32, 64, 1, V, H // 2, W // 2, 0, 3))                 # f.out3a: up-2 conv on the coarse grid
+        # conv1.0 / conv2.0: 5x5 stride 2 (pd carries the kernel size, D H W are the output dims)
+        for cin, npad, sc in [(8, 16, 2), (16, 32, 4)]:
+            shapes.append((cin, npad, 1, V, H // sc, W // sc, 5, 400))
         for s, D in enumerate(Ds):
             sc = 4 >> s
             h, w = H // sc, W // sc
@@ -128,15 +133,27 @@ def test_tcgen05_tile_planner_invariants():
             for lvl, (cin, npad) in enumerate([(16, 64), (32, 128), (64, 64)]):
                 d2, h2, w2 = max(D >> (lvl + 1), 1), h >> (lvl + 1), w >> (lvl + 1)
                 shapes.append((cin, npad, 2, d2, h2, w2, 1, 1))             # conv11 / conv9 / conv7 (transposed as GEMM)
+            for lvl, (cin, npad) in enumerate([(8, 16), (16, 32), (32, 32)]):
+                d2, h2, w2 = max(D >> (lvl + 1), 1), h >> (lvl + 1), w >> (lvl + 1)
+                shapes.append((cin, npad, 3, d2, h2, w2, 3, 400))           # conv1 / conv3 / conv5: 3x3x3 stride 2
     assert len(shapes) > 40
     for (cin, npad, kd, D, H, W, pd, mode) in shapes:
         rc = l.tdm_debug_conv_plan(cin, npad, kd, D, H, W, pd, mode, 225, out)
         assert rc == 0, (cin, npad, kd, D, H, W, mode, l.tdm_last_error())
         S, R, TW, P, DR, nch, slot_pos, tw, th, td, grid, smem = [int(x) for x in out]
-        if mode >= 100:
+        if mode >= 100 and mode != 400:
             assert td == 1 and DR == D, (D, H, W, DR, td)
             mode -= 100
         key = (cin, npad, kd, D, H, W, mode)
+        if mode == 400:
+            ks = pd
+            # 4 parity sub-tiles per channel group, each (R + KS/2) rows of P positions, and the A reads of the last chunk
+            assert P == TW + ks // 2 and 2 * P <= 256 and R >= 1 and DR >= 1 and 2 <= S <= 5, key
+            assert tw * TW >= W and (tw - 1) * TW < W and th * R >= H and (th - 1) * R < H and td * DR >= D and (td - 1) * DR < D, key
+            assert grid == tw * th * td and grid >= 1 and nch == (R * P + 127) // 128, key
+            assert slot_pos % 8 == 0 and slot_pos >= (R + ks // 2) * P and slot_pos >= nch * 128 + (ks // 2) * (P + 1), key
+            assert smem <= 225 * 1024 and 4 * slot_pos <= 32767, key
+            continue
         assert P == TW + 2 and P <= 256 and R >= 1 and DR >= 1 and 2 <= S <= 4, key
         assert tw * TW >= W and (tw - 1) * TW < W and th * R >= H and (th - 1) * R < H and td * DR >= D and (td - 1) * DR < D, key
         assert grid == tw * th * td and grid >= 1, key
