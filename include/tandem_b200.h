@@ -218,17 +218,11 @@ long long tdm_fusion_dump_blocks(tdm_fusion* h, int* coords, void* voxels, size_
  * tdm_fusion_last_alloc_ms: the allocation kernel's share of ms_integrate, per iteration. */
 int tdm_fusion_run_resident(tdm_fusion* h, int iters, float* ms_integrate, float* ms_render);
 int tdm_fusion_last_alloc_ms(tdm_fusion* h, float* ms);
-/* A/B switches for measurements (results are bit-identical either way): "alloc_filter" (CTA-level shared-memory filter in
- * front of the hash table during allocation), "raycast_cache8" (8-entry per-ray block cache); both default to 0 (the table
- * probes are L2 hits behind other latency); "raycast_persistent" (warps pull rays from a
- * counter and refill finished lanes; default 0 = one ray per thread), "raycast_shared" (index arithmetic shared between the nine voxel reads of a sample, one block lookup when they sit in one
- * block; default 1), "integrate_compact" (visibility pass + update of the
- * visible blocks only, default 1; 0 = every CTA scans the whole block list); "raycast_tile" (0: 16x16-pixel CTAs, 1: 8x8
- * (default), 2: 8x4, 3: 16x8); "raycast_dedup" (a sample whose eight corners straddle voxel-block faces looks every distinct
- * block up once instead of corner by corner; default 1: 0.31 vs 0.38 ms); "fast_div" (constant-divisor FMA division in the
- * ray-cast, exhaustively checked correctly rounded; default 0: 0.316 vs 0.311 ms); "occ_skip" (dilated block-occupancy bitmap
- * in front of the sampler; default 0: 0.330 vs 0.311 ms, a frustum-allocated map has no unallocated space on a ray's way);
- * "slab_clip" / "slab_exchange" (Z-slab volumes, see above). */
+/* Options.  "raycast_shared" (default 1: the production ray-cast, index arithmetic shared between the nine voxel reads of a
+ * sample, one block lookup per distinct block; 0: the comparator shaped after the reference's sampler, one hash lookup per
+ * voxel read) and "fast_div" (constant-divisor FMA division in the production ray-cast, exhaustively checked correctly
+ * rounded; default 0) leave every rendered bit unchanged; "slab_clip" / "slab_exchange" (Z-slab volumes, see above).  Any
+ * other name fails with "unknown fusion option". */
 int tdm_fusion_set_option(tdm_fusion* h, const char* name, int value);
 
 /* ------------------------------------------------------------------------------------------------

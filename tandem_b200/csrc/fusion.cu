@@ -15,6 +15,8 @@
 //                 allocated; per-axis index arithmetic shared by the nine voxel reads of a sample, ONE hash probe per
 //                 distinct voxel block of a sample (one-entry pointer cache in front), division-free bucket index,
 //                 colour blend only for the final hit.  Every sample sits where the reference's march puts it.
+//                 k_raycast (option "raycast_shared" = 0) is the comparator: the reference's sampler voxel by voxel, one
+//                 hash probe per voxel read; the production kernel must render the same volume bit for bit.
 // The hash function, bucket structure (full bucket -> block dropped), voxel record (8 B) and all geometry are
 // the reference's; geometry that decides integers uses __f*_rn intrinsics so it is bit-identical to the CPU
 // oracle (oracle/tsdf_oracle.c) which evaluates the same expressions without FMA contraction.
@@ -54,7 +56,6 @@ struct FusionDev {
   float half_vs;             // RN(voxel_size / 2.0f): the sampler's half-voxel shift (tsdf_volume.cu:166), a per-volume constant
   unsigned long long mod_magic;   // ceil(2^64 / num_buckets): exact 32-bit remainder without a division (fast_umod)
   unsigned mod_c32;               // 2^32 mod num_buckets
-  unsigned* occ;             // [128*128*4] dilated block-occupancy bitmap of the blocks THIS volume stores (occ_mark below)
   // Interleaved Z-slab partition (il_k > 0): block z belongs to rank ((z - il_z0) div il_k) mod il_world; a rank STORES its own
   // blocks plus one halo block on either side of each of its slabs.  Thin interleaved slabs keep the per-frame work of every
   // rank proportional to 1 / world for ANY view direction (contiguous slabs only balance memory: a camera looking along a slab
@@ -122,16 +123,6 @@ __device__ __forceinline__ float3 get_point3d(const tdm_fusion_options& o, int i
   p.y = div_(mul_(sub_((float)v, o.cy), p.z), o.fy);
   return p;
 }
-template <bool FAST>
-__device__ __forceinline__ float3 get_point3d_c(const FusionDev& d, int i, float depth) {  // get_point3d with constant-divisor division
-  const tdm_fusion_options& o = d.o;
-  const int v = i / o.width, u = i - o.width * v;
-  float3 p;
-  p.z = depth;
-  p.x = cdiv_<FAST>(mul_(sub_((float)u, o.cx), p.z), o.fx, d.r_fx);
-  p.y = cdiv_<FAST>(mul_(sub_((float)v, o.cy), p.z), o.fy, d.r_fy);
-  return p;
-}
 // the same with the pixel terms (u - cx), (v - cy) - loop invariants of a ray - computed once by the caller (same operations)
 template <bool FAST>
 __device__ __forceinline__ float3 get_point3d_px(const FusionDev& d, float ucx /* sub_(u, cx) */, float vcy /* sub_(v, cy) */, float depth) {
@@ -176,75 +167,33 @@ __device__ __forceinline__ long long hash_bucket(const FusionDev& d, int x, int 
   return (long long)hash_slot(x, y, z, d.o.num_buckets, d.mod_magic, d.mod_c32) * d.o.bucket_size;
 }
 
-// Dilated block-occupancy bitmap (the ray-cast's empty-space test).  One bit per block coordinate modulo 128 per axis
-// (word = x7 << 9 | y7 << 2 | z7 >> 5, bit = z7 & 31; 256 KB, L2- and mostly L1-resident).  Allocating block (x,y,z) sets the
-// bits of its 27 neighbours (x,y,z) + {-1,0,1}^3, so a CLEAR bit at c proves that no block within one block of c - in any alias
-// of c modulo 128 - is stored in this volume.  Bits are never cleared (blocks are never freed); aliasing and dilation only
-// make the test conservative.  The ray-cast asks for the bit of the block that an APPROXIMATE sample position falls into:
-// the exact centre voxel of a sample sits at most 1/16 block outside the block of the exact position (round-half-away,
-// tsdf_volume.cu:109-113), and the launch refuses the shortcut unless the linear ray model is good to 0.4 block, so the
-// exact centre voxel's block is one of the 27 - a clear bit means the sample reads "no voxel" and steps by tau.
-constexpr int kOccWords = 128 * 128 * 4;
-__device__ __forceinline__ unsigned occ_word(int bx, int by, int bz) {
-  return ((unsigned)(bx & 127) << 9) | ((unsigned)(by & 127) << 2) | ((unsigned)(bz & 127) >> 5);
-}
-__device__ __forceinline__ void occ_mark(const FusionDev& d, int x, int y, int z) {
-#pragma unroll
-  for (int dx = -1; dx <= 1; ++dx)
-#pragma unroll
-    for (int dy = -1; dy <= 1; ++dy)
-#pragma unroll
-      for (int dz = -1; dz <= 1; ++dz) {
-        unsigned* w = d.occ + occ_word(x + dx, y + dy, z + dz);
-        const unsigned bit = 1u << ((z + dz) & 31);
-        if (!(*w & bit)) atomicOr(w, bit);   // a stale read only costs a redundant atomic
-      }
-}
-
-// returns true when the block is in the table after the call (found or inserted), false when it was rejected / dropped
-__device__ bool insert_block(const FusionDev& d, int x, int y, int z) {
-  if (x <= -kKeyBias || x >= kKeyBias || y <= -kKeyBias || y >= kKeyBias || z <= -kKeyBias || z >= kKeyBias) return false;
-  if (!slab_stores(d, z)) return false;   // another rank's Z-slab
+__device__ void insert_block(const FusionDev& d, int x, int y, int z) {
+  if (x <= -kKeyBias || x >= kKeyBias || y <= -kKeyBias || y >= kKeyBias || z <= -kKeyBias || z >= kKeyBias) return;
+  if (!slab_stores(d, z)) return;   // another rank's Z-slab
   const unsigned long long key = pack_key(x, y, z);
   const long long b = hash_bucket(d, x, y, z);
   for (int i = 0; i < d.o.bucket_size; ++i) {
     unsigned long long cur = d.keys[b + i];
-    if (cur == key) return true;
+    if (cur == key) return;
     if (cur == kEmptyKey) {
       cur = atomicCAS(&d.keys[b + i], kEmptyKey, key);
-      if (cur == key) return true;      // somebody else inserted the same block
+      if (cur == key) return;           // somebody else inserted the same block
       if (cur == kEmptyKey) {           // we own the slot: take a voxel block and publish it in the list
         const int ptr = atomicAdd(&d.counters[0], 1);
         if (ptr >= d.o.num_blocks) {    // heap exhausted (heap.cu:16-18 aborts; we drop and count)
           atomicAdd(&d.counters[1], 1);
           d.ptrs[b + i] = -1;
-          return false;
+          return;
         }
         d.ptrs[b + i] = ptr;
         d.list[ptr] = make_int4(x, y, z, ptr);
         atomicAdd(&d.counters[3], 1);
-        occ_mark(d, x, y, z);
-        return true;
+        return;
       }
       // slot taken by a different block in the meantime: keep scanning
     }
   }
   atomicAdd(&d.counters[1], 1);  // bucket full: block dropped (hash_table.cu:103-115 returns without allocating)
-  return false;
-}
-
-// CTA-level filter in front of the table: the 128 rays of a CTA are neighbours and walk through the same few hundred blocks,
-// so most insert attempts are repeats.  Direct-mapped set of keys KNOWN to be in the table (only successful inserts / finds
-// are remembered, so drops are still counted per attempt as in the reference); races between threads are benign.
-constexpr int kAllocFilter = 1024;
-template <bool FILTER>
-__device__ __forceinline__ void insert_filtered(const FusionDev& d, unsigned long long* sfilter, int x, int y, int z) {
-  if (!FILTER) { insert_block(d, x, y, z); return; }
-  const unsigned long long key = pack_key(x, y, z);
-  const unsigned h = ((unsigned)x * 73856093u ^ (unsigned)y * 19349669u ^ (unsigned)z * 83492791u);
-  const int slot = (int)((h ^ (h >> 11)) & (kAllocFilter - 1));
-  if (sfilter[slot] == key) return;
-  if (insert_block(d, x, y, z)) sfilter[slot] = key;
 }
 
 __device__ __forceinline__ int find_in(const unsigned long long* __restrict__ keys, const int* __restrict__ ptrs, const FusionDev& d,
@@ -262,16 +211,10 @@ __device__ __forceinline__ int find_in(const unsigned long long* __restrict__ ke
 __device__ __forceinline__ int find_block(const FusionDev& d, int x, int y, int z) { return find_in(d.keys, d.ptrs, d, x, y, z); }
 
 // ---------------------------------------------------------------------------------------------- K5
-template <bool FILTER>
 __global__ void __launch_bounds__(128) k_allocate(FusionDev d, const float* __restrict__ depth, Mat4 T) {
   const tdm_fusion_options& o = d.o;
   const int n = o.height * o.width;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  __shared__ unsigned long long sfilter[FILTER ? kAllocFilter : 1];
-  if (FILTER) {
-    for (int k = threadIdx.x; k < kAllocFilter; k += blockDim.x) sfilter[k] = kEmptyKey;
-    __syncthreads();
-  }
   if (i >= n) return;
   const float dz = depth[i];
   if (dz < o.min_sensor_depth || dz > o.max_sensor_depth) return;
@@ -311,8 +254,8 @@ __global__ void __launch_bounds__(128) k_allocate(FusionDev d, const float* __re
       if (hi[a] > d.bbox[3 + a]) atomicMax(&d.bbox[3 + a], hi[a]);
     }
   }
-  insert_filtered<FILTER>(d, sfilter, bp.x, bp.y, bp.z);
-  if (neg) { bp.x += diff.x; bp.y += diff.y; bp.z += diff.z; insert_filtered<FILTER>(d, sfilter, bp.x, bp.y, bp.z); }
+  insert_block(d, bp.x, bp.y, bp.z);
+  if (neg) { bp.x += diff.x; bp.y += diff.y; bp.z += diff.z; insert_block(d, bp.x, bp.y, bp.z); }
   int guard = 0;
   while ((bp.x != be.x || bp.y != be.y || bp.z != be.z) && guard++ < 100000) {
     if (mt.x < mt.y) {
@@ -320,7 +263,7 @@ __global__ void __launch_bounds__(128) k_allocate(FusionDev d, const float* __re
     } else {
       if (mt.y < mt.z) { bp.y += step.y; mt.y = add_(mt.y, dt.y); } else { bp.z += step.z; mt.z = add_(mt.z, dt.z); }
     }
-    insert_filtered<FILTER>(d, sfilter, bp.x, bp.y, bp.z);
+    insert_block(d, bp.x, bp.y, bp.z);
   }
 }
 
@@ -341,56 +284,9 @@ __device__ __forceinline__ uint2 combine(uint2 v, float nsdf, const unsigned cha
   return make_uint2(__float_as_uint(sdf), out | ((unsigned)nw << 24));
 }
 
-__global__ void __launch_bounds__(256)
-k_integrate(FusionDev d, const unsigned char* __restrict__ bgr, const float* __restrict__ depth, Mat4 Ti) {
-  const tdm_fusion_options& o = d.o;
-  const int nblocks = min(d.counters[0], o.num_blocks);
-  const float vs = o.voxel_size, tau = o.truncation_distance;
-  const int B = 8;
-  for (int b = blockIdx.x; b < nblocks; b += gridDim.x) {
-    const int4 e = d.list[b];
-    const float3 pos = make_float3(mul_(mul_((float)e.x, vs), (float)B), mul_(mul_((float)e.y, vs), (float)B),
-                                   mul_(mul_((float)e.z, vs), (float)B));
-    const float3 pc = xform(Ti, pos);
-    if (pc.z < 0) continue;
-    const double half = 0.5 * (double)vs * (double)B;  // double as written in the reference (tsdf_volume.cu:460-463)
-    const float3 ctr = make_float3((float)((double)pc.x + half), (float)((double)pc.y + half), (float)((double)pc.z + half));
-    int2 px = project(o, ctr);
-    if (!(px.x >= 0 && px.y >= 0 && px.x < o.width && px.y < o.height)) continue;
-    if (threadIdx.x == 0) atomicAdd(&d.counters[2], 1);
-    // thread t owns voxels (bx,by,bz0) and (bx,by,bz0+1): adjacent in memory (index x*64+y*8+z)
-    const int t = threadIdx.x;
-    const int bx = t >> 5, by = (t >> 2) & 7, bz0 = (t & 3) * 2;
-    uint4* vp = reinterpret_cast<uint4*>(d.voxels + (size_t)e.w * 512 + bx * 64 + by * 8 + bz0);
-    uint4 raw = *vp;
-    uint2 vox[2] = {make_uint2(raw.x, raw.y), make_uint2(raw.z, raw.w)};
-    bool dirty = false;
-#pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      const float3 vw = make_float3(add_(pos.x, mul_((float)bx, vs)), add_(pos.y, mul_((float)by, vs)),
-                                    add_(pos.z, mul_((float)(bz0 + k), vs)));
-      const float3 vc = xform(Ti, vw);
-      if (vc.z == 0.0f) continue;
-      px = project(o, vc);
-      if (!(px.x >= 0 && px.y >= 0 && px.x < o.width && px.y < o.height)) continue;
-      const int idx = px.y * o.width + px.x;
-      const float dz = depth[idx];
-      if (dz <= 0 || dz < o.min_sensor_depth || dz > o.max_sensor_depth) continue;
-      const float sd = norm3(get_point3d(o, idx, dz)), vd = norm3(vc);
-      float nsdf;
-      if (vd > sub_(sd, tau) && vd < add_(sd, tau) && dz < o.max_sensor_depth) nsdf = sub_(sd, vd);
-      else if (vd < sub_(sd, tau)) nsdf = tau;
-      else continue;
-      vox[k] = combine(vox[k], nsdf, bgr + 3 * (size_t)idx, o.max_sdf_weight);
-      dirty = true;
-    }
-    if (dirty) *vp = make_uint4(vox[0].x, vox[0].y, vox[1].x, vox[1].y);
-  }
-}
-
-// K6, two-step form: only ~10 % of the allocated blocks are in view of a scan, and the map grows with every keyframe, so the
-// visibility test runs once per block in its own kernel (thread per block, warp-aggregated append to a compact list) and the
-// voxel update visits the visible blocks only.  Same expressions as k_integrate -> bit-identical voxels.
+// Only ~10 % of the allocated blocks are in view of a scan, and the map grows with every keyframe, so the visibility test runs
+// once per block in its own kernel (thread per block, warp-aggregated append to a compact list) and the voxel update visits
+// the visible blocks only.
 __global__ void __launch_bounds__(256) k_visible(FusionDev d, Mat4 Ti, int* __restrict__ vis_list) {
   const tdm_fusion_options& o = d.o;
   const int nblocks = min(d.counters[0], o.num_blocks);
@@ -456,12 +352,8 @@ k_integrate_list(FusionDev d, const unsigned char* __restrict__ bgr, const float
 }
 
 // ---------------------------------------------------------------------------------------------- K7
-// Per-ray block caches in front of the hash table.
-//  Cache1: the last block only.
-//  Cache8: eight entries, direct-mapped by the parity of the block coordinate (slot = x&1 | (y&1)<<1 | (z&1)<<2).  The nine
-//          voxel reads of one trilinear sample span at most two blocks per axis, which always land in different slots, so
-//          a sample never evicts what it still needs and a ray only probes the table when it ENTERS a block.
-//          Lives in shared memory (column per thread, conflict-free).
+// Per-ray last-block caches in front of the hash table.
+//  Cache1: the block index, for the reference-shaped comparator k_raycast.
 struct Cache1 {
   int x, y, z, ptr;
   __device__ __forceinline__ void init() { x = y = z = INT_MIN; ptr = -1; }
@@ -469,15 +361,9 @@ struct Cache1 {
     if (bx != x || by != y || bz != z) { x = bx; y = by; z = bz; ptr = find_block(d, bx, by, bz); }
     return ptr;
   }
-  __device__ __forceinline__ const uint2* block(const FusionDev& d, int bx, int by, int bz) {   // base of the 512-voxel block or null
-    const int p = find(d, bx, by, bz);
-    return p < 0 ? nullptr : d.voxels + (size_t)p * 512;
-  }
-  __device__ __forceinline__ bool holds(int bx, int by, int bz) const { return bx == x && by == y && bz == z; }
-  __device__ __forceinline__ const uint2* held(const FusionDev& d) const { return ptr < 0 ? nullptr : d.voxels + (size_t)ptr * 512; }
 };
 // Cache1 holding the block's BASE POINTER: a hit costs the three compares only (ncu: re-deriving voxels + ptr * 512 on every
-// hit was 4.5 % of the ray-cast's instructions).  Used by the production ray-cast; Cache1 stays with the reference-shaped kernels.
+// hit was 4.5 % of the ray-cast's instructions).  Used by the production ray-cast.
 struct Cache1P {
   int x, y, z;
   const uint2* base;
@@ -515,27 +401,7 @@ struct CachePeer {
   __device__ __forceinline__ bool holds(int bx, int by, int bz) const { return bx == x && by == y && bz == z; }
   __device__ __forceinline__ const uint2* held(const FusionDev&) const { return base; }
 };
-struct Cache8 {
-  unsigned long long* keys;   // [8][256] in shared memory, this thread's column
-  int* ptrs;
-  __device__ __forceinline__ void init() {
-#pragma unroll
-    for (int k = 0; k < 8; ++k) keys[k * 256] = kEmptyKey;
-  }
-  __device__ __forceinline__ int find(const FusionDev& d, int bx, int by, int bz) {
-    if (bx <= -kKeyBias || bx >= kKeyBias || by <= -kKeyBias || by >= kKeyBias || bz <= -kKeyBias || bz >= kKeyBias) return -1;
-    const int slot = ((bx & 1) | ((by & 1) << 1) | ((bz & 1) << 2)) * 256;
-    const unsigned long long key = pack_key(bx, by, bz);
-    if (keys[slot] == key) return ptrs[slot];
-    const int p = find_block(d, bx, by, bz);
-    keys[slot] = key;
-    ptrs[slot] = p;
-    return p;
-  }
-};
-
-template <class Cache>
-__device__ __forceinline__ uint2 get_voxel(const FusionDev& d, float3 p, Cache& bc) {  // tsdf_volume.cu:109-159
+__device__ __forceinline__ uint2 get_voxel(const FusionDev& d, float3 p, Cache1& bc) {  // tsdf_volume.cu:109-159
   const float s = d.o.voxel_size;
   const int gx = (int)add_(div_(p.x, s), mul_((float)sgn(p.x), 0.5f));
   const int gy = (int)add_(div_(p.y, s), mul_((float)sgn(p.y), 0.5f));
@@ -545,8 +411,7 @@ __device__ __forceinline__ uint2 get_voxel(const FusionDev& d, float3 p, Cache& 
   return __ldg(d.voxels + (size_t)ptr * 512 + (gx & 7) * 64 + (gy & 7) * 8 + (gz & 7));
 }
 
-template <class Cache>
-__device__ uint2 get_interpolated(const FusionDev& d, float3 p, Cache& bc) {  // tsdf_volume.cu:161-289
+__device__ uint2 get_interpolated(const FusionDev& d, float3 p, Cache1& bc) {  // tsdf_volume.cu:161-289
   const uint2 v0 = get_voxel(d, p, bc);
   if ((v0.y >> 24) == 0) return v0;
   const float s = d.o.voxel_size;
@@ -592,7 +457,7 @@ __device__ __forceinline__ uint2 voxel_at(const FusionDev& d, int gx, int gy, in
 }
 // COLOR = false: the marching steps only consume the interpolated sdf and the centre voxel's weight; the colour blend (8 corners
 // x 3 channels of unpack / convert / multiply-add: a fifth of the sample's instructions) is only evaluated for the final hit.
-template <class Cache, bool COLOR = true, bool FAST = false, bool DEDUP = true>
+template <class Cache, bool COLOR, bool FAST>
 __device__ uint2 get_interpolated_shared(const FusionDev& d, float3 p, Cache& bc) {
   const float s = d.o.voxel_size, rs = d.r_vs;
   const float3 vp = make_float3(cdiv_<FAST>(p.x, s, rs), cdiv_<FAST>(p.y, s, rs), cdiv_<FAST>(p.z, s, rs));
@@ -619,7 +484,7 @@ __device__ uint2 get_interpolated_shared(const FusionDev& d, float3 p, Cache& bc
       c[0] = __ldg(b); c[1] = __ldg(b + 64); c[2] = __ldg(b + 8); c[3] = __ldg(b + 1);
       c[4] = __ldg(b + 72); c[5] = __ldg(b + 9); c[6] = __ldg(b + 65); c[7] = __ldg(b + 73);
     }
-  } else if constexpr (DEDUP) {
+  } else {
     // The eight corners span at most two block rows per axis.  Reading them corner by corner through the one-entry cache
     // ping-pongs between the blocks (order 000,100,010,001,...: up to seven hash probes per sample, and - SIMT - every warp
     // has lanes on this path at every step: ncu counted ~600 warp instructions per marching step, two thirds of them probes).
@@ -647,10 +512,6 @@ __device__ uint2 get_interpolated_shared(const FusionDev& d, float3 p, Cache& bc
     c[0] = rd(pA, ox0 + oy0 + oz0);   c[1] = rd(p100, ox1 + oy0 + oz0); c[2] = rd(p010, ox0 + oy1 + oz0);
     c[3] = rd(p001, ox0 + oy0 + oz1); c[4] = rd(p110, ox1 + oy1 + oz0); c[5] = rd(p011, ox0 + oy1 + oz1);
     c[6] = rd(p101, ox1 + oy0 + oz1); c[7] = rd(pZ, ox1 + oy1 + oz1);
-  } else {
-    c[0] = voxel_at(d, gx0, gy0, gz0, bc); c[1] = voxel_at(d, gx1, gy0, gz0, bc); c[2] = voxel_at(d, gx0, gy1, gz0, bc);
-    c[3] = voxel_at(d, gx0, gy0, gz1, bc); c[4] = voxel_at(d, gx1, gy1, gz0, bc); c[5] = voxel_at(d, gx0, gy1, gz1, bc);
-    c[6] = voxel_at(d, gx1, gy0, gz1, bc); c[7] = voxel_at(d, gx1, gy1, gz1, bc);
   }
   float dist = 0.f, cf[3] = {0.f, 0.f, 0.f};
   const int ox[8] = {0, 1, 0, 0, 1, 0, 1, 1}, oy[8] = {0, 0, 1, 0, 1, 1, 0, 1}, oz[8] = {0, 0, 0, 1, 0, 1, 1, 1};
@@ -675,7 +536,8 @@ __device__ uint2 get_interpolated_shared(const FusionDev& d, float3 p, Cache& bc
 
 // one ray per thread, shared-index sampling (the default ray-cast).  The kernel is latency-bound (a step is one long dependent
 // chain: divide -> convert -> address -> load -> interpolate -> next t) and rays differ a lot in length, so small CTAs (8x8
-// pixels) at high residency balance better than 16x16 ones: TW x TH pixel tiles, MINB CTAs per SM requested.
+// pixels, 20 CTAs per SM requested, which holds the kernel at 48 registers) at high residency balance better than 16x16,
+// 16x8 or 8x4 ones (DESIGN.md, "TSDF variants removed").
 // SLAB (Z-slab partition, SURVEY.md 8e): this rank stores only the blocks z in [slab_lo, slab_hi), so every sample whose
 // trilinear neighbourhood lies outside that z range reads "no voxel" (weight 0) and advances the ray by exactly tau.  Those
 // samples are not taken: before the ray enters the slab's z range `cur` is advanced by the same fp32 additions (cur += tau)
@@ -692,17 +554,13 @@ __device__ __forceinline__ long long pack_hit_key(float depth, unsigned bgr24) {
 // NVLink P2P).  Each sample therefore sees exactly the voxels of the un-partitioned volume at exactly the same positions: the
 // union of the ranks' tiles is bit-identical to the single-volume render, occluders in other slabs included.  Foreign tiles
 // get the "miss" key, so the same MIN all-reduce assembles the image.
-// OCC (empty-space shortcut, bit-identical): before a sample is evaluated, the block that the linear ray model
-// O + cur * D falls into is looked up in the dilated occupancy bitmap (occ_mark); a clear bit proves the sample's centre voxel
-// lies in a block this volume does not store, i.e. the sample would return weight 0 and the ray would step by exactly tau - so
-// only `cur += tau` is executed (3 FMA + 3 floor + one L1-resident load instead of the pixel -> world transform, three
-// divisions, the hash probe and its dependent L2 miss).  Every sample that IS evaluated sits where the un-shortcut march puts it.
-template <int TW, int TH, int MINB, bool SLAB, bool FAST, bool PEER = false, bool OCC = false, bool DEDUP = true>
-__global__ void __launch_bounds__(TW * TH, MINB)
+// FAST: constant-divisor division (cdiv_), bit-identical to the IEEE division (option "fast_div", off by default).
+template <bool SLAB, bool FAST, bool PEER>
+__global__ void __launch_bounds__(64, 20)
 k_raycast_shared(FusionDev d, Mat4 T, unsigned char* __restrict__ bgr_out, float* __restrict__ depth_out, long long* __restrict__ keys) {
   const tdm_fusion_options& o = d.o;
-  const int x = blockIdx.x * TW + (threadIdx.x % TW);
-  const int y = blockIdx.y * TH + (threadIdx.x / TW);
+  const int x = blockIdx.x * 8 + (threadIdx.x % 8);
+  const int y = blockIdx.y * 8 + (threadIdx.x / 8);
   if (x >= o.width || y >= o.height) return;
   const int i = y * o.width + x;
   const float ucx = sub_((float)x, o.cx), vcy = sub_((float)y, o.cy);   // get_point3d's pixel terms (utils.h:93-101)
@@ -718,7 +576,6 @@ k_raycast_shared(FusionDev d, Mat4 T, unsigned char* __restrict__ bgr_out, float
   bc.init();
   float cur = 0.f;
   float t_exit = FLT_MAX;
-  float occ_d[3] = {0.f, 0.f, 0.f}, occ_o[3] = {0.f, 0.f, 0.f};   // sample position in BLOCK units = occ_o + cur * occ_d (linear model)
   {
     // Clip the march to the bounding box of everything any scan ever allocated (d.bbox, replicated on every rank): outside it
     // every sample reads "no voxel" and advances by tau, so the leading ones are replaced by the same fp32 additions without
@@ -732,7 +589,6 @@ k_raycast_shared(FusionDev d, Mat4 T, unsigned char* __restrict__ bgr_out, float
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
       const float D = T.m[4 * a] * ux + T.m[4 * a + 1] * uy + T.m[4 * a + 2], O = T.m[4 * a + 3];
-      if constexpr (OCC) { occ_d[a] = D / s8; occ_o[a] = O / s8; }
       const float lo = (float)d.bbox[a] * s8 - slack, hi = (float)(d.bbox[3 + a] + 1) * s8 + slack;
       if (fabsf(D) < 1e-12f) {
         if (O < lo || O > hi) t_in = FLT_MAX;
@@ -781,12 +637,7 @@ k_raycast_shared(FusionDev d, Mat4 T, unsigned char* __restrict__ bgr_out, float
       }
     }
     if (cur > t_exit) break;
-    if constexpr (OCC) {
-      const int bx = __float2int_rd(fmaf(occ_d[0], cur, occ_o[0])), by = __float2int_rd(fmaf(occ_d[1], cur, occ_o[1]));
-      const int bz = __float2int_rd(fmaf(occ_d[2], cur, occ_o[2]));
-      if (!((__ldg(d.occ + occ_word(bx, by, bz)) >> (bz & 31)) & 1u)) { cur = add_(cur, o.truncation_distance); continue; }
-    }
-    const uint2 v = get_interpolated_shared<decltype(bc), false, FAST, DEDUP>(d, xform(T, get_point3d_px<FAST>(d, ucx, vcy, cur)), bc);
+    const uint2 v = get_interpolated_shared<decltype(bc), false, FAST>(d, xform(T, get_point3d_px<FAST>(d, ucx, vcy, cur)), bc);
     const unsigned w = v.y >> 24;
     const float sdf = __uint_as_float(v.x);
     cur = add_(cur, w == 0 ? o.truncation_distance : sdf);
@@ -794,7 +645,7 @@ k_raycast_shared(FusionDev d, Mat4 T, unsigned char* __restrict__ bgr_out, float
   }
   // (un-clipped march: a ray that runs out of range ends with cur >= max_sensor_depth; the slab march may also stop behind the slab)
   if (hit && cur < o.max_sensor_depth) {
-    const uint2 v = get_interpolated_shared<decltype(bc), true, FAST, DEDUP>(d, xform(T, get_point3d_px<FAST>(d, ucx, vcy, cur)), bc);
+    const uint2 v = get_interpolated_shared<decltype(bc), true, FAST>(d, xform(T, get_point3d_px<FAST>(d, ucx, vcy, cur)), bc);
     bgr_out[3 * i] = v.y & 0xFF; bgr_out[3 * i + 1] = (v.y >> 8) & 0xFF; bgr_out[3 * i + 2] = (v.y >> 16) & 0xFF;
     depth_out[i] = cur;
     if (keys) keys[i] = pack_hit_key(cur, v.y);
@@ -805,18 +656,17 @@ k_raycast_shared(FusionDev d, Mat4 T, unsigned char* __restrict__ bgr_out, float
   }
 }
 
-template <bool CACHE8>
+// The comparator (option "raycast_shared" = 0): the reference's march and sampler (tsdf_volume.cu:600-632, 161-289) restated
+// voxel by voxel - one hash probe per voxel read behind a last-block cache, IEEE divisions, sgn().  Every production variant of
+// k_raycast_shared must render the same volume bit for bit (tests/test_fusion_gpu.py::test_raycast_is_bit_identical_to_reference_sampler).
 __global__ void __launch_bounds__(256)
 k_raycast(FusionDev d, Mat4 T, unsigned char* __restrict__ bgr_out, float* __restrict__ depth_out) {
   const tdm_fusion_options& o = d.o;
-  __shared__ unsigned long long skeys[CACHE8 ? 8 * 256 : 1];
-  __shared__ int sptrs[CACHE8 ? 8 * 256 : 1];
   const int x = blockIdx.x * 16 + (threadIdx.x & 15);
   const int y = blockIdx.y * 16 + (threadIdx.x >> 4);
   if (x >= o.width || y >= o.height) return;
   const int i = y * o.width + x;
-  typename std::conditional<CACHE8, Cache8, Cache1>::type bc;
-  if constexpr (CACHE8) { bc.keys = skeys + threadIdx.x; bc.ptrs = sptrs + threadIdx.x; }
+  Cache1 bc;
   bc.init();
   float cur = 0.f;
   int guard = 0;
@@ -834,65 +684,6 @@ k_raycast(FusionDev d, Mat4 T, unsigned char* __restrict__ bgr_out, float* __res
   } else {
     bgr_out[3 * i] = bgr_out[3 * i + 1] = bgr_out[3 * i + 2] = 0;
     depth_out[i] = 0.f;
-  }
-}
-
-// K7, persistent form.  Rays differ a lot in length (a few steps next to the camera's near surfaces, > 100 through free space),
-// so with one ray per thread a CTA - and every lane of a warp - idles until its slowest ray is done (a profile showed a third of the
-// warps active and two thirds of their lanes executing).  Here a fixed grid of warps pulls rays from a global counter: every trip of the warp's
-// loop first refills the lanes whose ray has finished (one warp-aggregated atomicAdd), then advances every lane's ray by ONE
-// sphere-tracing step.  Rays are numbered in 8x4 pixel tiles so a warp's 32 rays stay neighbours.  Per-ray arithmetic is the
-// same expression sequence as k_raycast, so the output is bit-identical.
-__global__ void __launch_bounds__(256)
-k_raycast_persistent(FusionDev d, Mat4 T, unsigned char* __restrict__ bgr_out, float* __restrict__ depth_out, int* __restrict__ ray_counter) {
-  const tdm_fusion_options& o = d.o;
-  const unsigned full = 0xffffffffu;
-  const int lane = threadIdx.x & 31;
-  const int tiles_x = (o.width + 7) >> 3, tiles_y = (o.height + 3) >> 2;
-  const int n_padded = tiles_x * tiles_y * 32;
-  Cache1 bc;
-  bc.init();
-  int i = 0, steps = 0;
-  float cur = 0.f;
-  bool have = false, exhausted = false;   // exhausted: the counter has passed the last ray (warp-uniform)
-  for (;;) {
-    if (!exhausted) {
-      const unsigned need = __ballot_sync(full, !have);
-      if (need) {
-        const int leader = __ffs(need) - 1;
-        int base = 0;
-        if (lane == leader) base = atomicAdd(ray_counter, __popc(need));
-        base = __shfl_sync(full, base, leader);
-        if (!have) {
-          const int idx = base + __popc(need & ((1u << lane) - 1u));
-          if (idx < n_padded) {
-            const int tile = idx >> 5, within = idx & 31;
-            const int x = (tile % tiles_x) * 8 + (within & 7), y = (tile / tiles_x) * 4 + (within >> 3);
-            if (x < o.width && y < o.height) { i = y * o.width + x; cur = 0.f; steps = 0; have = true; }
-          }
-        }
-        exhausted = base + __popc(need) >= n_padded;
-      }
-    }
-    if (exhausted && !__any_sync(full, have)) break;
-    if (have) {
-      const uint2 v = get_interpolated(d, xform(T, get_point3d(o, i, cur)), bc);
-      const unsigned w = v.y >> 24;
-      const float sdf = __uint_as_float(v.x);
-      cur = add_(cur, w == 0 ? o.truncation_distance : sdf);
-      ++steps;
-      if ((w != 0 && sdf < o.voxel_size) || !(cur < o.max_sensor_depth) || steps >= 100000) {
-        if (cur < o.max_sensor_depth) {
-          const uint2 c = get_interpolated(d, xform(T, get_point3d(o, i, cur)), bc);
-          bgr_out[3 * i] = c.y & 0xFF; bgr_out[3 * i + 1] = (c.y >> 8) & 0xFF; bgr_out[3 * i + 2] = (c.y >> 16) & 0xFF;
-          depth_out[i] = cur;
-        } else {
-          bgr_out[3 * i] = bgr_out[3 * i + 1] = bgr_out[3 * i + 2] = 0;
-          depth_out[i] = 0.f;
-        }
-        have = false;
-      }
-    }
   }
 }
 
@@ -1008,7 +799,7 @@ class FusionImpl final : public FusionIface {
       };
       fast_div_ok_ = ok(o.voxel_size) && ok(o.fx) && ok(o.fy);
       // div.rn.f32's fast path is already ~8 instructions and the ray-cast is latency-, not issue-bound.  Kept as an A/B option
-      // (bit-identical), off by default.
+      // (bit-identical), off by default; DESIGN.md ("TSDF variants removed") records its timings.
       const char* e = getenv("TDM_FAST_DIV");
       fast_div_ = fast_div_ok_ && e && e[0] == '1';
     }
@@ -1024,19 +815,11 @@ class FusionImpl final : public FusionIface {
     TDM_CUDA(cudaMalloc(&d_.list, (size_t)o.num_blocks * sizeof(int4)));
     TDM_CUDA(cudaMalloc(&d_.counters, 8 * sizeof(int)));
     TDM_CUDA(cudaMalloc(&d_.bbox, 6 * sizeof(int)));
-    TDM_CUDA(cudaMalloc(&d_.occ, kOccWords * sizeof(unsigned)));
-    TDM_CUDA(cudaMemsetAsync(d_.occ, 0, kOccWords * sizeof(unsigned), stream_));
     {
       const int init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
       TDM_CUDA(cudaMemcpy(d_.bbox, init, sizeof(init), cudaMemcpyHostToDevice));
     }
     TDM_CUDA(cudaMalloc(&d_vis_list_, (size_t)o.num_blocks * sizeof(int)));
-    {
-      int per_sm = 0, sms = 0;
-      TDM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_raycast_persistent, 256, 0));
-      TDM_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_));
-      raycast_grid_ = std::max(1, per_sm) * std::max(1, sms);
-    }
     TDM_CUDA(cudaMemsetAsync(d_.voxels, 0, (size_t)o.num_blocks * 512 * 8, stream_));
     TDM_CUDA(cudaMemsetAsync(d_.counters, 0, 8 * sizeof(int), stream_));
     k_fill_keys<<<cdiv(n_entries_, 256), 256, 0, stream_>>>(d_.keys, d_.ptrs, n_entries_);
@@ -1066,7 +849,7 @@ class FusionImpl final : public FusionIface {
     cudaSetDevice(device_);
     cudaStreamSynchronize(stream_);
     for (void* q : ipc_opened_) cudaIpcCloseMemHandle(q);
-    cudaFree(d_.keys); cudaFree(d_.ptrs); cudaFree(d_.voxels); cudaFree(d_.list); cudaFree(d_.counters); cudaFree(d_.bbox); cudaFree(d_.occ); cudaFree(d_vis_list_);
+    cudaFree(d_.keys); cudaFree(d_.ptrs); cudaFree(d_.voxels); cudaFree(d_.list); cudaFree(d_.counters); cudaFree(d_.bbox); cudaFree(d_vis_list_);
     cudaFreeHost(h_bgr_in_); cudaFreeHost(h_depth_in_); cudaFree(d_bgr_in_); cudaFree(d_depth_in_);
     for (int half = 0; half < 2; ++half) { cudaFreeHost(h_bgr_out_[half]); cudaFreeHost(h_depth_out_[half]); }
     cudaFree(d_bgr_out_); cudaFree(d_depth_out_); cudaFreeHost(h_counters_);
@@ -1111,7 +894,7 @@ class FusionImpl final : public FusionIface {
     TDM_CUDA(cudaEventRecord(ev_int_, stream_));
     have_scan_ = true;
     ++volume_epoch_;   // a pending mesh extracted before this scan no longer describes the volume
-    next_ = d_.o.num_render_streams > 0 ? kRender : kRender;
+    next_ = kRender;
   }
 
   // RenderAsync, tsdf_volume.cu:634-700
@@ -1279,17 +1062,10 @@ class FusionImpl final : public FusionIface {
   float last_alloc_ms() override { return last_alloc_ms_; }
   void set_option(const char* name, int value) override {
     const std::string n(name);
-    if (n == "alloc_filter") alloc_filter_ = value != 0;
-    else if (n == "raycast_cache8") raycast_cache8_ = value != 0;
-    else if (n == "raycast_persistent") raycast_persistent_ = value != 0;
-    else if (n == "raycast_shared") raycast_shared_ = value != 0;
-    else if (n == "raycast_tile") raycast_tile_ = value;
-    else if (n == "integrate_compact") integrate_compact_ = value != 0;
+    if (n == "raycast_shared") raycast_shared_ = value != 0;
     else if (n == "slab_clip") slab_clip_ = value != 0;
     else if (n == "fast_div") fast_div_ = value != 0 && fast_div_ok_;
     else if (n == "slab_exchange") slab_exchange_ = value != 0;
-    else if (n == "occ_skip") occ_skip_ = value != 0;
-    else if (n == "raycast_dedup") raycast_dedup_ = value != 0;
     else throw Error("unknown fusion option " + n);
   }
   bool mesh_pending() override { return mesh_kind_ != kMeshNone; }
@@ -1362,84 +1138,40 @@ class FusionImpl final : public FusionIface {
   void launch_integrate() {
     const int npx = d_.o.height * d_.o.width;
     TDM_CUDA(cudaMemsetAsync(d_.counters + 2, 0, 2 * sizeof(int), stream_));
-    if (alloc_filter_) k_allocate<true><<<cdiv(npx, 128), 128, 0, stream_>>>(d_, d_depth_in_, pose_);
-    else k_allocate<false><<<cdiv(npx, 128), 128, 0, stream_>>>(d_, d_depth_in_, pose_);
+    k_allocate<<<cdiv(npx, 128), 128, 0, stream_>>>(d_, d_depth_in_, pose_);
     TDM_CUDA(cudaGetLastError());
     if (ev_split_) TDM_CUDA(cudaEventRecord(ev_split_, stream_));
-    if (integrate_compact_) {
-      k_visible<<<cdiv(d_.o.num_blocks, 256), 256, 0, stream_>>>(d_, pose_inv_, d_vis_list_);
-      TDM_CUDA(cudaGetLastError());
-      k_integrate_list<<<132 * 8, 256, 0, stream_>>>(d_, d_bgr_in_, d_depth_in_, pose_inv_, d_vis_list_);
-    } else {
-      k_integrate<<<132 * 8, 256, 0, stream_>>>(d_, d_bgr_in_, d_depth_in_, pose_inv_);
-    }
+    k_visible<<<cdiv(d_.o.num_blocks, 256), 256, 0, stream_>>>(d_, pose_inv_, d_vis_list_);
+    TDM_CUDA(cudaGetLastError());
+    k_integrate_list<<<132 * 8, 256, 0, stream_>>>(d_, d_bgr_in_, d_depth_in_, pose_inv_, d_vis_list_);
     TDM_CUDA(cudaGetLastError());
   }
   void launch_render(int n, bool copy_back) {
     const size_t npx = (size_t)d_.o.height * d_.o.width;
-    dim3 grid(cdiv(d_.o.width, 16), cdiv(d_.o.height, 16));
+    const dim3 grid8(cdiv(d_.o.width, 8), cdiv(d_.o.height, 8));
+    const bool peer = d_.pr_world > 1;
+    const bool slab = !peer && (d_.slab_lo != INT_MIN || d_.slab_hi != INT_MAX) && slab_clip_;
     for (int i = 0; i < n; ++i) {
-      if (raycast_shared_ && !raycast_persistent_ && !raycast_cache8_) {
-        unsigned char* bo = d_bgr_out_ + (size_t)i * npx * 3;
-        float* dout_i = d_depth_out_ + (size_t)i * npx;
-        const bool peer = d_.pr_world > 1;
-        const bool slab = !peer && (d_.slab_lo != INT_MIN || d_.slab_hi != INT_MAX) && slab_clip_;
-        const bool occ = occ_skip_ && occ_model_ok(render_poses_[i]);
-        long long* keys = nullptr;
-        if (slab_exchange_ && i == 0) {
-          if (!d_hit_keys_) TDM_CUDA(cudaMalloc(&d_hit_keys_, npx * sizeof(long long)));
-          keys = d_hit_keys_;
-        }
-#define TDM_RAY2(TW_, TH_, MB_, GRID_, THREADS_, OCC_, DD_)                                                       \
-  do {                                                                                                             \
-    if (slab && fast_div_) k_raycast_shared<TW_, TH_, MB_, true, true, false, OCC_, DD_><<<GRID_, THREADS_, 0, stream_>>>(d_, render_poses_[i], bo, dout_i, keys);   \
-    else if (slab) k_raycast_shared<TW_, TH_, MB_, true, false, false, OCC_, DD_><<<GRID_, THREADS_, 0, stream_>>>(d_, render_poses_[i], bo, dout_i, keys);   \
-    else if (fast_div_) k_raycast_shared<TW_, TH_, MB_, false, true, false, OCC_, DD_><<<GRID_, THREADS_, 0, stream_>>>(d_, render_poses_[i], bo, dout_i, keys);   \
-    else k_raycast_shared<TW_, TH_, MB_, false, false, false, OCC_, DD_><<<GRID_, THREADS_, 0, stream_>>>(d_, render_poses_[i], bo, dout_i, keys);       \
-  } while (0)
-  /* MB_: residency asked for by the corner-by-corner sampler (round-2 tuning), MBD_: by the block-deduplicating sampler, */ \
-  /* MBO_: with the occupancy shortcut on top (6 more live registers) */                                           \
-#define TDM_RAY(TW_, TH_, MB_, MBD_, MBO_, GRID_, THREADS_)                                                       \
-  do {                                                                                                             \
-    if (occ) TDM_RAY2(TW_, TH_, MBO_, GRID_, THREADS_, true, true);                                                \
-    else if (raycast_dedup_) TDM_RAY2(TW_, TH_, MBD_, GRID_, THREADS_, false, true);                               \
-    else TDM_RAY2(TW_, TH_, MB_, GRID_, THREADS_, false, false);                                                   \
-  } while (0)
-        if (peer) k_raycast_shared<8, 8, 20, false, false, true><<<dim3(cdiv(d_.o.width, 8), cdiv(d_.o.height, 8)), 64, 0, stream_>>>(d_, render_poses_[i], bo, dout_i, keys);
-        else if (raycast_tile_ == 0) TDM_RAY(16, 16, 5, 5, 5, grid, 256);
-        else if (raycast_tile_ == 1) TDM_RAY(8, 8, 24, 20, 20, dim3(cdiv(d_.o.width, 8), cdiv(d_.o.height, 8)), 64);
-        else if (raycast_tile_ == 2) TDM_RAY(8, 4, 48, 40, 40, dim3(cdiv(d_.o.width, 8), cdiv(d_.o.height, 4)), 32);
-        else TDM_RAY(16, 8, 12, 10, 10, dim3(cdiv(d_.o.width, 16), cdiv(d_.o.height, 8)), 128);
-#undef TDM_RAY2
-#undef TDM_RAY
-      } else if (raycast_persistent_) {
-        TDM_CUDA(cudaMemsetAsync(d_.counters + 4, 0, sizeof(int), stream_));
-        k_raycast_persistent<<<raycast_grid_, 256, 0, stream_>>>(d_, render_poses_[i], d_bgr_out_ + (size_t)i * npx * 3,
-                                                                 d_depth_out_ + (size_t)i * npx, d_.counters + 4);
-      } else if (raycast_cache8_) k_raycast<true><<<grid, 256, 0, stream_>>>(d_, render_poses_[i], d_bgr_out_ + (size_t)i * npx * 3, d_depth_out_ + (size_t)i * npx);
-      else k_raycast<false><<<grid, 256, 0, stream_>>>(d_, render_poses_[i], d_bgr_out_ + (size_t)i * npx * 3, d_depth_out_ + (size_t)i * npx);
+      unsigned char* bo = d_bgr_out_ + (size_t)i * npx * 3;
+      float* dout_i = d_depth_out_ + (size_t)i * npx;
+      long long* keys = nullptr;
+      if (slab_exchange_ && raycast_shared_ && i == 0) {   // k_raycast writes no keys
+        if (!d_hit_keys_) TDM_CUDA(cudaMalloc(&d_hit_keys_, npx * sizeof(long long)));
+        keys = d_hit_keys_;
+      }
+      const Mat4& T = render_poses_[i];
+      if (!raycast_shared_) k_raycast<<<dim3(cdiv(d_.o.width, 16), cdiv(d_.o.height, 16)), 256, 0, stream_>>>(d_, T, bo, dout_i);
+      else if (peer) k_raycast_shared<false, false, true><<<grid8, 64, 0, stream_>>>(d_, T, bo, dout_i, keys);
+      else if (slab && fast_div_) k_raycast_shared<true, true, false><<<grid8, 64, 0, stream_>>>(d_, T, bo, dout_i, keys);
+      else if (slab) k_raycast_shared<true, false, false><<<grid8, 64, 0, stream_>>>(d_, T, bo, dout_i, keys);
+      else if (fast_div_) k_raycast_shared<false, true, false><<<grid8, 64, 0, stream_>>>(d_, T, bo, dout_i, keys);
+      else k_raycast_shared<false, false, false><<<grid8, 64, 0, stream_>>>(d_, T, bo, dout_i, keys);
       TDM_CUDA(cudaGetLastError());
     }
     if (copy_back && !slab_exchange_) {   // slab exchange mode: the per-slab render is only an operand of the exchange step
       TDM_CUDA(cudaMemcpyAsync(h_bgr_out_[free_half_], d_bgr_out_, npx * 3 * n, cudaMemcpyDeviceToHost, stream_));
       TDM_CUDA(cudaMemcpyAsync(h_depth_out_[free_half_], d_depth_out_, npx * 4 * n, cudaMemcpyDeviceToHost, stream_));
     }
-  }
-  // The occupancy shortcut locates a sample with the linear ray model O + cur * D in fp32; the exact position goes through a
-  // few more roundings (pixel -> camera -> world), each relative 2^-24 of a coordinate.  Bound every coordinate the march can
-  // reach by B = |t|_max + max_sensor_depth * (|row|_1 of R scaled by the widest pixel ray) and require 16 ulp(B) (a generous
-  // count of the roundings involved) to stay below 0.4 block; otherwise (tiny voxels far from the origin) the shortcut is off.
-  bool occ_model_ok(const Mat4& T) const {
-    const tdm_fusion_options& o = d_.o;
-    const float ux = std::max(std::fabs((0.f - o.cx) / o.fx), std::fabs(((float)o.width - o.cx) / o.fx));
-    const float uy = std::max(std::fabs((0.f - o.cy) / o.fy), std::fabs(((float)o.height - o.cy) / o.fy));
-    float B = 0.f;
-    for (int a = 0; a < 3; ++a) {
-      const float reach = std::fabs(T.m[4 * a + 3]) +
-                          o.max_sensor_depth * (std::fabs(T.m[4 * a]) * ux + std::fabs(T.m[4 * a + 1]) * uy + std::fabs(T.m[4 * a + 2]));
-      B = std::max(B, reach);
-    }
-    return B == B && B * (16.f / 8388608.f) < 0.4f * 8.f * o.voxel_size;
   }
   static constexpr int kMeshGrid = 132 * 8;   // 8 CTAs per SM of an H100 SXM
   // count + scan + emit + total on stream_ (no host sync)
@@ -1581,24 +1313,13 @@ class FusionImpl final : public FusionIface {
   int n_rendered_ = 0;
   bool have_scan_ = false;
   Next next_ = kIntegrate;
-  bool alloc_filter_ = false, raycast_cache8_ = false;   // tdm_fusion_set_option A/B switches (bit-identical), off by default
-  bool raycast_shared_ = true;
-  int raycast_tile_ = 1;   // 0: 16x16 px CTAs, 1: 8x8, 2: 8x4 (one warp), 3: 16x8
-  bool raycast_persistent_ = false, integrate_compact_ = true;
+  bool raycast_shared_ = true;   // false: the reference-shaped comparator k_raycast
   bool fast_div_ok_ = false, fast_div_ = false;   // constant-divisor division in the ray-cast (cdiv_): bit-identical, 3 instructions per division
   std::vector<void*> ipc_opened_;   // peers' allocations mapped with cudaIpcOpenMemHandle (closed in the destructor)
   bool slab_clip_ = true;        // Z-slab volumes: rays are only sampled inside the slab's z range (bit-identical, see k_raycast_shared)
-  bool raycast_dedup_ = true;    // ray-cast: samples whose corners straddle block faces look every distinct block up once
-  bool occ_skip_ = false;        // ray-cast: dilated occupancy bitmap in front of the sampler (bit-identical, see k_raycast_shared OCC).
-                                 // Off by default: the
-                                 // reference's allocation DDA walks every ray from the CAMERA to the surface (tsdf_volume.cu:317-434),
-                                 // so the free space a later ray crosses is itself allocated (sdf ~ tau, weight > 0) and every
-                                 // sample there must be interpolated; the bitmap only ever skips what the bounding-box clip
-                                 // already skips.  Kept as an A/B option, off by default.
   bool slab_exchange_ = false;   // Z-slab volumes: the ray-cast emits packed nearest-hit keys for the exchange step, the per-slab
                                  // render is not copied back and GetRenderResult does not wait (tandem_b200.parallel)
   int* d_vis_list_ = nullptr;
-  int raycast_grid_ = 132;
   cudaEvent_t ev_split_ = nullptr;
   float last_alloc_ms_ = 0.f;
   long long* d_hit_keys_ = nullptr;

@@ -207,11 +207,8 @@ st = f.stats()
 vis = st["visible_blocks"]
 alg = vis * 512 * 16 + 7 * H * W
 res = {}
-DEFAULTS = {"alloc_filter": 0, "raycast_cache8": 0, "raycast_persistent": 0, "integrate_compact": 1, "raycast_shared": 1, "raycast_tile": 1, "occ_skip": 0, "raycast_dedup": 1, "fast_div": 0}
-for name, opts in (("default", {}), ("alloc_filter", {"alloc_filter": 1}), ("raycast_persistent", {"raycast_persistent": 1}),
-                   ("raycast_cache8", {"raycast_cache8": 1}), ("raycast_lookup_per_voxel", {"raycast_shared": 0}), ("raycast_tile_16x16", {"raycast_tile": 0}), ("raycast_tile_8x4", {"raycast_tile": 2}), ("raycast_tile_16x8", {"raycast_tile": 3}), ("integrate_full_scan", {"integrate_compact": 0}), ("occupancy_shortcut", {"occ_skip": 1}),
-                   ("raycast_corner_by_corner", {"raycast_dedup": 0}), ("fast_div", {"fast_div": 1}), ("fast_div_tile_16x8", {"fast_div": 1, "raycast_tile": 3}),
-                   ("fast_div_tile_8x4", {"fast_div": 1, "raycast_tile": 2})):
+DEFAULTS = {"raycast_shared": 1, "fast_div": 0}
+for name, opts in (("default", {}), ("raycast_lookup_per_voxel", {"raycast_shared": 0}), ("fast_div", {"fast_div": 1})):
     for k, dv in DEFAULTS.items():
         f.set_option(k, opts.get(k, dv))
     f.run_resident(3)
