@@ -14,10 +14,11 @@
 // Outputs computed for the 2 pad columns of each row are garbage and masked in the epilogue (utilisation TW/(TW+2)).
 // B (weights, all taps) is pre-arranged on the host in the same canonical core-matrix order and stays resident.
 //
-// Roles (288 threads): warpgroups 0 and 1 consume, warp 8 produces (one lane issues the TMA copies).  A plane's
-// 64-position sub-chunks alternate between the two consumer warpgroups; each accumulates its sub-chunk in registers
-// (m64nNk16, one instruction per K=16 step) and runs the epilogue (bias / ReLU / skip / store) straight from the
-// accumulator fragment, so one warpgroup's epilogue overlaps the other's MMAs.
+// Roles (128 * NWG + 32 threads): warpgroups 0 .. NWG-1 consume, warp 4 * NWG produces (one lane issues the TMA copies).
+// NWG is 4 (544 threads) where the instantiation fits 96 registers without spills, else 2 (288 threads); see conv_nwg.
+// A plane's 64-position sub-chunks are dealt round-robin to the consumer warpgroups; each accumulates its sub-chunk in
+// registers (m64nNk16, one instruction per K=16 step), waits for the chain and runs the epilogue (bias / ReLU / skip /
+// store) straight from the accumulator fragment, so one warpgroup's drain and epilogue overlap the other warpgroups' MMAs.
 //
 // This file also holds what the stride-2 (conv_tc_s2.cuh) and input-stationary (conv_tc_is.cuh) kernels share with
 // k_conv_tc: the TMA ring and its prologue, the tile decode, the fragment-row -> pixel map, the bias registers, the
@@ -157,9 +158,19 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* tmap, 
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-constexpr int kConsumerWG = 2;                       // consumer warpgroups (warps 0..7)
-constexpr int kThreads = 128 * kConsumerWG + 32;     // + the producer warp
-constexpr int kProducerWarp = 4 * kConsumerWG;
+// Consumer warpgroups (warps 0 .. 4*NWG-1; warp 4*NWG produces) of one instantiation, fixed at build time.  Four keep up
+// to four MMA chains in flight per SM, so that one warpgroup's drain and epilogue are covered by three others' MMAs.  At
+// 544 threads (17 warps, five of them on one SM sub-partition) ptxas allows 96 registers per thread; two warpgroups (288
+// threads, 168 registers) remain only where that cap spills (-Xptxas -v, DESIGN.md section 5): the N = 64 transposed
+// convs (MODE 1), which keep their bias and the early-fetched skip operand in registers (the N = 128 one loads both in
+// the epilogue and fits), and the prob layer's soft-argmin tail for more than 32 planes (RegressTail<48 / 64>).
+// mode: k_conv_tc's MODE (0 for the stride-2 and input-stationary kernels); n: instruction N; tail_d: Tail::max_d, 0
+// without a tail.  The planners read the same function with their full-depth tile's D for tail_d (D <= 32 exactly when
+// the tail's bucket max_d is), so their warpgroup balance matches the kernel they plan for.
+__host__ __device__ constexpr int conv_nwg(int mode, int n, int tail_d) { return (mode == 1 && n <= 64) || tail_d > 32 ? 2 : 4; }
+__host__ __device__ constexpr int conv_threads(int nwg) { return 128 * nwg + 32; }
+// Tile-time factor of a plane's 2*nch sub-chunks dealt round-robin to nwg warpgroups: the last round may leave some idle
+inline double wg_balance(int nch, int nwg) { return (double)((2 * nch + nwg - 1) / nwg * nwg) / (2 * nch); }
 
 // ---------------------------------------------------------------------------------------------------------------
 // K-step pairing of taps, shared by the kernels' A descriptors and the host B images
@@ -192,8 +203,9 @@ __device__ __forceinline__ uint32_t kstep_alo(int b, uint32_t cgb16, TapOff off)
 // The TMA ring
 // ---------------------------------------------------------------------------------------------------------------
 // Shared memory: [B image, 128-byte aligned][S slots of slot_bytes][full[S] at +0, empty[S] at +8, b_full at +16 (8-byte
-// barriers, S <= 8)].  Input plane rp goes to slot rp % S; full[s] counts its TMA bytes, empty[s] the 8 consumer warps'
-// releases of it.
+// barriers, S <= 8)].  Input plane rp goes to slot rp % S; full[s] counts its TMA bytes, empty[s] the 4 * NWG consumer
+// warps' releases of it.
+template <int NWG>
 struct Ring {
   uint8_t* a;             // slot 0
   uint32_t slot_bytes;
@@ -210,7 +222,7 @@ struct Ring {
     Ring r{smem + (b_bytes + 127) / 128 * 128, slot_bytes, S, nullptr, 0};
     r.bars = reinterpret_cast<uint64_t*>(r.a + (size_t)slot_bytes * S);
     if (threadIdx.x == 0) {
-      for (int s = 0; s < S; ++s) { mbar_init(r.full(s), 1); mbar_init(r.empty(s), 4 * kConsumerWG); }
+      for (int s = 0; s < S; ++s) { mbar_init(r.full(s), 1); mbar_init(r.empty(s), 4 * NWG); }
       mbar_init(r.bars + 16, 1);
       asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
       mbar_expect_tx(r.bars + 16, b_bytes);
@@ -236,7 +248,7 @@ struct Ring {
   }
 
   // Consumers: the weight image, every input plane up to `plane`, the shared address (16-byte units) of a plane's slot,
-  // and the release of a plane this warp no longer reads (the producer may refill its slot once all 8 warps released it).
+  // and the release of a plane this warp no longer reads (the producer may refill its slot once all consumer warps released it).
   __device__ __forceinline__ void wait_weights() const { mbar_wait(bars + 16, 0); }
   __device__ __forceinline__ void wait(int plane) {
     for (; waited <= plane; ++waited) mbar_wait(full(waited % S), (waited / S) & 1);
@@ -288,14 +300,15 @@ __device__ __forceinline__ void load_bias(float (&bv)[NB][2], const float* bias,
 // (softmax / soft-argmin / confidence, module.py:1116-1133) without another launch.  NoTail = plain convolution.
 struct NoTail {
   static constexpr bool enabled = false;
+  static constexpr int max_d = 0;
   __device__ __forceinline__ void operator()(const float*, int, int, int, int) const {}
 };
 // Runs the tail over this thread's pixels once the tile is stored.  ndo == D (host-checked): the thread wrote all D
 // logits of its pixels itself (program order makes them visible to it).
-template <typename Tail>
+template <int NWG, typename Tail>
 __device__ __forceinline__ void run_tail(const Tail& tail, float* plain_out, const Tile& t, const TileOrigin& o, int wg, int wq, int lane) {
   if ((lane & 3) == 0) {
-    for (int sc = wg; sc < 2 * t.nch; sc += kConsumerWG)
+    for (int sc = wg; sc < 2 * t.nch; sc += NWG)
       for (int i = 0; i < 2; ++i) {
         // each row half decoded on its own: carried over from half 0, its pixel would stay live across the tail call, and
         // RegressTail<64> already sits at the register cap
@@ -346,8 +359,9 @@ __device__ __forceinline__ int stencil_off(int t, int P) { return (t / 3) * P + 
 // per plane at offsets {0,1}^2 (stencil positions (1..2,1..2)), 2 planes, N = 8 output parity classes x COUT.
 // MODE 3: 2-D "conv3x3 of a nearest-x2 up-sampled map" evaluated on the COARSE grid: 9 taps, N = 4 output parity
 // classes x COUT (the 3x3 fine taps collapse onto 2x2 coarse neighbours; weights pre-summed on the host).
-template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool OUT_PLAIN, int MODE = 0, bool HILO = false, typename Tail = NoTail>
-__global__ void __launch_bounds__(kThreads, 1)
+// NWG: consumer warpgroups, conv_nwg(MODE, instruction N, Tail::max_d).
+template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool OUT_PLAIN, int MODE, bool HILO, typename Tail, int NWG>
+__global__ void __launch_bounds__(conv_threads(NWG), 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, groups*planes}, box {8, P, R+2, 1}*/,
           const TIn* __restrict__ bimg /*host-arranged B image*/, const float* __restrict__ bias,
           const TOut* __restrict__ res, TOut* __restrict__ out, float* __restrict__ plain_out, const __grid_constant__ Geom g,
@@ -367,13 +381,13 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
   // N-slicing (blockIdx.y): wide outputs (CIN = 64 layers, whose full B image would not fit shared memory) are split into
   // slices of NPAD columns, each with its own contiguous B image; slice ns produces output columns [ns*NPAD, (ns+1)*NPAD).
   const int ns = blockIdx.y;
-  Ring ring = Ring::start(smem, B_BYTES, bimg + (size_t)ns * (B_BYTES / sizeof(TIn)), cg_bytes * CG, g.S);
+  Ring<NWG> ring = Ring<NWG>::start(smem, B_BYTES, bimg + (size_t)ns * (B_BYTES / sizeof(TIn)), cg_bytes * CG, g.S);
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // provably warp-uniform (uniform datapath)
   const int lane = threadIdx.x & 31;
   const TileOrigin o = tile_origin(g);
   const int nin = o.ndo + KD - 1;                  // input planes to stream
 
-  if (warp == kProducerWarp) {
+  if (warp == 4 * NWG) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       // one tiled TMA per (plane, channel group): box = (R+2) rows x P positions, rows / columns beyond the tensor are
@@ -428,7 +442,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
 #pragma unroll
     for (int kd = 0; kd < KD; ++kd) slot16[kd] = ring.slot16(od + kd);
     const int d = o.d0 + od;
-    for (int sc = wg; sc < nsub; sc += kConsumerWG) {
+    for (int sc = wg; sc < nsub; sc += NWG) {
       const int l = sc * 64 + wq * 16 + (lane >> 2);
       // the skip operand is fetched before the MMA chain, so that its load latency overlaps the chain (except for N = 128,
       // whose accumulators leave no room for it)
@@ -496,7 +510,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
     }
     ring.release(od);   // oldest input plane of od
   }
-  if constexpr (Tail::enabled) run_tail(tail, plain_out, g, o, wg, wq, lane);
+  if constexpr (Tail::enabled) run_tail<NWG>(tail, plain_out, g, o, wg, wq, lane);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -609,7 +623,8 @@ struct Plan {
 //        x wave quantisation on the 132 SMs of an H100 SXM (one CTA per SM: time ~ ceil(T/132) tile-times for T tiles)
 // tile_clk(DR, nch) is the estimated time of one tile in clocks: a per-CTA fixed cost + the instruction stream.  Its
 // constants are a model (instruction cost growing with N, a fixed per-CTA prologue, fill and drain), not a measurement;
-// they only rank tilings against each other.  A limit below 225 KB is soft: if nothing fits it, 225 KB is searched.
+// they only rank tilings against each other; callers scale it by wg_balance for the kernel's consumer warpgroups.  A limit
+// below 225 KB is soft: if nothing fits it, 225 KB is searched.
 template <typename Amp, typename Clk>
 inline Tile plan_tiles(int D, int H, int W, int cg, size_t b_bytes, size_t smem_limit, const TileLimits& lim, Amp amp, Clk tile_clk,
                        size_t& smem_out) {
@@ -666,9 +681,10 @@ inline Plan make_plan(int cin, int npad, int kd, int D, int H, int W, int pd, in
   auto amp = [&](int R, int TW, int P, int DR) {
     return (double)(R + 2) / R * (double)P / TW * (kd == 3 ? (double)(DR + 2) / DR : (kd == 2 ? (double)(DR + 1) / DR : 1.0));
   };
+  const int nwg = conv_nwg(mode, npad, full_depth ? D : 0);
   auto tile_clk = [&](int DR, int nch) {
     const double clk_mma = mode == 1 ? 35.0 + 0.45 * npad : 45.0 + 0.35 * npad;
-    return 8500.0 + (double)DR * nch * nblk * kd * clk_mma;
+    return (8500.0 + (double)DR * nch * nblk * kd * clk_mma) * wg_balance(nch, nwg);
   };
   static_cast<Tile&>(p.g) = plan_tiles(D, H, W, cin / 8, b_image_bytes(kd, nblk, npad), smem_limit, lim, amp, tile_clk, p.smem);
   p.g.Hp = H + 2; p.g.Wp = W + 2; p.g.pd = pd;

@@ -12,23 +12,24 @@
 // The blocks are folded into two rolling fp32 partials per sub-chunk, held in registers:
 //   output p-1 = partial(p-1) + block kd=2   -> complete: bias / ReLU / store
 //   partial(p) += block kd=1,   partial(p+1) = block kd=0
-// so a consumer warpgroup owns the same sub-chunks on every plane of the tile, and the planner bounds the sub-chunks per
-// warpgroup by kIsMaxCh (registers).  As in k_conv_tc, a warpgroup waits for its chain before it folds and stores, and the
-// other consumer warpgroup's MMAs overlap that epilogue (keeping the next chain in flight with wgmma.wait_group 1 made
-// ptxas serialise every wgmma, C7514).  Ring, producer warp, roles and tile geometry are those of k_conv_tc.
+// so consumer warpgroup wg owns sub-chunks NWG * k + wg on every plane of the tile, and the planner bounds the chunks per
+// plane by kIsMaxCh (registers: 2 * kIsMaxCh / NWG sub-chunks per warpgroup).  As in k_conv_tc, a warpgroup waits for its
+// chain before it folds and stores, and the other consumer warpgroups' MMAs overlap that epilogue (keeping the next chain
+// in flight with wgmma.wait_group 1 made ptxas serialise every wgmma, C7514).  Ring, producer warp, roles and tile
+// geometry are those of k_conv_tc.
 #pragma once
 #include "conv_tc.cuh"
 
 namespace tdm {
 namespace tc {
 
-// 128-position chunks per plane, i.e. 64-position sub-chunks per consumer warpgroup: two rolling partials of 4 floats each
-// per sub-chunk stay in registers
+// Most 128-position chunks per plane, i.e. 2 * kIsMaxCh / NWG 64-position sub-chunks per consumer warpgroup: two rolling
+// partials of 4 floats each per sub-chunk stay in registers
 constexpr int kIsMaxCh = 8;
 
 // Tail: the prob layer's softmax / soft-argmin / confidence, as in k_conv_tc (tiles that span all D planes, make_plan_is(full_depth)).
-template <typename TIn, typename TOut, int CIN, int CPK, bool OUT_PLAIN, typename Tail = NoTail>
-__global__ void __launch_bounds__(kThreads, 1)
+template <typename TIn, typename TOut, int CIN, int CPK, bool OUT_PLAIN, typename Tail, int NWG>
+__global__ void __launch_bounds__(conv_threads(NWG), 1)
 k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/, const TIn* __restrict__ bimg /*build_b_image_is*/,
              const float* __restrict__ bias, TOut* __restrict__ out, float* __restrict__ plain_out, const __grid_constant__ Geom g,
              const __grid_constant__ Tail tail) {
@@ -39,16 +40,18 @@ k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/
   constexpr int N = 3 * CPK;                    // instruction N
   constexpr int B_BYTES = NBLK * N * 32;
   constexpr int PN = CPK == 16 ? 4 : 2;         // folded values per thread and sub-chunk: (row half i, column e) or row half i
+  constexpr int KSUB = 2 * kIsMaxCh / NWG;      // most sub-chunks per plane that one warpgroup owns
+  static_assert((2 * kIsMaxCh) % NWG == 0, "the partial arrays hold exactly this warpgroup's share of 2 * kIsMaxCh sub-chunks");
 
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t cg_bytes = (uint32_t)g.slot_pos * 16u;
-  Ring ring = Ring::start(smem, B_BYTES, bimg, cg_bytes * CG, g.S);
+  Ring<NWG> ring = Ring<NWG>::start(smem, B_BYTES, bimg, cg_bytes * CG, g.S);
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   const TileOrigin o = tile_origin(g);
   const int nin = o.ndo + 2;             // padded input planes d0 .. d0+ndo+1 (the zero D halos cover the borders)
 
-  if (warp == kProducerWarp) {
+  if (warp == 4 * NWG) {
     if (lane == 0) {
       const uint32_t box_bytes = (uint32_t)g.P * (uint32_t)(g.R + 2) * 16u;
       ring.produce(nin, box_bytes * CG, [&](uint8_t* dst, int rp, uint64_t* bar) {
@@ -64,10 +67,10 @@ k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/
   const uint32_t sB16 = smem_u32(smem) >> 4;
   const uint32_t b_lbo16 = (uint32_t)(N * 16 >> 4);
   auto tap_off = [&](int t) -> int { return stencil_off(t, P); };
-  const int nch = g.nch;                         // sub-chunks sc = 2k + wg, k < nch, of every plane belong to this warpgroup
-  float pa[kIsMaxCh][PN], pb[kIsMaxCh][PN];      // partials of output planes rp-1 and rp (after input plane rp)
+  const int nsub = 2 * g.nch;                    // sub-chunks sc = NWG * k + wg < nsub of every plane belong to this warpgroup
+  float pa[KSUB][PN], pb[KSUB][PN];              // partials of output planes rp-1 and rp (after input plane rp)
 #pragma unroll
-  for (int k = 0; k < kIsMaxCh; ++k)
+  for (int k = 0; k < KSUB; ++k)
 #pragma unroll
     for (int q = 0; q < PN; ++q) pa[k][q] = pb[k][q] = 0.f;
   float fr[N / 2];
@@ -94,7 +97,7 @@ k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       int h, w;
-      if (!frag_pixel(g, o, (2 * k + wg) * 64 + wq * 16 + (lane >> 2), i, h, w)) continue;
+      if (!frag_pixel(g, o, (NWG * k + wg) * 64 + wq * 16 + (lane >> 2), i, h, w)) continue;
       if constexpr (OUT_PLAIN) {
         if ((lane & 3) == 0) plain_out[((long long)d * g.H + h) * g.W + w] = x[i] + bv[0][0];
       } else {
@@ -116,9 +119,9 @@ k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/
     ring.wait(rp);
     const uint32_t slot16 = ring.slot16(rp);
 #pragma unroll
-    for (int k = 0; k < kIsMaxCh; ++k) {
-      if (k < nch) {
-        const uint32_t a0 = slot16 + (uint32_t)(2 * k + wg) * 64u;
+    for (int k = 0; k < KSUB; ++k) {
+      if (NWG * k + wg < nsub) {
+        const uint32_t a0 = slot16 + (uint32_t)(NWG * k + wg) * 64u;
         fence_frag(fr);
         wgmma_fence();
 #pragma unroll
@@ -133,7 +136,7 @@ k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/
     }
     ring.release(rp);   // this warp no longer reads input plane rp
   }
-  if constexpr (Tail::enabled) run_tail(tail, plain_out, g, o, wg, wq, lane);
+  if constexpr (Tail::enabled) run_tail<NWG>(tail, plain_out, g, o, wg, wq, lane);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -176,7 +179,8 @@ inline Plan make_plan_is(int cin, int cpk, int D, int H, int W, size_t smem_limi
   const int n3 = 3 * cpk;
   const TileLimits lim{3, 2, 2, 1, 256, 30, kIsMaxCh, 1, full_depth};
   auto amp = [&](int R, int TW, int P, int DR) { return (double)(R + 2) / R * (double)P / TW * (double)(DR + 2) / DR; };
-  auto tile_clk = [&](int DR, int nch) { return 8500.0 + (double)(DR + 2) * nch * nblk * (45.0 + 0.35 * n3); };
+  const int nwg = conv_nwg(0, n3, full_depth ? D : 0);
+  auto tile_clk = [&](int DR, int nch) { return (8500.0 + (double)(DR + 2) * nch * nblk * (45.0 + 0.35 * n3)) * wg_balance(nch, nwg); };
   static_cast<Tile&>(p.g) = plan_tiles(D, H, W, cin / 8, b_image_bytes(1, nblk, n3), smem_limit, lim, amp, tile_clk, p.smem);
   p.g.Hp = H + 2; p.g.Wp = W + 2; p.g.pd = 1;
   p.grid = p.g.tiles_w * p.g.tiles_h * p.g.tiles_d;

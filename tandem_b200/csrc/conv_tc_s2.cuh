@@ -27,8 +27,8 @@ struct GeomS2 : Tile {     // Tile: OUTPUT grid; P = TW + KS/2, slot_pos = one p
   short tap_off[kMaxTaps + 1];   // position offset of tap t inside a channel group's 4 sub-tiles (table order)
 };
 
-template <typename TIn, typename TOut, int CIN, int NPAD, int KD, int KS>
-__global__ void __launch_bounds__(kThreads, 1)
+template <typename TIn, typename TOut, int CIN, int NPAD, int KD, int KS, int NWG>
+__global__ void __launch_bounds__(conv_threads(NWG), 1)
 k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ bimg, const float* __restrict__ bias,
              TOut* __restrict__ out, const __grid_constant__ GeomS2 g) {
   constexpr int CG = CIN / 8;
@@ -40,13 +40,13 @@ k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ b
   const int ns = blockIdx.y;
   const uint32_t sub_bytes = (uint32_t)g.slot_pos * 16u;
   const uint32_t cg_bytes = sub_bytes * 4u;
-  Ring ring = Ring::start(smem, B_BYTES, bimg + (size_t)ns * (B_BYTES / sizeof(TIn)), cg_bytes * CG, g.S);
+  Ring<NWG> ring = Ring<NWG>::start(smem, B_BYTES, bimg + (size_t)ns * (B_BYTES / sizeof(TIn)), cg_bytes * CG, g.S);
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   const TileOrigin o = tile_origin(g);
   const int nin = KD == 3 ? 2 * o.ndo + 1 : o.ndo;
 
-  if (warp == kProducerWarp) {
+  if (warp == 4 * NWG) {
     // ===================== TMA producer: 4 parity sub-tiles per channel group per input plane =====================
     if (lane == 0) {
       const uint32_t box_bytes = (uint32_t)g.P * (uint32_t)g.RR * 16u;
@@ -84,7 +84,7 @@ k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ b
 #pragma unroll
     for (int kd = 0; kd < KD; ++kd) slot16[kd] = ring.slot16(first + kd);
     const int d = o.d0 + od;
-    for (int sc = wg; sc < nsub; sc += kConsumerWG) {
+    for (int sc = wg; sc < nsub; sc += NWG) {
       float acc[NPAD / 2];
       mma_subchunk<NPAD, TIn, KD, NBLK>(acc, slot16, (uint32_t)sc * 64u, sB16, b_lbo16, aoff, alo);
 #pragma unroll
@@ -144,7 +144,8 @@ inline PlanS2 make_plan_s2(int cin, int npad, int kd, int ks, int D, int H, int 
   auto amp = [&](int R, int TW, int, int DR) {
     return (double)(2 * R + ks - 2) / (2 * R) * (double)(2 * TW + ks - 2) / (2 * TW) * (kd == 3 ? (double)(2 * DR + 1) / (2 * DR) : 1.0);
   };
-  auto tile_clk = [&](int DR, int nch) { return 8500.0 + (double)DR * nch * nblk * kd * (45.0 + 0.35 * npad); };
+  const int nwg = conv_nwg(0, npad, 0);
+  auto tile_clk = [&](int DR, int nch) { return (8500.0 + (double)DR * nch * nblk * kd * (45.0 + 0.35 * npad)) * wg_balance(nch, nwg); };
   static_cast<Tile&>(p.g) = plan_tiles(D, H, W, cin / 8, b_image_bytes(kd, nblk, npad), smem_limit, lim, amp, tile_clk, p.smem);
   TDM_CHECK(4 * p.g.slot_pos <= SHRT_MAX, "conv_tc_s2: tap offsets overflow");
   p.g.RR = p.g.R + hk;

@@ -777,17 +777,23 @@ class MvsnetEngine final : public MvsnetIface {
 
   // Tensor-core kernels are launched with programmatic stream serialization (PDL): their prologue and weight-image
   // load overlap the tail of the previous kernel (see Ring::start in conv_tc.cuh).  Each kernel's shared-memory limit
-  // is raised once, on its first launch.
+  // is raised once, on its first launch.  The block size is read from the instantiation itself: its
+  // __launch_bounds__(tc::conv_threads(NWG), 1) is the kernel's maxThreadsPerBlock, i.e. its NWG consumer warpgroups and
+  // the producer warp, so the launch cannot disagree with the barrier counts and the producer index compiled into it.
   template <auto Kern, typename... Args>
   void launch_tc(dim3 grid, size_t smem, Args... args) {
-    static bool attr_set = false;
-    if (!attr_set) {
+    static int threads = 0;
+    if (!threads) {
       TDM_CUDA(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      attr_set = true;
+      cudaFuncAttributes fa{};
+      TDM_CUDA(cudaFuncGetAttributes(&fa, Kern));
+      TDM_CHECK(fa.maxThreadsPerBlock == tc::conv_threads(2) || fa.maxThreadsPerBlock == tc::conv_threads(4),
+                "tensor-core conv: unexpected block size " + std::to_string(fa.maxThreadsPerBlock));
+      threads = fa.maxThreadsPerBlock;
     }
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid;
-    cfg.blockDim = dim3(tc::kThreads);
+    cfg.blockDim = dim3(threads);
     // with PDL an early-launched dependent must not stack several CTAs on the few SMs its predecessor left idle (they would
     // compete for those SMs' issue slots while the rest of the GPU waits): ask for enough shared memory that one CTA fills an SM
     cfg.dynamicSmemBytes = use_pdl_ ? std::max(smem, (size_t)pdl_min_smem_kb_ * 1024) : smem;
@@ -852,7 +858,8 @@ class MvsnetEngine final : public MvsnetIface {
     });
     const tc::Plan& pl = tcx.plan;
     if (profiling_) recs_.back().name = wkey + "[tc-is]";   // the record conv() opened as "[tc]"
-    launch_tc<tc::k_conv_tc_is<TIn, TA, CIN, CPK, PLAIN, Tail>>(dim3(pl.grid), pl.smem, tcx.tmap, (const TIn*)c.bimg_is, (const float*)c.bias,
+    constexpr int NWG = tc::conv_nwg(0, 3 * CPK, Tail::max_d);
+    launch_tc<tc::k_conv_tc_is<TIn, TA, CIN, CPK, PLAIN, Tail, NWG>>(dim3(pl.grid), pl.smem, tcx.tmap, (const TIn*)c.bimg_is, (const float*)c.bias,
                                                                PLAIN ? (TA*)nullptr : (TA*)out.p, PLAIN ? (float*)out.p : (float*)nullptr, pl.g, tail);
   }
 
@@ -890,7 +897,8 @@ class MvsnetEngine final : public MvsnetIface {
       op = (TOut*)out.p;
       if (res) rp = (const TOut*)res->p;
     }
-    launch_tc<tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail>>(dim3(pl.grid, c.nsplit), pl.smem, tcx.tmap, (const TIn*)c.bimg,
+    constexpr int NWG = tc::conv_nwg(MODE, HILO ? 2 * NPAD : NPAD, Tail::max_d);
+    launch_tc<tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail, NWG>>(dim3(pl.grid, c.nsplit), pl.smem, tcx.tmap, (const TIn*)c.bimg,
                                                                               (const float*)c.bias, rp, op, plain, pl.g, tail);
   }
 
@@ -913,7 +921,8 @@ class MvsnetEngine final : public MvsnetIface {
       return x;
     });
     const tc::PlanS2& pl = tcx.plan_s2;
-    launch_tc<tc::k_conv_tc_s2<TA, TA, CIN, NPAD, KD, KS>>(dim3(pl.grid, c.nsplit_s2), pl.smem, tcx.tmap, (const TA*)c.bimg_s2,
+    constexpr int NWG = tc::conv_nwg(0, NPAD, 0);
+    launch_tc<tc::k_conv_tc_s2<TA, TA, CIN, NPAD, KD, KS, NWG>>(dim3(pl.grid, c.nsplit_s2), pl.smem, tcx.tmap, (const TA*)c.bimg_s2,
                                                           (const float*)c.bias, (TA*)out.p, pl.g);
   }
 

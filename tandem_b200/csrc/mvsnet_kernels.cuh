@@ -805,6 +805,7 @@ __global__ void k_regress(const float* __restrict__ logits /*[D][H][W]*/, const 
 template <int MAXD>
 struct RegressTail {
   static constexpr bool enabled = true;
+  static constexpr int max_d = MAXD;
   DminSrc dsrc;
   float* depth;
   float* conf;
