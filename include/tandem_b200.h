@@ -105,6 +105,9 @@ int tdm_debug_homography(const float* K3x3, const float* c2w_ref, const float* c
  * out12 = {ring slots, tile rows, tile cols, pitch, planes per tile, 128-row chunks per plane, slot positions, tiles_w,
  * tiles_h, tiles_d, grid, shared-memory bytes}. */
 int tdm_debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out12);
+/* The same plan with an explicit output count: writes the first n (1..13) values of out12 followed by the consumer
+ * warpgroups of the kernel the plan is made for (the count its tile cost was balanced for). */
+int tdm_debug_conv_plan_n(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out, int n);
 /* Per-kernel CUDA-event timing of one resident forward: writes lines "name ms algorithmic_bytes flops\n"
  * into buf (NUL terminated). Returns bytes written or <0. */
 long long tdm_mvsnet_profile(tdm_mvsnet* h, char* buf, size_t capacity);

@@ -370,13 +370,12 @@ def plan_args(L: Layer, path: str, T_shapes: Dict[str, tuple], precision_tail: b
 
 def query_plan(args, smem_kb: int = 225):
     import ctypes
-    from tandem_b200._lib import lib
-    out = (ctypes.c_longlong * 12)()
-    rc = lib().tdm_debug_conv_plan(*args, smem_kb, out)
+    from tandem_b200._lib import CONV_PLAN_KEYS, lib
+    out = (ctypes.c_longlong * len(CONV_PLAN_KEYS))()
+    rc = lib().tdm_debug_conv_plan_n(*args, smem_kb, out, len(out))
     if rc != 0:
-        raise RuntimeError(f"tdm_debug_conv_plan{args}: {lib().tdm_last_error()}")
-    keys = ("S", "R", "TW", "P", "DR", "nch", "slot_pos", "tiles_w", "tiles_h", "tiles_d", "grid", "smem")
-    return dict(zip(keys, (int(v) for v in out)))
+        raise RuntimeError(f"tdm_debug_conv_plan_n{args}: {lib().tdm_last_error()}")
+    return dict(zip(CONV_PLAN_KEYS, (int(v) for v in out)))
 
 
 def tile_of(args, plan, c, d, h, w):
@@ -385,6 +384,180 @@ def tile_of(args, plan, c, d, h, w):
     if mode in (1, 3):
         d, h, w = (d // 2 if mode == 1 else d), h // 2, w // 2
     return (d // plan["DR"], h // plan["R"], w // plan["TW"])
+
+
+# -------------------------------------------------------------------------------------------------------- launch classes
+# The situations a tensor-core launch can put its kernel in, from its plan_args and plan.  The GPU layer test runs a table
+# of windows (WINDOWS) chosen so that every class the product can reach is run; tests/test_mvsnet_layers_cpu.py enumerates
+# the reachable launches and checks that.
+IS_MAX_CH = 8       # kIsMaxCh (conv_tc_is.cuh): most 128-position chunks per plane of the input-stationary kernel
+
+FAMILY = {0: "k_conv_tc mode 0", 1: "k_conv_tc mode 1 (deconv)", 3: "k_conv_tc mode 3 (up-2)", 100: "k_conv_tc prob tail",
+          200: "k_conv_tc_is", 300: "k_conv_tc_is prob tail", 400: "k_conv_tc_s2"}
+
+
+def shapes(V, H, W, dn):
+    """debug-tensor shapes (C, D, H, W) of the forward (mvsnet.cu ensure_plan)."""
+    S = {"f.img": (8, V, H, W), "f.c0_0": (8, V, H, W), "f.c3": (8, V, H, W), "f.c1_0": (16, V, H // 2, W // 2),
+         "f.c1_1": (16, V, H // 2, W // 2), "f.c2": (16, V, H // 2, W // 2), "f.c2_0": (32, V, H // 4, W // 4),
+         "f.c2_1": (32, V, H // 4, W // 4), "f.c1": (32, V, H // 4, W // 4), "feat1": (32, V, H // 4, W // 4),
+         "f.i2": (32, V, H // 2, W // 2), "f.i2b": (32, V, H // 2, W // 2), "feat2": (16, V, H // 2, W // 2),
+         "f.i3": (32, V, H, W), "feat3": (8, V, H, W)}
+    for s in (1, 2, 3):
+        sc = 1 << (3 - s)
+        h, w, D = H // sc, W // sc, dn[s - 1]
+        D3 = D // 4 if D == 4 else D // 8
+        S.update({f"s{s}.volume": (32 >> (s - 1), D, h, w), f"s{s}.c0": (8, D, h, w), f"s{s}.c1": (16, D // 2, h // 2, w // 2),
+                  f"s{s}.c2": (16, D // 2, h // 2, w // 2), f"s{s}.c3": (32, D // 4, h // 4, w // 4),
+                  f"s{s}.c4": (32, D // 4, h // 4, w // 4), f"s{s}.c5": (64, D3, h // 8, w // 8), f"s{s}.c6": (64, D3, h // 8, w // 8),
+                  f"s{s}.x7": (32, D // 4, h // 4, w // 4), f"s{s}.x9": (16, D // 2, h // 2, w // 2), f"s{s}.x11": (8, D, h, w),
+                  f"s{s}.logits": (1, D, h, w)})
+    return S
+
+
+def default_path(L: Layer, use_is: bool = True) -> str:
+    """The launch a 16-bit engine picks for L with the fused FPN and the direct conv0.0 (mvsnet.cu conv / conv_tc_dispatch)."""
+    if L.out in ("feat1", "f.i2", "f.i2b", "f.i3"):
+        return ""
+    if L.dim == 2:
+        return "tc-s2" if L.stride[0] == 2 else "tc"
+    if L.out.endswith((".c0", ".logits")):
+        return "tc-is" if use_is else "tc"
+    if L.transposed:
+        return "tc" if L.stride[0] == 2 else ""
+    if L.stride == (2, 2, 2):
+        return "tc-s2"
+    return "" if L.stride != (1, 1, 1) else "tc"
+
+
+def window_launches(V: int, H: int, W: int, dn, opts=None, layers=None):
+    """(name, plan_args) of every tensor-core launch of one forward with options opts (use_is, fused_regress; the other
+    options either leave the launches alone or are not modelled here).  layers: only these debug names (None: all)."""
+    opts = opts or {}
+    use_is, tail = opts.get("use_is", 1) == 1, opts.get("fused_regress", 0) == 1
+    S = shapes(V, H, W, dn)
+    out = []
+    for L in layer_table(dn, True, True):
+        if layers is not None and L.out not in layers:
+            continue
+        args = plan_args(L, default_path(L, use_is), S, tail and L.plain)
+        if args is not None:
+            out.append((L.out, args))
+    if layers is None or "feat3" in layers:
+        out.append(("feat3 (out3a)", (32, 64, 1, V, H // 2, W // 2, 0, 3)))
+        out.append(("feat3 (out3b)", (8, 32, 1, V, H, W, 0, 0)))
+    return out
+
+
+def tail_bucket(args) -> int:
+    """RegressTail<MAXD> of a prob launch with the soft-argmin tail (mvsnet.cu TDM_TAIL), 0 without one."""
+    if args[-1] not in (100, 300):
+        return 0
+    D = args[3]
+    return 8 if D <= 8 else 32 if D <= 32 else 48 if D <= 48 else 64
+
+
+def nsplit_of(args) -> int:
+    """blockIdx.y slices of the output columns: the 64-channel layers (conv6, the conv7 deconv) and the stride-2 conv5
+    (32 -> 64) do not fit one B image."""
+    cin, npad, kd, mode = args[0], args[1], args[2], args[-1]
+    if mode == 400:
+        return 2 if (cin == 32 and kd == 3) else 1
+    if mode == 1:
+        return 4 if cin == 64 else 1
+    return 2 if cin == 64 else 1
+
+
+def ring_nin(args, ndo: int) -> int:
+    """Input planes a tile of ndo output planes streams through the ring."""
+    kd, mode = args[2], args[-1]
+    if mode == 400:
+        return 2 * ndo + 1 if kd == 3 else ndo
+    if mode >= 200:
+        return ndo + 2
+    return ndo + kd - 1
+
+
+def launch_classes(args, plan):
+    """(key, classes) of one launch: key = (kernel family, consumer warpgroups, tail bucket), classes the set of situations
+    it puts its kernel in (tile edges, warpgroup occupancy, register partials, ring depth, row pitch, N slicing)."""
+    mode = args[-1]
+    D, H, W = args[3:6]
+    nwg, nsub, S = plan["nwg"], 2 * plan["nch"], plan["S"]
+    c = set()
+    if plan["tiles_w"] == plan["tiles_h"] == plan["tiles_d"] == 1:
+        c.add("single tile")
+    if W % plan["TW"]:
+        c.add("partial W tile")
+    if H % plan["R"]:
+        c.add("partial H tile")
+    if D % plan["DR"]:
+        c.add("partial D tile")
+    # 2 * nch sub-chunks dealt round-robin to nwg warpgroups
+    c.add("idle warpgroups" if nsub < nwg else ("ragged last round" if nsub % nwg else "even rounds"))
+    if mode in (200, 300) and plan["nch"] == IS_MAX_CH:
+        c.add("nch == kIsMaxCh")
+    for ndo in {plan["DR"], D - (plan["tiles_d"] - 1) * plan["DR"]}:
+        nin = ring_nin(args, ndo)
+        c.add("ring nin <= S" if nin <= S else ("ring S < nin <= 2S" if nin <= 2 * S else "ring nin > 2S"))
+    if plan["P"] <= 8:
+        c.add("pitch P <= 8")
+    if nsplit_of(args) > 1:
+        c.add("nsplit > 1")
+    return (FAMILY[mode], nwg, tail_bucket(args)), c
+
+
+# Windows of tests/test_mvsnet_layers_gpu.py::test_layers_launch_classes, each run in both 16-bit precisions on a fresh engine
+# with debug_poison: (V, H, W, depth numbers, options, the (family, NWG, tail bucket, class) it alone runs).  Together they
+# run every launch class the product can reach (tests/test_mvsnet_layers_cpu.py::test_gpu_windows_reach_every_launch_class
+# computes that set and checks it).  Picked greedily by classes run per unit of window size; a window with a depth number
+# of 4 runs the abl04 checkpoint.
+WINDOWS = [
+    (2, 32, 32, (40, 16, 4), {'fused_regress': 1},
+     (('k_conv_tc_is prob tail', 2, 48, 'single tile'),)),
+    (2, 32, 224, (40, 16, 8), {'fused_regress': 1, 'use_is': 0},
+     (('k_conv_tc prob tail', 4, 32, 'even rounds'),)),
+    (2, 32, 32, (8, 56, 40), {'fused_regress': 1},
+     (('k_conv_tc_is prob tail', 4, 8, 'idle warpgroups'), ('k_conv_tc_is prob tail', 4, 8, 'single tile'))),
+    (2, 32, 32, (8, 56, 4), {'fused_regress': 1, 'use_is': 0},
+     (('k_conv_tc prob tail', 2, 64, 'partial H tile'), ('k_conv_tc prob tail', 4, 8, 'idle warpgroups'), ('k_conv_tc prob tail', 4, 8, 'single tile'))),
+    (2, 32, 352, (40, 4, 16), {'fused_regress': 1},
+     (('k_conv_tc_is prob tail', 2, 48, 'partial W tile'),)),
+    (2, 32, 32, (16, 4, 4), {'fused_regress': 1},
+     (('k_conv_tc_is prob tail', 4, 32, 'idle warpgroups'), ('k_conv_tc_is prob tail', 4, 32, 'single tile'))),
+    (2, 32, 32, (16, 40, 4), {'fused_regress': 1, 'use_is': 0},
+     (('k_conv_tc prob tail', 2, 48, 'partial H tile'), ('k_conv_tc prob tail', 4, 32, 'idle warpgroups'), ('k_conv_tc prob tail', 4, 32, 'single tile'))),
+    (13, 96, 448, (8, 4, 4), {'tc_smem_kb': 113},
+     (('k_conv_tc mode 3 (up-2)', 4, 0, 'partial D tile'), ('k_conv_tc mode 3 (up-2)', 4, 0, 'ring nin > 2S'))),
+    (2, 32, 352, (56, 40, 4), {'fused_regress': 1, 'use_is': 0},
+     (('k_conv_tc prob tail', 2, 48, 'partial W tile'), ('k_conv_tc prob tail', 2, 64, 'partial W tile'))),
+    (2, 32, 32, (40, 4, 4), {'fused_regress': 1, 'use_is': 0},
+     (('k_conv_tc prob tail', 2, 48, 'single tile'),)),
+    (2, 32, 32, (56, 4, 4), {'fused_regress': 1},
+     (('k_conv_tc_is prob tail', 2, 64, 'single tile'),)),
+    (2, 32, 32, (56, 4, 4), {'fused_regress': 1, 'use_is': 0},
+     (('k_conv_tc prob tail', 2, 64, 'single tile'),)),
+    (2, 32, 352, (56, 4, 4), {'fused_regress': 1},
+     (('k_conv_tc_is prob tail', 2, 64, 'partial W tile'),)),
+    (5, 160, 608, (8, 4, 4), {'fused_regress': 1},
+     (('k_conv_tc_is prob tail', 4, 8, 'nch == kIsMaxCh'),)),
+    (2, 256, 640, (8, 4, 4), {'fused_regress': 1, 'use_is': 0, 'tc_smem_kb': 113},
+     (('k_conv_tc prob tail', 4, 8, 'ragged last round'),)),
+    (3, 288, 448, (8, 4, 8), {},
+     (('k_conv_tc mode 3 (up-2)', 4, 0, 'ragged last round'), ('k_conv_tc_s2', 4, 0, 'ragged last round'))),
+    (2, 160, 608, (8, 4, 16), {'fused_regress': 1},
+     (('k_conv_tc_is prob tail', 4, 32, 'nch == kIsMaxCh'),)),
+    (2, 288, 448, (8, 24, 4), {'tc_smem_kb': 113},
+     (('k_conv_tc_is', 4, 0, 'ragged last round'),)),
+    (2, 416, 256, (8, 4, 24), {'tc_smem_kb': 113},
+     (('k_conv_tc mode 1 (deconv)', 4, 0, 'ring nin > 2S'),)),
+    (2, 256, 640, (8, 4, 16), {'fused_regress': 1, 'use_is': 0, 'tc_smem_kb': 113},
+     (('k_conv_tc prob tail', 4, 32, 'ragged last round'),)),
+    (2, 224, 512, (8, 4, 40), {'fused_regress': 1},
+     (('k_conv_tc_is prob tail', 2, 48, 'nch == kIsMaxCh'),)),
+    (2, 224, 512, (8, 4, 56), {'fused_regress': 1},
+     (('k_conv_tc_is prob tail', 2, 64, 'nch == kIsMaxCh'),)),
+]
 
 
 # ------------------------------------------------------------------------------------------------------------ cost volume

@@ -33,6 +33,11 @@ def check(rc):
     return rc
 
 
+#: the values tdm_debug_conv_plan_n writes, in order (include/tandem_b200.h; tdm_debug_conv_plan writes the first 12); nwg
+#: is the consumer-warpgroup count of the kernel the plan is made for
+CONV_PLAN_KEYS = ("S", "R", "TW", "P", "DR", "nch", "slot_pos", "tiles_w", "tiles_h", "tiles_d", "grid", "smem", "nwg")
+
+
 class FusionOptions(ctypes.Structure):
     """Field-for-field DrFusionOptions (dr_fusion.h:18-36)."""
     _fields_ = [("voxel_size", ctypes.c_float), ("num_buckets", ctypes.c_int), ("bucket_size", ctypes.c_int),
@@ -107,6 +112,7 @@ def _declare(l):
         "tdm_mvsnet_run_resident_multi": (i, [P(vp), i, i, fp, ip]),
         "tdm_debug_homography": (i, [fp, fp, fp, fp, fp]),
         "tdm_debug_conv_plan": (i, [i, i, i, i, i, i, i, i, i, P(c.c_longlong)]),
+        "tdm_debug_conv_plan_n": (i, [i, i, i, i, i, i, i, i, i, P(c.c_longlong), i]),
         "tdm_mvsnet_profile": (c.c_longlong, [vp, cp, c.c_size_t]),
         "tdm_fusion_create": (i, [P(FusionOptions), i, P(vp)]),
         "tdm_fusion_destroy": (None, [vp]),

@@ -49,12 +49,16 @@ int tdm_debug_homography(const float* K3x3, const float* c2w_ref, const float* c
   TDM_API_END
 }
 
-int tdm_debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out12) {
+int tdm_debug_conv_plan_n(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out, int n) {
   TDM_API_BEGIN
-  TDM_CHECK(out12 && cin >= 8 && npad >= 8 && (kd == 1 || kd == 2 || kd == 3) && D > 0 && H > 0 && W > 0, "bad argument");
-  tdm::debug_conv_plan(cin, npad, kd, D, H, W, pd, mode, smem_kb, out12);
+  TDM_CHECK(out && n >= 1 && n <= 13 && cin >= 8 && npad >= 8 && (kd == 1 || kd == 2 || kd == 3) && D > 0 && H > 0 && W > 0, "bad argument");
+  tdm::debug_conv_plan(cin, npad, kd, D, H, W, pd, mode, smem_kb, out, n);
   return TDM_OK;
   TDM_API_END
+}
+
+int tdm_debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out12) {
+  return tdm_debug_conv_plan_n(cin, npad, kd, D, H, W, pd, mode, smem_kb, out12, 12);
 }
 
 int tdm_mvsnet_create(const char* weights_path, int precision, int device, tdm_mvsnet** out) {

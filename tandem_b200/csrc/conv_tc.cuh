@@ -614,6 +614,7 @@ struct Plan {
   Geom g;
   int grid;
   size_t smem;
+  int nwg;                // consumer warpgroups the tiling was balanced for (conv_nwg); the launch checks its kernel's NWG
 };
 
 // Searches (ring depth, tile width, tile rows, planes per tile) for the cheapest tiling whose B image (b_bytes), ring
@@ -689,6 +690,7 @@ inline Plan make_plan(int cin, int npad, int kd, int D, int H, int W, int pd, in
   static_cast<Tile&>(p.g) = plan_tiles(D, H, W, cin / 8, b_image_bytes(kd, nblk, npad), smem_limit, lim, amp, tile_clk, p.smem);
   p.g.Hp = H + 2; p.g.Wp = W + 2; p.g.pd = pd;
   p.grid = p.g.tiles_w * p.g.tiles_h * p.g.tiles_d;
+  p.nwg = nwg;
   return p;
 }
 

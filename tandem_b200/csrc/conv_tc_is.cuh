@@ -184,6 +184,7 @@ inline Plan make_plan_is(int cin, int cpk, int D, int H, int W, size_t smem_limi
   static_cast<Tile&>(p.g) = plan_tiles(D, H, W, cin / 8, b_image_bytes(1, nblk, n3), smem_limit, lim, amp, tile_clk, p.smem);
   p.g.Hp = H + 2; p.g.Wp = W + 2; p.g.pd = 1;
   p.grid = p.g.tiles_w * p.g.tiles_h * p.g.tiles_d;
+  p.nwg = nwg;
   return p;
 }
 

@@ -132,6 +132,7 @@ struct PlanS2 {
   GeomS2 g;
   int grid;
   size_t smem;
+  int nwg;                 // as Plan::nwg
 };
 
 // D,H,W: OUTPUT dims.  kd in {1,3}.
@@ -150,6 +151,7 @@ inline PlanS2 make_plan_s2(int cin, int npad, int kd, int ks, int D, int H, int 
   TDM_CHECK(4 * p.g.slot_pos <= SHRT_MAX, "conv_tc_s2: tap offsets overflow");
   p.g.RR = p.g.R + hk;
   p.grid = p.g.tiles_w * p.g.tiles_h * p.g.tiles_d;
+  p.nwg = nwg;
   return p;
 }
 

@@ -196,11 +196,15 @@ class MvsnetEngine final : public MvsnetIface {
     else if (key == "pdl_min_smem_kb") { TDM_CHECK(value >= 0 && value <= 225, "pdl_min_smem_kb out of range"); pdl_min_smem_kb_ = value; }
     else if (key == "cv_variant") { TDM_CHECK(value >= 0 && value <= 5, "cv_variant out of range"); cv_variant_ = value; }
     else if (key == "tc_smem_kb") { TDM_CHECK(value >= 48 && value <= 225, "tc_smem_kb out of range"); tc_smem_kb_ = value; tc_cache_.clear(); }
-    else if (key.rfind("depth_num_stage", 0) == 0 && key.size() == 16 && key[15] >= '1' && key[15] <= '3') {
-      // override the checkpoint's MODEL.DEPTH_NUM for one stage (BASELINE.json configs[0] uses 32 stage-1 hypotheses;
-      // CostRegNet is fully convolutional in D).  Forces a re-plan.
-      TDM_CHECK(value == 4 || (value > 0 && value % 8 == 0 && value <= 64), "depth_num must be 4 or a multiple of 8 up to 64");
-      depth_num_[key[15] - '1'] = value;
+    else if ((key.rfind("depth_num_stage", 0) == 0 && key.size() == 16 && key[15] >= '1' && key[15] <= '3') || key == "debug_poison") {
+      // depth_num_stageN: override the checkpoint's MODEL.DEPTH_NUM for one stage (BASELINE.json configs[0] uses 32 stage-1
+      // hypotheses; CostRegNet is fully convolutional in D).  debug_poison: see alloc.  Both force a re-plan.
+      if (key == "debug_poison") {
+        debug_poison_ = value != 0;
+      } else {
+        TDM_CHECK(value == 4 || (value > 0 && value % 8 == 0 && value <= 64), "depth_num must be 4 or a multiple of 8 up to 64");
+        depth_num_[key[15] - '1'] = value;
+      }
       // the old plan's buffers are sized for the old D: drop them together with the resident window, so that neither
       // run_resident / profile nor a stale logits buffer can be used before the next CallAsync re-plans
       free_plan();
@@ -633,6 +637,22 @@ class MvsnetEngine final : public MvsnetIface {
     }
     TDM_CUDA(cudaMalloc(&b.p, b.bytes));
     TDM_CUDA(cudaMemsetAsync(b.p, 0, b.bytes, stream_));  // halos stay zero forever: kernels only write the interior
+    if (debug_poison_) {
+      // all-ones bytes are a NaN in fp32, fp16 and bf16: a position the forward should have stored but did not reads as
+      // non-finite instead of as a plausible 0 (which a ReLU layer's true output often is).  The P8 interiors and the
+      // logits are poisoned; the other fp32 maps are not all written by every forward (depth / confidence / edge of the
+      // stages the edge filter skips, dmin with inline_dmin, thr's spare entry) and keep their zeros.
+      if (!f32) {
+        const size_t row = (size_t)(W + 2) * 8 * es;
+        for (int p = 0; p < (C / 8) * (D + 2 * b.pd); ++p) {
+          const int d = p % (D + 2 * b.pd);
+          if (d < b.pd || d >= D + b.pd) continue;
+          TDM_CUDA(cudaMemset2DAsync((uint8_t*)b.p + ((size_t)p * (H + 2) + 1) * row + 8 * es, row, 0xFF, (size_t)W * 8 * es, H, stream_));
+        }
+      } else if (name.size() >= 6 && name.compare(name.size() - 6, 6, "logits") == 0) {
+        TDM_CUDA(cudaMemsetAsync(b.p, 0xFF, b.bytes, stream_));
+      }
+    }
     bufs_[name] = b;
     return bufs_[name];
   }
@@ -859,6 +879,7 @@ class MvsnetEngine final : public MvsnetIface {
     const tc::Plan& pl = tcx.plan;
     if (profiling_) recs_.back().name = wkey + "[tc-is]";   // the record conv() opened as "[tc]"
     constexpr int NWG = tc::conv_nwg(0, 3 * CPK, Tail::max_d);
+    TDM_CHECK(pl.nwg == NWG, wkey + ": tile plan balanced for another warpgroup count than the kernel's");
     launch_tc<tc::k_conv_tc_is<TIn, TA, CIN, CPK, PLAIN, Tail, NWG>>(dim3(pl.grid), pl.smem, tcx.tmap, (const TIn*)c.bimg_is, (const float*)c.bias,
                                                                PLAIN ? (TA*)nullptr : (TA*)out.p, PLAIN ? (float*)out.p : (float*)nullptr, pl.g, tail);
   }
@@ -898,6 +919,7 @@ class MvsnetEngine final : public MvsnetIface {
       if (res) rp = (const TOut*)res->p;
     }
     constexpr int NWG = tc::conv_nwg(MODE, HILO ? 2 * NPAD : NPAD, Tail::max_d);
+    TDM_CHECK(pl.nwg == NWG, wkey + ": tile plan balanced for another warpgroup count than the kernel's");
     launch_tc<tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail, NWG>>(dim3(pl.grid, c.nsplit), pl.smem, tcx.tmap, (const TIn*)c.bimg,
                                                                               (const float*)c.bias, rp, op, plain, pl.g, tail);
   }
@@ -922,6 +944,7 @@ class MvsnetEngine final : public MvsnetIface {
     });
     const tc::PlanS2& pl = tcx.plan_s2;
     constexpr int NWG = tc::conv_nwg(0, NPAD, 0);
+    TDM_CHECK(pl.nwg == NWG, wkey + ": tile plan balanced for another warpgroup count than the kernel's");
     launch_tc<tc::k_conv_tc_s2<TA, TA, CIN, NPAD, KD, KS, NWG>>(dim3(pl.grid, c.nsplit_s2), pl.smem, tcx.tmap, (const TA*)c.bimg_s2,
                                                           (const float*)c.bias, (TA*)out.p, pl.g);
   }
@@ -1540,6 +1563,7 @@ class MvsnetEngine final : public MvsnetIface {
   cudaStream_t side_stream_ = nullptr;
   cudaEvent_t ev_fork_ = nullptr, ev_join_ = nullptr;
   bool filter_all_ = false, keep_ = true, use_tc_ = (sizeof(TA) == 2);  // tensor-core convs are the default on 16-bit engines
+  bool debug_poison_ = false;  // set_option("debug_poison", 1): activation interiors start as NaN (alloc), for the layer tests
   bool profiling_ = false;
   int launch_count_ = 0, launches_per_forward_ = 0;
   std::vector<LaunchRec> recs_;
@@ -1579,9 +1603,10 @@ void debug_homography(const float* K3x3, const float* c2w_ref, const float* c2w_
   }
 }
 
-// host-only view of the tensor-core tile planner (no GPU involved; used by the CPU test-suite): out12 = {S, R, TW, P, DR, nch,
-// slot_pos, tiles_w, tiles_h, tiles_d, grid, smem_bytes}
-void debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out12) {
+// host-only view of the tensor-core tile planner (no GPU involved; used by the CPU test-suite): the first n (<= 13) of {S, R,
+// TW, P, DR, nch, slot_pos, tiles_w, tiles_h, tiles_d, grid, smem_bytes, nwg}; nwg is the consumer-warpgroup count the plan
+// was made for, which every launch checks against its kernel's NWG
+void debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out, int n) {
   // mode + 100 = the same mode with tiles that span all D planes (the prob layer with the soft-argmin tail);
   // mode 200 = the input-stationary planner (make_plan_is) with npad = columns per kd block (kd and pd are implied: 3, 1),
   // mode 300 = the same with tiles that span all D planes,
@@ -1590,15 +1615,15 @@ void debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int
     TDM_CHECK((kd == 1 || kd == 3) && (pd == 3 || pd == 5), "mode 400: kd must be 1 or 3 and pd the kernel size 3 or 5");
     const tc::PlanS2 p = tc::make_plan_s2(cin, npad, kd, pd, D, H, W, (size_t)smem_kb * 1024);
     const tc::GeomS2& g = p.g;
-    const long long v[12] = {g.S, g.R, g.TW, g.P, g.DR, g.nch, g.slot_pos, g.tiles_w, g.tiles_h, g.tiles_d, p.grid, (long long)p.smem};
-    for (int i = 0; i < 12; ++i) out12[i] = v[i];
+    const long long v[13] = {g.S, g.R, g.TW, g.P, g.DR, g.nch, g.slot_pos, g.tiles_w, g.tiles_h, g.tiles_d, p.grid, (long long)p.smem, p.nwg};
+    for (int i = 0; i < n; ++i) out[i] = v[i];
     return;
   }
   const tc::Plan p = mode >= 200 ? tc::make_plan_is(cin, npad, D, H, W, (size_t)smem_kb * 1024, mode == 300)
                                  : tc::make_plan(cin, npad, kd, D, H, W, pd, mode % 100, (size_t)smem_kb * 1024, mode >= 100);
   const tc::Geom& g = p.g;
-  const long long v[12] = {g.S, g.R, g.TW, g.P, g.DR, g.nch, g.slot_pos, g.tiles_w, g.tiles_h, g.tiles_d, p.grid, (long long)p.smem};
-  for (int i = 0; i < 12; ++i) out12[i] = v[i];
+  const long long v[13] = {g.S, g.R, g.TW, g.P, g.DR, g.nch, g.slot_pos, g.tiles_w, g.tiles_h, g.tiles_d, p.grid, (long long)p.smem, p.nwg};
+  for (int i = 0; i < n; ++i) out[i] = v[i];
 }
 
 }  // namespace tdm

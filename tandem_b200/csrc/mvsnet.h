@@ -26,6 +26,6 @@ class MvsnetIface {
 
 MvsnetIface* make_mvsnet(const std::string& weights_path, int precision, int device);
 void debug_homography(const float* K3x3, const float* c2w_ref, const float* c2w_src, float* rot9, float* trans3);
-void debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out12);
+void debug_conv_plan(int cin, int npad, int kd, int D, int H, int W, int pd, int mode, int smem_kb, long long* out, int n);
 
 }  // namespace tdm

@@ -110,7 +110,7 @@ def test_wgmma_tile_planner_invariants():
     memory, the wgmma N limit and the TMA box limit.  Stride-2 plans (mode 400) read sub-tiles of pitch P = TW + KS/2,
     whose TMA boxes span 2 * P columns."""
     l = lib()
-    out = (ctypes.c_longlong * 12)()
+    out = (ctypes.c_longlong * 13)()
     shapes = []
     for (H, W, V, Ds) in [(480, 640, 7, (48, 32, 8)), (256, 320, 4, (32, 32, 8)), (96, 128, 2, (32, 8, 8))]:
         # FeatureNet: 2-D convs over V planes (kd = 1, pd = 0)
@@ -138,9 +138,10 @@ def test_wgmma_tile_planner_invariants():
                 shapes.append((cin, npad, 3, d2, h2, w2, 3, 400))           # conv1 / conv3 / conv5: 3x3x3 stride 2
     assert len(shapes) > 40
     for (cin, npad, kd, D, H, W, pd, mode) in shapes:
-        rc = l.tdm_debug_conv_plan(cin, npad, kd, D, H, W, pd, mode, 225, out)
+        rc = l.tdm_debug_conv_plan_n(cin, npad, kd, D, H, W, pd, mode, 225, out, 13)
         assert rc == 0, (cin, npad, kd, D, H, W, mode, l.tdm_last_error())
-        S, R, TW, P, DR, nch, slot_pos, tw, th, td, grid, smem = [int(x) for x in out]
+        S, R, TW, P, DR, nch, slot_pos, tw, th, td, grid, smem, nwg = [int(x) for x in out]
+        assert nwg in (2, 4), (cin, npad, kd, D, H, W, mode, nwg)       # consumer warpgroups of 128 threads + 1 producer warp
         if mode >= 100 and mode != 400:
             assert td == 1 and DR == D, (D, H, W, DR, td)
             mode -= 100
@@ -159,6 +160,18 @@ def test_wgmma_tile_planner_invariants():
         assert grid == tw * th * td and grid >= 1, key
         assert nch == (R * P + 127) // 128 and npad % 8 == 0 and npad <= 256, key      # wgmma m64nNk16: N <= 256
         assert smem <= 225 * 1024 and slot_pos % 8 == 0 and slot_pos >= (R + 2) * P, key
+
+
+def test_conv_plan_twelve_value_entry_point_writes_twelve():
+    """tdm_debug_conv_plan keeps its 12-entry output for existing callers; tdm_debug_conv_plan_n adds the warpgroup count."""
+    l = lib()
+    for args in [(8, 32, 1, 7, 480, 640, 0, 0), (8, 8, 3, 48, 120, 160, 1, 300), (32, 32, 3, 8, 30, 40, 3, 400)]:
+        a = (ctypes.c_longlong * 13)(*([-7] * 13))
+        b = (ctypes.c_longlong * 13)()
+        assert l.tdm_debug_conv_plan(*args, 225, a) == 0 and l.tdm_debug_conv_plan_n(*args, 225, b, 13) == 0, l.tdm_last_error()
+        assert list(a[:12]) == list(b[:12]) and a[12] == -7 and b[12] in (2, 4), (args, list(a), list(b))
+    c = (ctypes.c_longlong * 14)()
+    assert l.tdm_debug_conv_plan_n(8, 32, 1, 7, 480, 640, 0, 0, 225, c, 14) != 0
 
 
 def test_constant_division_is_correctly_rounded(tmp_path):

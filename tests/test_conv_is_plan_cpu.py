@@ -1,5 +1,5 @@
 """CPU-side invariants of the input-stationary tile planner (make_plan_is in tandem_b200/csrc/conv_tc_is.cuh), queried
-through tdm_debug_conv_plan mode 200 (300: tiles span all D planes) for every stride-1 3x3x3 layer it serves: each stage's conv0 and prob."""
+through tdm_debug_conv_plan_n mode 200 (300: tiles span all D planes) for every stride-1 3x3x3 layer it serves: each stage's conv0 and prob."""
 import ctypes
 
 from tandem_b200._lib import lib
@@ -23,13 +23,15 @@ def _shapes():
 
 def test_input_stationary_plans_cover_the_layer_and_fit_the_sm():
     l = lib()
-    out = (ctypes.c_longlong * 12)()
+    out = (ctypes.c_longlong * 13)()
     for (cin, cpk, D, H, W, *mode) in _shapes():
         mode = mode[0] if mode else IS_MODE
-        rc = l.tdm_debug_conv_plan(cin, cpk, 3, D, H, W, 1, mode, 225, out)
+        rc = l.tdm_debug_conv_plan_n(cin, cpk, 3, D, H, W, 1, mode, 225, out, 13)
         key = (cin, cpk, D, H, W, mode)
         assert rc == 0, (key, l.tdm_last_error())
-        S, R, TW, P, DR, nch, slot_pos, tw, th, td, grid, smem = [int(x) for x in out]
+        S, R, TW, P, DR, nch, slot_pos, tw, th, td, grid, smem, nwg = [int(x) for x in out]
+        # the kernel's partial arrays hold 2 * MAX_CH / nwg sub-chunks per warpgroup, exactly its share
+        assert nwg in (2, 4) and (2 * MAX_CH) % nwg == 0, (key, nwg)
         # coverage: the tiles partition the output exactly
         assert P == TW + 2 and P <= 256 and R >= 1 and DR >= 1, key
         assert tw * TW >= W and (tw - 1) * TW < W and th * R >= H and (th - 1) * R < H, key

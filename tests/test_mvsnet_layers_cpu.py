@@ -1,6 +1,8 @@
 """CPU checks of the fp64 per-layer reference (oracle/mvsnet_layers.py) that tests/test_mvsnet_layers_gpu.py applies to
 the engine: a faithful simulation of a 16-bit layer never exceeds the bound, the subtle kernel faults the GPU test exists
-to catch always do, and the GPU test's windows drive every tile planner into single tiles and partial last tiles."""
+to catch always do (also at the plan geometry of the four-warpgroup kernels), and the GPU test's windows run every launch
+class (tile edges, warpgroup occupancy, register partials, ring depth: oracle/mvsnet_layers.py launch_classes) the product
+can reach."""
 import numpy as np
 import pytest
 import torch
@@ -13,23 +15,7 @@ W_ABL03, _, _ = load_tdmw(default_weights("abl03_view_aggregation"))
 DT = {"mixed16": torch.float16, "bf16": torch.bfloat16}
 
 
-def shapes(V, H, W, dn):
-    """debug-tensor shapes (C, D, H, W) of the forward (mvsnet.cu ensure_plan)."""
-    S = {"f.img": (8, V, H, W), "f.c0_0": (8, V, H, W), "f.c3": (8, V, H, W), "f.c1_0": (16, V, H // 2, W // 2),
-         "f.c1_1": (16, V, H // 2, W // 2), "f.c2": (16, V, H // 2, W // 2), "f.c2_0": (32, V, H // 4, W // 4),
-         "f.c2_1": (32, V, H // 4, W // 4), "f.c1": (32, V, H // 4, W // 4), "feat1": (32, V, H // 4, W // 4),
-         "f.i2": (32, V, H // 2, W // 2), "f.i2b": (32, V, H // 2, W // 2), "feat2": (16, V, H // 2, W // 2),
-         "f.i3": (32, V, H, W), "feat3": (8, V, H, W)}
-    for s in (1, 2, 3):
-        sc = 1 << (3 - s)
-        h, w, D = H // sc, W // sc, dn[s - 1]
-        D3 = D // 4 if D == 4 else D // 8
-        S.update({f"s{s}.volume": (32 >> (s - 1), D, h, w), f"s{s}.c0": (8, D, h, w), f"s{s}.c1": (16, D // 2, h // 2, w // 2),
-                  f"s{s}.c2": (16, D // 2, h // 2, w // 2), f"s{s}.c3": (32, D // 4, h // 4, w // 4),
-                  f"s{s}.c4": (32, D // 4, h // 4, w // 4), f"s{s}.c5": (64, D3, h // 8, w // 8), f"s{s}.c6": (64, D3, h // 8, w // 8),
-                  f"s{s}.x7": (32, D // 4, h // 4, w // 4), f"s{s}.x9": (16, D // 2, h // 2, w // 2), f"s{s}.x11": (8, D, h, w),
-                  f"s{s}.logits": (1, D, h, w)})
-    return S
+shapes = ML.shapes
 
 
 def r16(t, precision):
@@ -251,82 +237,189 @@ def test_regress_and_filter_mutations_are_caught():
     assert ML.edge_cutoff(H * W, 0.0) == H * W - 1 and ML.edge_cutoff(H * W, 100.0) == 0
 
 
-# ------------------------------------------------------------------------------------------------------------ tile coverage
-# the windows of tests/test_mvsnet_layers_gpu.py: (V, H, W, depth numbers)
-# (V, H, W, depth numbers, prob tails run there: "is" fused_regress=1, "os" fused_regress=1 with use_is=0)
-GPU_WINDOWS = [(7, 480, 640, (48, 32, 8), ()), (7, 320, 512, (48, 4, 4), ()), (2, 96, 128, (16, 24, 40), ()),
-               (16, 224, 288, (56, 64, 8), ()), (4, 352, 480, (24, 40, 56), ("is", "os")), (2, 96, 128, (16, 24, 8), ("is",)),
-               (2, 32, 64, (8, 8, 8), ())]
+# ------------------------------------------------------------------------------------------------------------ launch classes
+# What the product can launch: H and W multiples of 32 up to 480 x 640, 2 to 16 views, every legal depth number per stage
+# (4 at stages 2 and 3 as in the abl04 checkpoint, 8 to 64 in steps of 8), use_is 1 / 0, the fused soft-argmin tails, and
+# tc_smem_kb 225 / 113.  The 2-D layers depend on (V, H, W) only, a stage's 3-D layers on its depth number and (H, W) only.
+OPTS_3D = ({}, {"use_is": 0}, {"fused_regress": 1}, {"fused_regress": 1, "use_is": 0})
 
 
-def _default_path(L, dn):
-    """The launch the mixed16 engine picks for L with default options (mvsnet.cu conv / conv_tc_dispatch)."""
-    if L.out in ("feat1", "f.i2", "f.i2b", "f.i3"):
-        return ""
-    if L.dim == 2:
-        return "tc-s2" if L.stride[0] == 2 else "tc"
-    if L.out.endswith((".c0", ".logits")):
-        return "tc-is"
-    if L.transposed:
-        return "tc" if L.stride[0] == 2 else ""
-    if L.stride == (2, 2, 2):
-        return "tc-s2"
-    return "" if L.stride != (1, 1, 1) else "tc"
+def _reachable_launches():
+    """{(plan_args, smem_kb)} of every tensor-core launch the product can make (deduplicated: the plan depends on nothing else)."""
+    table = ML.layer_table((8, 8, 8), True, True)
+    names2d = [L.out for L in table if L.dim == 2] + ["feat3"]
+    sizes = [(H, W) for H in range(32, 481, 32) for W in range(32, 641, 32)]
+    args = set()
+    for V in range(2, 17):
+        for H, W in sizes:
+            args.update(a for _, a in ML.window_launches(V, H, W, (8, 8, 8), None, names2d))
+    for s in (1, 2, 3):
+        names = [L.out for L in table if L.out.startswith(f"s{s}.")]
+        for D in ([4] if s > 1 else []) + list(range(8, 65, 8)):
+            dn = tuple(D if i == s - 1 else 8 for i in range(3))
+            for H, W in sizes:
+                for opts in OPTS_3D:
+                    args.update(a for _, a in ML.window_launches(2, H, W, dn, opts, names))
+    return {(a, smem) for a in args for smem in (225, 113)}
 
 
-def _family(args):
-    mode = args[-1]
-    return {0: "mode 0 (stride 1)", 1: "mode 1 (deconv)", 3: "mode 3 (up-2)", 100: "mode 100 (prob tail)",
-            200: "mode 200 (input-stationary)", 300: "mode 300 (input-stationary prob tail)", 400: "stride-2"}[mode]
+def _window_classes(windows):
+    """(key, class) -> first window of the table that runs it."""
+    hit = {}
+    for V, H, W, dn, opts, *_ in windows:
+        smem = opts.get("tc_smem_kb", 225)
+        for name, args in ML.window_launches(V, H, W, dn, opts):
+            key, cls = ML.launch_classes(args, ML.query_plan(args, smem))
+            for c in cls:
+                hit.setdefault((key, c), f"{W}x{H}v{V} {dn} {opts or ''} {name}")
+    return hit
 
 
-# what these windows do not reach: no single-tile layer of the input-stationary and up-2 planners or of the prob tails (their
-# smallest layers are still split), no partial W tile of the input-stationary tail, and the 2-D up-2 layer splits its view
-# axis only at 113 KB.  The tails span all of D by construction.
-NO_SINGLE = ("mode 200 (input-stationary)", "mode 3 (up-2)", "mode 100 (prob tail)", "mode 300 (input-stationary prob tail)")
-NO_PARTIAL_D = ("mode 3 (up-2)", "mode 100 (prob tail)", "mode 300 (input-stationary prob tail)")
-NO_PARTIAL_W = ("mode 300 (input-stationary prob tail)",)
+def _unrun(windows, reachable):
+    hit = _window_classes(windows)
+    return sorted(kc for kc in reachable if kc not in hit), hit
 
 
-@pytest.mark.parametrize("smem_kb", [225, 113])
-def test_gpu_windows_reach_single_and_partial_tiles(smem_kb):
-    seen = {}
-    for V, H, W, dn, tails in GPU_WINDOWS:
-        S = shapes(V, H, W, dn)
-        todo = []
+def test_gpu_windows_reach_every_launch_class():
+    """Every (kernel family, consumer warpgroups, tail bucket, class) a product launch can reach is run by a window of
+    ML.WINDOWS, which tests/test_mvsnet_layers_gpu.py runs in both 16-bit precisions."""
+    reachable = {}
+    for args, smem in _reachable_launches():
+        key, cls = ML.launch_classes(args, ML.query_plan(args, smem))
+        for c in cls:
+            reachable.setdefault((key, c), (args, smem))
+    unrun, hit = _unrun(ML.WINDOWS, reachable)
+    print(f"\n{len(reachable)} reachable launch classes, {len(ML.WINDOWS)} windows:")
+    for (fam, nwg, bucket), c in sorted(reachable):
+        where = hit.get(((fam, nwg, bucket), c), "NOT RUN")
+        print(f"  {fam:28s} NWG {nwg} tail {bucket:2d}  {c:20s} {where}")
+    assert not unrun, "reachable but run by no window: " + "; ".join(
+        f"{k} {c} (e.g. plan_args {reachable[(k, c)][0]} at {reachable[(k, c)][1]} KB)" for k, c in unrun)
+    # the table is minimal in the sense that each window runs a class no other window runs
+    for i in range(len(ML.WINDOWS)):
+        rest = ML.WINDOWS[:i] + ML.WINDOWS[i + 1:]
+        assert _unrun(rest, reachable)[0], f"window {ML.WINDOWS[i]} runs no class of its own"
+
+
+# -------------------------------------------------------------------------------------------- mutations at the plan geometry
+def _find_launch(fam, cls, paths=("tc", "tc-is"), need=None):
+    """The smallest layer of the GPU windows whose launch (family fam, on a path simulate() models) reaches class cls and
+    satisfies need(args, plan): (layer, path, shapes, plan_args, plan)."""
+    best = None
+    for V, H, W, dn, opts, _ in ML.WINDOWS:
+        S = ML.shapes(V, H, W, dn)
+        smem = opts.get("tc_smem_kb", 225)
+        use_is, tail = opts.get("use_is", 1) == 1, opts.get("fused_regress", 0) == 1
         for L in ML.layer_table(dn, True, True):
-            path = _default_path(L, dn)
-            args = ML.plan_args(L, path, S)
-            if args is not None:
-                todo.append((L.out, args))
-                if path == "tc-is" and (V, H, W) == (2, 96, 128):          # the use_is=0 option runs this window
-                    todo.append((L.out + " (use_is=0)", ML.plan_args(L, "tc", S)))
-                if L.plain:
-                    for t in tails:
-                        todo.append((L.out + f" ({t} tail)", ML.plan_args(L, "tc-is" if t == "is" else "tc", S, True)))
-        todo.append(("feat3 (out3a)", (32, 64, 1, V, H // 2, W // 2, 0, 3)))
-        todo.append(("feat3 (out3b)", (8, 32, 1, V, H, W, 0, 0)))
-        for name, args in todo:
-            pl = ML.query_plan(args, smem_kb)
-            D, Hh, Ww = args[3:6]
-            fam = _family(args)
-            hit = seen.setdefault(fam, {"single": [], "W": [], "H": [], "D": []})
-            where = f"{W}x{H}v{V} {name} ({D}x{Hh}x{Ww}: TW {pl['TW']} R {pl['R']} DR {pl['DR']})"
-            if pl["tiles_w"] == pl["tiles_h"] == pl["tiles_d"] == 1:
-                hit["single"].append(where)
-            if Ww % pl["TW"]:
-                hit["W"].append(where)
-            if Hh % pl["R"]:
-                hit["H"].append(where)
-            if D % pl["DR"]:
-                hit["D"].append(where)
-    print(f"\ntile coverage at {smem_kb} KB:")
-    for fam, hit in sorted(seen.items()):
-        for k in ("single", "W", "H", "D"):
-            print(f"  {fam:30s} {k:6s} {len(hit[k]):3d}  e.g. {hit[k][0] if hit[k] else '-'}")
-    for fam, hit in seen.items():
-        assert (hit["W"] or fam in NO_PARTIAL_W) and hit["H"], (fam, {k: len(v) for k, v in hit.items()})
-        if fam not in NO_SINGLE:
-            assert hit["single"], (fam, "no single-tile layer")
-        if fam not in NO_PARTIAL_D:
-            assert hit["D"], (fam, "no partial depth tile")
+            path = ML.default_path(L, use_is)
+            if path not in paths or L.transposed:
+                continue
+            args = ML.plan_args(L, path, S, tail and L.plain)
+            pl = ML.query_plan(args, smem)
+            key, c = ML.launch_classes(args, pl)
+            size = int(np.prod(S[L.out]))
+            if key[0] == fam and cls in c and (need is None or need(args, pl)) and (best is None or size < best[0]):
+                best = (size, L, path, S, args, pl)
+    assert best is not None, (fam, cls)
+    return best[1:]
+
+
+def _subchunk_pixels(args, pl, sc, tile=(0, 0)):
+    """{tile position l: (h, w)} of the output pixels sub-chunk sc of tile (th, tw) stores (frag_pixel: l = row * P + col,
+    pad columns and positions beyond the grid dropped)."""
+    H, W = args[4], args[5]
+    h0, w0 = tile[0] * pl["R"], tile[1] * pl["TW"]
+    out = {}
+    for l in range(sc * 64, sc * 64 + 64):
+        hh, ww = divmod(l, pl["P"])
+        if hh < pl["R"] and ww < pl["TW"] and h0 + hh < H and w0 + ww < W:
+            out[l] = (h0 + hh, w0 + ww)
+    return out
+
+
+def _sim(L, path, S, rng, weights=W_ABL03, T=None):
+    T = T or {n: rand16(S[n], "mixed16", rng) for n in (L.inp, L.res) if n}
+    y, ar = simulate(L, T, "mixed16", path, weights=weights)
+    return T, y, ar
+
+
+def test_warpgroup_and_ring_mutations_are_caught():
+    """Faults of the four-warpgroup kernels, simulated at the plan the planner makes for a layer of the GPU windows: a
+    position a kernel does not store holds the debug_poison NaN."""
+    rng = np.random.default_rng(5)
+    caught = {}
+    # ragged last round: the last round's sub-chunks of tile (0, 0), plane 0 not stored / copied from sub-chunk sc - NWG
+    for fam in ("k_conv_tc mode 0", "k_conv_tc_is"):
+        L, path, S, args, pl = _find_launch(fam, "ragged last round")
+        T, y, ar = _sim(L, path, S, rng)
+        nsub, nwg = 2 * pl["nch"], pl["nwg"]
+        last = range(nsub - nsub % nwg, nsub)
+        yn, yc = y.copy(), y.copy()
+        for sc in last:
+            src = _subchunk_pixels(args, pl, sc - nwg)
+            for l, (h, w) in _subchunk_pixels(args, pl, sc).items():
+                yn[:, 0, h, w] = np.nan
+                if l - 64 * nwg in src:
+                    yc[:, 0, h, w] = y[(slice(None), 0) + src[l - 64 * nwg]]
+        what = f"{L.out} [{fam}, nch {pl['nch']}, NWG {nwg}]: last round's sub-chunks {list(last)}"
+        caught[what + " not stored"] = _caught(L, T, yn, ar)
+        caught[what + f" copied from sub-chunk sc - {nwg}"] = _caught(L, T, yc, ar)
+    # idle warpgroups (nch == 1): sub-chunk 1 not stored, on every plane of tile (0, 0)
+    for fam in ("k_conv_tc mode 0", "k_conv_tc_is"):
+        L, path, S, args, pl = _find_launch(fam, "idle warpgroups", need=lambda a, p: _subchunk_pixels(a, p, 1))
+        T, y, ar = _sim(L, path, S, rng)
+        yn = y.copy()
+        for h, w in _subchunk_pixels(args, pl, 1).values():
+            yn[:, :pl["DR"], h, w] = np.nan
+        caught[f"{L.out} [{fam}, nch {pl['nch']}, NWG {pl['nwg']}]: sub-chunk 1 not stored"] = _caught(L, T, yn, ar)
+    # nch == kIsMaxCh: sub-chunks NWG * (KSUB - 1) + wg (the last entries of the partial arrays) miss the kd = 1 fold
+    L, path, S, args, pl = _find_launch("k_conv_tc_is", "nch == kIsMaxCh")
+    T, y, ar = _sim(L, path, S, rng)
+    w_nokd1 = dict(W_ABL03)
+    w_nokd1[L.conv_w] = np.asarray(W_ABL03[L.conv_w]).copy()
+    w_nokd1[L.conv_w][:, :, 1] = 0
+    _, yk, _ = _sim(L, path, S, rng, weights=w_nokd1, T=T)
+    nwg = pl["nwg"]
+    ksub = 2 * ML.IS_MAX_CH // nwg
+    yb = y.copy()
+    for th in range(pl["tiles_h"]):
+        for tw in range(pl["tiles_w"]):
+            for wg in range(nwg):
+                for h, w in _subchunk_pixels(args, pl, nwg * (ksub - 1) + wg, (th, tw)).values():
+                    yb[:, :, h, w] = yk[:, :, h, w]
+    caught[f"{L.out} [k_conv_tc_is, nch {pl['nch']} == kIsMaxCh, NWG {nwg}]: sub-chunks {nwg * (ksub - 1)}.. miss the kd=1 fold"] = \
+        _caught(L, T, yb, ar)
+    # ring wrap: output plane od = S - 1 of tile 0 reads its newest input plane from the slot S planes stale
+    for fam in ("k_conv_tc mode 0", "k_conv_tc_is"):
+        L, path, S, args, pl = _find_launch(fam, "ring nin > 2S")
+        if L.dim != 3:
+            continue
+        T, y, ar = _sim(L, path, S, rng)
+        od = pl["S"] - 1                      # newest padded input plane od + 2 >= S: its slot held plane od + 2 - S before
+        x = T[L.inp]
+        T2 = dict(T)
+        T2[L.inp] = x.copy()
+        stale = od + 1 - pl["S"]
+        T2[L.inp][:, od + 1] = x[:, stale] if stale >= 0 else 0
+        _, y2, _ = _sim(L, path, S, rng, T=T2)
+        yb = y.copy()
+        yb[:, od] = y2[:, od]
+        caught[f"{L.out} [{fam}, S {pl['S']}, DR {pl['DR']}]: output plane {od} from an input plane {pl['S']} slots stale"] = \
+            _caught(L, T, yb, ar)
+    assert len(caught) == 9 and all(caught.values()), {k: v for k, v in caught.items() if not v} or caught
+    print("\n" + "\n".join(f"caught: {k}" for k in caught))
+
+
+@pytest.mark.parametrize("precision", ["mixed16", "bf16"])
+def test_faithful_16bit_layer_stays_within_bound_at_window_plans(precision):
+    """The faithful simulation of the layers the mutation test picks from the GPU windows stays within the bound."""
+    rng = np.random.default_rng(6)
+    for fam, cls in (("k_conv_tc mode 0", "ragged last round"), ("k_conv_tc_is", "ragged last round"),
+                     ("k_conv_tc mode 0", "idle warpgroups"), ("k_conv_tc_is", "idle warpgroups"),
+                     ("k_conv_tc_is", "nch == kIsMaxCh"), ("k_conv_tc mode 0", "ring nin > 2S"), ("k_conv_tc_is", "ring nin > 2S")):
+        L, path, S, args, pl = _find_launch(fam, cls)
+        T = {n: rand16(S[n], precision, rng) for n in (L.inp, L.res) if n}
+        y, ar = simulate(L, T, precision, path)
+        r = ratio(L, T, y, ar)
+        print(f"{precision} {fam} {cls}: {L.out} {S[L.out]} ratio {r.worst[1]:.3f}")
+        assert r.worst[1] <= 1.0, (fam, cls, L.out, r.worst)

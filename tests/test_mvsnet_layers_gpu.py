@@ -1,7 +1,7 @@
 """Every layer of the 16-bit MVSNet forward against an fp64 reference computed on the engine's own stored input
 (oracle/mvsnet_layers.py), with an a-priori per-element error bound; the soft-argmin against fp64, the edge filter bit for
-bit.  Windows and options are chosen so that the tile planners produce single tiles and partial last tiles along W, H and D
-(tests/test_mvsnet_layers_cpu.py checks that they do)."""
+bit.  test_layers_launch_classes runs the windows of oracle/mvsnet_layers.py WINDOWS in fp16 and bf16, which together run
+every launch class the tile planners can reach (tests/test_mvsnet_layers_cpu.py checks that they do)."""
 import time
 
 import numpy as np
@@ -268,27 +268,71 @@ OPTIONS = [dict(use_is=0), dict(use_tc=0), dict(prob_direct=1, fused_regress=1, 
            dict(tc_smem_kb=113), dict(fork_fpn=0, use_pdl=2), dict(cv_variant=0), dict(cv_variant=4), dict(cv_variant=5)]
 
 
-@pytest.mark.parametrize("opts", OPTIONS, ids=["-".join(f"{k}{v}" for k, v in o.items()) for o in OPTIONS])
-def test_layers_options(opts):
+def _run_options(opts, precision, **extra):
     V, H, W, dn = 2, 96, 128, (16, 24, 8)
     win = _synthetic(V, H, W)
-    m = _engine("abl03_view_aggregation", "mixed16", dn, **opts)
+    m = _engine("abl03_view_aggregation", precision, dn, **opts, **extra)
     _submit(m, win)
-    check_forward(m, win, "abl03_view_aggregation", "mixed16", dn, opts, "128x96v2 " + ",".join(f"{k}={v}" for k, v in opts.items()), REPORT,
+    check_forward(m, win, "abl03_view_aggregation", precision, dn, opts, "128x96v2 " + ",".join(f"{k}={v}" for k, v in opts.items()), REPORT,
                   volume="cv_variant" in opts)
+
+
+@pytest.mark.parametrize("opts", OPTIONS, ids=["-".join(f"{k}{v}" for k, v in o.items()) for o in OPTIONS])
+def test_layers_options(opts):
+    _run_options(opts, "mixed16")
+
+
+@pytest.mark.parametrize("opts", OPTIONS, ids=["-".join(f"{k}{v}" for k, v in o.items()) for o in OPTIONS])
+def test_layers_options_bf16(opts):
+    """The bf16 engine's own instantiation of every kernel an option selects, with NaN-poisoned activation interiors."""
+    _run_options(opts, "bf16", debug_poison=1)
+
+
+def _run_prob_tail(use_is, precision, **extra):
+    V, H, W, dn = 4, 352, 480, (24, 40, 56)
+    win = _synthetic(V, H, W)
+    opts = dict(fused_regress=1, use_is=use_is)
+    m = _engine("abl03_view_aggregation", precision, dn, **opts, **extra)
+    _submit(m, win)
+    assert sum(r[0].startswith("s") and r[0].endswith("regress") for r in m.profile()) == 0
+    check_forward(m, win, "abl03_view_aggregation", precision, dn, opts, f"480x352v4 fused_regress use_is={use_is}", REPORT)
 
 
 @pytest.mark.parametrize("use_is", [1, 0])
 def test_layers_prob_tail_partial_tiles(use_is):
     """fused_regress at 480x352 (D 24 / 40 / 56: RegressTail<32>, <48>, <64>): the soft-argmin tail of the input-stationary
     (use_is=1) and the output-stationary (use_is=0) prob kernel, with partial last tiles along H (and W for the latter)."""
-    V, H, W, dn = 4, 352, 480, (24, 40, 56)
+    _run_prob_tail(use_is, "mixed16")
+
+
+@pytest.mark.parametrize("use_is", [1, 0])
+def test_layers_prob_tail_partial_tiles_bf16(use_is):
+    _run_prob_tail(use_is, "bf16", debug_poison=1)
+
+
+def _window_id(w):
+    V, H, W, dn, opts, _ = w
+    return f"{W}x{H}v{V}-" + "-".join(map(str, dn)) + "".join(f"-{k}{v}" for k, v in opts.items())
+
+
+@pytest.mark.parametrize("precision", ["mixed16", "bf16"])
+@pytest.mark.parametrize("window", ML.WINDOWS, ids=[_window_id(w) for w in ML.WINDOWS])
+def test_layers_launch_classes(window, precision):
+    """Every launch class the tile planners can reach (tile edges, idle / ragged warpgroups, full register partials, ring
+    depth, narrow pitch, N slicing: oracle/mvsnet_layers.py launch_classes), on a fresh engine whose activation interiors
+    start as NaN, so that a store a kernel skipped cannot pass as a zero or as a previous forward's value."""
+    V, H, W, dn, opts, listed = window
+    smem = opts.get("tc_smem_kb", 225)
+    hit = set()
+    for _, args in ML.window_launches(V, H, W, dn, opts):
+        key, cls = ML.launch_classes(args, ML.query_plan(args, smem))
+        hit |= {key + (c,) for c in cls}
+    assert set(listed) <= hit, f"the window no longer reaches {sorted(set(listed) - hit)}"
+    weights = "abl04_fewer_depth_planes" if 4 in dn else "abl03_view_aggregation"
     win = _synthetic(V, H, W)
-    opts = dict(fused_regress=1, use_is=use_is)
-    m = _engine("abl03_view_aggregation", "mixed16", dn, **opts)
+    m = _engine(weights, precision, dn, debug_poison=1, **opts)
     _submit(m, win)
-    assert sum(r[0].startswith("s") and r[0].endswith("regress") for r in m.profile()) == 0
-    check_forward(m, win, "abl03_view_aggregation", "mixed16", dn, opts, f"480x352v4 fused_regress use_is={use_is}", REPORT)
+    check_forward(m, win, weights, precision, dn, opts, _window_id(window), REPORT)
 
 
 def test_layers_smem_113_at_view_maximum():
