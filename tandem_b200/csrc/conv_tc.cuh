@@ -163,7 +163,9 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 // 544 threads (17 warps, five of them on one SM sub-partition) ptxas allows 96 registers per thread; two warpgroups (288
 // threads, 168 registers) remain only where that cap spills (-Xptxas -v, DESIGN.md section 5): the N = 64 transposed
 // convs (MODE 1), which keep their bias and the early-fetched skip operand in registers (the N = 128 one loads both in
-// the epilogue and fits), and the prob layer's soft-argmin tail for more than 32 planes (RegressTail<48 / 64>).
+// the epilogue and fits), and the prob layer's soft-argmin tail for more than 32 planes (RegressTail<48 / 64>).  The
+// N = 64 transposed convs spilled at 96 with 4-byte epilogue accesses; their 8-byte ones build at 88 with two warpgroups,
+// and four have not been tried since.
 // mode: k_conv_tc's MODE (0 for the stride-2 and input-stationary kernels); n: instruction N; tail_d: Tail::max_d, 0
 // without a tail.  The planners read the same function with their full-depth tile's D for tail_d (D <= 32 exactly when
 // the tail's bucket max_d is), so their warpgroup balance matches the kernel they plan for.
@@ -339,9 +341,12 @@ __device__ __forceinline__ void mma_subchunk(float (&acc)[N / 2], const uint32_t
 
 // Two consecutive channels of an 8-channel group: one 4-byte store / load (the load is split into its issue, a plain
 // 4-byte __ldg, and unpack2, so that it can be issued early).
-template <typename T> __device__ __forceinline__ void store2(T* p, float x0, float x1) {
+template <typename T> __device__ __forceinline__ uint32_t pack2(float x0, float x1) {
   T v[2] = {from_f<T>(x0), from_f<T>(x1)};
-  *reinterpret_cast<uint32_t*>(p) = *reinterpret_cast<const uint32_t*>(v);
+  return *reinterpret_cast<const uint32_t*>(v);
+}
+template <typename T> __device__ __forceinline__ void store2(T* p, float x0, float x1) {
+  *reinterpret_cast<uint32_t*>(p) = pack2<T>(x0, x1);
 }
 template <typename T> __device__ __forceinline__ void unpack2(uint32_t u, float& x0, float& x1) {
   const T* v = reinterpret_cast<const T*>(&u);
@@ -436,6 +441,24 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
   float bv[OUT_PLAIN || !BIAS_REG ? 1 : NPAD / 8][2];
   if constexpr (OUT_PLAIN) bv[0][0] = bias ? bias[0] : 0.f;
   else if constexpr (BIAS_REG) load_bias<CLASS_EPI>(bv, bias, ns * NPAD, g.cout, lane);
+  // PAIR_EPI (CLASS_EPI with N <= 64) moves whole 32-byte sectors.  Classes pw = 0 and pw = 1 of one (pd, ph, output
+  // channel group) are column blocks j0 and j0 + PWS (cout = CIN / 2 for the deconvs, 8 for up-2; the host checks it), and their output pixels 2w
+  // and 2w + 1 are adjacent: 32 bytes per input position.  Lanes q and q ^ 1 of a fragment row swap one packed word, so
+  // that lane q reads and writes 8 contiguous bytes, channels 4 * (q >> 1) .. +3 of class pw = q & 1.  A warp access then
+  // covers its 8 positions' 32-byte runs in full, where two 4-byte accesses per lane filled half of each sector apiece.
+  // The N = 128 deconv (conv9), which fetches its skip operand after the chain, keeps 4-byte accesses: there the exchange
+  // puts a shuffle behind each skip load and measured slower.
+  constexpr bool PAIR_EPI = CLASS_EPI && NPAD <= 64;
+  constexpr int PWS = MODE == 1 ? CIN / 16 : 1;
+  const int pq = lane & 1;
+  auto pair_j0 = [](int k) { return k / PWS * 2 * PWS + k % PWS; };
+  // element offset of the 8 bytes this lane moves for block pair k of pixel (d, h, w), in a tensor of group stride gs
+  auto pair_at = [&](int d, int h, int w, int k, long long gs) -> long long {
+    long long pos;
+    int co;
+    out_at(d, h, w, pair_j0(k) + pq * PWS, pos, co);
+    return pos + (co >> 3) * gs + 4 * ((lane & 3) >> 1);
+  };
   for (int od = 0; od < o.ndo; ++od) {
     ring.wait(od + KD - 1);
     uint32_t slot16[KD];
@@ -454,12 +477,21 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
           for (int i = 0; i < 2; ++i) {
             int h, w;
             const bool in = frag_pixel(g, o, l, i, h, w);
+            if constexpr (PAIR_EPI) {
+              // rv[i][2k .. 2k+1]: this lane's 8 bytes of block pair k, exchanged after the chain
 #pragma unroll
-            for (int j = 0; j < NPAD / 8; ++j) {
-              long long pos;
-              int co;
-              rv[i][j] = in && out_at(d, h, w, j, pos, co)
-                             ? __ldg(reinterpret_cast<const unsigned int*>(res + pos + (co >> 3) * g.res_gs + (co & 7))) : 0u;
+              for (int k = 0; k < NPAD / 16; ++k) {
+                const uint2 r = in ? __ldg(reinterpret_cast<const uint2*>(res + pair_at(d, h, w, k, g.res_gs))) : make_uint2(0u, 0u);
+                rv[i][2 * k] = r.x; rv[i][2 * k + 1] = r.y;
+              }
+            } else {
+#pragma unroll
+              for (int j = 0; j < NPAD / 8; ++j) {
+                long long pos;
+                int co;
+                rv[i][j] = in && out_at(d, h, w, j, pos, co)
+                               ? __ldg(reinterpret_cast<const unsigned int*>(res + pos + (co >> 3) * g.res_gs + (co & 7))) : 0u;
+              }
             }
           }
         }
@@ -469,8 +501,42 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         int h, w;
-        if (!frag_pixel(g, o, l, i, h, w)) continue;
-        if constexpr (OUT_PLAIN) {
+        const bool in = frag_pixel(g, o, l, i, h, w);
+        if (!in && !PAIR_EPI) continue;   // PAIR_EPI: every lane takes part in the word exchange
+        if constexpr (PAIR_EPI) {
+#pragma unroll
+          for (int k = 0; k < NPAD / 16; ++k) {
+            const int j0 = pair_j0(k);
+            uint32_t r[2] = {0u, 0u};   // skip words of blocks j0 and j0 + PWS at this lane's channels 2q, 2q + 1
+            if (g.has_res) {
+              const uint2 rr = make_uint2(rv[i][2 * k], rv[i][2 * k + 1]);
+              // rr holds channels 2(q & ~1) .. +3 of class pq: this lane's own word and the partner's
+              const uint32_t own = pq ? rr.y : rr.x, other = __shfl_xor_sync(0xffffffffu, pq ? rr.x : rr.y, 1);
+              r[0] = pq ? other : own; r[1] = pq ? own : other;
+            }
+            uint32_t v[2];
+#pragma unroll
+            for (int p = 0; p < 2; ++p) {
+              const int j = j0 + p * PWS;
+              float x[2];
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                x[e] = acc[4 * j + 2 * i + e];
+                if constexpr (HILO) x[e] += acc[4 * (j + NPAD / 8) + 2 * i + e];
+                x[e] += bv[j][e];
+                if (g.relu) x[e] = fmaxf(x[e], 0.f);
+              }
+              if (g.has_res) {
+                float r0, r1;
+                unpack2<TOut>(r[p], r0, r1);
+                x[0] += r0; x[1] += r1;
+              }
+              v[p] = pack2<TOut>(x[0], x[1]);
+            }
+            const uint32_t own = pq ? v[1] : v[0], other = __shfl_xor_sync(0xffffffffu, pq ? v[0] : v[1], 1);
+            if (in) *reinterpret_cast<uint2*>(out + pair_at(d, h, w, k, g.out_gs)) = pq ? make_uint2(other, own) : make_uint2(own, other);
+          }
+        } else if constexpr (OUT_PLAIN) {
           if ((lane & 3) == 0) {
             float x = acc[2 * i];
             if constexpr (HILO) x += acc[4 * (NPAD / 8) + 2 * i];

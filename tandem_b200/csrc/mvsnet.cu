@@ -920,6 +920,8 @@ class MvsnetEngine final : public MvsnetIface {
     }
     constexpr int NWG = tc::conv_nwg(MODE, HILO ? 2 * NPAD : NPAD, Tail::max_d);
     TDM_CHECK(pl.nwg == NWG, wkey + ": tile plan balanced for another warpgroup count than the kernel's");
+    // the parity-class epilogue pairs column blocks pw = 0 / 1 at a compile-time distance of cout / 8 blocks
+    TDM_CHECK((MODE != 1 || c.cout == CIN / 2) && (MODE != 3 || c.cout == 8), wkey + ": parity-class layer with an unexpected cout");
     launch_tc<tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail, NWG>>(dim3(pl.grid, c.nsplit), pl.smem, tcx.tmap, (const TIn*)c.bimg,
                                                                               (const float*)c.bias, rp, op, plain, pl.g, tail);
   }
