@@ -1,7 +1,7 @@
 """ORACLE (test infrastructure, never shipped, never on the product path).
 
-Layer-by-layer fp64 reference of the CVA-MVSNet forward for the 16-bit engines.  Every layer is recomputed in float64 on
-the engine's OWN stored input (DrMvsnet.debug_tensor: the exact 16-bit values the kernel consumed, converted to fp32
+Layer-by-layer fp64 reference of the CVA-MVSNet forward for the 16-bit and the fp32 engines.  Every layer is recomputed in float64 on
+the engine's OWN stored input (DrMvsnet.debug_tensor: the exact 16-bit or fp32 values the kernel consumed, converted to fp32
 without loss), so no upstream rounding leaks in, and the engine's output must lie inside an a-priori per-element bound:
 
     |y - y_ref| <= (1 + u_out) * E + u_out * |y_ref| + a_out (+ u_out * |partial| where a partial result is stored)
@@ -24,6 +24,15 @@ The per-class constants are derived from the arithmetic of the kernels (conv_tc*
                          last fp32 add is one of the n epilogue adds).
 
 u16 is 2^-11 for fp16 and 2^-8 for bf16 (unit roundoff of an 11- / 8-bit significand).
+
+The fp32 engine runs every layer on the direct FFMA kernels (k_conv_direct, its transposed gather, the prob layer), with
+fp32 weights, fp32 activations and no fused FPN tail:
+  * weights / accumulation  u_w = 2^-24, u_acc = 2^-24, a_w = 0 (fp32 keeps the exponent range of the folded weights)
+  * output               fp32 stores: u_out = 0, the last rounding (bias add, ReLU is exact) is one of the n epilogue adds, as
+                         for the logits.  A residual is added after that and rounds once more, relative to the stored value:
+                         u_out = 2^-24 for the layers that carry one (the deconvolutions and the FPN top-down sums).
+  * input                f.img = fl32(u8 / 255) (IEEE division, k_preprocess_bgr<float>): f.conv0.0 runs on the generic
+                         direct kernel against the stored image, so the division's rounding is not part of its error.
 """
 import math
 from dataclasses import dataclass
@@ -147,9 +156,24 @@ def is_hilo_tc(cin: int, cout: int, kd: int) -> bool:
     return npad <= 32 and cin <= 32 and not (kd == 3 and cin == 32 and cout == 32)
 
 
-def arith_for(path: str, precision: str, cin: int, cout: int, kd: int, plain: bool, transposed: bool = False) -> Arith:
+def direct_family(L: Layer, out_shape) -> str:
+    """The k_conv_direct instantiation that computes L on the fp32 engine (mvsnet.cu conv_inst): with at least 16 output
+    channels and fewer than 128 * 592 output positions a thread owns 8 channels and blockIdx.y picks the group."""
+    if L.plain:
+        return "k_conv_direct prob, fp32 logits"
+    split = out_shape[0] >= 16 and int(np.prod(out_shape[1:])) < 128 * 592
+    kind = f"transposed {L.stride}" if L.transposed else ("2-D" if L.dim == 2 else "3-D")
+    return f"k_conv_direct {kind}, " + ("8-channel split" if split else "all channels") + (", + residual" if L.res or L.res_up2 else "")
+
+
+def arith_for(path: str, precision: str, cin: int, cout: int, kd: int, plain: bool, transposed: bool = False,
+              residual: bool = False, family: str = "") -> Arith:
     """path: the profile suffix of the launch ('' direct, 'tc', 'tc-is', 'tc-s2', 'tc-up2', 'direct', 'u8-direct').
-    The transposed-conv and stride-2 images are single 16-bit."""
+    The transposed-conv and stride-2 images are single 16-bit.  fp32: every layer is direct (residual: a residual is added
+    after the accumulation; family: the report's name of the instantiation, direct_family)."""
+    if precision == "fp32":
+        assert path == "", f"the fp32 engine has no {path} launch"
+        return Arith(U_FP32, U_ACC["fma"], 0.0, U_FP32 if residual else 0.0, 0.0, family or "fp32 weights, FFMA, fp32 store")
     u16, a16 = U16[precision], A16[precision]
     u_out, a_out = (0.0, 0.0) if plain else (u16, a16)
     if path in ("", "direct", "u8-direct"):
@@ -594,7 +618,10 @@ class CvArith:
       u_dot, dot_steps  gate weights in fp16 (2^-11) and C/2 HFMA2 partial roundings (va16), or fp32 FFMA over C channels
       u_acc    rounding of the accumulation over views per view: fp16 (ACC16) or fp32
       a_acc    subnormal grid of the fp16 accumulator in true units (2^-25 * 4096)
-      u_out, a_out  the stored volume: fp16 x 2^-5 (subnormal grid 2^-25 * 32) or bf16"""
+      u_out, a_out  the stored volume: fp16 x 2^-5 (subnormal grid 2^-25 * 32), bf16, or fp32 (0: the division by the view
+               count is the last rounding and is counted below)
+      grid_sample  the fp32 engine's sample coordinate: ix = ((qx / qz / half_w - 1 + 1) * 0.5) * (W - 1), the normalise /
+               un-normalise round trip of grid_sample, four more roundings after the division"""
     u_bil: float
     ref_chain: bool
     a_diff: float
@@ -607,10 +634,14 @@ class CvArith:
     u_out: float
     a_out: float
     desc: str
+    grid_sample: bool = False
 
 
 def cv_arith(precision: str, cv_variant: int, C: int, D: int) -> CvArith:
     u, h = U_FP32, 2.0 ** -11
+    if precision == "fp32":        # generic kernel, fp32 features / math / volume: bilinear weights (1 - ax)(1 - ay) carry 3
+        # roundings, the 4-tap FMA chain 4 more
+        return CvArith(7 * u, False, 0.0, u, 0.0, u, C, u, 0.0, 0.0, 0.0, "generic, fp32 math, fp32 volume", grid_sample=True)
     if precision == "bf16":        # generic kernel, fp32 arithmetic on bf16 features, bf16 volume
         return CvArith(6 * u, False, 0.0, u, 0.0, u, C, u, 0.0, 2.0 ** -8, 0.0, "generic, fp32 math, bf16 volume")
     a_out = 2.0 ** -25 * 32.0
@@ -663,6 +694,10 @@ def cost_volume_reference(w, s: int, feats: np.ndarray, hyps: np.ndarray, K, c2w
                 # rcp (approx, 2^-23) and the product (2^-24) on top of the propagated errors of qx, qy, qz
                 eix = (eq[0] + np.abs(ix) * eq[2]) / np.abs(q[2]) + 3 * u * np.abs(ix)
                 eiy = (eq[1] + np.abs(iy) * eq[2]) / np.abs(q[2]) + 3 * u * np.abs(iy)
+            if ar.grid_sample:
+                # / half_w, - 1, + 1 and * (W - 1): u |ix| each, except that - 1 rounds at |ix| + half_w in pixel units
+                eix = eix + u * (4 * np.abs(ix) + 0.5 * (W - 1))
+                eiy = eiy + u * (4 * np.abs(iy) + 0.5 * (H - 1))
             valid = (q[2] >= 0.001) & (ix >= -1) & (iy >= -1) & (ix < W) & (iy < H)
             near = (q[2] >= 0.001) & (ix >= -1 - eix) & (iy >= -1 - eiy) & (ix < W + eix) & (iy < H + eiy)
             excl[d] |= np.abs(q[2] - 0.001) <= eq[2]

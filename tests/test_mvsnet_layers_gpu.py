@@ -1,4 +1,4 @@
-"""Every layer of the 16-bit MVSNet forward against an fp64 reference computed on the engine's own stored input
+"""Every layer of the 16-bit and fp32 MVSNet forwards against an fp64 reference computed on the engine's own stored input
 (oracle/mvsnet_layers.py), with an a-priori per-element error bound; the soft-argmin against fp64, the edge filter bit for
 bit.  test_layers_launch_classes runs the windows of oracle/mvsnet_layers.py WINDOWS in fp16 and bf16, which together run
 every launch class the tile planners can reach (tests/test_mvsnet_layers_cpu.py checks that they do)."""
@@ -91,8 +91,9 @@ def check_forward(m, win, weights, precision, dn, opts, label, report, volume=Fa
     reference).  Returns the number of layers checked."""
     w, dn0, _ = _weights(weights)
     dn = tuple(dn or dn0)
-    fused_fpn = opts.get("use_tc", 1) == 1
-    direct00 = opts.get("direct_conv00", 1) == 1
+    fp32 = precision == "fp32"              # no fused FPN tail, no k_conv00_u8: f.conv0.0 is a direct conv of f.img
+    fused_fpn = not fp32 and opts.get("use_tc", 1) == 1
+    direct00 = not fp32 and opts.get("direct_conv00", 1) == 1
     layers = ML.layer_table(dn, fused_fpn, direct00)
     T = _tensors(m, layers)
     outs = {(s, k): m.stage_output(s, k) for s in (1, 2, 3) for k in ("depth", "confidence", "depth_dense", "confidence_dense")}
@@ -127,17 +128,23 @@ def check_forward(m, win, weights, precision, dn, opts, label, report, volume=Fa
         y_ref, bound, ar = ML.conv00_u8_reference(w, np.stack([win["bgrs"][v] for v in order]), precision)
         record("f.c0_0", paths.get("f.conv0.0", ""), ar, T["f.c0_0"], y_ref, bound)
     else:
-        # k_preprocess_bgr: RGB of the reference-first window as exact u8 / 256, channels 3..7 zero
-        u8 = np.stack([win["bgrs"][v] for v in order])[..., ::-1].transpose(3, 0, 1, 2).astype(np.float32) / 256
-        assert np.array_equal(T["f.img"][:3], u8) and not T["f.img"][3:].any(), f"{label}: f.img is not u8/256 of the window"
+        # k_preprocess_bgr: RGB of the reference-first window as exact u8 / 256 (16-bit engines) or as fl32(u8 / 255) (fp32
+        # engine, IEEE division as numpy's), channels 3..7 zero
+        u8 = np.stack([win["bgrs"][v] for v in order])[..., ::-1].transpose(3, 0, 1, 2).astype(np.float32)
+        img = u8 / np.float32(255) if fp32 else u8 / 256
+        got = T["f.img"][:3]
+        report.append((label, precision, "f.img", "preprocess", "u8 / 255" if fp32 else "u8 / 256", float(np.any(got != img))))
+        assert np.array_equal(got.view(np.uint32), img.view(np.uint32)) and not T["f.img"][3:].any(), \
+            f"{label}: f.img is not {'u8/255' if fp32 else 'u8/256'} of the window on {int((got != img).sum())} values"
     checked = 0
     for L in layers:
         path = paths.get(L.wkey, "")
         Wt, _ = ML.fold(w, L.conv_w, L.bn, L.bias, L.transposed)
         cin, cout = (Wt.shape[0], Wt.shape[1]) if L.transposed else (Wt.shape[1], Wt.shape[0])
-        ar = ML.arith_for(path, precision, cin, cout, 1 if L.dim == 2 else 3, L.plain, L.transposed)
+        ar = ML.arith_for(path, precision, cin, cout, 1 if L.dim == 2 else 3, L.plain, L.transposed,
+                          residual=bool(L.res or L.res_up2), family=ML.direct_family(L, shapes[L.out]) if fp32 else "")
         # f.img is stored as exact u8/256 on the 16-bit engines: the remaining 256/255 lives in the weights
-        scale = 256.0 / 255.0 if L.out == "f.c0_0" else 1.0
+        scale = 256.0 / 255.0 if L.out == "f.c0_0" and not fp32 else 1.0
         y_ref, bound = ML.reference(L, w, T, ar, scale)
         record(L.out, path, ar, T[L.out], y_ref, bound, L)
         checked += 1
@@ -238,14 +245,30 @@ SYNTH = [  # (V, H, W, depth numbers): every MAXD instantiation of the regressio
     (4, 352, 480, (24, 40, 56)),
     (2, 32, 64, (8, 8, 8)),           # single-tile stride-2 layers
 ]
+# fp32: the direct kernels split the output channels of a layer with >= 16 of them over blockIdx.y below 128 * 592 output
+# positions (mvsnet.cu conv_inst); 128x96v2 runs every such layer split, 288x224v16 and 480x352v4 run the full-resolution
+# FeatureNet layers unsplit and the coarse CostRegNet layers split
+SYNTH_PRECISIONS = [(c, "mixed16") for c in SYNTH] + [(c, "fp32") for c in SYNTH if c[0] * c[1] * c[2] <= 4 * 352 * 480]
 
 
-@pytest.mark.parametrize("V,H,W,dn", SYNTH, ids=[f"{c[2]}x{c[1]}v{c[0]}" for c in SYNTH])
-def test_layers_synthetic_windows(V, H, W, dn):
+@pytest.mark.parametrize("V,H,W,dn,precision", [c + (p,) for c, p in SYNTH_PRECISIONS],
+                         ids=[f"{c[2]}x{c[1]}v{c[0]}" + ("-fp32" if p == "fp32" else "") for c, p in SYNTH_PRECISIONS])
+def test_layers_synthetic_windows(V, H, W, dn, precision):
     win = _synthetic(V, H, W)
-    m = _engine("abl03_view_aggregation", "mixed16", dn)
+    m = _engine("abl03_view_aggregation", precision, dn)
     _submit(m, win)
-    check_forward(m, win, "abl03_view_aggregation", "mixed16", dn, {}, f"{W}x{H}v{V}", REPORT, volume=H <= 96)
+    if precision == "fp32":
+        split = [L.out for L in ML.layer_table(dn, False, False)
+                 if not L.plain and "split" in ML.direct_family(L, ML.shapes(V, H, W, dn)[L.out])]
+        print(f"{W}x{H}v{V} fp32: {len(split)} layers with the 8-channel split: {split}")
+    check_forward(m, win, "abl03_view_aggregation", precision, dn, {}, f"{W}x{H}v{V}", REPORT, volume=H <= 96)
+
+
+def test_fp32_windows_straddle_the_channel_split():
+    """The fp32 windows of test_layers_synthetic_windows run k_conv_direct both with and without the 8-channel split."""
+    fams = {ML.direct_family(L, ML.shapes(V, H, W, dn)[L.out])
+            for (V, H, W, dn), p in SYNTH_PRECISIONS if p == "fp32" for L in ML.layer_table(dn, False, False)}
+    assert any("8-channel split" in f for f in fams) and any("all channels" in f for f in fams), fams
 
 
 def test_layers_benchmark_window(golden_full):
@@ -255,7 +278,7 @@ def test_layers_benchmark_window(golden_full):
     check_forward(m, win, "abl03_view_aggregation", "mixed16", None, {}, "640x480", REPORT)
 
 
-@pytest.mark.parametrize("precision", ["mixed16", "bf16"])
+@pytest.mark.parametrize("precision", ["mixed16", "bf16", "fp32"])
 def test_layers_four_depth_planes(golden_small, precision):
     """abl04: D = 4 at stages 2 and 3, where conv5 / conv7 run with stride (1, 2, 2) on the direct kernels."""
     win = _golden(golden_small)
