@@ -13,10 +13,12 @@
 //   output p-1 = partial(p-1) + block kd=2   -> complete: bias / ReLU / store
 //   partial(p) += block kd=1,   partial(p+1) = block kd=0
 // so consumer warpgroup wg owns sub-chunks NWG * k + wg on every plane of the tile, and the planner bounds the chunks per
-// plane by kIsMaxCh (registers: 2 * kIsMaxCh / NWG sub-chunks per warpgroup).  As in k_conv_tc, a warpgroup waits for its
-// chain before it folds and stores, and the other consumer warpgroups' MMAs overlap that epilogue (keeping the next chain
-// in flight with wgmma.wait_group 1 made ptxas serialise every wgmma, C7514).  Ring, producer warp, roles and tile
-// geometry are those of k_conv_tc.
+// plane by kIsMaxCh (registers: 2 * kIsMaxCh / NWG sub-chunks per warpgroup).  The chains are short (5 to 18 wgmma), so a
+// warpgroup issues the chains of KB = is_batch(...) of its sub-chunks of a plane back to back, each into its own fragment,
+// then commits once, waits once (wait_group 0) and folds them in sub-chunk order; nothing stays in flight across the wait
+// (keeping a chain in flight with wgmma.wait_group 1 made ptxas serialise every wgmma, C7514).  The other consumer
+// warpgroups' MMAs overlap the folds and stores.  Every output comes from the same chain and the same fold order as with
+// one chain per wait.  Ring, producer warp, roles and tile geometry are those of k_conv_tc.
 #pragma once
 #include "conv_tc.cuh"
 
@@ -26,6 +28,12 @@ namespace tc {
 // Most 128-position chunks per plane, i.e. 2 * kIsMaxCh / NWG 64-position sub-chunks per consumer warpgroup: two rolling
 // partials of 4 floats each per sub-chunk stay in registers
 constexpr int kIsMaxCh = 8;
+
+// Chains a consumer warpgroup issues back to back before one wait (a divisor of its 2 * kIsMaxCh / NWG sub-chunks), the
+// most that build without spills (-Xptxas -v, DESIGN.md section 5): the prob layer's 12-float fragments four at a time
+// with four warpgroups.  conv0's 24-float fragments spill with two next to the partials and the output offsets, and
+// keep one chain per wait, as do the prob tail's two-warpgroup instantiations, already at 168 registers.
+__host__ __device__ constexpr int is_batch(int cpk, int nwg) { return cpk == 8 && nwg == 4 ? 4 : 1; }
 
 // Tail: the prob layer's softmax / soft-argmin / confidence, as in k_conv_tc (tiles that span all D planes, make_plan_is(full_depth)).
 template <typename TIn, typename TOut, int CIN, int CPK, bool OUT_PLAIN, typename Tail, int NWG>
@@ -42,6 +50,8 @@ k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/
   constexpr int PN = CPK == 16 ? 4 : 2;         // folded values per thread and sub-chunk: (row half i, column e) or row half i
   constexpr int KSUB = 2 * kIsMaxCh / NWG;      // most sub-chunks per plane that one warpgroup owns
   static_assert((2 * kIsMaxCh) % NWG == 0, "the partial arrays hold exactly this warpgroup's share of 2 * kIsMaxCh sub-chunks");
+  constexpr int KB = is_batch(CPK, NWG);        // chains in flight per warpgroup between two waits
+  static_assert(KSUB % KB == 0, "a warpgroup's sub-chunks split into whole batches");
 
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t cg_bytes = (uint32_t)g.slot_pos * 16u;
@@ -73,11 +83,29 @@ k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/
   for (int k = 0; k < KSUB; ++k)
 #pragma unroll
     for (int q = 0; q < PN; ++q) pa[k][q] = pb[k][q] = 0.f;
-  float fr[N / 2];
   // channels 2 * (lane % 4) + e, or the single prob channel
   float bv[1][2];
   if constexpr (OUT_PLAIN) bv[0][0] = bias ? bias[0] : 0.f;
   else load_bias<false>(bv, bias, 0, 8, lane);
+
+  // A sub-chunk covers the same pixels on every plane: the in-plane element offset of each fragment row half this thread
+  // stores (h * W + w, or the P8 position ((h + 1) * Wp + w + 1) * 8), -1 for pad columns and positions beyond the grid.
+  // Four warpgroups keep them in registers, decoded once per CTA; the two-warpgroup tail instantiations, which own twice
+  // the sub-chunks and sit at 168 registers, would spill and decode them in every fold.
+  constexpr bool POFF_REG = NWG == 4;
+  const long long pstride = OUT_PLAIN ? (long long)g.H * g.W : (long long)g.Hp * g.Wp * 8;
+  auto pix_off = [&](int k, int i) -> int {
+    int h, w;
+    const bool in = frag_pixel(g, o, (NWG * k + wg) * 64 + wq * 16 + (lane >> 2), i, h, w);
+    return !in ? -1 : OUT_PLAIN ? h * g.W + w : ((h + 1) * g.Wp + (w + 1)) * 8;
+  };
+  int poff[POFF_REG ? KSUB : 1][2];
+  if constexpr (POFF_REG) {
+#pragma unroll
+    for (int k = 0; k < KSUB; ++k)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) poff[k][i] = pix_off(k, i);
+  }
 
   // value q of column block s (0: kd=2, 1: kd=1, 2: kd=0) of fragment f, hi + lo
   auto blk = [&](const float (&f)[N / 2], int s, int q) -> float {
@@ -93,13 +121,13 @@ k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/
       pb[k][q] = blk(f, 2, q);
     }
     if (rp < 2) return;
-    const int d = o.d0 + rp - 2;
+    const long long plane = (long long)(o.d0 + rp - 2 + (OUT_PLAIN ? 0 : 1)) * pstride;   // output plane d (padded: d + 1)
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      int h, w;
-      if (!frag_pixel(g, o, (NWG * k + wg) * 64 + wq * 16 + (lane >> 2), i, h, w)) continue;
+      const int off = POFF_REG ? poff[POFF_REG ? k : 0][i] : pix_off(k, i);
+      if (off < 0) continue;
       if constexpr (OUT_PLAIN) {
-        if ((lane & 3) == 0) plain_out[((long long)d * g.H + h) * g.W + w] = x[i] + bv[0][0];
+        if ((lane & 3) == 0) plain_out[plane + off] = x[i] + bv[0][0];
       } else {
         const int co = 2 * (lane & 3);
         float y[2];
@@ -108,8 +136,7 @@ k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/
           y[e] = x[2 * i + e] + bv[0][e];
           if (g.relu) y[e] = fmaxf(y[e], 0.f);
         }
-        const long long pos = ((((long long)(d + 1)) * g.Hp + (h + 1)) * g.Wp + (w + 1)) * 8;
-        store2<TOut>(out + pos + co, y[0], y[1]);
+        store2<TOut>(out + plane + off + co, y[0], y[1]);
       }
     }
   };
@@ -119,19 +146,33 @@ k_conv_tc_is(const __grid_constant__ CUtensorMap tmap /*P8 input, as k_conv_tc*/
     ring.wait(rp);
     const uint32_t slot16 = ring.slot16(rp);
 #pragma unroll
-    for (int k = 0; k < KSUB; ++k) {
-      if (NWG * k + wg < nsub) {
-        const uint32_t a0 = slot16 + (uint32_t)(NWG * k + wg) * 64u;
-        fence_frag(fr);
+    for (int k0 = 0; k0 < KSUB; k0 += KB) {
+      // sub-chunks NWG * k + wg grow with k: if the batch's first one is beyond the plane, all of them are
+      if (NWG * k0 + wg < nsub) {
+        // the batch's chains are issued back to back into their own fragments and retired by one wait
+        float fr[KB][N / 2];
+#pragma unroll
+        for (int j = 0; j < KB; ++j) fence_frag(fr[j]);
         wgmma_fence();
 #pragma unroll
-        for (int b = 0; b < NBLK; ++b)
-          wgmma<N, TIn>(fr, desc(a0 + kstep_aoff<CIN, 9>(b, cgb16, tap_off), kstep_alo<CIN, 9>(b, cgb16, tap_off)),
-                        desc(sB16 + (uint32_t)(b * N * 2), b_lbo16), b != 0 ? 1u : 0u);
+        for (int j = 0; j < KB; ++j) {
+          if (NWG * (k0 + j) + wg < nsub) {
+            const uint32_t a0 = slot16 + (uint32_t)(NWG * (k0 + j) + wg) * 64u;
+#pragma unroll
+            for (int b = 0; b < NBLK; ++b)
+              wgmma<N, TIn>(fr[j], desc(a0 + kstep_aoff<CIN, 9>(b, cgb16, tap_off), kstep_alo<CIN, 9>(b, cgb16, tap_off)),
+                            desc(sB16 + (uint32_t)(b * N * 2), b_lbo16), b != 0 ? 1u : 0u);
+          }
+        }
         wgmma_commit();
         wgmma_wait_all();
-        fence_frag(fr);
-        fold(k, fr, rp);
+#pragma unroll
+        for (int j = 0; j < KB; ++j) {
+          if (NWG * (k0 + j) + wg < nsub) {
+            fence_frag(fr[j]);
+            fold(k0 + j, fr[j], rp);
+          }
+        }
       }
     }
     ring.release(rp);   // this warp no longer reads input plane rp
