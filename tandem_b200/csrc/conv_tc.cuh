@@ -152,6 +152,25 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* tmap, 
       "l"(tmap), "r"(x0), "r"(x1), "r"(x2), "r"(x3), "r"(smem_u32(bar))
       : "memory");
 }
+// The same for a 5-D tensor map, and its reverse: a whole box shared -> global (SASS: UTMASTG), elements beyond the
+// tensor are not written.  Stores are tracked in bulk groups: commit closes one, wait_read(0) returns once every
+// committed store has finished reading shared memory, so that its source may be overwritten (or the CTA exit).
+__device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* tmap, int x0, int x1, int x2, int x3, int x4, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];" ::"r"(
+          smem_u32(dst)),
+      "l"(tmap), "r"(x0), "r"(x1), "r"(x2), "r"(x3), "r"(x4), "r"(smem_u32(bar))
+      : "memory");
+}
+__device__ __forceinline__ void tma_store_5d(const CUtensorMap* tmap, const void* src, int x0, int x1, int x2, int x3, int x4) {
+  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(tmap),
+               "r"(smem_u32(src)), "r"(x0), "r"(x1), "r"(x2), "r"(x3), "r"(x4)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// Makes this thread's generic-proxy writes to shared memory visible to later TMA (async-proxy) reads of it
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // Programmatic dependent launch: a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start
 // while its predecessor drains (see Ring::start for what runs before pdl_wait()).
@@ -161,15 +180,18 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 // Consumer warpgroups (warps 0 .. 4*NWG-1; warp 4*NWG produces) of one instantiation, fixed at build time.  Four keep up
 // to four MMA chains in flight per SM, so that one warpgroup's drain and epilogue are covered by three others' MMAs.  At
 // 544 threads (17 warps, five of them on one SM sub-partition) ptxas allows 96 registers per thread; two warpgroups (288
-// threads, 168 registers) remain only where that cap spills (-Xptxas -v, DESIGN.md section 5): the N = 64 transposed
-// convs (MODE 1), which keep their bias and the early-fetched skip operand in registers (the N = 128 one loads both in
-// the epilogue and fits), and the prob layer's soft-argmin tail for more than 32 planes (RegressTail<48 / 64>).  The
-// N = 64 transposed convs spilled at 96 with 4-byte epilogue accesses; their 8-byte ones build at 88 with two warpgroups,
-// and four have not been tried since.
+// threads, 168 registers) remain only where that cap spills (-Xptxas -v, DESIGN.md section 5): the prob layer's
+// soft-argmin tail for more than 32 planes (RegressTail<48 / 64>), and the N = 64 transposed convs (MODE 1: conv11 and
+// the conv7 slices).  Those build at 58 registers with four since their skip operand comes through the shared-memory
+// output box, but their tile plans, and with them the launch situations the layer tests are built around
+// (oracle/mvsnet_layers.py WINDOWS), are those of two warpgroups; the N = 128 one (conv9) runs four.
 // mode: k_conv_tc's MODE (0 for the stride-2 and input-stationary kernels); n: instruction N; tail_d: Tail::max_d, 0
 // without a tail.  The planners read the same function with their full-depth tile's D for tail_d (D <= 32 exactly when
 // the tail's bucket max_d is), so their warpgroup balance matches the kernel they plan for.
 __host__ __device__ constexpr int conv_nwg(int mode, int n, int tail_d) { return (mode == 1 && n <= 64) || tail_d > 32 ? 2 : 4; }
+// Most 128-position chunks per input plane of a transposed-conv (MODE 1) tile: its consumers keep the output-box offsets
+// of their fragment rows in registers, 2 * ceil(2 * kDeconvMaxCh / NWG) of them
+constexpr int kDeconvMaxCh = 8;
 __host__ __device__ constexpr int conv_threads(int nwg) { return 128 * nwg + 32; }
 // Tile-time factor of a plane's 2*nch sub-chunks dealt round-robin to nwg warpgroups: the last round may leave some idle
 inline double wg_balance(int nch, int nwg) { return (double)((2 * nch + nwg - 1) / nwg * nwg) / (2 * nch); }
@@ -205,8 +227,9 @@ __device__ __forceinline__ uint32_t kstep_alo(int b, uint32_t cgb16, TapOff off)
 // The TMA ring
 // ---------------------------------------------------------------------------------------------------------------
 // Shared memory: [B image, 128-byte aligned][S slots of slot_bytes][full[S] at +0, empty[S] at +8, b_full at +16 (8-byte
-// barriers, S <= 8)].  Input plane rp goes to slot rp % S; full[s] counts its TMA bytes, empty[s] the 4 * NWG consumer
-// warps' releases of it.
+// barriers, S <= 8; k_conv_tc's MODE 1 adds its output-box barriers at +17 .. +20), 256 bytes][MODE 1: two output
+// boxes].  Input plane rp goes to slot rp % S; full[s] counts its TMA bytes, empty[s] the 4 * NWG consumer warps'
+// releases of it.
 template <int NWG>
 struct Ring {
   uint8_t* a;             // slot 0
@@ -368,6 +391,8 @@ __device__ __forceinline__ int stencil_off(int t, int P) { return (t / 3) * P + 
 template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool OUT_PLAIN, int MODE, bool HILO, typename Tail, int NWG>
 __global__ void __launch_bounds__(conv_threads(NWG), 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, groups*planes}, box {8, P, R+2, 1}*/,
+          const __grid_constant__ CUtensorMap tmap_res /*MODE 1: skip operand, see OutBox*/,
+          const __grid_constant__ CUtensorMap tmap_out /*MODE 1: output*/,
           const TIn* __restrict__ bimg /*host-arranged B image*/, const float* __restrict__ bias,
           const TOut* __restrict__ res, TOut* __restrict__ out, float* __restrict__ plain_out, const __grid_constant__ Geom g,
           const __grid_constant__ Tail tail) {
@@ -392,17 +417,74 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
   const TileOrigin o = tile_origin(g);
   const int nin = o.ndo + KD - 1;                  // input planes to stream
 
+  // MODE 1 output boxes: input plane d of the tile yields output planes 2d, 2d + 1, rows 2h0 .. 2h0 + 2R - 1 and columns
+  // 2w0 .. 2w0 + 2TW - 1.  Its box holds them for the OBG output channel groups of this N slice, in P8 order
+  // [group][2][2R][2TW][8]; the skip operand comes in by TMA into the box, the consumers turn it into the output in
+  // place, and the producer stores the box by TMA.  Two boxes alternate, so that plane od + 1 never waits for od's store.
+  constexpr int OBG = MODE == 1 ? NPAD / 64 : 1;
+  const uint32_t obox_bytes = MODE == 1 ? 128u * (uint32_t)(g.R * g.TW * OBG) : 0u;
+  uint8_t* const obox0 = reinterpret_cast<uint8_t*>(ring.bars) + 256;
+  uint64_t* const obox_full = ring.bars + 17;     // [2] skip operand landed (or the box is free, without one)
+  uint64_t* const obox_filled = ring.bars + 19;   // [2] the 4 * NWG consumer warps wrote their outputs
+  if constexpr (MODE == 1) {
+    if (threadIdx.x == 0) {
+      for (int b = 0; b < 2; ++b) { mbar_init(obox_full + b, 1); mbar_init(obox_filled + b, 4 * NWG); }
+      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+  }
+
   if (warp == 4 * NWG) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       // one tiled TMA per (plane, channel group): box = (R+2) rows x P positions, rows / columns beyond the tensor are
       // zero-filled by the TMA engine, so partial tiles need no special casing
       const uint32_t box_bytes = (uint32_t)g.P * (uint32_t)(g.R + 2) * 16u;
-      ring.produce(nin, box_bytes * CG, [&](uint8_t* dst, int rp, uint64_t* bar) {
+      auto boxes = [&](uint8_t* dst, int rp, uint64_t* bar) {
         const int pp = o.d0 + rp + PLANE0;  // padded plane index (pd == 1: plane d-1+kd+1; pd == 0: plane d)
 #pragma unroll 1
         for (int cg = 0; cg < CG; ++cg) tma_load_4d(dst + (size_t)cg * cg_bytes, &tmap, 0, o.w0, o.h0, cg * g.iDp + pp, bar);
-      });
+      };
+      if constexpr (MODE == 1) {
+        // input planes, skip boxes and output stores interleaved: plane od's consumers need input planes od, od + 1 and
+        // box od % 2; the box of od + 2 is refilled once od's store has read it.  Skip and output tensor maps cover
+        // the interior of the P8 tensors: rows / columns beyond the grid read as zero and are never written.
+        const int og = OBG == 1 ? ns : 0;   // first output channel group of this slice
+        auto fill = [&](int od) {
+          uint64_t* bar = obox_full + (od & 1);
+          if (g.has_res) {
+            mbar_expect_tx(bar, obox_bytes);
+            tma_load_5d(obox0 + (size_t)(od & 1) * obox_bytes, &tmap_res, 0, 2 * o.w0, 2 * o.h0, 2 * (o.d0 + od), og, bar);
+          } else {
+            mbar_arrive(bar);
+          }
+        };
+        int rp = 0;
+        auto feed = [&](int upto) {
+          for (; rp < upto && rp < nin; ++rp) {
+            const int slot = rp % g.S;
+            if (rp >= g.S) mbar_wait(ring.empty(slot), ((rp / g.S) - 1) & 1);
+            mbar_expect_tx(ring.full(slot), box_bytes * CG);
+            boxes(ring.a + (size_t)slot * ring.slot_bytes, rp, ring.full(slot));
+          }
+        };
+        feed(g.S);
+        fill(0);
+        if (o.ndo > 1) fill(1);
+        for (int od = 0; od < o.ndo; ++od) {
+          mbar_wait(obox_filled + (od & 1), (od >> 1) & 1);
+          tma_store_5d(&tmap_out, obox0 + (size_t)(od & 1) * obox_bytes, 0, 2 * o.w0, 2 * o.h0, 2 * (o.d0 + od), og);
+          bulk_commit();
+          feed(od + 1 + g.S);   // the consumers released plane od before they signalled its box
+          if (od + 2 < o.ndo) {
+            bulk_wait_read0();
+            fill(od + 2);
+          }
+        }
+        bulk_wait_read0();
+      } else {
+        ring.produce(nin, box_bytes * CG, boxes);
+      }
     }
     return;
   }
@@ -423,12 +505,12 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
   // P8 position and first channel of column block j of pixel (d, h, w); false for blocks beyond COUT
   auto out_at = [&](int d, int h, int w, int j, long long& pos, int& co) -> bool {
     const int n = ns * NPAD + 8 * j + 2 * (lane & 3);
-    if constexpr (CLASS_EPI) {
-      // N = 8 (MODE 1) or 4 (MODE 3) parity classes x COUT: class (pd,ph,pw) of input position (d,h,w) is output (2d+pd, 2h+ph, 2w+pw)
+    if constexpr (MODE == 3) {
+      // N = 4 parity classes x COUT: class (ph,pw) of input position (d,h,w) is output (d, 2h+ph, 2w+pw)
       const int cls = n / g.cout;
       co = n % g.cout;
-      const int od2 = MODE == 1 ? 2 * d + (cls >> 2) : d, oh2 = 2 * h + ((cls >> 1) & 1), ow2 = 2 * w + (cls & 1);
-      pos = ((((long long)(od2 + g.opd)) * g.oHp + (oh2 + 1)) * g.oWp + (ow2 + 1)) * 8;
+      const int oh2 = 2 * h + ((cls >> 1) & 1), ow2 = 2 * w + (cls & 1);
+      pos = ((((long long)(d + g.opd)) * g.oHp + (oh2 + 1)) * g.oWp + (ow2 + 1)) * 8;
     } else {
       co = n;
       if (ns * NPAD + 8 * j >= g.cout) return false;
@@ -436,40 +518,60 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
     }
     return true;
   };
-  // bias in registers, except for N = 128, whose 32 more registers would spill: it loads them in the epilogue
+  // bias in registers, except for N = 128, whose 32 more registers would spill: it loads them in the epilogue.  MODE 1
+  // slice ns holds output channels ns * CPS .. + CPS - 1 of all 8 classes (build_b_image_deconv): column n is class
+  // n / CPS, channel ns * CPS + n % CPS.
   constexpr bool BIAS_REG = NPAD <= 64;
+  constexpr int CPS = NPAD / 8;
+  const float* const bias_s = MODE == 1 && bias ? bias + ns * CPS : bias;
   float bv[OUT_PLAIN || !BIAS_REG ? 1 : NPAD / 8][2];
   if constexpr (OUT_PLAIN) bv[0][0] = bias ? bias[0] : 0.f;
+  else if constexpr (BIAS_REG && MODE == 1) load_bias<true>(bv, bias_s, 0, CPS, lane);
   else if constexpr (BIAS_REG) load_bias<CLASS_EPI>(bv, bias, ns * NPAD, g.cout, lane);
-  // PAIR_EPI (CLASS_EPI with N <= 64) moves whole 32-byte sectors.  Classes pw = 0 and pw = 1 of one (pd, ph, output
-  // channel group) are column blocks j0 and j0 + PWS (cout = CIN / 2 for the deconvs, 8 for up-2; the host checks it), and their output pixels 2w
-  // and 2w + 1 are adjacent: 32 bytes per input position.  Lanes q and q ^ 1 of a fragment row swap one packed word, so
-  // that lane q reads and writes 8 contiguous bytes, channels 4 * (q >> 1) .. +3 of class pw = q & 1.  A warp access then
-  // covers its 8 positions' 32-byte runs in full, where two 4-byte accesses per lane filled half of each sector apiece.
-  // The N = 128 deconv (conv9), which fetches its skip operand after the chain, keeps 4-byte accesses: there the exchange
-  // puts a shuffle behind each skip load and measured slower.
-  constexpr bool PAIR_EPI = CLASS_EPI && NPAD <= 64;
-  constexpr int PWS = MODE == 1 ? CIN / 16 : 1;
+  // PAIR_EPI (MODE 3) moves whole 32-byte sectors.  Classes pw = 0 and pw = 1 of one (ph, output channel group) are
+  // column blocks 2k and 2k + 1 (cout = 8; the host checks it), and their output pixels 2w and 2w + 1 are adjacent: 32
+  // bytes per input position.  Lanes q and q ^ 1 of a fragment row swap one packed word, so that lane q writes 8
+  // contiguous bytes, channels 4 * (q >> 1) .. +3 of class pw = q & 1.  A warp access then covers its 8 positions'
+  // 32-byte runs in full, where two 4-byte accesses per lane filled half of each sector apiece.
+  constexpr bool PAIR_EPI = MODE == 3;
   const int pq = lane & 1;
-  auto pair_j0 = [](int k) { return k / PWS * 2 * PWS + k % PWS; };
   // element offset of the 8 bytes this lane moves for block pair k of pixel (d, h, w), in a tensor of group stride gs
   auto pair_at = [&](int d, int h, int w, int k, long long gs) -> long long {
     long long pos;
     int co;
-    out_at(d, h, w, pair_j0(k) + pq * PWS, pos, co);
+    out_at(d, h, w, 2 * k + pq, pos, co);
     return pos + (co >> 3) * gs + 4 * ((lane & 3) >> 1);
   };
+  // MODE 1: box element offset of this lane's channels 2q, 2q + 1 of class 0 for fragment row half i of this
+  // warpgroup's k-th sub-chunk (sub-chunk wg + k * NWG), -1 for pad columns and rows beyond the tile; decoded once per
+  // CTA.  Class (pd, ph, pw) and channel group c of the slice add c * 2 * PD_STR + pd * PD_STR + ph * PH_STR + pw * 8.
+  constexpr int MAXSC = MODE == 1 ? (2 * kDeconvMaxCh + NWG - 1) / NWG : 1;
+  int boff[MAXSC][2];
+  const int PH_STR = 16 * g.TW, PD_STR = 32 * g.R * g.TW;
+  if constexpr (MODE == 1) {
+#pragma unroll
+    for (int k = 0; k < MAXSC; ++k)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int l = (wg + k * NWG) * 64 + wq * 16 + (lane >> 2) + 8 * i;
+        const int hh = l / P, ww = l - hh * P;
+        boff[k][i] = hh < g.R && ww < g.TW ? (4 * hh * g.TW + 2 * ww) * 8 + 2 * (lane & 3) : -1;
+      }
+  }
   for (int od = 0; od < o.ndo; ++od) {
     ring.wait(od + KD - 1);
     uint32_t slot16[KD];
 #pragma unroll
     for (int kd = 0; kd < KD; ++kd) slot16[kd] = ring.slot16(od + kd);
     const int d = o.d0 + od;
-    for (int sc = wg; sc < nsub; sc += NWG) {
+    TOut* const box = reinterpret_cast<TOut*>(obox0 + (size_t)(od & 1) * obox_bytes);
+    if constexpr (MODE == 1) mbar_wait(obox_full + (od & 1), (od >> 1) & 1);
+#pragma unroll 1
+    for (int k = 0; wg + k * NWG < nsub; ++k) {
+      const int sc = wg + k * NWG;
       const int l = sc * 64 + wq * 16 + (lane >> 2);
-      // the skip operand is fetched before the MMA chain, so that its load latency overlaps the chain (except for N = 128,
-      // whose accumulators leave no room for it)
-      constexpr bool RES_EARLY = !OUT_PLAIN && NPAD <= 64;
+      // the skip operand is fetched before the MMA chain, so that its load latency overlaps the chain
+      constexpr bool RES_EARLY = !OUT_PLAIN && NPAD <= 64 && MODE != 1;
       uint32_t rv[2][RES_EARLY ? NPAD / 8 : 1];
       if constexpr (RES_EARLY) {
         if (g.has_res) {
@@ -477,27 +579,49 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
           for (int i = 0; i < 2; ++i) {
             int h, w;
             const bool in = frag_pixel(g, o, l, i, h, w);
-            if constexpr (PAIR_EPI) {
-              // rv[i][2k .. 2k+1]: this lane's 8 bytes of block pair k, exchanged after the chain
 #pragma unroll
-              for (int k = 0; k < NPAD / 16; ++k) {
-                const uint2 r = in ? __ldg(reinterpret_cast<const uint2*>(res + pair_at(d, h, w, k, g.res_gs))) : make_uint2(0u, 0u);
-                rv[i][2 * k] = r.x; rv[i][2 * k + 1] = r.y;
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < NPAD / 8; ++j) {
-                long long pos;
-                int co;
-                rv[i][j] = in && out_at(d, h, w, j, pos, co)
-                               ? __ldg(reinterpret_cast<const unsigned int*>(res + pos + (co >> 3) * g.res_gs + (co & 7))) : 0u;
-              }
+            for (int j = 0; j < NPAD / 8; ++j) {
+              long long pos;
+              int co;
+              rv[i][j] = in && out_at(d, h, w, j, pos, co)
+                             ? __ldg(reinterpret_cast<const unsigned int*>(res + pos + (co >> 3) * g.res_gs + (co & 7))) : 0u;
             }
           }
         }
       }
       float acc[NMMA / 2];
       mma_subchunk<NMMA, TIn, KD, NBLK>(acc, slot16, (uint32_t)sc * 64u, sB16, b_lbo16, aoff, alo);
+      if constexpr (MODE == 1) {
+        // acc + bias -> ReLU -> + skip -> one rounding, in place in the box
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          int bo = boff[0][i];
+#pragma unroll
+          for (int kk = 1; kk < MAXSC; ++kk)
+            if (k == kk) bo = boff[kk][i];
+          if (bo < 0) continue;
+#pragma unroll
+          for (int j = 0; j < NPAD / 8; ++j) {
+            const int cls = j / OBG, c = j % OBG;
+            uint32_t* const p = reinterpret_cast<uint32_t*>(box + bo + (2 * c + (cls >> 2)) * PD_STR + ((cls >> 1) & 1) * PH_STR + (cls & 1) * 8);
+            float x[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              x[e] = acc[4 * j + 2 * i + e];
+              if constexpr (BIAS_REG) x[e] += bv[j][e];
+              else x[e] += bias_s ? __ldg(bias_s + (8 * j + 2 * (lane & 3)) % CPS + e) : 0.f;
+              if (g.relu) x[e] = fmaxf(x[e], 0.f);
+            }
+            if (g.has_res) {
+              float r0, r1;
+              unpack2<TOut>(*p, r0, r1);
+              x[0] += r0; x[1] += r1;
+            }
+            *p = pack2<TOut>(x[0], x[1]);
+          }
+        }
+        continue;
+      }
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         int h, w;
@@ -505,19 +629,11 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
         if (!in && !PAIR_EPI) continue;   // PAIR_EPI: every lane takes part in the word exchange
         if constexpr (PAIR_EPI) {
 #pragma unroll
-          for (int k = 0; k < NPAD / 16; ++k) {
-            const int j0 = pair_j0(k);
-            uint32_t r[2] = {0u, 0u};   // skip words of blocks j0 and j0 + PWS at this lane's channels 2q, 2q + 1
-            if (g.has_res) {
-              const uint2 rr = make_uint2(rv[i][2 * k], rv[i][2 * k + 1]);
-              // rr holds channels 2(q & ~1) .. +3 of class pq: this lane's own word and the partner's
-              const uint32_t own = pq ? rr.y : rr.x, other = __shfl_xor_sync(0xffffffffu, pq ? rr.x : rr.y, 1);
-              r[0] = pq ? other : own; r[1] = pq ? own : other;
-            }
+          for (int k2 = 0; k2 < NPAD / 16; ++k2) {
             uint32_t v[2];
 #pragma unroll
             for (int p = 0; p < 2; ++p) {
-              const int j = j0 + p * PWS;
+              const int j = 2 * k2 + p;
               float x[2];
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
@@ -526,15 +642,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
                 x[e] += bv[j][e];
                 if (g.relu) x[e] = fmaxf(x[e], 0.f);
               }
-              if (g.has_res) {
-                float r0, r1;
-                unpack2<TOut>(r[p], r0, r1);
-                x[0] += r0; x[1] += r1;
-              }
               v[p] = pack2<TOut>(x[0], x[1]);
             }
             const uint32_t own = pq ? v[1] : v[0], other = __shfl_xor_sync(0xffffffffu, pq ? v[0] : v[1], 1);
-            if (in) *reinterpret_cast<uint2*>(out + pair_at(d, h, w, k, g.out_gs)) = pq ? make_uint2(other, own) : make_uint2(own, other);
+            if (in) *reinterpret_cast<uint2*>(out + pair_at(d, h, w, k2, g.out_gs)) = pq ? make_uint2(other, own) : make_uint2(own, other);
           }
         } else if constexpr (OUT_PLAIN) {
           if ((lane & 3) == 0) {
@@ -573,6 +684,12 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
           }
         }
       }
+    }
+    if constexpr (MODE == 1) {
+      // this warp's outputs of plane od are in the box: hand it to the producer's TMA store
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(obox_filled + (od & 1));
     }
     ring.release(od);   // oldest input plane of od
   }
@@ -616,6 +733,8 @@ inline void build_b_image(const float* w, int cin, int cout, int npad, int kd_n,
 // Transposed conv (k3 s2 p1 op1) B image: w is the gather-form folded weight [tap27][cin][cout] (tap index = kernel index
 // of the ConvTranspose3d).  Per axis, output parity p and input offset t (0 = same index, 1 = next index) select the
 // kernel index: p=0:t=0 -> k=1 ; p=1:t=0 -> k=2, t=1 -> k=0 ; (p=0,t=1) contributes nothing.
+// nsplit > 1: slice s holds output channels s * cout / nsplit .. + cout / nsplit - 1 of all 8 classes, column
+// cls * cout / nsplit + channel % (cout / nsplit), so that each slice writes whole output channel groups.
 template <typename T>
 inline void build_b_image_deconv(const float* w, int cin, int cout, std::vector<T>& img, T (*cvt)(float), int nsplit = 1) {
   const int nblk = ksteps(cin, 4);
@@ -633,8 +752,8 @@ inline void build_b_image_deconv(const float* w, int cin, int cout, std::vector<
               const int th = t / 2, tw = t % 2;
               const int kd = kidx(cls >> 2, td), kh = kidx((cls >> 1) & 1, th), kw = kidx(cls & 1, tw);
               if (kd < 0 || kh < 0 || kw < 0 || ci >= cin) continue;
-              const int nfull = cls * cout + co, n = nfull % npad;
-              T* simg = img.data() + slice * (nfull / npad);
+              const int cps = cout / nsplit, n = cls * cps + co % cps;   // slice co / cps: channels co / cps * cps .. + cps - 1
+              T* simg = img.data() + slice * (co / cps);
               const float val = w[((size_t)((kd * 3 + kh) * 3 + kw) * cin + ci) * cout + co];
               simg[b_index(td * nblk + b, half, n, e, npad)] = cvt(val);
             }
@@ -674,6 +793,11 @@ struct TileLimits {
   int nch_max;            // most 128-position chunks per plane
   int dr_min;             // fewest planes per tile (when D >= 2)
   bool full_depth;        // tiles span all D planes (the prob layer's soft-argmin tail needs a pixel's D logits in one CTA)
+  int out_box = 0;        // shared-memory bytes of output boxes per tile position (R x TW), 0 without them.  They count
+                          // against the 225 KB an SM offers, not against a lower budget (see plan_tiles)
+  int tw_max = INT_MAX;   // widest tile
+  int whole_rounds = 0;   // > 0: a plane of more than one chunk deals its 2 * nch sub-chunks in whole rounds of this many
+                          // warpgroups (no warpgroup idles through the last round)
 };
 
 struct Plan {
@@ -691,24 +815,29 @@ struct Plan {
 // tile_clk(DR, nch) is the estimated time of one tile in clocks: a per-CTA fixed cost + the instruction stream.  Its
 // constants are a model (instruction cost growing with N, a fixed per-CTA prologue, fill and drain), not a measurement;
 // they only rank tilings against each other; callers scale it by wg_balance for the kernel's consumer warpgroups.  A limit
-// below 225 KB is soft: if nothing fits it, 225 KB is searched.
+// below 225 KB is soft: if nothing fits it, 225 KB is searched.  It bounds the B image and the ring; output boxes
+// (TileLimits::out_box) count against the 225 KB only.
 template <typename Amp, typename Clk>
 inline Tile plan_tiles(int D, int H, int W, int cg, size_t b_bytes, size_t smem_limit, const TileLimits& lim, Amp amp, Clk tile_clk,
                        size_t& smem_out) {
-  auto smem_of = [&](int S, int R, int P) { return b_bytes + (size_t)S * cg * lim.boxes * box_positions(R, P, lim.halo) * 16 + 256; };
+  auto box_bytes = [&](int R, int P) { return (size_t)lim.out_box * R * (P - lim.halo); };
+  auto smem_of = [&](int S, int R, int P) {
+    return b_bytes + (size_t)S * cg * lim.boxes * box_positions(R, P, lim.halo) * 16 + 256 + box_bytes(R, P);
+  };
   double best_cost = 1e30;
   int bestR = 0, bestTW = 0, bestS = 0, bestDR = 0;
   for (int S = lim.s_hi; S >= lim.s_lo; --S) {
     for (int tiles_w = 1; tiles_w <= 20; ++tiles_w) {
       const int TW = (W + tiles_w - 1) / tiles_w;
-      if (TW + lim.halo > lim.p_max) continue;
+      if (TW + lim.halo > lim.p_max || TW > lim.tw_max) continue;
       if (tiles_w > 1 && TW < lim.tw_min) break;
       const int tw_n = (W + TW - 1) / TW;
       const int P = TW + lim.halo;
       for (int R = 1; R <= 32 && R <= H; ++R) {
         const int nch = (R * P + 127) / 128;
         if (nch > lim.nch_max) break;
-        if (smem_of(S, R, P) > smem_limit) break;
+        if (smem_of(S, R, P) - box_bytes(R, P) > smem_limit || smem_of(S, R, P) > 225 * 1024) break;
+        if (lim.whole_rounds && nch > 1 && (2 * nch) % lim.whole_rounds) continue;
         const int th_n = (H + R - 1) / R;
         for (int dsplit = 1; dsplit <= (lim.full_depth ? 1 : D); ++dsplit) {
           const int DR = (D + dsplit - 1) / dsplit;
@@ -744,7 +873,17 @@ inline Plan make_plan(int cin, int npad, int kd, int D, int H, int W, int pd, in
   Plan p{};
   const int nblk = ksteps(cin, mode == 1 ? 4 : 9);
   const int s_hi = kd == 3 ? 4 : 3, s_lo = kd == 3 ? 3 : 2;   // kd == 2 (deconv): 2 live + 1 prefetch
-  const TileLimits lim{s_hi, s_lo, 2, 1, 256, 30, INT_MAX, kd >= 2 ? 2 : 1, full_depth};
+  TileLimits lim{s_hi, s_lo, 2, 1, 256, 30, INT_MAX, kd >= 2 ? 2 : 1, full_depth};
+  if (mode == 1) {
+    // two output boxes of npad / 64 channel groups, 8 output positions of 16 bytes per input position; a box spans 2 TW
+    // columns (TMA box dimensions <= 256)
+    lim.out_box = 2 * (npad / 64) * 128;
+    lim.tw_max = 128;
+    lim.nch_max = kDeconvMaxCh;
+    // with four warpgroups an odd chunk count leaves two of them idle for one chain per plane, and the plane's box store
+    // waits for the slowest warpgroup: tiles of 1 or an even number of chunks only
+    lim.whole_rounds = conv_nwg(1, npad, 0);
+  }
   auto amp = [&](int R, int TW, int P, int DR) {
     return (double)(R + 2) / R * (double)P / TW * (kd == 3 ? (double)(DR + 2) / DR : (kd == 2 ? (double)(DR + 1) / DR : 1.0));
   };

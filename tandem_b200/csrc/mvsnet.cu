@@ -828,7 +828,7 @@ class MvsnetEngine final : public MvsnetIface {
 
   // Tile plan and input tensor map of one layer's tensor-core launch, made on first use.  Keys: the layer, + "#tail" (prob
   // with the soft-argmin tail), "#is" / "#is#tail" (input-stationary kernel), "#s2" (stride-2 kernel).
-  struct TcCache { tc::Plan plan; tc::PlanS2 plan_s2; CUtensorMap tmap; };
+  struct TcCache { tc::Plan plan; tc::PlanS2 plan_s2; CUtensorMap tmap, tmap_res, tmap_out; };
   std::map<std::string, TcCache> tc_cache_;
 
   template <typename Make>
@@ -858,6 +858,26 @@ class MvsnetEngine final : public MvsnetIface {
                                              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     TDM_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed for " + wkey + " (" + std::to_string((int)r) + ")");
+    return tmap;
+  }
+
+  // tensor map over the interior of a 3-D P8 output (or skip) tensor {8 channels, W, H, D, channel group} for the output
+  // boxes of the transposed convs: box 2 tw columns x 2 r rows x 2 planes x groups channel groups.  Boxes are moved as
+  // 16-bit words, fp16 or bf16 alike; elements beyond the interior are zero-filled on loads and skipped on stores, so the
+  // halos stay zero.
+  CUtensorMap p8_interior_tmap(const std::string& wkey, const DevBuf& t, int tw, int r, int groups) {
+    TDM_CHECK(t.pd == 1 && 2 * tw <= 256 && 2 * r <= 256, wkey + ": output box out of the TMA limits");
+    CUtensorMap tmap;
+    const P8<TA> v = p8<TA>(t);
+    TA* base = v.p + ((long long)(v.Hp + 1) * v.Wp + 1) * 8;   // plane 1 (the first interior one), row 1, column 1
+    const cuuint64_t dims[5] = {8, (cuuint64_t)t.W, (cuuint64_t)t.H, (cuuint64_t)t.D, (cuuint64_t)(t.C / 8)};
+    const cuuint64_t strides[4] = {16, (cuuint64_t)v.Wp * 16, (cuuint64_t)v.Wp * v.Hp * 16, (cuuint64_t)v.gs * 2};
+    const cuuint32_t box[5] = {8, (cuuint32_t)(2 * tw), (cuuint32_t)(2 * r), 2, (cuuint32_t)groups};
+    const cuuint32_t es[5] = {1, 1, 1, 1, 1};
+    const CUresult res = tc::encode_tiled_fn()(&tmap, CU_TENSOR_MAP_DATA_TYPE_UINT16, 5, base, dims, strides, box, es,
+                                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                                               CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    TDM_CHECK(res == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed for the output box of " + wkey + " (" + std::to_string((int)res) + ")");
     return tmap;
   }
 
@@ -904,6 +924,11 @@ class MvsnetEngine final : public MvsnetIface {
         if (res) g.res_gs = p8<const TOut>(*res).gs;
       }
       x.tmap = p8_tmap<TIn>(wkey, in, CIN / 8, g.iDp, g.P, g.R + 2, 1);
+      x.tmap_res = x.tmap_out = x.tmap;   // read by MODE 1 only
+      if constexpr (MODE == 1) {
+        x.tmap_out = p8_interior_tmap(wkey, out, g.TW, g.R, NPAD / 64);
+        if (res) x.tmap_res = p8_interior_tmap(wkey, *res, g.TW, g.R, NPAD / 64);
+      }
       debug_plan(wkey, "mode " + std::to_string(MODE) + " cin " + std::to_string(CIN) + " N " + std::to_string(HILO ? 2 * NPAD : NPAD) +
                  " kd " + std::to_string(KD) + " in", g, x.plan.grid, c.nsplit, x.plan.smem);
       return x;
@@ -920,9 +945,13 @@ class MvsnetEngine final : public MvsnetIface {
     }
     constexpr int NWG = tc::conv_nwg(MODE, HILO ? 2 * NPAD : NPAD, Tail::max_d);
     TDM_CHECK(pl.nwg == NWG, wkey + ": tile plan balanced for another warpgroup count than the kernel's");
-    // the parity-class epilogue pairs column blocks pw = 0 / 1 at a compile-time distance of cout / 8 blocks
-    TDM_CHECK((MODE != 1 || c.cout == CIN / 2) && (MODE != 3 || c.cout == 8), wkey + ": parity-class layer with an unexpected cout");
-    launch_tc<tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail, NWG>>(dim3(pl.grid, c.nsplit), pl.smem, tcx.tmap, (const TIn*)c.bimg,
+    // MODE 1: each N slice of NPAD columns is 8 classes x NPAD / 8 channels, whole output channel groups of the box;
+    // MODE 3: the epilogue pairs column blocks pw = 0 / 1 of cout = 8
+    TDM_CHECK((MODE != 1 || (c.cout == CIN / 2 && c.cout == c.nsplit * NPAD / 8 && NPAD % 64 == 0 && (NPAD == 64 || c.nsplit == 1))) &&
+              (MODE != 3 || c.cout == 8), wkey + ": parity-class layer with an unexpected cout");
+    TDM_CHECK(MODE != 1 || (out.pd == 1 && (!res || (res->D == out.D && res->H == out.H && res->W == out.W && res->C == out.C))),
+              wkey + ": transposed conv skip / output shapes differ");
+    launch_tc<tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail, NWG>>(dim3(pl.grid, c.nsplit), pl.smem, tcx.tmap, tcx.tmap_res, tcx.tmap_out, (const TIn*)c.bimg,
                                                                               (const float*)c.bias, rp, op, plain, pl.g, tail);
   }
 
