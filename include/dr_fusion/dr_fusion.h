@@ -9,6 +9,7 @@
 #include <vector>
 
 struct tdm_fusion;  // include/tandem_b200.h
+class DrMvsnet;     // include/dr_mvsnet/dr_mvsnet.h
 
 struct DrFusionOptions {
     float voxel_size;
@@ -43,6 +44,11 @@ public:
     ~DrFusion();
 
     void IntegrateScanAsync(unsigned char *bgr, float *depth, float const *pose);
+
+    // Extension: integrates the result mvsnet.GetResult() last returned where it sits on the device - its depth, the
+    // window's reference BGR image and (pose == nullptr) reference cam_to_world, i.e. what tandem_backend.cpp:166 passes -
+    // with no host round trip.  Legal until the next GetResult, also after the next CallAsync (tdm_fusion_integrate_mvsnet).
+    void IntegrateScanAsync(DrMvsnet const &mvsnet, float const *pose = nullptr);
 
     void RenderAsync(std::vector<float const *> camera_poses);
 

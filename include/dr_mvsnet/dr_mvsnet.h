@@ -9,6 +9,7 @@
 #include <utility>
 
 class DrMvsnetImpl;  // opaque: owns a tdm_mvsnet handle (shims/dr_mvsnet.cpp)
+struct tdm_mvsnet;   // include/tandem_b200.h
 
 class DrMvsnetOutput {
 public:
@@ -54,6 +55,9 @@ public:
 
   // Non-blocking
   bool Ready();
+
+  // Extension: the C-ABI handle, so that DrFusion::IntegrateScanAsync(DrMvsnet const&) can read the result on the device.
+  tdm_mvsnet* handle() const;
 
 private:
   DrMvsnetImpl *impl;

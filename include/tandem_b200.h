@@ -136,6 +136,19 @@ void tdm_fusion_destroy(tdm_fusion* h);
 /* DrFusion::IntegrateScanAsync (dr_fusion.h:50): bgr H*W*3 u8, depth H*W f32 metric z-depth, pose 4x4
  * row-major cam->world; inputs are copied into pinned staging before returning (tsdf_volume.cu:542-543). */
 int tdm_fusion_integrate_async(tdm_fusion* h, const unsigned char* bgr, const float* depth, const float* pose);
+/* Extension: IntegrateScanAsync of the result the last tdm_mvsnet_get_result of m returned, read on the device
+ * (tandem_backend.cpp:166 passes that result's depth, the window's reference BGR image and its cam_to_world; the
+ * reference's IntegrateScanAsync, tsdf_volume.cu:515-598, then uploads both images again).  Integrates the filtered
+ * stage-3 depth and the reference view's BGR image - the bytes tdm_mvsnet_get_result wrote and the caller passed to
+ * tdm_mvsnet_call_async - with pose, or with the window's reference cam_to_world when pose is NULL: the volume is the one
+ * tdm_fusion_integrate_async builds from the same inputs, bit for bit.
+ * get_result keeps that result on the device (a device-to-device copy on the engine's stream) until the next get_result, so
+ * the call may come after the next window's call_async, as in TANDEM; the same result may be integrated again, into this
+ * or other fusion handles.  Same call order as tdm_fusion_integrate_async; returns once the work is enqueued (no host
+ * synchronisation).  Either handle may be destroyed right after the call.  Errors, with nothing launched: a null handle,
+ * no result fetched from m yet, a fusion height / width that differs from the window's, handles on different devices, a
+ * singular pose, the wrong call order. */
+int tdm_fusion_integrate_mvsnet(tdm_fusion* h, tdm_mvsnet* m, const float* pose);
 /* DrFusion::RenderAsync (dr_fusion.h:52): n_poses must equal num_render_streams (tsdf_volume.cu:643-648). */
 int tdm_fusion_render_async(tdm_fusion* h, const float* const* camera_poses, int n_poses);
 /* DrFusion::GetRenderResult (dr_fusion.h:54): pointers into a pinned double buffer owned by the handle,

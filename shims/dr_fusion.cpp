@@ -1,6 +1,7 @@
 // class DrFusion over the tandem_b200 C ABI (replaces tandem/libdr/dr_fusion/src/dr_fusion/dr_fusion.cpp).
 // Error convention of the reference: print + exit(EXIT_FAILURE) (tsdf_volume.cu:520-524).
 #include "dr_fusion/dr_fusion.h"
+#include "dr_mvsnet/dr_mvsnet.h"
 
 #include <cstdio>
 #include <cstdlib>
@@ -32,6 +33,10 @@ DrFusion::~DrFusion() {
 
 void DrFusion::IntegrateScanAsync(unsigned char* bgr, float* depth, float const* pose) {
   if (tdm_fusion_integrate_async(handle_, bgr, depth, pose) != TDM_OK) die("DrFusion::IntegrateScanAsync");
+}
+
+void DrFusion::IntegrateScanAsync(DrMvsnet const& mvsnet, float const* pose) {
+  if (tdm_fusion_integrate_mvsnet(handle_, mvsnet.handle(), pose) != TDM_OK) die("DrFusion::IntegrateScanAsync(DrMvsnet)");
 }
 
 void DrFusion::RenderAsync(std::vector<float const*> camera_poses) {

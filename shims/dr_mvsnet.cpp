@@ -77,6 +77,8 @@ void DrMvsnet::Wait() {
 
 bool DrMvsnet::Ready() { return tdm_mvsnet_ready(impl->h) == 1; }
 
+tdm_mvsnet* DrMvsnet::handle() const { return impl->h; }
+
 // ---- known-answer test on the converted golden container -------------------------------------------------------
 // sample_inputs.bin (tools/convert_sample_inputs.py): "TDMS0001", i32 V,H,W, f32 K[9] (stage 3), f32 dmin,dmax,discard,
 // f32 c2w[V*16], u8 bgr[V*H*W*3] (window order, reference at V-2), f32 depth[H*W], f32 confidence[H*W] (stage 3 filtered).

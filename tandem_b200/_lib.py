@@ -117,6 +117,7 @@ def _declare(l):
         "tdm_fusion_create": (i, [P(FusionOptions), i, P(vp)]),
         "tdm_fusion_destroy": (None, [vp]),
         "tdm_fusion_integrate_async": (i, [vp, vp, fp, fp]),
+        "tdm_fusion_integrate_mvsnet": (i, [vp, vp, fp]),
         "tdm_fusion_render_async": (i, [vp, P(fp), i]),
         "tdm_fusion_get_render_result": (i, [vp, P(vp), P(fp), i]),
         "tdm_fusion_synchronize": (i, [vp]),

@@ -3,9 +3,13 @@
 #include "capi_common.h"
 #include "common.cuh"
 #include "fusion.h"
+#include "mvsnet.h"
 
 struct tdm_fusion {
   tdm::FusionIface* impl;
+};
+struct tdm_mvsnet {   // same layout as in capi_mvsnet.cu (one pointer)
+  tdm::MvsnetIface* impl;
 };
 
 extern "C" {
@@ -26,6 +30,16 @@ int tdm_fusion_integrate_async(tdm_fusion* h, const unsigned char* bgr, const fl
   TDM_API_BEGIN
   TDM_CHECK(h && bgr && depth && pose, "null argument");
   h->impl->integrate_async(bgr, depth, pose);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_fusion_integrate_mvsnet(tdm_fusion* h, tdm_mvsnet* m, const float* pose) {
+  TDM_API_BEGIN
+  TDM_CHECK(h && m, "null handle");
+  tdm::FusionIface* f = h->impl;
+  m->impl->read_handoff(f->stream(), [f, pose](const tdm::MvsnetIface::Handoff& ho) {
+    f->integrate_device(ho.bgr, ho.depth, ho.H, ho.W, ho.device, ho.ready, pose ? pose : ho.c2w);
+  });
   return TDM_OK;
   TDM_API_END
 }

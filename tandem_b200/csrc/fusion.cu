@@ -897,6 +897,32 @@ class FusionImpl final : public FusionIface {
     next_ = kRender;
   }
 
+  // IntegrateScanAsync from device memory (the MVSNet keyframe handoff, tdm_fusion_integrate_mvsnet): the same scan buffers
+  // and the same launch_integrate as above, filled device to device; no host synchronisation.  Checks everything before
+  // anything is enqueued.
+  void integrate_device(const unsigned char* bgr, const float* depth, int height, int width, int device, void* ready,
+                        const float* pose) override {
+    if (next_ != kIntegrate)
+      throw Error("call order is IntegrateScanAsync -> RenderAsync -> GetRenderResult (tsdf_volume.cu:520-525)");
+    TDM_CHECK(device == device_, "the MVSNet handle and the fusion live on different devices");
+    TDM_CHECK(height == d_.o.height && width == d_.o.width, "the MVSNet window's height / width differ from the fusion's");
+    Mat4 p, pinv;
+    std::memcpy(p.m, pose, 64);
+    if (!inv4_f32(p.m, pinv.m)) throw Error("camera pose is singular");
+    TDM_CUDA(cudaSetDevice(device_));
+    const size_t npx = (size_t)d_.o.height * d_.o.width;
+    TDM_CUDA(cudaStreamWaitEvent(stream_, (cudaEvent_t)ready, 0));
+    TDM_CUDA(cudaMemcpyAsync(d_bgr_in_, bgr, npx * 3, cudaMemcpyDeviceToDevice, stream_));
+    TDM_CUDA(cudaMemcpyAsync(d_depth_in_, depth, npx * 4, cudaMemcpyDeviceToDevice, stream_));
+    pose_ = p;
+    pose_inv_ = pinv;
+    launch_integrate();
+    TDM_CUDA(cudaEventRecord(ev_int_, stream_));
+    have_scan_ = true;
+    ++volume_epoch_;
+    next_ = kRender;
+  }
+
   // RenderAsync, tsdf_volume.cu:634-700
   void render_async(const float* const* poses, int n) override {
     if (next_ != kRender) throw Error("call order is IntegrateScanAsync -> RenderAsync -> GetRenderResult (tsdf_volume.cu:635-640)");

@@ -12,6 +12,10 @@ class FusionIface {
  public:
   virtual ~FusionIface() = default;
   virtual void integrate_async(const unsigned char* bgr, const float* depth, const float* pose) = 0;
+  // The same scan from device memory of this handle's device (height x width, as the options): the stream waits for `ready`
+  // (a cudaEvent_t) and copies bgr / depth into the scan buffers; every read of them is enqueued on stream() when it returns.
+  virtual void integrate_device(const unsigned char* bgr, const float* depth, int height, int width, int device, void* ready,
+                                const float* pose) = 0;
   virtual void render_async(const float* const* poses, int n) = 0;
   virtual void get_render_result(unsigned char** bgr, float** depth, int n) = 0;
   virtual void set_slab(int z_block_lo, int z_block_hi) = 0;

@@ -158,6 +158,12 @@ class MvsnetEngine final : public MvsnetIface {
     cv_work_.notify_all();
     if (worker_.joinable()) worker_.join();
     cudaSetDevice(device_);
+    // consumers of the keyframe handoff may still be reading it: read_handoff returns once their reads are enqueued
+    cudaStreamSynchronize(stream_);
+    for (int i = 0; i < n_ho_release_; ++i) cudaEventSynchronize(ev_ho_release_[i]);
+    for (cudaEvent_t e : ev_ho_release_) cudaEventDestroy(e);
+    if (ev_ho_ready_) cudaEventDestroy(ev_ho_ready_);
+    cudaFree(d_ho_depth_); cudaFree(d_ho_bgr_);
     free_plan();
     for (auto& kv : convs_) { cudaFree(kv.second.w); cudaFree(kv.second.bias); cudaFree(kv.second.bimg); cudaFree(kv.second.bimg_s2); cudaFree(kv.second.bimg_is); }
     if (d_cv_stats_) {
@@ -332,7 +338,28 @@ class MvsnetEngine final : public MvsnetIface {
           }
       CopyPool::shared().run(jobs);
     }
+    fill_handoff();
     has_result_ = false;
+  }
+
+  void read_handoff(void* stream, const std::function<void(const Handoff&)>& consume) override {
+    std::unique_lock<std::mutex> lk(mu_);
+    if (!ho_valid_) throw Error("no MVSNet result to integrate: call GetResult first");
+    Handoff h;
+    h.depth = d_ho_depth_;
+    h.bgr = d_ho_bgr_;
+    std::memcpy(h.c2w, ho_c2w_, sizeof(ho_c2w_));
+    h.H = ho_H_; h.W = ho_W_; h.device = device_;
+    h.ready = (void*)ev_ho_ready_;
+    try {
+      consume(h);
+    } catch (...) {
+      // consume may have enqueued reads before it failed: mark them too (on another device's stream this fails, and then
+      // consume enqueued nothing)
+      if (!record_release(stream)) cudaGetLastError();
+      throw;
+    }
+    TDM_CHECK(record_release(stream), "keyframe handoff: cannot record the release event");
   }
 
   void stage_output(int stage, const std::string& which, float* out, size_t cap) override {
@@ -1510,6 +1537,43 @@ class MvsnetEngine final : public MvsnetIface {
     }
   }
 
+  // Keyframe handoff.  Invariant: the handoff buffers are written only by this fill, enqueued on stream_ behind every release
+  // event recorded since the previous fill, and freed only after those events have completed; so a consumer's reads, which
+  // wait for ev_ho_ready_ and end before their release event, always see exactly the result the last GetResult returned,
+  // however far the next window's upload and forward (which overwrite d_bgr_ and s3.depth) have got.
+  void fill_handoff() {
+    const size_t n = (size_t)H_ * W_;
+    ho_valid_ = false;
+    if (ho_H_ != H_ || ho_W_ != W_) {
+      for (int i = 0; i < n_ho_release_; ++i) TDM_CUDA(cudaEventSynchronize(ev_ho_release_[i]));
+      n_ho_release_ = 0;
+      cudaFree(d_ho_depth_); cudaFree(d_ho_bgr_);
+      d_ho_depth_ = nullptr; d_ho_bgr_ = nullptr; ho_H_ = ho_W_ = 0;
+      TDM_CUDA(cudaMalloc(&d_ho_depth_, n * 4));
+      TDM_CUDA(cudaMalloc(&d_ho_bgr_, n * 3));
+      ho_H_ = H_; ho_W_ = W_;
+    }
+    if (!ev_ho_ready_) TDM_CUDA(cudaEventCreateWithFlags(&ev_ho_ready_, cudaEventDisableTiming));
+    for (int i = 0; i < n_ho_release_; ++i) TDM_CUDA(cudaStreamWaitEvent(stream_, ev_ho_release_[i], 0));
+    n_ho_release_ = 0;
+    TDM_CUDA(cudaMemcpyAsync(d_ho_depth_, fbuf("s3.depth"), n * 4, cudaMemcpyDeviceToDevice, stream_));
+    TDM_CUDA(cudaMemcpyAsync(d_ho_bgr_, d_bgr_, n * 3, cudaMemcpyDeviceToDevice, stream_));   // view 0 = the reference view
+    TDM_CUDA(cudaEventRecord(ev_ho_ready_, stream_));
+    std::memcpy(ho_c2w_, c2w_[0], sizeof(ho_c2w_));
+    ho_valid_ = true;
+  }
+  bool record_release(void* stream) {
+    if (cudaSetDevice(device_) != cudaSuccess) return false;
+    if (n_ho_release_ == (int)ev_ho_release_.size()) {
+      cudaEvent_t e = nullptr;
+      if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) return false;
+      ev_ho_release_.push_back(e);
+    }
+    if (cudaEventRecord(ev_ho_release_[n_ho_release_], (cudaStream_t)stream) != cudaSuccess) return false;
+    ++n_ho_release_;
+    return true;
+  }
+
   // true when every non-null pointer is page-locked host memory the device can DMA from / into directly
   static bool all_page_locked(const void* const* ptrs, int n) {
     for (int i = 0; i < n; ++i) {
@@ -1569,6 +1633,15 @@ class MvsnetEngine final : public MvsnetIface {
   bool eager_d2h_ = true;   // worker copies the four maps into pinned staging right behind the forward (pageable callers);
                             // 0: GetResult copies back itself - for callers that pass page-locked result buffers
   float c2w_[kMaxSrc + 1][16];
+  // keyframe handoff (fill_handoff / read_handoff): the last fetched result, kept until the next GetResult
+  float* d_ho_depth_ = nullptr;
+  unsigned char* d_ho_bgr_ = nullptr;
+  float ho_c2w_[16];
+  int ho_H_ = 0, ho_W_ = 0;
+  bool ho_valid_ = false;
+  cudaEvent_t ev_ho_ready_ = nullptr;
+  std::vector<cudaEvent_t> ev_ho_release_;   // pool; the first n_ho_release_ were recorded by consumers since the last fill
+  int n_ho_release_ = 0;
   float K_[27];
   float dmin_ = 0, dmax_ = 0, discard_ = 0;
   float* d_bs3_ = nullptr;

@@ -1,11 +1,21 @@
 // Type-erased interface of the CVA-MVSNet engine (implemented in mvsnet.cu for fp32 and bf16 storage).
 #pragma once
+#include <functional>
 #include <string>
 
 namespace tdm {
 
 class MvsnetIface {
  public:
+  // The result the last GetResult returned, kept on the engine's device until the next GetResult (the keyframe handoff to the
+  // TSDF, tdm_fusion_integrate_mvsnet): filtered stage-3 depth, the reference view's BGR and its cam_to_world.
+  struct Handoff {
+    const float* depth;          // H*W
+    const unsigned char* bgr;    // H*W*3, view 0 after the ref-first reorder
+    float c2w[16];
+    int H, W, device;
+    void* ready;                 // cudaEvent_t recorded behind the copy that filled the buffers
+  };
   virtual ~MvsnetIface() = default;
   virtual void set_option(const std::string& key, int value) = 0;
   // K3x3x3: three row-major 3x3 intrinsics, stage1..stage3.
@@ -14,6 +24,10 @@ class MvsnetIface {
   virtual bool ready() = 0;
   virtual void wait() = 0;
   virtual void get_result(float* depth, float* conf, float* depth_dense, float* conf_dense) = 0;
+  // Calls consume(handoff) under the engine's lock.  consume enqueues every read of the handoff on `stream` (a cudaStream_t
+  // of the handoff's device) behind handoff.ready; the engine then records a release event on `stream` that the next
+  // GetResult's fill and the destructor wait for.  Throws when no result has been fetched yet.
+  virtual void read_handoff(void* stream, const std::function<void(const Handoff&)>& consume) = 0;
   virtual void stage_output(int stage, const std::string& which, float* out, size_t cap) = 0;
   virtual long long debug_tensor(const std::string& name, float* out, size_t cap, int* dims4) = 0;
   virtual void run_resident(int iters, float* ms_total, int* launches) = 0;

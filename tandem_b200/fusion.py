@@ -64,6 +64,20 @@ class DrFusion:
         fp = ctypes.POINTER(ctypes.c_float)
         check(lib().tdm_fusion_integrate_async(self._h, bgr.ctypes.data, depth.ctypes.data_as(fp), pose.ctypes.data_as(fp)))
 
+    def IntegrateScanFromMvsnet(self, mvsnet, pose=None):
+        """IntegrateScanAsync of the result mvsnet.GetResult() last returned, read where it sits on the device: its filtered
+        depth, the window's reference BGR image and, with pose=None, the window's reference cam->world pose (what
+        tandem_backend.cpp:166 passes).  Non-blocking; legal until the next GetResult replaces the result, also after the
+        next CallAsync (include/tandem_b200.h: tdm_fusion_integrate_mvsnet)."""
+        fp = ctypes.POINTER(ctypes.c_float)
+        if pose is None:
+            check(lib().tdm_fusion_integrate_mvsnet(self._h, mvsnet._h, None))
+            return
+        pose = np.ascontiguousarray(pose, np.float32)
+        if pose.size != 16:
+            raise TandemError("IntegrateScanFromMvsnet: pose must be 4x4")
+        check(lib().tdm_fusion_integrate_mvsnet(self._h, mvsnet._h, pose.ctypes.data_as(fp)))
+
     def RenderAsync(self, camera_poses):
         poses = [np.ascontiguousarray(p, np.float32) for p in camera_poses]
         fp = ctypes.POINTER(ctypes.c_float)

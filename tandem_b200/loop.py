@@ -84,8 +84,8 @@ class TandemLoop:
             td = prev["true_depth"]
             m = (td > 0) & (out_prev.depth_dense > 0)
             self.stats["mvs_absrel"].append(float(np.mean(np.abs(out_prev.depth_dense[m] - td[m]) / td[m])))
-        if out_prev is not None and self.integrate == "mvsnet":        # (3) integrate the previous result
-            self.fusion.IntegrateScanAsync(prev["bgr"], out_prev.depth, prev["c2w"])
+        if out_prev is not None and self.integrate == "mvsnet":        # (3) integrate the previous result, read on the device
+            self.fusion.IntegrateScanFromMvsnet(self.mvsnet)            # (= its depth, prev["bgr"] and prev["c2w"])
         else:
             self.fusion.IntegrateScanAsync(bgr, sensor_depth, c2w)
         self.fusion.RenderAsync([np.asarray(c2w, np.float32)])          # (4) at the new keyframe's pose
