@@ -256,7 +256,8 @@ int tdm_tracker_set_new(tdm_tracker* t, const float* dInew /* h*w*3: (I,dx,dy) i
 /* calcRes: refToNew 4x4 row-major double; res6 = [E, numTermsInE, flowT, 0, flowRT, saturatedRatio]. */
 int tdm_tracker_calc_res(tdm_tracker* t, const double* refToNew, float new_exposure,
                          const double aff_g2l[2], float cutoffTH, double res6[6]);
-/* calcG: H 8x8 row-major, b 8; uses the warped buffers of the last calc_res. */
+/* calcG: H 8x8 row-major, b 8; uses the warped buffers of the last calc_res (tdm_tracker_calc_res_g, _calc_res_batch and
+ * _track write none and leave what calcG refers to unchanged; before any calc_res it fails). */
 int tdm_tracker_calc_g(tdm_tracker* t, float new_exposure, const double aff_g2l[2], double H[64], double b[8]);
 /* Fused single-launch calcRes+calcG (no warped buffers), same outputs. */
 int tdm_tracker_calc_res_g(tdm_tracker* t, const double* refToNew, float new_exposure,
@@ -269,6 +270,10 @@ int tdm_tracker_calc_res_batch(tdm_tracker* t, int n_hyp, const double* refToNew
                                float cutoffTH, double* res6);
 int tdm_tracker_synchronize(tdm_tracker* t);
 int tdm_tracker_run_resident(tdm_tracker* t, int iters, float* ms_total);
+/* Test accessor (not for hot paths): copies the first n (<= n_max) entries of the seven per-point arrays the last calc_res
+ * wrote - u, v, dx, dy, idepth, residual, huber weight; zero at every point not accepted - to out (7 x n, array-major).
+ * Synchronises the tracker's stream. */
+int tdm_tracker_get_warped(tdm_tracker* t, int n, float* out);
 
 /* ------------------------------------------------------------------------------------------------
  * SURVEY.md 8(f) "next" rows: the host stages either side of the evaluation, moved onto the device.  These entry

@@ -150,6 +150,7 @@ def _declare(l):
         "tdm_tracker_calc_res_batch": (i, [vp, i, dp, f, dp, f, dp]),
         "tdm_tracker_synchronize": (i, [vp]),
         "tdm_tracker_run_resident": (i, [vp, i, fp]),
+        "tdm_tracker_get_warped": (i, [vp, i, fp]),
         "tdm_pyramid_create": (i, [i, i, i, i, P(vp)]),
         "tdm_pyramid_destroy": (None, [vp]),
         "tdm_pyramid_build": (i, [vp, fp]),

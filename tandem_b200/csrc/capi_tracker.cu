@@ -180,6 +180,13 @@ int tdm_tracker_get_reference(tdm_tracker* t, int n, float* pc_u, float* pc_v, f
   return TDM_OK;
   TDM_API_END
 }
+int tdm_tracker_get_warped(tdm_tracker* t, int n, float* out) {
+  TDM_API_BEGIN
+  TDM_CHECK(t && out, "null argument");
+  t->impl->get_warped(n, out);
+  return TDM_OK;
+  TDM_API_END
+}
 
 /* ---- SURVEY 8(f) n3: one pyramid level's LM loop on the device ---- */
 int tdm_tracker_track(tdm_tracker* t, const double refToNew[16], const double aff_g2l[2], float new_exposure,

@@ -828,13 +828,24 @@ class TrackerImpl final : public TrackerIface {
     TDM_CUDA(cudaStreamSynchronize(stream_));
     finish_g(H, b);
   }
+  // The fused path writes no warped buffers, so what a later calc_g refers to - the parameters and count of the last
+  // calc_res - is put back afterwards (as calc_res_batch does); on error too.
   void calc_res_g(const double* refToNew, float new_exposure, const double aff[2], float cutoffTH, double res6[6],
                   double H[64], double b[8]) override {
-    prepare(refToNew, new_exposure, aff, cutoffTH);
-    launch(2);
-    TDM_CUDA(cudaStreamSynchronize(stream_));
-    finish_res(res6);
-    finish_g(H, b);
+    const TrkParams saved = p_;
+    const bool saved_have = have_params_;
+    const int saved_warped = num_warped_;
+    try {
+      prepare(refToNew, new_exposure, aff, cutoffTH);
+      launch(2);
+      TDM_CUDA(cudaStreamSynchronize(stream_));
+      finish_res(res6);
+      finish_g(H, b);
+    } catch (...) {
+      p_ = saved; have_params_ = saved_have; num_warped_ = saved_warped;
+      throw;
+    }
+    p_ = saved; have_params_ = saved_have; num_warped_ = saved_warped;
   }
 
   // ---------------------------------------------------------------------------------------------- n1
@@ -847,18 +858,8 @@ class TrackerImpl final : public TrackerIface {
     TDM_CUDA(cudaStreamSynchronize(stream_));
     const size_t npx = (size_t)w_ * h_, nm = (size_t)n_max_;
     ensure_front_buffers();
-    // sparse points [0, n_sparse] (the last one is the reference's stale slot, CoarseTracker.cpp:717-722)
     const int ns1 = a.n_sparse + 1;
     if ((long long)ns1 > n_max_) throw Error("setReferenceDense: more sparse points than n_max");
-    const float* src[4] = {a.pc_u, a.pc_v, a.pc_idepth, a.pc_color};
-    for (int k = 0; k < 4; ++k) {
-      if (src[k]) {
-        std::memcpy(h_pc_ + k * nm, src[k], 4 * (size_t)ns1);
-        TDM_CUDA(cudaMemcpyAsync(d_pc_ + k * nm, h_pc_ + k * nm, 4 * (size_t)ns1, cudaMemcpyHostToDevice, stream_));
-      } else {
-        TDM_CUDA(cudaMemsetAsync(d_pc_ + k * nm, 0, 4, stream_));
-      }
-    }
     const float* d_depth = a.depth;
     if (!a.depth_on_device) {
       std::memcpy(h_front_, a.depth, 4 * npx);
@@ -920,6 +921,17 @@ class TrackerImpl final : public TrackerIface {
     TDM_CUDA(cudaStreamSynchronize(stream_));
     const int total = *h_total_;
     if ((long long)a.n_sparse + 1 + total > n_max_) throw Error("setReferenceDense: n_max too small for the dense points");
+    // Only now is the current reference overwritten, so that a call refused above leaves it as it was.
+    // Sparse points [0, n_sparse] (the last one is the reference's stale slot, CoarseTracker.cpp:717-722).
+    const float* src[4] = {a.pc_u, a.pc_v, a.pc_idepth, a.pc_color};
+    for (int k = 0; k < 4; ++k) {
+      if (src[k]) {
+        std::memcpy(h_pc_ + k * nm, src[k], 4 * (size_t)ns1);
+        TDM_CUDA(cudaMemcpyAsync(d_pc_ + k * nm, h_pc_ + k * nm, 4 * (size_t)ns1, cudaMemcpyHostToDevice, stream_));
+      } else {
+        TDM_CUDA(cudaMemsetAsync(d_pc_ + k * nm, 0, 4, stream_));
+      }
+    }
     k_dense_emit<<<h_, 256, 0, stream_>>>(d_proj_, d_id0, a.dense_only, w_, h_, d_rowoff_, d_gray, gstride, a.n_sparse + 1,
                                           d_pc_, d_pc_ + nm, d_pc_ + 2 * nm, d_pc_ + 3 * nm);
     TDM_CUDA(cudaGetLastError());
@@ -940,6 +952,13 @@ class TrackerImpl final : public TrackerIface {
     float* dst[4] = {u, v, idepth, color};
     for (int k = 0; k < 4; ++k)
       if (dst[k]) TDM_CUDA(cudaMemcpyAsync(dst[k], d_pc_ + k * nm, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_));
+  }
+  void get_warped(int n, float* out) override {
+    TDM_CHECK(n >= 0 && n <= n_max_, "get_warped: bad n");
+    TDM_CUDA(cudaSetDevice(device_));
+    for (int k = 0; k < 7; ++k)
+      TDM_CUDA(cudaMemcpyAsync(out + (size_t)k * n, d_warped_ + (size_t)k * n_max_, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream_));
     TDM_CUDA(cudaStreamSynchronize(stream_));
   }
   // ---------------------------------------------------------------------------------------------- n2
@@ -967,7 +986,7 @@ class TrackerImpl final : public TrackerIface {
     r->aff[0] = o->aff[0]; r->aff[1] = o->aff[1];
     for (int i = 0; i < 6; ++i) r->res[i] = o->res[0][i];
     r->iterations = o->iterations[0]; r->evaluations = o->evaluations[0]; r->cutoff_repeat = o->repeat[0];
-    num_warped_ = o->num_warped;
+    // num_warped_ stays that of the last calc_res: the loop writes no warped buffers, calc_g still refers to them
   }
   // ---------------------------------------------------------------------------------------------- n5
   void track_pyramid(TrackerIface* const* levels, int coarsest, const PyramidArgs& a, PyramidResult* r) override {

@@ -18,6 +18,8 @@ class TrackerIface {
                           double H[64], double b[8]) = 0;
   virtual void synchronize() = 0;
   virtual void run_resident(int iters, float* ms) = 0;
+  // test accessor: the first n entries of the 7 warped arrays of the last calc_res (u, v, dx, dy, idepth, residual, weight)
+  virtual void get_warped(int n, float* out /* 7 x n */) = 0;
   // ---- SURVEY 8(f) n1-n3: the stages either side of the evaluation, kept on the device ----
   struct DenseRefArgs {
     const float* depth = nullptr;       // h*w, host or device

@@ -170,6 +170,13 @@ class CudaCoarseTracker:
                     res=np.array(r.res, np.float64), iterations=r.iterations, evaluations=r.evaluations,
                     cutoff_repeat=r.cutoff_repeat, device_ms=r.device_ms)
 
+    def getWarped(self, n):
+        """Test accessor: (7, n) float32 - u, v, dx, dy, idepth, residual, weight of the first n points as the last calcRes
+        wrote them (zeros at points it did not accept)."""
+        out = np.empty((7, n), np.float32)
+        check(lib().tdm_tracker_get_warped(self._h, n, out.ctypes.data_as(_fp)))
+        return out
+
     def synchronize(self):
         check(lib().tdm_tracker_synchronize(self._h))
 
