@@ -7,6 +7,7 @@
 #include <cstdlib>
 #include <memory>
 #include <utility>
+#include <vector>
 
 class DrMvsnetImpl;  // opaque: owns a tdm_mvsnet handle (shims/dr_mvsnet.cpp)
 struct tdm_mvsnet;   // include/tandem_b200.h
@@ -46,6 +47,13 @@ public:
   void CallAsync(int height, int width, int view_num, int ref_index, unsigned char **bgrs, float const *intrinsic_matrix,
                  float **cam_to_worlds, float depth_min, float depth_max, float discard_percentage,
                  bool debug_print = false);
+
+  // Extension: the same call with the feature cache (tdm_mvsnet_call_async_ids).  view_ids[i] names view i (TANDEM:
+  // frameHessians[i]->shell->id); FeatureNet runs only for the ids the previous such call did not hold.  bgrs[i] may be
+  // NULL for a held id and is ignored for one.
+  void CallAsync(int height, int width, int view_num, int ref_index, std::vector<long long> const &view_ids,
+                 unsigned char **bgrs, float const *intrinsic_matrix, float **cam_to_worlds, float depth_min,
+                 float depth_max, float discard_percentage, bool debug_print = false);
 
   // Blocking. Ownership of the result passes to the caller (delete it).
   DrMvsnetOutput *GetResult();

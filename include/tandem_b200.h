@@ -66,6 +66,23 @@ int tdm_mvsnet_call_async_k(tdm_mvsnet* h, int height, int width, int view_num, 
                             unsigned char* const* bgrs, const float* intrinsics_stage123,
                             float* const* cam_to_worlds, float depth_min, float depth_max,
                             float discard_percentage);
+/* Extension: CallAsync with a feature cache.  view_ids[i] names view i (a caller-chosen keyframe id, e.g. DSO's
+ * FrameShell::id).  The handle keeps, per id of the last such call, the view's image and its FeatureNet outputs on the
+ * device, and runs FeatureNet only for the ids it does not hold; ids that left the window are evicted.  The result is
+ * the one tdm_mvsnet_call_async gives for the same images.  bgrs[i] may be NULL for an id the handle holds; a non-NULL
+ * bgrs[i] of a held id is ignored (the id wins: the cached image and features are used).  intrinsics: the 3x3
+ * full-resolution K as in tdm_mvsnet_call_async, or with stage_k != 0 the 27 floats of tdm_mvsnet_call_async_k.
+ * Errors, with nothing launched and the cache unchanged: a NULL image for an id the handle does not hold (every id, when
+ * the size or view_num differs from the last call's), the same id twice, cv_variant 5, and every tdm_mvsnet_call_async
+ * error.  tdm_mvsnet_call_async / _call_async_k, a new size or view_num and any tdm_mvsnet_set_option except eager_d2h
+ * empty the cache. */
+int tdm_mvsnet_call_async_ids(tdm_mvsnet* h, int height, int width, int view_num, int ref_index, const long long* view_ids,
+                              unsigned char* const* bgrs, const float* intrinsics, int stage_k,
+                              float* const* cam_to_worlds, float depth_min, float depth_max, float discard_percentage);
+/* The feature cache after the last call (waits for it): *n_ids receives the number of ids held (view_num after a
+ * tdm_mvsnet_call_async_ids, 0 after a plain call), view_ids (capacity >= *n_ids, or NULL with capacity 0) those ids in
+ * the last window's order, *n_computed the views FeatureNet computed for the last call.  n_ids / n_computed may be NULL. */
+int tdm_mvsnet_feature_cache(tdm_mvsnet* h, long long* view_ids, int capacity, int* n_ids, int* n_computed);
 /* DrMvsnet::GetResult (blocking). Copies the stage-3 maps (H*W floats each; any pointer may be NULL)
  * into caller memory: depth/confidence are edge-filtered, *_dense unfiltered (dr_mvsnet.cpp:296-329).
  * Calling it twice without a new CallAsync is an error, as in the reference (dr_mvsnet.cpp:100-102). */
@@ -81,6 +98,8 @@ int tdm_mvsnet_set_option(tdm_mvsnet* h, const char* key, int value);
 /* Stage outputs of the last finished call: which = "depth"|"confidence"|"depth_dense"|"confidence_dense"|"edge". */
 int tdm_mvsnet_stage_output(tdm_mvsnet* h, int stage /*1..3*/, const char* which, float* out, size_t capacity);
 /* Test hook: copy a named intermediate of the last call as planar fp32 [C][D][H][W]; dims4 receives C,D,H,W.
+ * feat1..feat3 hold every view of the window in window order (reference first); the other FeatureNet tensors ("f.*")
+ * hold only the views the last forward computed (after a cached call: its new views, in window order).
  * Returns the number of floats written, or <0. */
 long long tdm_mvsnet_debug_tensor(tdm_mvsnet* h, const char* name, float* out, size_t capacity, int* dims4);
 
@@ -88,6 +107,9 @@ long long tdm_mvsnet_debug_tensor(tdm_mvsnet* h, const char* name, float* out, s
  * handle's stream with inputs already in HBM (no H2D/D2H inside), timed with CUDA events on that stream.
  * ms_total receives the elapsed milliseconds; launches (optional) the kernel launches per forward. */
 int tdm_mvsnet_run_resident(tdm_mvsnet* h, int iters, float* ms_total, int* launches);
+/* Same, with FeatureNet recomputing only the last n_new (1..view_num) views of the last window (window order) and the
+ * others read from the feature pool: the device time of a window that adds n_new keyframes to the cache. */
+int tdm_mvsnet_run_resident_new(tdm_mvsnet* h, int n_new, int iters, float* ms_total, int* launches);
 /* Same clock over n handles of one device: iters_total forwards issued round-robin, each handle on its own stream (the
  * windows are independent, so their kernels may overlap on the GPU); ms_total spans first launch .. last completion. */
 int tdm_mvsnet_run_resident_multi(tdm_mvsnet* const* hs, int n, int iters_total, float* ms_total, int* launches);

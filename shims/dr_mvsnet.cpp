@@ -64,6 +64,23 @@ void DrMvsnet::CallAsync(int height, int width, int view_num, int ref_index, uns
     die("DrMvsnet::CallAsync");
 }
 
+void DrMvsnet::CallAsync(int height, int width, int view_num, int ref_index, std::vector<long long> const& view_ids,
+                         unsigned char** bgrs, float const* intrinsic_matrix, float** cam_to_worlds, float depth_min,
+                         float depth_max, float discard_percentage, bool debug_print) {
+  if (debug_print)
+    printf("--- DrMvsnet::CallAsync (feature cache) --- W=%d, H=%d, view_num=%d, ref_index=%d, depth_min=%f, depth_max=%f, discard=%f\n",
+           width, height, view_num, ref_index, depth_min, depth_max, discard_percentage);
+  if ((int)view_ids.size() != view_num) {
+    std::cerr << "ERROR: DrMvsnet::CallAsync: " << view_ids.size() << " view ids for " << view_num << " views" << std::endl;
+    exit(EXIT_FAILURE);
+  }
+  impl->height = height;
+  impl->width = width;
+  if (tdm_mvsnet_call_async_ids(impl->h, height, width, view_num, ref_index, view_ids.data(), bgrs, intrinsic_matrix, 0,
+                                cam_to_worlds, depth_min, depth_max, discard_percentage) != TDM_OK)
+    die("DrMvsnet::CallAsync");
+}
+
 DrMvsnetOutput* DrMvsnet::GetResult() {
   DrMvsnetOutput* out = new DrMvsnetOutput(impl->height, impl->width);
   if (tdm_mvsnet_get_result(impl->h, out->depth, out->confidence, out->depth_dense, out->confidence_dense) != TDM_OK)

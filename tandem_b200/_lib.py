@@ -102,6 +102,9 @@ def _declare(l):
         "tdm_mvsnet_destroy": (None, [vp]),
         "tdm_mvsnet_call_async": (i, [vp, i, i, i, i, P(vp), fp, P(vp), f, f, f]),
         "tdm_mvsnet_call_async_k": (i, [vp, i, i, i, i, P(vp), fp, P(vp), f, f, f]),
+        "tdm_mvsnet_call_async_ids": (i, [vp, i, i, i, i, P(c.c_longlong), P(vp), fp, i, P(vp), f, f, f]),
+        "tdm_mvsnet_feature_cache": (i, [vp, P(c.c_longlong), i, ip, ip]),
+        "tdm_mvsnet_run_resident_new": (i, [vp, i, i, fp, ip]),
         "tdm_mvsnet_get_result": (i, [vp, fp, fp, fp, fp]),
         "tdm_mvsnet_ready": (i, [vp]),
         "tdm_mvsnet_wait": (i, [vp]),

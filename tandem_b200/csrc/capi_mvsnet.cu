@@ -82,19 +82,42 @@ int tdm_mvsnet_call_async_k(tdm_mvsnet* h, int height, int width, int view_num, 
   return TDM_OK;
   TDM_API_END
 }
-int tdm_mvsnet_call_async(tdm_mvsnet* h, int height, int width, int view_num, int ref_index,
-                          unsigned char* const* bgrs, const float* K, float* const* c2ws, float dmin,
-                          float dmax, float discard) {
-  TDM_API_BEGIN
-  TDM_CHECK(h && bgrs && K && c2ws, "null argument");
-  // K_stage3 = K, K_stage2 rows 0-1 * 0.5, K_stage1 rows 0-1 * 0.25 (dr_mvsnet.cpp:220-247, incl. its TODO)
-  float Ks[27];
+// K_stage3 = K, K_stage2 rows 0-1 * 0.5, K_stage1 rows 0-1 * 0.25 (dr_mvsnet.cpp:220-247, incl. its TODO)
+static void stage_intrinsics(const float* K, float* Ks) {
   const float sc[3] = {0.25f, 0.5f, 1.0f};
   for (int s = 0; s < 3; ++s)
     for (int i = 0; i < 3; ++i)
       for (int j = 0; j < 3; ++j)
         Ks[s * 9 + i * 3 + j] = (i < 2) ? (float)((double)sc[s] * (double)K[i * 3 + j]) : K[i * 3 + j];
+}
+
+int tdm_mvsnet_call_async(tdm_mvsnet* h, int height, int width, int view_num, int ref_index,
+                          unsigned char* const* bgrs, const float* K, float* const* c2ws, float dmin,
+                          float dmax, float discard) {
+  TDM_API_BEGIN
+  TDM_CHECK(h && bgrs && K && c2ws, "null argument");
+  float Ks[27];
+  stage_intrinsics(K, Ks);
   h->impl->call_async(height, width, view_num, ref_index, bgrs, Ks, c2ws, dmin, dmax, discard);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_mvsnet_call_async_ids(tdm_mvsnet* h, int height, int width, int view_num, int ref_index, const long long* view_ids,
+                              unsigned char* const* bgrs, const float* intrinsics, int stage_k, float* const* c2ws,
+                              float dmin, float dmax, float discard) {
+  TDM_API_BEGIN
+  TDM_CHECK(h && view_ids && bgrs && intrinsics && c2ws, "null argument");
+  float Ks[27];
+  if (stage_k) std::memcpy(Ks, intrinsics, sizeof(Ks));
+  else stage_intrinsics(intrinsics, Ks);
+  h->impl->call_async_ids(height, width, view_num, ref_index, view_ids, bgrs, Ks, c2ws, dmin, dmax, discard);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_mvsnet_feature_cache(tdm_mvsnet* h, long long* view_ids, int capacity, int* n_ids, int* n_computed) {
+  TDM_API_BEGIN
+  TDM_CHECK(h && capacity >= 0 && (view_ids || capacity == 0), "bad argument");
+  h->impl->feature_cache(view_ids, capacity, n_ids, n_computed);
   return TDM_OK;
   TDM_API_END
 }
@@ -142,6 +165,13 @@ int tdm_mvsnet_run_resident(tdm_mvsnet* h, int iters, float* ms_total, int* laun
   TDM_API_BEGIN
   TDM_CHECK(h && ms_total, "null argument");
   h->impl->run_resident(iters, ms_total, launches);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_mvsnet_run_resident_new(tdm_mvsnet* h, int n_new, int iters, float* ms_total, int* launches) {
+  TDM_API_BEGIN
+  TDM_CHECK(h && ms_total, "null argument");
+  h->impl->run_resident_new(n_new, iters, ms_total, launches);
   return TDM_OK;
   TDM_API_END
 }

@@ -177,6 +177,7 @@ class MvsnetEngine final : public MvsnetIface {
     release_slot(slot_);
     if (d_bs3_) cudaFree(d_bs3_);
     if (h_params_) cudaFreeHost(h_params_);
+    if (h_feat_slot_) cudaFreeHost(h_feat_slot_);
     if (d_params_) cudaFree(d_params_);
     for (auto& e : ev_out_) if (e) cudaEventDestroy(e);
     if (ev_in_) cudaEventDestroy(ev_in_);
@@ -196,6 +197,7 @@ class MvsnetEngine final : public MvsnetIface {
     TDM_CUDA(cudaStreamSynchronize(stream_));
     if (key == "eager_d2h") { eager_d2h_ = value != 0; return; }   // not part of the captured launch sequence
     drop_graph();
+    cache_valid_ = false;   // features computed under other options are not reused
     if (key == "filter_all_stages") filter_all_ = value != 0;
     else if (key == "use_graph") use_graph_ = value != 0;
     else if (key == "use_pdl") { TDM_CHECK(value >= 0 && value <= 2, "use_pdl: 0 off, 1 tensor-core kernels, 2 every kernel of the forward"); use_pdl_ = value; }
@@ -232,66 +234,96 @@ class MvsnetEngine final : public MvsnetIface {
   // "Blocking for last input. Non-blocking for this input." (dr_mvsnet.h:42)
   void call_async(int H, int W, int V, int ref_index, unsigned char* const* bgrs, const float* K3x3x3,
                   float* const* c2ws, float dmin, float dmax, float discard) override {
-    TDM_CHECK(V >= 2 && V <= kMaxSrc + 1, "view_num out of range");
-    TDM_CHECK(ref_index >= 0 && ref_index < V, "ref_index out of range");
-    TDM_CHECK(H % 32 == 0 && W % 32 == 0, "height and width must be multiples of 32 (three stride-2 levels at 1/4 resolution)");
+    check_window(H, W, V, ref_index);
     for (int i = 0; i < V - 1; ++i)
       for (int j = i + 1; j < V; ++j)
         if (bgrs[i] == bgrs[j] || c2ws[i] == c2ws[j])
           throw Error("CallAsync: the same data passed for two views (dr_mvsnet.cpp:153-160)");
     std::unique_lock<std::mutex> lk(mu_);
-    cv_done_.wait(lk, [this] { return !busy_; });
-    if (has_result_) throw Error("CallAsync while a result is un-fetched (dr_mvsnet.cpp:315-318)");
-    if (!worker_error_.empty()) { std::string e = worker_error_; worker_error_.clear(); throw Error(e); }
+    wait_idle_for_call(lk);
     TDM_CUDA(cudaSetDevice(device_));
     ensure_plan(V, H, W);
-    // copy inputs (owned by the caller only during this call); reference view first (dr_mvsnet.cpp:190-197)
-    const size_t img = (size_t)H * W * 3;
+    // copy inputs (owned by the caller only during this call); reference view first (dr_mvsnet.cpp:190-197).  Every view is
+    // computed, view vi in slot vi of both pools; the feature cache is emptied.
+    cache_valid_ = false;
+    std::vector<int> slots(V);
+    std::vector<const unsigned char*> srcs(V);
     for (int vi = 0; vi < V; ++vi) {
-      const int view = vi == 0 ? ref_index : (vi <= ref_index ? vi - 1 : vi);
-      std::memcpy(c2w_[vi], c2ws[view], 16 * sizeof(float));
+      view_slot_[vi] = vi;
+      slots[vi] = vi;
+      srcs[vi] = bgrs[window_view(vi, ref_index)];
     }
-    if (all_page_locked((const void* const*)bgrs, V)) {
-      // Page-locked caller images (cudaHostAlloc / cudaHostRegister): DMA straight from them - no staging copy, no copy
-      // threads.  The caller owns them only during this call, so the call returns once the seven DMAs have landed
-      // (6.45 MB over PCIe gen5: ~0.13 ms, less than the staging memcpy it replaces).
-      for (int vi = 0; vi < V; ++vi) {
-        const int view = vi == 0 ? ref_index : (vi <= ref_index ? vi - 1 : vi);
-        TDM_CUDA(cudaMemcpyAsync(d_bgr_ + (size_t)vi * img, bgrs[view], img, cudaMemcpyHostToDevice, stream_));
+    upload_images(V, slots.data(), srcs.data());
+    submit(V, ref_index, c2ws, K3x3x3, dmin, dmax, discard, lk);
+  }
+
+  // Feature cache.  Pools: plane s of d_bgr_ (u8 image) and of feat1..feat3 (FeatureNet outputs) is slot s, V slots; after
+  // a cached call they hold exactly that window's ids.  Ids that left the window are evicted and their slots take the new
+  // views, lowest free slot first in window order (reference first).  FeatureNet then runs on the k new views only and its
+  // outputs are scattered into their slots; the cost volumes read view v from slot view_slot_[v] (CvParams::plane).
+  void call_async_ids(int H, int W, int V, int ref_index, const long long* ids, unsigned char* const* bgrs, const float* K3x3x3,
+                      float* const* c2ws, float dmin, float dmax, float discard) override {
+    check_window(H, W, V, ref_index);
+    for (int i = 0; i < V - 1; ++i)
+      for (int j = i + 1; j < V; ++j) {
+        if (ids[i] == ids[j]) throw Error("CallAsyncIds: view id " + std::to_string(ids[i]) + " passed for two views");
+        if (c2ws[i] == c2ws[j]) throw Error("CallAsync: the same data passed for two views (dr_mvsnet.cpp:153-160)");
       }
-      TDM_CUDA(cudaEventRecord(ev_in_, stream_));
-      TDM_CUDA(cudaEventSynchronize(ev_in_));
-    } else {
-      // Pageable caller memory: staged through pinned memory.  The staging copy of view v+1 overlaps the DMA of view v (the
-      // worker is idle here, so this thread may enqueue on the engine's stream); each view is split into slices copied by the
-      // process-wide pool; a slice's H2D is enqueued by whichever thread finished copying it (CUDA stream calls are
-      // thread-safe; the order of the DMAs inside the stream does not matter, the forward is enqueued behind all of them).
-      std::vector<CopyPool::Job> jobs;
-      constexpr int kSlices = 2;
-      std::mutex err_mu;
-      cudaError_t first_err = cudaSuccess;
-      for (int vi = 0; vi < V; ++vi) {
-        const int view = vi == 0 ? ref_index : (vi <= ref_index ? vi - 1 : vi);
-        for (int sl = 0; sl < kSlices; ++sl) {
-          const size_t b0 = img * sl / kSlices, b1 = img * (sl + 1) / kSlices;
-          unsigned char* hp = h_bgr_ + (size_t)vi * img + b0;
-          unsigned char* dp = d_bgr_ + (size_t)vi * img + b0;
-          jobs.push_back({hp, bgrs[view] + b0, b1 - b0, [this, hp, dp, b0, b1, &err_mu, &first_err] {
-                            cudaSetDevice(device_);   // pool threads start on device 0
-                            const cudaError_t e = cudaMemcpyAsync(dp, hp, b1 - b0, cudaMemcpyHostToDevice, stream_);
-                            if (e != cudaSuccess) { std::lock_guard<std::mutex> lk(err_mu); first_err = e; }
-                          }});
-        }
-      }
-      CopyPool::shared().run(jobs);
-      TDM_CUDA(first_err);
+    std::unique_lock<std::mutex> lk(mu_);
+    wait_idle_for_call(lk);
+    TDM_CHECK(cv_variant_ != 5, "CallAsyncIds: cv_variant 5 reads the views in window order and cannot use the feature cache");
+    // everything below the checks changes state: decide first which views are held (a re-plan empties the pools)
+    const bool same_plan = V == V_ && H == H_ && W == W_;
+    int held_slot[kMaxSrc + 1];
+    for (int vi = 0; vi < V; ++vi) {
+      const int view = window_view(vi, ref_index);
+      held_slot[vi] = -1;
+      if (cache_valid_ && same_plan)
+        for (int s = 0; s < V_; ++s)
+          if (slot_id_[s] == ids[view]) held_slot[vi] = s;
+      if (held_slot[vi] < 0 && !bgrs[view])
+        throw Error("CallAsyncIds: no image for view id " + std::to_string(ids[view]) + ", which the handle does not hold");
     }
-    std::memcpy(K_, K3x3x3, 27 * sizeof(float));
-    dmin_ = dmin; dmax_ = dmax; discard_ = discard;
-    busy_ = true;
-    have_inputs_ = true;
-    lk.unlock();
-    cv_work_.notify_all();
+    TDM_CUDA(cudaSetDevice(device_));
+    ensure_plan(V, H, W);
+    bool used[kMaxSrc + 1] = {};
+    for (int vi = 0; vi < V; ++vi)
+      if (held_slot[vi] >= 0) used[held_slot[vi]] = true;
+    std::vector<int> slots;
+    std::vector<const unsigned char*> srcs;
+    int next_free = 0;
+    for (int vi = 0; vi < V; ++vi) {
+      if (held_slot[vi] < 0) {
+        while (used[next_free]) ++next_free;
+        held_slot[vi] = next_free;
+        used[next_free] = true;
+        slots.push_back(next_free);
+        srcs.push_back(bgrs[window_view(vi, ref_index)]);
+      }
+    }
+    const int k = (int)slots.size();
+    if (k > 0 && k < V) ensure_feature_scratch(k);
+    // the new images go into slots that no queued work reads any more: the last forward has finished (the worker is idle)
+    // and GetResult's handoff copy of the previous reference image is enqueued on stream_ ahead of these uploads
+    upload_images(k, slots.data(), srcs.data());
+    for (int vi = 0; vi < V; ++vi) {
+      view_slot_[vi] = held_slot[vi];
+      slot_id_[held_slot[vi]] = ids[window_view(vi, ref_index)];
+    }
+    cache_valid_ = true;
+    submit(k, ref_index, c2ws, K3x3x3, dmin, dmax, discard, lk, slots.data());
+  }
+
+  void feature_cache(long long* ids, int cap, int* n_ids, int* n_computed) override {
+    std::unique_lock<std::mutex> lk(mu_);
+    cv_done_.wait(lk, [this] { return !busy_; });
+    const int n = cache_valid_ ? V_ : 0;
+    if (n_ids) *n_ids = n;
+    if (n_computed) *n_computed = n_computed_;
+    if (ids) {
+      TDM_CHECK(cap >= n, "feature_cache: capacity too small");
+      for (int view = 0; view < n; ++view) ids[view] = slot_id_[view_slot_[window_index(view, last_ref_index_)]];
+    }
   }
 
   bool ready() override {
@@ -374,10 +406,12 @@ class MvsnetEngine final : public MvsnetIface {
     TDM_CUDA(cudaMemcpy(out, it->second.p, n * 4, cudaMemcpyDeviceToHost));
   }
 
+  // FeatureNet intermediates ("f.*") are those of the last forward, over the views it computed (k planes after a cached call);
+  // feat1..feat3 are returned in window order (reference first) whichever pool slots hold the views.
   long long debug_tensor(const std::string& name, float* out, size_t cap, int* dims4) override {
     wait();
     TDM_CUDA(cudaSetDevice(device_));
-    auto it = bufs_.find(name);
+    auto it = bufs_.find(fk_ < V_ && name.compare(0, 2, "f.") == 0 ? name + "@" + std::to_string(fk_) : name);
     if (it == bufs_.end()) throw Error("no such tensor: " + name);
     const DevBuf& b = it->second;
     const long long npos = (long long)b.D * b.H * b.W;
@@ -399,18 +433,31 @@ class MvsnetEngine final : public MvsnetIface {
     cudaFree(tmp);
     if (b.kind == 2 && kVolScale != 1.f)
       for (long long i = 0; i < n; ++i) out[i] *= 1.f / kVolScale;   // report the volume in its own units
+    if ((name == "feat1" || name == "feat2" || name == "feat3") && !slots_identity()) {
+      const std::vector<float> t(out, out + n);
+      const long long plane = (long long)b.H * b.W;
+      for (int c = 0; c < b.C; ++c)
+        for (int v = 0; v < b.D; ++v)
+          std::memcpy(out + ((long long)c * b.D + v) * plane, t.data() + ((long long)c * b.D + view_slot_[v]) * plane, plane * 4);
+    }
     return n;
   }
 
-  void run_resident(int iters, float* ms_total, int* launches) override {
+  void run_resident(int iters, float* ms_total, int* launches) override { run_resident_new(V_, iters, ms_total, launches); }
+
+  void run_resident_new(int n_new, int iters, float* ms_total, int* launches) override {
     wait();
     TDM_CHECK(have_inputs_, "run_resident: no window submitted yet");
+    TDM_CHECK(n_new >= 1 && n_new <= V_, "run_resident: n_new must be 1..view_num");
     TDM_CUDA(cudaSetDevice(device_));
+    int slots[kMaxSrc + 1];
+    for (int j = 0; j < n_new; ++j) slots[j] = view_slot_[window_index(V_ - n_new + j, last_ref_index_)];
+    if (n_new < V_) ensure_feature_scratch(n_new);
     cudaEvent_t e0, e1;
     TDM_CUDA(cudaEventCreate(&e0));
     TDM_CUDA(cudaEventCreate(&e1));
     TDM_CUDA(cudaEventRecord(e0, stream_));
-    for (int i = 0; i < iters; ++i) forward(false);
+    for (int i = 0; i < iters; ++i) forward(n_new, slots, false);
     TDM_CUDA(cudaEventRecord(e1, stream_));
     TDM_CUDA(cudaEventSynchronize(e1));
     TDM_CUDA(cudaEventElapsedTime(ms_total, e0, e1));
@@ -425,7 +472,7 @@ class MvsnetEngine final : public MvsnetIface {
     wait();
     TDM_CHECK(have_inputs_, "run_resident: no window submitted yet");
     TDM_CUDA(cudaSetDevice(device_));
-    for (int i = 0; i < iters; ++i) forward(false);
+    for (int i = 0; i < iters; ++i) forward(V_, nullptr, false);
     return launches_per_forward_;
   }
 
@@ -433,9 +480,9 @@ class MvsnetEngine final : public MvsnetIface {
     wait();
     TDM_CHECK(have_inputs_, "profile: no window submitted yet");
     TDM_CUDA(cudaSetDevice(device_));
-    forward(false);  // warm
+    forward(V_, nullptr, false);  // warm
     recs_.clear();
-    forward(true);
+    forward(V_, nullptr, true);
     TDM_CUDA(cudaStreamSynchronize(stream_));
     std::ostringstream os;
     for (auto& r : recs_) {
@@ -644,6 +691,8 @@ class MvsnetEngine final : public MvsnetIface {
     TDM_CUDA(cudaMemset(select2_, 0, sizeof(SelectState2)));
     TDM_CUDA(cudaMallocHost(&h_params_, sizeof(CallParams)));
     TDM_CUDA(cudaMalloc(&d_params_, sizeof(CallParams)));
+    TDM_CUDA(cudaMallocHost(&h_feat_slot_, sizeof(c_feat_slot[0])));
+    for (int v = 0; v <= kMaxSrc; ++v) view_slot_[v] = v;
   }
 
   // ---------------------------------------------------------------- buffers
@@ -702,6 +751,32 @@ class MvsnetEngine final : public MvsnetIface {
     if (h_out_) cudaFreeHost(h_out_);
     if (d_bgr_) cudaFree(d_bgr_);
     h_bgr_ = nullptr; h_out_ = nullptr; d_bgr_ = nullptr;
+    cache_valid_ = false;
+    for (int v = 0; v <= kMaxSrc; ++v) view_slot_[v] = v;
+  }
+  // FeatureNet's buffers over D views; sfx "" = the whole window (feat1..feat3 are then the feature pool), "@k" = the scratch
+  // of a cached forward over k new views
+  void alloc_featurenet(int D, const std::string& sfx) {
+    const int H = H_, W = W_;
+    alloc("f.img" + sfx, 8, D, H, W);
+    alloc("f.c0_0" + sfx, 8, D, H, W);
+    alloc("f.c3" + sfx, 8, D, H, W);
+    alloc("f.c1_0" + sfx, 16, D, H / 2, W / 2);
+    alloc("f.c1_1" + sfx, 16, D, H / 2, W / 2);
+    alloc("f.c2" + sfx, 16, D, H / 2, W / 2);
+    alloc("f.c2_0" + sfx, 32, D, H / 4, W / 4);
+    alloc("f.c2_1" + sfx, 32, D, H / 4, W / 4);
+    alloc("f.c1" + sfx, 32, D, H / 4, W / 4);
+    alloc("feat1" + sfx, 32, D, H / 4, W / 4);
+    alloc("f.i2" + sfx, 32, D, H / 2, W / 2);
+    alloc("f.i2b" + sfx, 32, D, H / 2, W / 2);
+    alloc("feat2" + sfx, 16, D, H / 2, W / 2);
+    alloc("f.i3" + sfx, 32, D, H, W);
+    alloc("feat3" + sfx, 8, D, H, W);
+  }
+  // made once per k and plan (freed with the plan), outside any capture: the forward over k views then replays as its own graph
+  void ensure_feature_scratch(int k) {
+    if (!bufs_.count("feat1@" + std::to_string(k))) alloc_featurenet(k, "@" + std::to_string(k));
   }
   void ensure_plan(int V, int H, int W) {
     if (V == V_ && H == H_ && W == W_) return;
@@ -710,21 +785,7 @@ class MvsnetEngine final : public MvsnetIface {
     TDM_CUDA(cudaMallocHost(&h_bgr_, (size_t)V * H * W * 3));
     TDM_CUDA(cudaMallocHost(&h_out_, (size_t)4 * H * W * sizeof(float)));
     TDM_CUDA(cudaMalloc(&d_bgr_, (size_t)V * H * W * 3));
-    alloc("f.img", 8, V, H, W);
-    alloc("f.c0_0", 8, V, H, W);
-    alloc("f.c3", 8, V, H, W);
-    alloc("f.c1_0", 16, V, H / 2, W / 2);
-    alloc("f.c1_1", 16, V, H / 2, W / 2);
-    alloc("f.c2", 16, V, H / 2, W / 2);
-    alloc("f.c2_0", 32, V, H / 4, W / 4);
-    alloc("f.c2_1", 32, V, H / 4, W / 4);
-    alloc("f.c1", 32, V, H / 4, W / 4);
-    alloc("feat1", 32, V, H / 4, W / 4);
-    alloc("f.i2", 32, V, H / 2, W / 2);
-    alloc("f.i2b", 32, V, H / 2, W / 2);
-    alloc("feat2", 16, V, H / 2, W / 2);
-    alloc("f.i3", 32, V, H, W);
-    alloc("feat3", 8, V, H, W);
+    alloc_featurenet(V, "");
     for (int s = 1; s <= 3; ++s) {
       const std::string k = "s" + std::to_string(s) + ".";
       const int sc = 1 << (3 - s);
@@ -854,7 +915,8 @@ class MvsnetEngine final : public MvsnetIface {
   }
 
   // Tile plan and input tensor map of one layer's tensor-core launch, made on first use.  Keys: the layer, + "#tail" (prob
-  // with the soft-argmin tail), "#is" / "#is#tail" (input-stationary kernel), "#s2" (stride-2 kernel).
+  // with the soft-argmin tail), "#is" / "#is#tail" (input-stationary kernel), "#s2" (stride-2 kernel); the output-stationary
+  // and stride-2 keys end in "@" + the input's D.
   struct TcCache { tc::Plan plan; tc::PlanS2 plan_s2; CUtensorMap tmap, tmap_res, tmap_out; };
   std::map<std::string, TcCache> tc_cache_;
 
@@ -934,7 +996,8 @@ class MvsnetEngine final : public MvsnetIface {
   template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool PLAIN, int MODE = 0, bool HILO = false, typename Tail = tc::NoTail>
   void tc_inst(const std::string& wkey, const DevBuf& in, const DevConv& c, const DevBuf* res, const DevBuf& out, bool relu,
                const Tail& tail = Tail()) {
-    const TcCache& tcx = tc_cached(wkey + (Tail::enabled ? "#tail" : ""), [&] {
+    // FeatureNet layers run over V planes or, with the feature cache, over k: one plan and tensor map per plane count
+    const TcCache& tcx = tc_cached(wkey + (Tail::enabled ? "#tail" : "") + "@" + std::to_string(in.D), [&] {
       TcCache x{};
       x.plan = tc::make_plan(CIN, HILO ? 2 * NPAD : NPAD, KD, in.D, in.H, in.W, in.pd, MODE, (size_t)tc_smem_kb_ * 1024,   // tiles live on the INPUT grid
                              Tail::enabled);
@@ -984,7 +1047,7 @@ class MvsnetEngine final : public MvsnetIface {
 
   template <int CIN, int NPAD, int KD, int KS>
   void tc_s2_inst(const std::string& wkey, const DevBuf& in, const DevConv& c, const DevBuf& out, bool relu) {
-    const TcCache& tcx = tc_cached(wkey + "#s2", [&] {
+    const TcCache& tcx = tc_cached(wkey + "#s2@" + std::to_string(in.D), [&] {
       TcCache x{};
       x.plan_s2 = tc::make_plan_s2(CIN, NPAD, KD, KS, out.D, out.H, out.W, (size_t)tc_smem_kb_ * 1024);
       tc::GeomS2& g = x.plan_s2.g;
@@ -1186,6 +1249,7 @@ class MvsnetEngine final : public MvsnetIface {
     const DevBuf& vb = bufs_.at(k + "volume");
     std::memset(&p, 0, sizeof(p));
     p.nsrc = V_ - 1; p.D = vb.D; p.H = vb.H; p.W = vb.W;
+    for (int v = 0; v < V_; ++v) p.plane[v] = view_slot_[v];
     const float* K = K_ + 9 * (s - 1);
     double Pr[16], Pri[16];
     world_to_pixel(K, c2w_[0], Pr);
@@ -1233,6 +1297,8 @@ class MvsnetEngine final : public MvsnetIface {
     TDM_CUDA(cudaMemcpyAsync(d_params_, h_params_, sizeof(CallParams), cudaMemcpyHostToDevice, stream_));
     TDM_CUDA(cudaMemcpyToSymbolAsync(c_call_params, h_params_, sizeof(CallParams), (size_t)slot_ * sizeof(CallParams),
                                      cudaMemcpyHostToDevice, stream_));
+    TDM_CUDA(cudaMemcpyToSymbolAsync(c_feat_slot, h_feat_slot_, sizeof(c_feat_slot[0]), (size_t)slot_ * sizeof(c_feat_slot[0]),
+                                     cudaMemcpyHostToDevice, stream_));
   }
 
   void cost_volume(int s) {
@@ -1248,6 +1314,7 @@ class MvsnetEngine final : public MvsnetIface {
     if constexpr (std::is_same<TA, __half>::value) {
       if (va_ && cv_variant_ == 5 && fb.C == 8 && vb.D == 8) {
         // A/B: source-view tiles staged in shared memory by TMA (cost_volume_tma.cuh); other stages run variant 3
+        TDM_CHECK(slots_identity(), "cv_variant 5 reads the views in window order, not through the feature pool's slots");
         if (!cv_tmap_ok_) {
           const cuuint64_t dims[4] = {8, (cuuint64_t)(fb.W + 2), (cuuint64_t)(fb.H + 2), (cuuint64_t)(fb.D + 2 * fb.pd)};
           const cuuint64_t strides[3] = {16, (cuuint64_t)(fb.W + 2) * 16, (cuuint64_t)(fb.W + 2) * (fb.H + 2) * 16};
@@ -1353,12 +1420,16 @@ class MvsnetEngine final : public MvsnetIface {
 
   // Per-call parameters are refreshed in device memory, then the (otherwise argument-invariant) kernel sequence is
   // replayed as a CUDA graph: captured on the second forward of a plan (the first one warms the tensor-map / attribute
-  // caches), invalidated by free_plan() and by option changes.
-  void forward(bool profiling) {
+  // caches), invalidated by free_plan() and by option changes.  k = the views FeatureNet computes: V (every slot, the
+  // identity table) or, for the feature cache, the k views in slots fslots[0..k-1]; one graph per k, the slots are data.
+  void forward(int k, const int* fslots, bool profiling) {
+    fk_ = k;
+    for (int j = 0; j <= kMaxSrc; ++j) h_feat_slot_[j] = k == V_ || j >= k ? j : fslots[j];
     upload_call_params();
     if (profiling || !use_graph_) { forward_launches(profiling); return; }
-    if (graph_exec_) { TDM_CUDA(cudaGraphLaunch(graph_exec_, stream_)); return; }
-    if (!warmed_) { forward_launches(false); warmed_ = true; return; }
+    FwdGraph& fg = graphs_[k];
+    if (fg.exec) { TDM_CUDA(cudaGraphLaunch(fg.exec, stream_)); return; }
+    if (!fg.warmed) { forward_launches(false); fg.warmed = true; return; }
     cudaGraph_t graph = nullptr;
     TDM_CUDA(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
     try {
@@ -1369,55 +1440,71 @@ class MvsnetEngine final : public MvsnetIface {
       throw;
     }
     TDM_CUDA(cudaStreamEndCapture(stream_, &graph));
-    TDM_CUDA(cudaGraphInstantiate(&graph_exec_, graph, 0));
+    TDM_CUDA(cudaGraphInstantiate(&fg.exec, graph, 0));
     cudaGraphDestroy(graph);
-    TDM_CUDA(cudaGraphLaunch(graph_exec_, stream_));
+    TDM_CUDA(cudaGraphLaunch(fg.exec, stream_));
   }
   void drop_graph() {
-    if (graph_exec_) cudaGraphExecDestroy(graph_exec_);
-    graph_exec_ = nullptr;
-    warmed_ = false;
+    for (auto& kv : graphs_)
+      if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+    graphs_.clear();
   }
 
-  // The whole graph of cva_mvsnet.py:98-184 on stream_, inputs already in d_bgr_.
+  // feature cache: FeatureNet output `name` over the fk_ computed views -> their pool slots (c_feat_slot) of `name` over V
+  void scatter_features(const std::string& name) {
+    if (fk_ == V_) return;
+    const DevBuf& src = bufs_.at(name + "@" + std::to_string(fk_));
+    const DevBuf& dst = bufs_.at(name);
+    TDM_CHECK(src.pd == 0 && dst.pd == 0 && src.C == dst.C && src.H == dst.H && src.W == dst.W, "feature scatter: shape mismatch");
+    const int plane_vec = (int)((size_t)(src.H + 2) * (src.W + 2) * 8 * sizeof(TA) / 16);
+    rec_begin(name + "[scatter]", 2.0 * src.alg_bytes, 0);
+    launch_k(k_scatter_planes, dim3(cdiv(plane_vec, 256), (src.C / 8) * fk_), dim3(256), (const uint4*)src.p, (uint4*)dst.p,
+             plane_vec, fk_, V_, slot_);
+    TDM_CUDA(cudaGetLastError());
+    rec_end();
+  }
+
+  // The whole graph of cva_mvsnet.py:98-184 on stream_, inputs already in d_bgr_.  FeatureNet runs over the fk_ views of
+  // c_feat_slot: all V into feat1..feat3 directly, or (feature cache) fk_ < V views into the "@fk_" scratch, scattered after.
   void forward_launches(bool profiling) {
     profiling_ = profiling;
     launch_count_ = 0;
-    const int V = V_, H = H_, W = W_;
+    const int H = H_, W = W_, k = fk_;
+    const std::string fs = k == V_ ? "" : "@" + std::to_string(k);
+    auto fb = [&fs](const char* name) { return name + fs; };
+    const bool fork = fork_fpn_ && !profiling && k > 0;
+    if (k > 0) {   // k == 0: a cached window of held views only, every feature is in the pool
     {
-      ViewPtrs vp;
-      for (int v = 0; v < V; ++v) vp.v[v] = d_bgr_ + (size_t)v * H * W * 3;
-      const long long n = (long long)V * H * W;
+      const long long n = (long long)k * H * W;
       bool fused = false;
       if constexpr (kRawInput) {
         if (direct_conv00_) {
           fused = true;
           rec_begin("f.conv0.0[u8-direct]", 3.0 * n + 8.0 * n * sizeof(TA), 2.0 * 27 * 8 * (double)n);
-          launch_k(k_conv00_u8<TA>, dim3(cdiv(W, 32), cdiv(H, 8), V), dim3(256), d_bgr_, p8<TA>(bufs_.at("f.c0_0")), H, W, slot_);
+          launch_k(k_conv00_u8<TA>, dim3(cdiv(W, 32), cdiv(H, 8), k), dim3(256), d_bgr_, p8<TA>(bufs_.at(fb("f.c0_0"))), H, W, slot_);
           TDM_CUDA(cudaGetLastError());
           rec_end();
         }
       }
       if (!fused) {
         rec_begin("preprocess", 3.0 * n + 8.0 * n * sizeof(TA), 0);
-        k_preprocess_bgr<TA, kRawInput><<<cdiv(n, 256), 256, 0, stream_>>>(vp, p8<TA>(bufs_.at("f.img")), V, H * W);
+        k_preprocess_bgr<TA, kRawInput><<<cdiv(n, 256), 256, 0, stream_>>>(d_bgr_, p8<TA>(bufs_.at(fb("f.img"))), k, H * W, slot_);
         TDM_CUDA(cudaGetLastError());
         rec_end();
-        conv("f.conv0.0", "f.img", "f.c0_0", 1, 1, 1, true);
+        conv("f.conv0.0", fb("f.img"), fb("f.c0_0"), 1, 1, 1, true);
       }
     }
-    conv("f.conv0.1", "f.c0_0", "f.c3", 1, 1, 1, true);
-    conv("f.conv1.0", "f.c3", "f.c1_0", 1, 2, 2, true);
-    conv("f.conv1.1", "f.c1_0", "f.c1_1", 1, 1, 1, true);
-    conv("f.conv1.2", "f.c1_1", "f.c2", 1, 1, 1, true);
-    conv("f.conv2.0", "f.c2", "f.c2_0", 1, 2, 2, true);
-    conv("f.conv2.1", "f.c2_0", "f.c2_1", 1, 1, 1, true);
-    conv("f.conv2.2", "f.c2_1", "f.c1", 1, 1, 1, true);
+    conv("f.conv0.1", fb("f.c0_0"), fb("f.c3"), 1, 1, 1, true);
+    conv("f.conv1.0", fb("f.c3"), fb("f.c1_0"), 1, 2, 2, true);
+    conv("f.conv1.1", fb("f.c1_0"), fb("f.c1_1"), 1, 1, 1, true);
+    conv("f.conv1.2", fb("f.c1_1"), fb("f.c2"), 1, 1, 1, true);
+    conv("f.conv2.0", fb("f.c2"), fb("f.c2_0"), 1, 2, 2, true);
+    conv("f.conv2.1", fb("f.c2_0"), fb("f.c2_1"), 1, 1, 1, true);
+    conv("f.conv2.2", fb("f.c2_1"), fb("f.c1"), 1, 1, 1, true);
     // The pyramid's upper outputs (feat2, feat3) are only read by stages 2 and 3, while stage 1 needs feat1 alone and its
     // coarse U-Net levels leave most SMs idle: the FPN tail runs on a second stream, forked here and joined before the
     // stage-2 cost volume (inside the captured graph these are two parallel branches).  Not while profiling: the per-kernel
     // events assume one stream.
-    const bool fork = fork_fpn_ && !profiling;
     struct SwapBack {   // an exception inside the branch must not leave the engine on the side stream
       cudaStream_t &a, &b; bool on;
       ~SwapBack() { if (on) std::swap(a, b); }
@@ -1428,25 +1515,30 @@ class MvsnetEngine final : public MvsnetIface {
       std::swap(stream_, side_stream_);
       side.on = true;
     } else {
-      conv("f.out1", "f.c1", "feat1", 1, 1, 1, false);
+      conv("f.out1", fb("f.c1"), fb("feat1"), 1, 1, 1, false);
+      scatter_features("feat1");
     }
     if (fused_fpn_ && use_tc_) {
-      conv("f.skip2", "f.c2", "f.i2", 1, 1, 1, false, 2, "f.c1", "f.i2b", d_bs3_);
-      conv("f.out2", "f.i2", "feat2", 1, 1, 1, false);
-      conv_up2("f.out3a", "f.i2b", "feat3");
-      conv("f.out3b", "f.c3", "feat3", 1, 1, 1, false, 1, "feat3");
+      conv("f.skip2", fb("f.c2"), fb("f.i2"), 1, 1, 1, false, 2, fb("f.c1"), fb("f.i2b"), d_bs3_);
+      conv("f.out2", fb("f.i2"), fb("feat2"), 1, 1, 1, false);
+      conv_up2("f.out3a", fb("f.i2b"), fb("feat3"));
+      conv("f.out3b", fb("f.c3"), fb("feat3"), 1, 1, 1, false, 1, fb("feat3"));
     } else {
-      conv("f.skip2", "f.c2", "f.i2", 1, 1, 1, false, 2, "f.c1");
-      conv("f.out2", "f.i2", "feat2", 1, 1, 1, false);
-      conv("f.skip3", "f.c3", "f.i3", 1, 1, 1, false, 2, "f.i2");
-      conv("f.out3", "f.i3", "feat3", 1, 1, 1, false);
+      conv("f.skip2", fb("f.c2"), fb("f.i2"), 1, 1, 1, false, 2, fb("f.c1"));
+      conv("f.out2", fb("f.i2"), fb("feat2"), 1, 1, 1, false);
+      conv("f.skip3", fb("f.c3"), fb("f.i3"), 1, 1, 1, false, 2, fb("f.i2"));
+      conv("f.out3", fb("f.i3"), fb("feat3"), 1, 1, 1, false);
     }
+    scatter_features("feat2");
+    scatter_features("feat3");
     if (fork) {
       TDM_CUDA(cudaEventRecord(ev_join_, stream_));      // stream_ is the side stream here
       std::swap(stream_, side_stream_);
       side.on = false;
-      conv("f.out1", "f.c1", "feat1", 1, 1, 1, false);
+      conv("f.out1", fb("f.c1"), fb("feat1"), 1, 1, 1, false);
+      scatter_features("feat1");
     }
+    }  // k > 0
 
     for (int s = 1; s <= 3; ++s) {
       const std::string k = "s" + std::to_string(s) + ".";
@@ -1512,7 +1604,7 @@ class MvsnetEngine final : public MvsnetIface {
       std::string err;
       try {
         const size_t n = (size_t)H_ * W_;
-        forward(false);
+        forward(call_k_, call_slots_, false);
         if (eager_d2h_) {
           const char* names[4] = {"s3.depth", "s3.confidence", "s3.depth_dense", "s3.confidence_dense"};
           for (int k = 0; k < 4; ++k) {
@@ -1530,6 +1622,7 @@ class MvsnetEngine final : public MvsnetIface {
         std::lock_guard<std::mutex> lk(mu_);
         worker_error_ = err;
         has_result_ = err.empty();
+        if (!err.empty()) cache_valid_ = false;   // the pool may not hold the features of the ids it lists
         busy_ = false;
         started_ = false;
       }
@@ -1540,7 +1633,8 @@ class MvsnetEngine final : public MvsnetIface {
   // Keyframe handoff.  Invariant: the handoff buffers are written only by this fill, enqueued on stream_ behind every release
   // event recorded since the previous fill, and freed only after those events have completed; so a consumer's reads, which
   // wait for ev_ho_ready_ and end before their release event, always see exactly the result the last GetResult returned,
-  // however far the next window's upload and forward (which overwrite d_bgr_ and s3.depth) have got.
+  // however far the next window's upload and forward (which overwrite d_bgr_ and s3.depth) have got.  The image is copied
+  // from the reference view's pool slot, which is enqueued on stream_ before any later upload into that slot.
   void fill_handoff() {
     const size_t n = (size_t)H_ * W_;
     ho_valid_ = false;
@@ -1557,7 +1651,7 @@ class MvsnetEngine final : public MvsnetIface {
     for (int i = 0; i < n_ho_release_; ++i) TDM_CUDA(cudaStreamWaitEvent(stream_, ev_ho_release_[i], 0));
     n_ho_release_ = 0;
     TDM_CUDA(cudaMemcpyAsync(d_ho_depth_, fbuf("s3.depth"), n * 4, cudaMemcpyDeviceToDevice, stream_));
-    TDM_CUDA(cudaMemcpyAsync(d_ho_bgr_, d_bgr_, n * 3, cudaMemcpyDeviceToDevice, stream_));   // view 0 = the reference view
+    TDM_CUDA(cudaMemcpyAsync(d_ho_bgr_, d_bgr_ + (size_t)view_slot_[0] * n * 3, n * 3, cudaMemcpyDeviceToDevice, stream_));
     TDM_CUDA(cudaEventRecord(ev_ho_ready_, stream_));
     std::memcpy(ho_c2w_, c2w_[0], sizeof(ho_c2w_));
     ho_valid_ = true;
@@ -1571,6 +1665,80 @@ class MvsnetEngine final : public MvsnetIface {
     }
     if (cudaEventRecord(ev_ho_release_[n_ho_release_], (cudaStream_t)stream) != cudaSuccess) return false;
     ++n_ho_release_;
+    return true;
+  }
+
+  static void check_window(int H, int W, int V, int ref_index) {
+    TDM_CHECK(V >= 2 && V <= kMaxSrc + 1, "view_num out of range");
+    TDM_CHECK(ref_index >= 0 && ref_index < V, "ref_index out of range");
+    TDM_CHECK(H % 32 == 0 && W % 32 == 0, "height and width must be multiples of 32 (three stride-2 levels at 1/4 resolution)");
+  }
+  // the caller's view at position vi of the reference-first order (dr_mvsnet.cpp:190-197), and back
+  static int window_view(int vi, int ref_index) { return vi == 0 ? ref_index : (vi <= ref_index ? vi - 1 : vi); }
+  static int window_index(int view, int ref_index) { return view == ref_index ? 0 : (view < ref_index ? view + 1 : view); }
+
+  void wait_idle_for_call(std::unique_lock<std::mutex>& lk) {
+    cv_done_.wait(lk, [this] { return !busy_; });
+    if (has_result_) throw Error("CallAsync while a result is un-fetched (dr_mvsnet.cpp:315-318)");
+    if (!worker_error_.empty()) { std::string e = worker_error_; worker_error_.clear(); throw Error(e); }
+  }
+
+  // srcs[j] (H*W*3 u8, owned by the caller only during this call) -> slot slots[j] of d_bgr_
+  void upload_images(int n, const int* slots, const unsigned char* const* srcs) {
+    const size_t img = (size_t)H_ * W_ * 3;
+    if (all_page_locked((const void* const*)srcs, n)) {
+      // Page-locked caller images (cudaHostAlloc / cudaHostRegister): DMA straight from them - no staging copy, no copy
+      // threads.  The caller owns them only during this call, so the call returns once the seven DMAs have landed
+      // (6.45 MB over PCIe gen5: ~0.13 ms, less than the staging memcpy it replaces).
+      for (int j = 0; j < n; ++j)
+        TDM_CUDA(cudaMemcpyAsync(d_bgr_ + (size_t)slots[j] * img, srcs[j], img, cudaMemcpyHostToDevice, stream_));
+      TDM_CUDA(cudaEventRecord(ev_in_, stream_));
+      TDM_CUDA(cudaEventSynchronize(ev_in_));
+    } else {
+      // Pageable caller memory: staged through pinned memory.  The staging copy of view v+1 overlaps the DMA of view v (the
+      // worker is idle here, so this thread may enqueue on the engine's stream); each view is split into slices copied by the
+      // process-wide pool; a slice's H2D is enqueued by whichever thread finished copying it (CUDA stream calls are
+      // thread-safe; the order of the DMAs inside the stream does not matter, the forward is enqueued behind all of them).
+      std::vector<CopyPool::Job> jobs;
+      constexpr int kSlices = 2;
+      std::mutex err_mu;
+      cudaError_t first_err = cudaSuccess;
+      for (int j = 0; j < n; ++j) {
+        for (int sl = 0; sl < kSlices; ++sl) {
+          const size_t b0 = img * sl / kSlices, b1 = img * (sl + 1) / kSlices;
+          unsigned char* hp = h_bgr_ + (size_t)slots[j] * img + b0;
+          unsigned char* dp = d_bgr_ + (size_t)slots[j] * img + b0;
+          jobs.push_back({hp, srcs[j] + b0, b1 - b0, [this, hp, dp, b0, b1, &err_mu, &first_err] {
+                            cudaSetDevice(device_);   // pool threads start on device 0
+                            const cudaError_t e = cudaMemcpyAsync(dp, hp, b1 - b0, cudaMemcpyHostToDevice, stream_);
+                            if (e != cudaSuccess) { std::lock_guard<std::mutex> lk(err_mu); first_err = e; }
+                          }});
+        }
+      }
+      CopyPool::shared().run(jobs);
+      TDM_CUDA(first_err);
+    }
+  }
+
+  // hands the window to the worker: FeatureNet on the k views in slots new_slots[0..k-1] (k == V: every slot)
+  void submit(int k, int ref_index, float* const* c2ws, const float* K3x3x3, float dmin, float dmax, float discard,
+              std::unique_lock<std::mutex>& lk, const int* new_slots = nullptr) {
+    for (int vi = 0; vi < V_; ++vi) std::memcpy(c2w_[vi], c2ws[window_view(vi, ref_index)], 16 * sizeof(float));
+    std::memcpy(K_, K3x3x3, 27 * sizeof(float));
+    dmin_ = dmin; dmax_ = dmax; discard_ = discard;
+    call_k_ = k;
+    for (int j = 0; j < k; ++j) call_slots_[j] = new_slots ? new_slots[j] : j;
+    n_computed_ = k;
+    last_ref_index_ = ref_index;
+    busy_ = true;
+    have_inputs_ = true;
+    lk.unlock();
+    cv_work_.notify_all();
+  }
+
+  bool slots_identity() const {
+    for (int v = 0; v < V_; ++v)
+      if (view_slot_[v] != v) return false;
     return true;
   }
 
@@ -1647,14 +1815,25 @@ class MvsnetEngine final : public MvsnetIface {
   float* d_bs3_ = nullptr;
   CallParams* h_params_ = nullptr;   // pinned
   CallParams* d_params_ = nullptr;
-  cudaGraphExec_t graph_exec_ = nullptr;
+  int* h_feat_slot_ = nullptr;       // pinned [kMaxSrc + 1]: the table c_feat_slot[slot_] the next forward uses
+  // feature cache (call_async_ids): slot s of d_bgr_ / feat1..3 holds the view with id slot_id_[s] when cache_valid_; view vi of
+  // the last window (reference first) is in slot view_slot_[vi] (the identity after a plain call_async)
+  long long slot_id_[kMaxSrc + 1] = {};
+  int view_slot_[kMaxSrc + 1];
+  bool cache_valid_ = false;
+  int last_ref_index_ = 0;
+  int n_computed_ = 0;                                 // views FeatureNet computed for the last call
+  int call_k_ = 0, call_slots_[kMaxSrc + 1] = {};      // the submitted window's FeatureNet views, for the worker
+  int fk_ = 0;                                         // views FeatureNet computes in the forward being enqueued / last enqueued
+  struct FwdGraph { cudaGraphExec_t exec = nullptr; bool warmed = false; };
+  std::map<int, FwdGraph> graphs_;   // one captured forward per FeatureNet view count
   CUtensorMap cv_tmap_{};      // cv_variant 5 (A/B): tiled view of feat3 for the TMA-staged cost volume
   bool cv_tmap_ok_ = false;
   unsigned* d_cv_stats_ = nullptr;
   int cv_variant_ = 3;   // 0: generic cost-volume kernel; 1-4: k_cost_volume_va16 (ND 2/2/4 | 4/4/4, fp32 | fp16 accumulate)
   // Programmatic dependent launch of the tensor-core kernels: the trigger sits after griddepcontrol.wait (a trigger before it
   // lets the whole chain of later kernels become resident early), and pdl_min_smem_kb_ = 120 keeps one tensor-core CTA per SM.
-  bool warmed_ = false, use_graph_ = true;
+  bool use_graph_ = true;
   int use_pdl_ = 1;   // 2: the FMA-pipe kernels (cost volume, soft-argmin, edge filter ...) are launched with the attribute as well
   int slot_ = 0;           // index into c_call_params
   int tc_smem_kb_ = 225;   // shared-memory budget of the tile planner (<= 113 lets two CTAs share an SM)

@@ -11,7 +11,7 @@ class MvsnetIface {
   // TSDF, tdm_fusion_integrate_mvsnet): filtered stage-3 depth, the reference view's BGR and its cam_to_world.
   struct Handoff {
     const float* depth;          // H*W
-    const unsigned char* bgr;    // H*W*3, view 0 after the ref-first reorder
+    const unsigned char* bgr;    // H*W*3, the reference view's image
     float c2w[16];
     int H, W, device;
     void* ready;                 // cudaEvent_t recorded behind the copy that filled the buffers
@@ -21,6 +21,12 @@ class MvsnetIface {
   // K3x3x3: three row-major 3x3 intrinsics, stage1..stage3.
   virtual void call_async(int H, int W, int V, int ref_index, unsigned char* const* bgrs, const float* K3x3x3,
                           float* const* c2ws, float dmin, float dmax, float discard) = 0;
+  // Feature cache (tdm_mvsnet_call_async_ids): views are named by caller ids; FeatureNet runs only for the ids the handle does
+  // not hold, whose bgrs[i] must be non-null (the bgrs of held ids are ignored).
+  virtual void call_async_ids(int H, int W, int V, int ref_index, const long long* ids, unsigned char* const* bgrs,
+                              const float* K3x3x3, float* const* c2ws, float dmin, float dmax, float discard) = 0;
+  // ids held (the last cached call's window, in its order; none after a plain call_async) and the views the last call computed
+  virtual void feature_cache(long long* ids, int cap, int* n_ids, int* n_computed) = 0;
   virtual bool ready() = 0;
   virtual void wait() = 0;
   virtual void get_result(float* depth, float* conf, float* depth_dense, float* conf_dense) = 0;
@@ -31,6 +37,8 @@ class MvsnetIface {
   virtual void stage_output(int stage, const std::string& which, float* out, size_t cap) = 0;
   virtual long long debug_tensor(const std::string& name, float* out, size_t cap, int* dims4) = 0;
   virtual void run_resident(int iters, float* ms_total, int* launches) = 0;
+  // the last window's forward with FeatureNet recomputing only its last n_new views (window order), the others read from the pool
+  virtual void run_resident_new(int n_new, int iters, float* ms_total, int* launches) = 0;
   virtual std::string profile() = 0;
   // building blocks of tdm_mvsnet_run_resident_multi (several engines of one device timed together)
   virtual void* resident_stream() = 0;                 // cudaStream_t

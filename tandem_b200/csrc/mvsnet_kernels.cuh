@@ -46,13 +46,16 @@ struct P8 {
   }
 };
 
+// Which slot of the engine's image / feature pool FeatureNet plane v works on: c_feat_slot[engine][v].  The identity for a
+// forward over the whole window; the slots of the views a cached call adds when FeatureNet runs on those views only (the
+// image is read from that slot of the u8 pool and k_scatter_planes copies the features into it).  Refreshed stream-ordered
+// before each forward, like c_call_params, so that captured graphs replay with the current table.
+__constant__ int c_feat_slot[8 /* kMaxEngines */][16 /* kMaxSrc + 1 */];
+
 // ------------------------------------------------------------------------------------------------
-// a1: u8 BGR HWC (window order) -> T [V][H][W][4] RGB/255 (+ zero 4th channel), reference view first.
+// a1: u8 BGR HWC (image pool, plane v read from slot c_feat_slot[engine][v]) -> T [V][H][W][4] RGB/255 (+ zero 4th channel).
 // Replaces the scalar CPU loop + 25.8 MB pageable H2D of dr_mvsnet.cpp:190-217,260.
 // ------------------------------------------------------------------------------------------------
-struct ViewPtrs {
-  const unsigned char* v[16];
-};
 
 // RAW255: the 16-bit engines store u8/256 - exact in fp16 / bf16 (8 significant bits, power-of-two scale) - and fold the
 // remaining 256/255 of dr_mvsnet.cpp:203-210 into the first convolution's weights (which keeps the weights' magnitude, so
@@ -60,12 +63,12 @@ struct ViewPtrs {
 // rounded to 16 bit would inject a relative error of up to 2^-11 into every feature.  The fp32 parity engine divides as the
 // reference does.
 template <typename T, bool RAW255 = false>
-__global__ void k_preprocess_bgr(ViewPtrs src, P8<T> out, int V, int HW) {
+__global__ void k_preprocess_bgr(const unsigned char* __restrict__ bgr /*[slots][H][W][3]*/, P8<T> out, int V, int HW, int slot) {
   long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= (long long)V * HW) return;
   int v = (int)(i / HW);
   int p = (int)(i - (long long)v * HW);
-  const unsigned char* s = src.v[v] + 3ll * p;
+  const unsigned char* s = bgr + 3ll * ((long long)c_feat_slot[slot][v] * HW + p);
   float o[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   if (RAW255) {
     o[0] = (float)s[2] * 0.00390625f; o[1] = (float)s[1] * 0.00390625f; o[2] = (float)s[0] * 0.00390625f;
@@ -93,14 +96,14 @@ struct Conv00Weights {
 __constant__ Conv00Weights c_conv00[8 /* kMaxEngines */];
 
 template <typename T>
-__global__ void __launch_bounds__(256) k_conv00_u8(const unsigned char* __restrict__ bgr /*[V][H][W][3], reference view first*/, P8<T> out, int H, int W, int slot) {
+__global__ void __launch_bounds__(256) k_conv00_u8(const unsigned char* __restrict__ bgr /*image pool [slots][H][W][3]*/, P8<T> out, int H, int W, int slot) {
   grid_dep_sync();
   constexpr int TX = 32, TY = 8;
   __shared__ float tile[TY + 2][(TX + 2) * 3];   // x = u8 / 255 formed ONCE per input value (IEEE division, dr_mvsnet.cpp:203-210)
   const Conv00Weights& cw = c_conv00[slot];
   const int v = blockIdx.z;
   const int x0 = blockIdx.x * TX, y0 = blockIdx.y * TY;
-  const unsigned char* img = bgr + (size_t)v * H * W * 3;
+  const unsigned char* img = bgr + (size_t)c_feat_slot[slot][v] * H * W * 3;
   for (int i = threadIdx.x; i < (TY + 2) * (TX + 2); i += 256) {
     const int ty = i / (TX + 2), tx = i - ty * (TX + 2);
     const int yy = y0 + ty - 1, xx = x0 + tx - 1;
@@ -131,6 +134,17 @@ __global__ void __launch_bounds__(256) k_conv00_u8(const unsigned char* __restri
 #pragma unroll
   for (int c = 0; c < 8; ++c) acc[c] = fmaxf(acc[c], 0.f);
   store_vec<T, 8>(out.p + out.pos(v, y, x), acc);
+}
+
+// Feature cache: copies the k planes FeatureNet computed (a 2-D P8 map over k planes, pd = 0) into pool slots
+// c_feat_slot[engine][0..k-1] of the same map over V planes.  Whole padded planes are moved (the halos are zero on both
+// sides), 16 bytes per thread; blockIdx.y = channel group * k + plane.
+__global__ void k_scatter_planes(const uint4* __restrict__ src, uint4* __restrict__ dst, int plane_vec, int k, int V, int slot) {
+  grid_dep_sync();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= plane_vec) return;
+  const int g = blockIdx.y / k, j = blockIdx.y - g * k;
+  dst[((long long)g * V + c_feat_slot[slot][j]) * plane_vec + i] = src[(long long)blockIdx.y * plane_vec + i];
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -410,6 +424,7 @@ struct CvParams {
   HypSpec hyp;
   float vol_scale;     // the volume is STORED as value * vol_scale (1 for fp32 / bf16 volumes; 2^-5 for the fp16 volume of the
                        // mixed16 engine, whose conv0 weights carry the inverse): a power of two, i.e. exact
+  int plane[kMaxSrc + 1];   // feature-map plane of view v (0 = reference, 1.. = sources): its slot in the engine's feature pool
 };
 
 // C = channels handled by ONE thread; CSPLIT adjacent lanes share a voxel and split its channels (C*CSPLIT in total):
@@ -430,7 +445,7 @@ __constant__ CallParams c_call_params[kMaxEngines];
 
 template <typename T, typename TV, int C, int CSPLIT = 1>
 __global__ void __launch_bounds__(128)
-k_cost_volume(P8<const T> feats /*views on the D axis, ref first*/, const DminSrc dsrc,
+k_cost_volume(P8<const T> feats /*views on the D axis, view v on plane p.plane[v]*/, const DminSrc dsrc,
               P8<TV> vol, int slot, int stage /*per-call parameters: c_call_params[slot].cv[stage] (graph-replayable)*/) {
   const CvParams& p = c_call_params[slot].cv[stage];
   const long long n = (long long)p.D * p.H * p.W;
@@ -448,7 +463,7 @@ k_cost_volume(P8<const T> feats /*views on the D axis, ref first*/, const DminSr
 
   float ref[C];
   {
-    const T* rp = feats.p + feats.pos(0, y, x);
+    const T* rp = feats.p + feats.pos(p.plane[0], y, x);
 #pragma unroll
     for (int c0 = 0; c0 < C; c0 += 8) {
       float t8[8];
@@ -490,7 +505,7 @@ k_cost_volume(P8<const T> feats /*views on the D axis, ref first*/, const DminSr
         const float x0f = floorf(ix), y0f = floorf(iy);
         const float ax = ix - x0f, ay = iy - y0f;
         const float w00 = (1.f - ax) * (1.f - ay), w01 = ax * (1.f - ay), w10 = (1.f - ax) * ay, w11 = ax * ay;
-        const T* tp = feats.p + feats.pos(s + 1, (int)y0f, (int)x0f);
+        const T* tp = feats.p + feats.pos(p.plane[s + 1], (int)y0f, (int)x0f);
         const int row = feats.Wp * 8;
         if constexpr (std::is_same<T, __half>::value) {
           // fp16 features: the 4-tap interpolation runs as packed HFMA2 (2 channels per instruction) and only the result is
@@ -545,7 +560,7 @@ k_cost_volume(P8<const T> feats /*views on the D axis, ref first*/, const DminSr
         const int xx = x0 + (k & 1), yy = y0 + (k >> 1);
         const float wgt = ((k & 1) ? ax : 1.f - ax) * ((k >> 1) ? ay : 1.f - ay);
         if (xx >= 0 && xx < p.W && yy >= 0 && yy < p.H) {
-          const T* tp = feats.p + feats.pos(s + 1, yy, xx);
+          const T* tp = feats.p + feats.pos(p.plane[s + 1], yy, xx);
 #pragma unroll
           for (int c0 = 0; c0 < C; c0 += 8) {
             float f[8];
@@ -644,7 +659,7 @@ k_cost_volume_va16(P8<const __half> feats, const DminSrc dsrc, P8<TV> vol, int s
 
   __half2 nref[C / 2], gwh[C / 2];
   {
-    const __half* rp = fbase + feats.pos(0, y, x);
+    const __half* rp = fbase + feats.pos(p.plane[0], y, x);
     const __half2 ms = __float2half2_rn(-kS);
 #pragma unroll
     for (int c0 = 0; c0 < C; c0 += 8) {
@@ -679,7 +694,7 @@ k_cost_volume_va16(P8<const __half> feats, const DminSrc dsrc, P8<TV> vol, int s
     const float ry = R[3] * fx + R[4] * fy + R[5];
     const float rz = R[6] * fx + R[7] * fy + R[8];
     const float t0 = t[0], t1 = t[1], t2 = t[2];
-    const int vbase = ((s + 1 + feats.pd) * feats.Hp + 1) * feats.Wp + 1;
+    const int vbase = ((p.plane[s + 1] + feats.pd) * feats.Hp + 1) * feats.Wp + 1;
 #pragma unroll
     for (int k = 0; k < ND; ++k) {
       const float qx = fmaf(rx, depth[k], t0), qy = fmaf(ry, depth[k], t1), qz = fmaf(rz, depth[k], t2);

@@ -26,8 +26,12 @@ GRAY_W = np.array([0.114, 0.587, 0.299], np.float32)
 class TandemLoop:
     def __init__(self, H, W, K4, weights, window=7, keyframe_every=5, depth_min=0.1, depth_max=8.0, discard=2.5,
                  precision="mixed16", device=0, integrate="mvsnet", max_iterations=(10, 20, 50, 50, 50), tracking_step=1,
-                 fusion_options=None, levels=None):
+                 fusion_options=None, levels=None, feature_cache=False):
+        """feature_cache=True submits each window through DrMvsnet.CallAsyncIds with the keyframe index as the view id,
+        so that FeatureNet runs only for the keyframe each window adds."""
         self.H, self.W, self.K4 = H, W, tuple(float(k) for k in K4)
+        self.feature_cache = feature_cache
+        self.n_keyframes = 0
         fx, fy, cx, cy = self.K4
         self.K = np.array([[fx, 0, cx], [0, fy, cy], [0, 0, 1]], np.float32)
         self.window, self.kf_every = window, keyframe_every
@@ -53,7 +57,7 @@ class TandemLoop:
         self.tracker = self.trackers[0]
         self.pyr = ImagePyramid(W, H, levels, device=device)       # new frame
         self.pyr_ref = ImagePyramid(W, H, levels, device=device)   # reference keyframe (grey values of the dense points)
-        self.kfs = []                 # (bgr, c2w) of the keyframes in the window
+        self.kfs = []                 # (bgr, c2w, true_depth, keyframe index) of the keyframes in the window
         self.pending = None           # window submitted to MVSNet whose result has not been fetched
         self.ref_c2w = None
         self.have_ref = False
@@ -66,7 +70,8 @@ class TandemLoop:
     # ------------------------------------------------------------------------------------------
     def _keyframe(self, bgr, gray, c2w, sensor_depth, true_depth):
         t0 = time.perf_counter()
-        self.kfs.append((bgr, np.asarray(c2w, np.float32), true_depth))
+        self.kfs.append((bgr, np.asarray(c2w, np.float32), true_depth, self.n_keyframes))
+        self.n_keyframes += 1
         if len(self.kfs) > self.window:
             self.kfs.pop(0)
         out_prev = None
@@ -78,7 +83,11 @@ class TandemLoop:
             ref_index = self.window - 2                                 # FullSystem.cpp:1127
             bgrs = [k[0] for k in self.kfs]
             c2ws = [k[1] for k in self.kfs]
-            self.mvsnet.CallAsync(self.H, self.W, self.window, ref_index, bgrs, self.K, c2ws, self.dmin, self.dmax, self.discard)
+            if self.feature_cache:
+                self.mvsnet.CallAsyncIds(self.H, self.W, self.window, ref_index, [k[3] for k in self.kfs], bgrs, self.K, c2ws,
+                                         self.dmin, self.dmax, self.discard)
+            else:
+                self.mvsnet.CallAsync(self.H, self.W, self.window, ref_index, bgrs, self.K, c2ws, self.dmin, self.dmax, self.discard)
             self.pending = dict(bgr=bgrs[ref_index], c2w=c2ws[ref_index], true_depth=self.kfs[ref_index][2])
         if out_prev is not None and prev.get("true_depth") is not None:
             td = prev["true_depth"]

@@ -79,6 +79,36 @@ class DrMvsnet:
                    np.asarray(K_stages, np.float32).reshape(27), cam_to_worlds, depth_min, depth_max,
                    discard_percentage)
 
+    def CallAsyncIds(self, height, width, view_num, ref_index, view_ids, bgrs, intrinsics, cam_to_worlds, depth_min,
+                     depth_max, discard_percentage, stage_k=False):
+        """CallAsync with the feature cache (tdm_mvsnet_call_async_ids): view_ids[i] names view i; FeatureNet runs only
+        for ids the handle does not hold.  bgrs[i] may be None for a held id (and is ignored for one).  intrinsics: the
+        3x3 full-resolution K, or with stage_k=True the three per-stage K's of CallAsyncStageK."""
+        if len(view_ids) != view_num or len(bgrs) != view_num or len(cam_to_worlds) != view_num:
+            raise TandemError("view_num does not match the number of ids / images / poses")
+        imgs = [None if b is None else np.ascontiguousarray(b, dtype=np.uint8) for b in bgrs]
+        for b in imgs:
+            if b is not None and b.size != height * width * 3:
+                raise TandemError("bgr image has the wrong size")
+        c2ws = [np.ascontiguousarray(c, dtype=np.float32) for c in cam_to_worlds]
+        K = np.ascontiguousarray(np.asarray(intrinsics, np.float32).reshape(27 if stage_k else 9))
+        ids = (ctypes.c_longlong * view_num)(*[int(i) for i in view_ids])
+        bp = (ctypes.c_void_p * view_num)(*[None if b is None else b.ctypes.data for b in imgs])
+        cp = (ctypes.c_void_p * view_num)(*[c.ctypes.data for c in c2ws])
+        check(lib().tdm_mvsnet_call_async_ids(self._h, height, width, view_num, ref_index, ids, bp,
+                                              K.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), int(bool(stage_k)), cp,
+                                              float(depth_min), float(depth_max), float(discard_percentage)))
+        self._hw = (height, width)
+
+    def feature_cache(self):
+        """(ids held in the last window's order, views FeatureNet computed for the last call)."""
+        n = ctypes.c_int()
+        nc = ctypes.c_int()
+        check(lib().tdm_mvsnet_feature_cache(self._h, None, 0, ctypes.byref(n), ctypes.byref(nc)))
+        ids = (ctypes.c_longlong * max(n.value, 1))()
+        check(lib().tdm_mvsnet_feature_cache(self._h, ids, n.value, ctypes.byref(n), ctypes.byref(nc)))
+        return [int(ids[i]) for i in range(n.value)], nc.value
+
     def GetResult(self, out=None):
         """Returns a fresh DrMvsnetOutput (the reference's ownership contract, dr_mvsnet.h:12-34), or fills `out` - a
         DrMvsnetOutput the caller recycles, e.g. DrMvsnetOutput(h, w, pinned=True) for a zero-copy read-back."""
@@ -119,6 +149,13 @@ class DrMvsnet:
         ms = ctypes.c_float()
         nl = ctypes.c_int()
         check(lib().tdm_mvsnet_run_resident(self._h, iters, ctypes.byref(ms), ctypes.byref(nl)))
+        return ms.value, nl.value
+
+    def run_resident_new(self, n_new, iters):
+        """run_resident with FeatureNet recomputing only the last n_new views of the last window."""
+        ms = ctypes.c_float()
+        nl = ctypes.c_int()
+        check(lib().tdm_mvsnet_run_resident_new(self._h, n_new, iters, ctypes.byref(ms), ctypes.byref(nl)))
         return ms.value, nl.value
 
     @staticmethod

@@ -20,3 +20,5 @@ leg pyramid_race $T2 racecheck tests/test_track_pyramid_gpu.py -k "equals_host a
 leg new_coarse_mem $T1 memcheck tests/test_track_new_coarse_gpu.py -k "not shim and not size1"
 leg new_coarse_race $T2 racecheck tests/test_track_new_coarse_gpu.py -k "host_loop and size0 and retrack"
 leg conv_is_mem $T1 memcheck tests/test_conv_is_gpu.py -k "abl04"
+leg feature_cache_mem $T1 memcheck tests/test_mvsnet_feature_cache_gpu.py -k "handoff or golden"
+leg feature_cache_race $T2 racecheck tests/test_mvsnet_feature_cache_gpu.py -k "handoff"
