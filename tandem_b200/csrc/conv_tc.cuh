@@ -52,8 +52,8 @@ struct Tile {
 struct Geom : Tile {
   int Hp, Wp;             // H+2, W+2
   int pd;                 // 1: 3-D conv (KD = 3, halo planes exist), 0: 2-D conv over independent planes (KD = 1)
-  long long in_gs, out_gs, res_gs;   // channel-group strides in elements
-  int relu, has_res;
+  long long in_gs, out_gs;   // channel-group strides in elements
+  int relu, has_res;         // has_res: MODE 1 adds its skip operand
   int cout;               // real output channels (<= NPAD)
   int oHp, oWp, opd;      // padded dims / D halo of the OUTPUT tensor (differs from the input in deconv mode)
   int iDp;                // padded plane count of the input: tensor-map dim 3 = channel_group * iDp + plane
@@ -385,19 +385,25 @@ __device__ __forceinline__ int stencil_off(int t, int P) { return (t / 3) * P + 
 // weight precision at the cost of a wider N.
 // MODE 0: 3x3 stencil per plane (9 taps).  MODE 1: transposed conv k3 s2 p1 op1 as a GEMM over the INPUT grid: 2x2 taps
 // per plane at offsets {0,1}^2 (stencil positions (1..2,1..2)), 2 planes, N = 8 output parity classes x COUT.
-// MODE 3: 2-D "conv3x3 of a nearest-x2 up-sampled map" evaluated on the COARSE grid: 9 taps, N = 4 output parity
-// classes x COUT (the 3x3 fine taps collapse onto 2x2 coarse neighbours; weights pre-summed on the host).
+// MODE 3: the fused FPN tail, out = conv3x3(up2(x)) + conv3x3(y) for a map x on the COARSE grid and y on the fine one,
+// evaluated on the coarse grid: 9 coarse taps, N = 4 output parity classes x COUT.  Fine tap k of output parity p reads
+// fine offset p + k - 1 = 2 * delta + q, i.e. coarse offset delta in {-1, 0, 1} and sub-position q in {0, 1}.  Channel
+// groups 0 .. 3 of a ring slot are x (tmap); groups 4 .. 7 are the four parity sub-tiles (qh, qw) of y's 8 channels
+// (tmap_res, every second fine row and column), so y's term is a 3x3 coarse-grid conv over 32 space-to-depth channels
+// like x's (weights pre-summed and placed per class, coarse tap and sub-position on the host).
 // NWG: consumer warpgroups, conv_nwg(MODE, instruction N, Tail::max_d).
 template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool OUT_PLAIN, int MODE, bool HILO, typename Tail, int NWG>
 __global__ void __launch_bounds__(conv_threads(NWG), 1)
 k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, groups*planes}, box {8, P, R+2, 1}*/,
-          const __grid_constant__ CUtensorMap tmap_res /*MODE 1: skip operand, see OutBox*/,
+          const __grid_constant__ CUtensorMap tmap_res /*MODE 1: skip operand, see OutBox; MODE 3: the fine input,
+                                                          box {8, 2P, 2(R+2), 1} with element strides 2 in W and H*/,
           const __grid_constant__ CUtensorMap tmap_out /*MODE 1: output*/,
           const TIn* __restrict__ bimg /*host-arranged B image*/, const float* __restrict__ bias,
-          const TOut* __restrict__ res, TOut* __restrict__ out, float* __restrict__ plain_out, const __grid_constant__ Geom g,
-          const __grid_constant__ Tail tail) {
+          TOut* __restrict__ out, float* __restrict__ plain_out, const __grid_constant__ Geom g, const __grid_constant__ Tail tail) {
   static_assert(!Tail::enabled || OUT_PLAIN, "a per-pixel tail only exists for the single-channel fp32 output");
+  static_assert(MODE != 3 || (CIN == 64 && KD == 1), "MODE 3 streams 4 coarse and 4 fine sub-tile channel groups");
   constexpr int CG = CIN / 8;
+  constexpr int CG_TMAP = MODE == 3 ? 4 : CG;     // channel groups from tmap; MODE 3 loads the rest from tmap_res
   constexpr int NTAPS = MODE == 1 ? 4 : 9;
   constexpr int NBLK = ksteps(CIN, NTAPS);
   constexpr int NMMA = HILO ? 2 * NPAD : NPAD;   // instruction N
@@ -443,7 +449,14 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
       auto boxes = [&](uint8_t* dst, int rp, uint64_t* bar) {
         const int pp = o.d0 + rp + PLANE0;  // padded plane index (pd == 1: plane d-1+kd+1; pd == 0: plane d)
 #pragma unroll 1
-        for (int cg = 0; cg < CG; ++cg) tma_load_4d(dst + (size_t)cg * cg_bytes, &tmap, 0, o.w0, o.h0, cg * g.iDp + pp, bar);
+        for (int cg = 0; cg < CG_TMAP; ++cg) tma_load_4d(dst + (size_t)cg * cg_bytes, &tmap, 0, o.w0, o.h0, cg * g.iDp + pp, bar);
+        if constexpr (MODE == 3) {
+          // box position (i, j) is coarse (h0 - 1 + i, w0 - 1 + j), like the coarse boxes; in sub-tile (qh, qw) it holds
+          // fine (2 (h0 - 1 + i) + qh, 2 (w0 - 1 + j) + qw), padded coordinates from (2 h0 - 1 + qh, 2 w0 - 1 + qw)
+#pragma unroll 1
+          for (int q = 0; q < 4; ++q)
+            tma_load_4d(dst + (size_t)(CG_TMAP + q) * cg_bytes, &tmap_res, 0, 2 * o.w0 - 1 + (q & 1), 2 * o.h0 - 1 + (q >> 1), pp, bar);
+        }
       };
       if constexpr (MODE == 1) {
         // input planes, skip boxes and output stores interleaved: plane od's consumers need input planes od, od + 1 and
@@ -570,25 +583,6 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
     for (int k = 0; wg + k * NWG < nsub; ++k) {
       const int sc = wg + k * NWG;
       const int l = sc * 64 + wq * 16 + (lane >> 2);
-      // the skip operand is fetched before the MMA chain, so that its load latency overlaps the chain
-      constexpr bool RES_EARLY = !OUT_PLAIN && NPAD <= 64 && MODE != 1;
-      uint32_t rv[2][RES_EARLY ? NPAD / 8 : 1];
-      if constexpr (RES_EARLY) {
-        if (g.has_res) {
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            int h, w;
-            const bool in = frag_pixel(g, o, l, i, h, w);
-#pragma unroll
-            for (int j = 0; j < NPAD / 8; ++j) {
-              long long pos;
-              int co;
-              rv[i][j] = in && out_at(d, h, w, j, pos, co)
-                             ? __ldg(reinterpret_cast<const unsigned int*>(res + pos + (co >> 3) * g.res_gs + (co & 7))) : 0u;
-            }
-          }
-        }
-      }
       float acc[NMMA / 2];
       mma_subchunk<NMMA, TIn, KD, NBLK>(acc, slot16, (uint32_t)sc * 64u, sB16, b_lbo16, aoff, alo);
       if constexpr (MODE == 1) {
@@ -671,14 +665,6 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
               if constexpr (BIAS_REG) x[e] += bv[j][e];
               else x[e] += bias ? bias[co + e] : 0.f;
               if (g.relu) x[e] = fmaxf(x[e], 0.f);
-            }
-            if (g.has_res) {
-              uint32_t r;
-              if constexpr (RES_EARLY) r = rv[i][j];
-              else r = __ldg(reinterpret_cast<const unsigned int*>(res + pos + (co >> 3) * g.res_gs + (co & 7)));
-              float r0, r1;
-              unpack2<TOut>(r, r0, r1);
-              x[0] += r0; x[1] += r1;
             }
             store2<TOut>(out + e0, x[0], x[1]);
           }
@@ -884,6 +870,9 @@ inline Plan make_plan(int cin, int npad, int kd, int D, int H, int W, int pd, in
     // waits for the slowest warpgroup: tiles of 1 or an even number of chunks only
     lim.whole_rounds = conv_nwg(1, npad, 0);
   }
+  // the fused FPN tail (MODE 3, CIN 64) also loads the fine input's parity sub-tiles: boxes of 2P columns (TMA box
+  // dimensions <= 256)
+  if (mode == 3 && cin == 64) lim.p_max = 128;
   auto amp = [&](int R, int TW, int P, int DR) {
     return (double)(R + 2) / R * (double)P / TW * (kd == 3 ? (double)(DR + 2) / DR : (kd == 2 ? (double)(DR + 1) / DR : 1.0));
   };

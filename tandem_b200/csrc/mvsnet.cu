@@ -111,7 +111,8 @@ struct DevConv {
   bool tc_deconv = false;  // transposed conv evaluated as a GEMM over the input grid (N = 8 parity classes x cout)
   int nsplit = 1;          // N slices (blockIdx.y) for the 64-channel layers
   bool hilo = false;       // weights carried as hi + lo 16-bit halves (N doubled), see conv_tc.cuh
-  bool tc_up2 = false;     // MODE 3: conv3x3 of a nearest-x2 up-sampled map on the coarse grid (fused FPN tail)
+  bool tc_up2 = false;     // MODE 3: the fused FPN tail, conv3x3 of a nearest-x2 up-sampled map + conv3x3 of a fine map,
+                           // on the coarse grid
   bool tc_s2 = false;      // stride-2 conv on the tensor-map (strided TMA) kernel, conv_tc_s2.cuh
   void* bimg_s2 = nullptr;
   int npad_s2 = 0, nsplit_s2 = 1;
@@ -561,41 +562,43 @@ class MvsnetEngine final : public MvsnetIface {
 
   // Algebraic fusion of the FPN tail for stage 3 (module.py:522-530): feat3 = out3(up2(i2) + skip3(c3) + b3) is linear,
   //   feat3 = [conv3x3(W3) o up2](i2 + b3)  +  conv3x3(W3 . Ws3)(c3)
-  // (adding b3 to i2 BEFORE the zero-padded up-sampling reproduces the bias' border behaviour exactly).  The first term
-  // is evaluated on the coarse grid (4 output parity classes, the 3x3 fine taps pre-summed onto the 3x3 coarse
-  // neighbourhood), the second is an 8->8 conv on c3 that adds the first as its residual.  The 138 MB tensor i3 is never
-  // formed.
+  // (adding b3 to i2 BEFORE the zero-padded up-sampling reproduces the bias' border behaviour exactly).  Both terms are
+  // evaluated in one launch on the coarse grid (k_conv_tc MODE 3), one fp32 accumulator and one rounding per output: 4
+  // output parity classes, the 3x3 fine taps of the first pre-summed onto the 3x3 coarse neighbourhood, those of the
+  // second placed per coarse tap and sub-position of c3's space-to-depth view.  The 138 MB tensor i3 is never formed.
   void build_fused_fpn() {
     const std::string f = "feature_net.";
     const FoldedConv w3 = fold_conv(wf_, f + "out.stage3.weight", "", "", false);                        // [9][32][8]
     const FoldedConv ws = fold_conv(wf_, f + "skip.stage3.weight", f + "skip.stage3.bias", "", false);   // [1][8][32]
-    FoldedConv a;   // coarse-grid operator: [9 coarse taps][32][4 classes * 8]
-    a.cin = 32; a.cout = 32; a.kd = 1; a.kh = 3; a.kw = 3;
-    a.w.assign((size_t)9 * 32 * 32, 0.f);
-    auto coarse = [](int p, int k) { return p == 0 ? (k == 0 ? -1 : 0) : (k == 2 ? 1 : 0); };  // fine tap k of parity p -> coarse offset
+    std::vector<double> b((size_t)9 * 8 * 8, 0.0);   // W3 . Ws3 : [9 fine taps][8][8]
+    for (int t = 0; t < 9; ++t)
+      for (int ci = 0; ci < 8; ++ci)
+        for (int co = 0; co < 8; ++co)
+          for (int m = 0; m < 32; ++m) b[((size_t)t * 8 + ci) * 8 + co] += (double)w3.w[((size_t)t * 32 + m) * 8 + co] * (double)ws.w[(size_t)ci * 32 + m];
+    // coarse-grid operator [9 coarse taps][64][4 classes * 8]: input channels 0..31 are i2b, 32 + 8 q + c is channel c
+    // of c3's sub-position q = (qh, qw).  Fine tap k of parity p reads fine offset p + k - 1 = 2 delta + q.
+    FoldedConv a;
+    a.cin = 64; a.cout = 32; a.kd = 1; a.kh = 3; a.kw = 3;
+    a.w.assign((size_t)9 * 64 * 32, 0.f);
+    auto delta = [](int p, int k) { return p + k - 1 < 0 ? -1 : (p + k - 1) / 2; };
+    auto sub = [](int p, int k) { return (p + k + 1) % 2; };
     for (int ph = 0; ph < 2; ++ph)
       for (int pw = 0; pw < 2; ++pw)
         for (int kh = 0; kh < 3; ++kh)
           for (int kw = 0; kw < 3; ++kw) {
-            const int ta = (coarse(ph, kh) + 1) * 3 + (coarse(pw, kw) + 1);
-            for (int m = 0; m < 32; ++m)
-              for (int co = 0; co < 8; ++co)
-                a.w[((size_t)ta * 32 + m) * 32 + (ph * 2 + pw) * 8 + co] += w3.w[((size_t)(kh * 3 + kw) * 32 + m) * 8 + co];
+            const int ta = (delta(ph, kh) + 1) * 3 + (delta(pw, kw) + 1), n0 = (ph * 2 + pw) * 8;
+            const int ci0 = 32 + 8 * (sub(ph, kh) * 2 + sub(pw, kw));
+            for (int co = 0; co < 8; ++co) {
+              for (int m = 0; m < 32; ++m) a.w[((size_t)ta * 64 + m) * 32 + n0 + co] += w3.w[((size_t)(kh * 3 + kw) * 32 + m) * 8 + co];
+              for (int c = 0; c < 8; ++c) a.w[((size_t)ta * 64 + ci0 + c) * 32 + n0 + co] = (float)b[((size_t)(kh * 3 + kw) * 8 + c) * 8 + co];
+            }
           }
-    FoldedConv b;   // W3 . Ws3 : [9][8][8]
-    b.cin = 8; b.cout = 8; b.kd = 1; b.kh = 3; b.kw = 3;
-    b.w.assign((size_t)9 * 8 * 8, 0.f);
-    for (int t = 0; t < 9; ++t)
-      for (int ci = 0; ci < 8; ++ci)
-        for (int co = 0; co < 8; ++co) {
-          double acc = 0;
-          for (int m = 0; m < 32; ++m) acc += (double)w3.w[((size_t)t * 32 + m) * 8 + co] * (double)ws.w[(size_t)ci * 32 + m];
-          b.w[((size_t)t * 8 + ci) * 8 + co] = (float)acc;
-        }
-    add_conv("f.out3a", a);
-    convs_["f.out3a"].cout = 8;          // real channels per class; N = 4 classes x 8 = npad
-    convs_["f.out3a"].tc_up2 = true;
-    add_conv("f.out3b", b);
+    add_conv("f.fpn3", a);
+    DevConv& dc = convs_["f.fpn3"];
+    dc.cout = 8;          // real channels per class; N = 4 classes x 8 = npad
+    dc.npad = 32;
+    dc.hilo = dc.tc_ok = dc.tc_up2 = true;
+    upload_bimgs<TA>(a, dc);
     TDM_CUDA(cudaMalloc(&d_bs3_, 32 * 4));
     TDM_CUDA(cudaMemcpy(d_bs3_, ws.bias.data(), 32 * 4, cudaMemcpyHostToDevice));
     fused_fpn_ = true;
@@ -996,6 +999,8 @@ class MvsnetEngine final : public MvsnetIface {
   template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool PLAIN, int MODE = 0, bool HILO = false, typename Tail = tc::NoTail>
   void tc_inst(const std::string& wkey, const DevBuf& in, const DevConv& c, const DevBuf* res, const DevBuf& out, bool relu,
                const Tail& tail = Tail()) {
+    // res: MODE 1's skip operand (optional), MODE 3's fine input (f.c3)
+    TDM_CHECK(MODE == 1 || (MODE == 3) == (res != nullptr), wkey + ": MODE 3 takes a fine input, MODE 0 no residual");
     // FeatureNet layers run over V planes or, with the feature cache, over k: one plan and tensor map per plane count
     const TcCache& tcx = tc_cached(wkey + (Tail::enabled ? "#tail" : "") + "@" + std::to_string(in.D), [&] {
       TcCache x{};
@@ -1009,16 +1014,14 @@ class MvsnetEngine final : public MvsnetIface {
       g.relu = relu ? 1 : 0;
       g.has_res = res ? 1 : 0;
       g.cout = c.cout;
-      if constexpr (!PLAIN) {
-        g.out_gs = p8<TOut>(out).gs;
-        if (res) g.res_gs = p8<const TOut>(*res).gs;
-      }
-      x.tmap = p8_tmap<TIn>(wkey, in, CIN / 8, g.iDp, g.P, g.R + 2, 1);
-      x.tmap_res = x.tmap_out = x.tmap;   // read by MODE 1 only
+      if constexpr (!PLAIN) g.out_gs = p8<TOut>(out).gs;
+      x.tmap = p8_tmap<TIn>(wkey, in, MODE == 3 ? 4 : CIN / 8, g.iDp, g.P, g.R + 2, 1);
+      x.tmap_res = x.tmap_out = x.tmap;   // read by MODE 1 and 3 only
       if constexpr (MODE == 1) {
         x.tmap_out = p8_interior_tmap(wkey, out, g.TW, g.R, NPAD / 64);
         if (res) x.tmap_res = p8_interior_tmap(wkey, *res, g.TW, g.R, NPAD / 64);
       }
+      if constexpr (MODE == 3) x.tmap_res = p8_tmap<TIn>(wkey, *res, 1, res->D, 2 * g.P, 2 * (g.R + 2), 2);
       debug_plan(wkey, "mode " + std::to_string(MODE) + " cin " + std::to_string(CIN) + " N " + std::to_string(HILO ? 2 * NPAD : NPAD) +
                  " kd " + std::to_string(KD) + " in", g, x.plan.grid, c.nsplit, x.plan.smem);
       return x;
@@ -1026,13 +1029,8 @@ class MvsnetEngine final : public MvsnetIface {
     const tc::Plan& pl = tcx.plan;
     TOut* op = nullptr;
     float* plain = nullptr;
-    const TOut* rp = nullptr;
-    if constexpr (PLAIN) {
-      plain = (float*)out.p;
-    } else {
-      op = (TOut*)out.p;
-      if (res) rp = (const TOut*)res->p;
-    }
+    if constexpr (PLAIN) plain = (float*)out.p;
+    else op = (TOut*)out.p;
     constexpr int NWG = tc::conv_nwg(MODE, HILO ? 2 * NPAD : NPAD, Tail::max_d);
     TDM_CHECK(pl.nwg == NWG, wkey + ": tile plan balanced for another warpgroup count than the kernel's");
     // MODE 1: each N slice of NPAD columns is 8 classes x NPAD / 8 channels, whole output channel groups of the box;
@@ -1042,7 +1040,7 @@ class MvsnetEngine final : public MvsnetIface {
     TDM_CHECK(MODE != 1 || (out.pd == 1 && (!res || (res->D == out.D && res->H == out.H && res->W == out.W && res->C == out.C))),
               wkey + ": transposed conv skip / output shapes differ");
     launch_tc<tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail, NWG>>(dim3(pl.grid, c.nsplit), pl.smem, tcx.tmap, tcx.tmap_res, tcx.tmap_out, (const TIn*)c.bimg,
-                                                                              (const float*)c.bias, rp, op, plain, pl.g, tail);
+                                                                              (const float*)c.bias, op, plain, pl.g, tail);
   }
 
   template <int CIN, int NPAD, int KD, int KS>
@@ -1098,6 +1096,7 @@ class MvsnetEngine final : public MvsnetIface {
         if (c.cin == 64) { tc_inst<TA, TA, 64, 64, 2, false, 1>(wkey, bi, c, rp, bo, relu); return true; }
         return false;
       }
+      if (rp) return false;   // the stride-1 kernel adds no residual
 #define TDM_TC(TI, CI, NP, KDV, HL)                                                        \
   if (c.cin == CI && c.npad == NP && c.kd == KDV && c.hilo == HL) {                        \
     tc_inst<TI, TA, CI, NP, KDV, false, 0, HL>(wkey, bi, c, rp, bo, relu);                       \
@@ -1152,18 +1151,23 @@ class MvsnetEngine final : public MvsnetIface {
     }
   }
 
-  void conv_up2(const std::string& wkey, const std::string& in, const std::string& out) {
+  // feat3 of the fused FPN tail (build_fused_fpn) from the coarse map `coarse` (f.i2b) and the fine map `fine` (f.c3)
+  void conv_fpn3(const std::string& wkey, const std::string& coarse, const std::string& fine, const std::string& out) {
     if constexpr (sizeof(TA) == 2) {
       const DevConv& c = convs_.at(wkey);
-      const DevBuf& bi = bufs_.at(in);
+      const DevBuf& bi = bufs_.at(coarse);
+      const DevBuf& bf = bufs_.at(fine);
       const DevBuf& bo = bufs_.at(out);
-      TDM_CHECK(c.tc_up2 && bo.H == 2 * bi.H && bo.W == 2 * bi.W && bo.D == bi.D, "conv_up2 shape mismatch");
-      rec_begin(wkey + "[tc-up2]", (double)bi.alg_bytes + (double)bo.alg_bytes, 2.0 * 9 * 32 * 8 * (double)bo.D * bo.H * bo.W);
-      tc_inst<TA, TA, 32, 32, 1, false, 3, true>(wkey, bi, c, nullptr, bo, false);
+      TDM_CHECK(c.tc_up2 && bo.H == 2 * bi.H && bo.W == 2 * bi.W && bo.D == bi.D && bi.C == 32 && bi.pd == 0 &&
+                    bf.C == 8 && bf.pd == 0 && bf.D == bo.D && bf.H == bo.H && bf.W == bo.W,
+                "conv_fpn3 shape mismatch");
+      rec_begin(wkey + "[tc-up2]", (double)bi.alg_bytes + (double)bf.alg_bytes + (double)bo.alg_bytes,
+                2.0 * 9 * (32 + 8) * 8 * (double)bo.D * bo.H * bo.W);
+      tc_inst<TA, TA, 64, 32, 1, false, 3, true>(wkey, bi, c, &bf, bo, false);
       TDM_CUDA(cudaGetLastError());
       rec_end();
     } else {
-      throw Error("conv_up2 needs a 16-bit engine");
+      throw Error("conv_fpn3 needs a 16-bit engine");
     }
   }
 
@@ -1521,8 +1525,7 @@ class MvsnetEngine final : public MvsnetIface {
     if (fused_fpn_ && use_tc_) {
       conv("f.skip2", fb("f.c2"), fb("f.i2"), 1, 1, 1, false, 2, fb("f.c1"), fb("f.i2b"), d_bs3_);
       conv("f.out2", fb("f.i2"), fb("feat2"), 1, 1, 1, false);
-      conv_up2("f.out3a", fb("f.i2b"), fb("feat3"));
-      conv("f.out3b", fb("f.c3"), fb("feat3"), 1, 1, 1, false, 1, fb("feat3"));
+      conv_fpn3("f.fpn3", fb("f.i2b"), fb("f.c3"), fb("feat3"));
     } else {
       conv("f.skip2", fb("f.c2"), fb("f.i2"), 1, 1, 1, false, 2, fb("f.c1"));
       conv("f.out2", fb("f.i2"), fb("feat2"), 1, 1, 1, false);
