@@ -105,6 +105,18 @@ public:
                                         float lambdaExtrapolationLimit, float affineOptModeA, float affineOptModeB,
                                         Eigen::Matrix<double, 5, 1> const &lastCoarseRMSE, float reTrackThreshold);
 
+  // Extension: CoarseTracker::setCoarseTrackingRef including makeCoarseDepthL0 (CoarseTracker.cpp:148-374, :633-733) for the
+  // trackers of levels 0..n-1 (the ones trackPyramid takes) in one call: the points the reference's loop uses, in its order
+  // (monocular: centerProjectedTo and efPoint->HdiF; rgbd_init: ph->u, ph->v, ph->idepth, ph->idepth_hessian), the colours from
+  // the keyframe's pyramid, and, when fusion is not null, the dense append of its render_index-th render.  Every level then
+  // holds its reference as after setReference.  Returns pc_n per level; throws std::runtime_error on invalid input.
+  static std::vector<int> setCoarseTrackingRef(std::vector<CudaCoarseTracker *> const &levels, bool rgbd_init, int n_points,
+                                               float const *pt_u, float const *pt_v, float const *pt_idepth,
+                                               float const *pt_hessian, tdm_pyramid *ref_pyramid, tdm_fusion *fusion,
+                                               int render_index, Eigen::Matrix<double, 4, 4> const &T_depth_to_ref,
+                                               int tracking_step, bool dense_only, float ref_exposure,
+                                               Eigen::Vector2d const &ref_aff);
+
   void synchronize();
 
   void startTiming();

@@ -407,6 +407,28 @@ int tdm_tracker_track_new_coarse(tdm_tracker* const* levels, int coarsest_level,
                                  const double last_coarse_rmse[5], float retrack_threshold, tdm_track_new_coarse_result* out,
                                  tdm_track_try* tries_out);
 
+/* n7  CoarseTracker::setCoarseTrackingRef (tandem/src/FullSystem/CoarseTracker.cpp:633-733) including makeCoarseDepthL0
+ *     (:148-374), for the trackers of levels 0..n_levels-1 ((w0>>l) x (h0>>l), as tdm_tracker_track_pyramid expects them) in
+ *     one call on levels[0]'s stream.  The points are the ones the reference uses, in its order (frameHessians x
+ *     pointHessians): rgbd_init == 0, those passing the lastResiduals[0] / ResState::IN test of :157 with pt_u/v/idepth =
+ *     centerProjectedTo[0..2] and pt_hessian = efPoint->HdiF; rgbd_init == 1, ph->u, ph->v, ph->idepth, ph->idepth_hessian.
+ *     Scatter (several points on one pixel are summed in input order), 2x2 sum pyramid, dilation, normalise-and-compact per
+ *     level with the colours dIp[l][i][0] of ref_pyramid; then, with a dense map (host `depth` or the render_index-th render of
+ *     depth_from_fusion, as in tdm_tracker_set_reference_dense; both NULL: none) n1's dense append behind level 0's points.
+ *     Like the reference's arrays, a tracker's reference arrays persist across calls: slot pc_n[l] keeps the last candidate the
+ *     reference wrote there and rejected, or what it held before.  Every level then holds pc_n[l] points with ref_exposure and
+ *     ref_aff_g2l, as after setReference.  Blocking, one host wait; ordered after the pending work of every level's stream, the
+ *     pyramid's build and the render.  Invalid input (null handles or arrays that are needed, n_levels outside 1..5, wrong level
+ *     sizes, no setK on level 0, a pyramid with fewer levels or another level-0 size, different devices, a point whose rounded
+ *     pixel - (int)(u + 0.5f) monocular, (int)(u + 0.5) RGB-D - lies outside the level-0 image) is an error and launches
+ *     nothing.  A level whose n_max cannot hold its points and the slot behind them is an error found after the launch; every
+ *     level's reference is then empty. */
+int tdm_tracker_set_coarse_tracking_ref(tdm_tracker* const* levels, int n_levels, int rgbd_init, int n_points, const float* pt_u,
+                                        const float* pt_v, const float* pt_idepth, const float* pt_hessian, tdm_pyramid* ref_pyramid,
+                                        const float* depth, tdm_fusion* depth_from_fusion, int render_index,
+                                        const double T_depth_to_ref[16], int tracking_step, int dense_only, float ref_exposure,
+                                        const double ref_aff_g2l[2], int pc_n[5]);
+
 #ifdef __cplusplus
 }
 #endif

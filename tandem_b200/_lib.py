@@ -164,6 +164,7 @@ def _declare(l):
         "tdm_tracker_track": (i, [vp, dp, dp, f, f, i, f, i, i, P(TrackResult)]),
         "tdm_tracker_track_pyramid": (i, [P(vp), i, dp, dp, f, f, ip, f, f, f, dp, P(TrackPyramidResult)]),
         "tdm_tracker_track_new_coarse": (i, [P(vp), i, dp, i, dp, f, f, ip, f, f, f, dp, f, P(TrackNewCoarseResult), P(TrackTry)]),
+        "tdm_tracker_set_coarse_tracking_ref": (i, [P(vp), i, i, i, fp, fp, fp, fp, vp, fp, vp, i, dp, i, i, f, dp, ip]),
     }
     missing = []
     for name, (res, args) in sigs.items():

@@ -274,4 +274,39 @@ int tdm_tracker_track_new_coarse(tdm_tracker* const* levels, int coarsest_level,
   TDM_API_END
 }
 
+/* ---- SURVEY 8(f) n7: CoarseTracker::setCoarseTrackingRef with makeCoarseDepthL0, every level on the device ---- */
+int tdm_tracker_set_coarse_tracking_ref(tdm_tracker* const* levels, int n_levels, int rgbd_init, int n_points, const float* pt_u,
+                                        const float* pt_v, const float* pt_idepth, const float* pt_hessian, tdm_pyramid* ref_pyramid,
+                                        const float* depth, tdm_fusion* depth_from_fusion, int render_index,
+                                        const double T_depth_to_ref[16], int tracking_step, int dense_only, float ref_exposure,
+                                        const double ref_aff_g2l[2], int pc_n[5]) {
+  TDM_API_BEGIN
+  TDM_CHECK(levels && ref_pyramid && ref_aff_g2l && pc_n, "null argument");
+  TDM_CHECK(n_levels >= 1 && n_levels <= 5, "n_levels must be in 1..5");
+  TDM_CHECK(!(depth && depth_from_fusion), "pass at most one of depth / depth_from_fusion");
+  tdm::TrackerIface* impl[5] = {};
+  for (int l = 0; l < n_levels; ++l) {
+    TDM_CHECK(levels[l], "set_coarse_tracking_ref level " + std::to_string(l) + ": null tracker");
+    impl[l] = levels[l]->impl;
+  }
+  tdm::TrackerIface::CoarseRefArgs a;
+  a.n_levels = n_levels; a.rgbd_init = rgbd_init != 0; a.n_points = n_points;
+  a.pt_u = pt_u; a.pt_v = pt_v; a.pt_idepth = pt_idepth; a.pt_hessian = pt_hessian;
+  a.ref_pyramid = ref_pyramid->impl;
+  if (depth_from_fusion) {
+    TDM_CHECK(T_depth_to_ref, "dense map without T_depth_to_ref");
+    int dev = -1;
+    a.depth = depth_from_fusion->impl->render_depth_device(render_index, &a.depth_ready, &dev);
+    a.depth_on_device = true;
+    TDM_CHECK(dev == impl[0]->device(), "fusion and tracker live on different devices");
+  } else {
+    a.depth = depth;
+  }
+  a.T_depth_to_ref = T_depth_to_ref; a.step = tracking_step; a.dense_only = dense_only;
+  a.ref_exposure = ref_exposure; a.ref_aff = ref_aff_g2l;
+  impl[0]->set_coarse_tracking_ref(impl, a, pc_n);
+  return TDM_OK;
+  TDM_API_END
+}
+
 }  // extern "C"

@@ -12,7 +12,10 @@
 // deterministic (the reference's float atomics are not), one launch, no memset, no D2H copy.
 #include <cmath>
 #include <cstring>
+#include <string>
 #include <vector>
+
+#include <cub/device/device_radix_sort.cuh>
 
 #include "tracker.h"
 
@@ -366,37 +369,103 @@ __global__ void k_dense_warp(const float* __restrict__ depth, int w, int h, int 
   if (pu > w - 4 || pv > h - 4 || pu < 3 || pv < 3) return;
   atomicMin(proj + pu + (size_t)pv * w, __float_as_uint(p[2]));
 }
-__device__ __forceinline__ bool dense_take(const unsigned* proj, const float* idepth0, int dense_only, int i) {
-  return proj[i] != 0xFFFFFFFFu && (dense_only || !idepth0 || idepth0[i] <= 0.f);
-}
-__global__ void __launch_bounds__(256) k_dense_rowcount(const unsigned* __restrict__ proj, const float* __restrict__ idepth0,
-                                                         int dense_only, int w, int h, int* __restrict__ rowcnt) {
+// The raster-order compaction (row counts -> row offsets -> ordered intra-row emit) is shared with n7's normalise-and-compact
+// pass: a selector classifies each pixel of [2, w-2) x [2, h-2) as 0 (skip), 1 (append) or 2 (a candidate the reference writes
+// to slot pc_n and then rejects, n7 only) and writes the point of an appended pixel.
+struct DenseSel {             // n1: the hit pixels of the warp that the sparse image leaves free
+  static constexpr bool kStale = false;
+  const unsigned* proj;
+  const float* idepth0;
+  int dense_only;
+  const float* gray;
+  int gstride;
+  __device__ __forceinline__ int cls(int i) const {
+    return proj[i] != 0xFFFFFFFFu && (dense_only || !idepth0 || idepth0[i] <= 0.f) ? 1 : 0;
+  }
+  __device__ __forceinline__ void emit(int o, int x, int y, int i, float* pc_u, float* pc_v, float* pc_idepth, float* pc_color) const {
+    pc_u[o] = (float)x;
+    pc_v[o] = (float)y;
+    pc_idepth[o] = __fdiv_rn(1.f, __uint_as_float(proj[i]));
+    pc_color[o] = gray[(size_t)i * gstride];
+  }
+  __device__ __forceinline__ void finish(int, int) const {}
+};
+struct NormSel {              // n7: CoarseTracker.cpp:346-370 on one level (idepth normalised in place, rejected -> -1)
+  static constexpr bool kStale = true;
+  float* idepth;
+  const float* wsum;
+  const float* gray;          // the level's (I, dx, dy) image
+  __device__ __forceinline__ int cls(int i) const {
+    if (!(wsum[i] > 0.f)) return 0;
+    const float d = __fdiv_rn(idepth[i], wsum[i]);
+    return isfinite(gray[3 * (size_t)i]) && d > 0.f ? 1 : 2;
+  }
+  __device__ __forceinline__ void emit(int o, int x, int y, int i, float* pc_u, float* pc_v, float* pc_idepth, float* pc_color) const {
+    pc_u[o] = (float)x;
+    pc_v[o] = (float)y;
+    pc_idepth[o] = __fdiv_rn(idepth[i], wsum[i]);
+    pc_color[o] = gray[3 * (size_t)i];
+  }
+  __device__ __forceinline__ void finish(int i, int c) const {   // after every read of pixel i (only its own thread reads it)
+    idepth[i] = c == 1 ? __fdiv_rn(idepth[i], wsum[i]) : -1.f;
+  }
+};
+// rowlast[y] = (last x of class 1, last x of class 2) in row y, -1 for none; only for selectors with kStale
+template <class Sel>
+__global__ void __launch_bounds__(256) k_compact_rowcount(Sel s, int w, int h, int* __restrict__ rowcnt, int2* __restrict__ rowlast) {
   const int y = blockIdx.x;
-  int c = 0;
+  int c = 0, la = 0, lr = 0;   // last x + 1
   if (y >= 2 && y < h - 2)
-    for (int x = 2 + threadIdx.x; x < w - 2; x += 256) c += dense_take(proj, idepth0, dense_only, x + y * w) ? 1 : 0;
-  __shared__ int sm[8];
+    for (int x = 2 + threadIdx.x; x < w - 2; x += 256) {
+      const int k = s.cls(x + y * w);
+      c += k == 1 ? 1 : 0;
+      if (Sel::kStale) {
+        if (k == 1) la = x + 1;
+        if (k == 2) lr = x + 1;
+      }
+    }
+  __shared__ int sm[3][8];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = c;
+  if (Sel::kStale) {
+    la = __reduce_max_sync(0xffffffffu, (unsigned)la);
+    lr = __reduce_max_sync(0xffffffffu, (unsigned)lr);
+  }
+  if ((threadIdx.x & 31) == 0) { sm[0][threadIdx.x >> 5] = c; sm[1][threadIdx.x >> 5] = la; sm[2][threadIdx.x >> 5] = lr; }
   __syncthreads();
   if (threadIdx.x == 0) {
-    int s = 0;
-    for (int k = 0; k < 8; ++k) s += sm[k];
-    rowcnt[y] = s;
+    int t = 0, a = 0, r = 0;
+    for (int k = 0; k < 8; ++k) { t += sm[0][k]; a = max(a, sm[1][k]); r = max(r, sm[2][k]); }
+    rowcnt[y] = t;
+    if (Sel::kStale) rowlast[y] = make_int2(a - 1, r - 1);
   }
 }
-__global__ void k_dense_rowscan(const int* __restrict__ rowcnt, int h, int* __restrict__ rowoff, int* __restrict__ total_out) {
+// rowoff[y] = (*start, or 0) + the counts of the rows above; *total_out = the count of all rows.  With rowlast: *stale_out = the
+// raster index of the last class-2 pixel behind the last class-1 pixel (the candidate left in slot pc_n), -1 for none.
+__global__ void k_compact_rowscan(const int* __restrict__ rowcnt, const int2* __restrict__ rowlast, int w, int h,
+                                  const int* __restrict__ start, int* __restrict__ rowoff, int* __restrict__ total_out,
+                                  int* __restrict__ stale_out) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  int s = 0;
-  for (int y = 0; y < h; ++y) { rowoff[y] = s; s += rowcnt[y]; }
-  *total_out = s;
+  const int s0 = start ? *start : 0;
+  int s = s0, la = -1, lr = -1;
+  for (int y = 0; y < h; ++y) {
+    rowoff[y] = s;
+    s += rowcnt[y];
+    if (rowlast && y >= 2 && y < h - 2) {
+      if (rowlast[y].x >= 0) la = rowlast[y].x + y * w;
+      if (rowlast[y].y >= 0) lr = rowlast[y].y + y * w;
+    }
+  }
+  *total_out = s - s0;
+  if (stale_out) *stale_out = lr > la ? lr : -1;
 }
-__global__ void __launch_bounds__(256) k_dense_emit(const unsigned* __restrict__ proj, const float* __restrict__ idepth0,
-                                                     int dense_only, int w, int h, const int* __restrict__ rowoff,
-                                                     const float* __restrict__ gray, int gstride, int first,
-                                                     float* __restrict__ pc_u, float* __restrict__ pc_v,
-                                                     float* __restrict__ pc_idepth, float* __restrict__ pc_color) {
+// Points go to slots first + rowoff[y] + (rank in the row), those at or beyond cap are dropped (the caller checks the count
+// against its capacity afterwards).  With kStale the class-2 pixel *stale goes to slot *total.
+template <class Sel>
+__global__ void __launch_bounds__(256) k_compact_emit(Sel s, int w, int h, const int* __restrict__ rowoff, int first, int cap,
+                                                       const int* __restrict__ stale, const int* __restrict__ total,
+                                                       float* __restrict__ pc_u, float* __restrict__ pc_v,
+                                                       float* __restrict__ pc_idepth, float* __restrict__ pc_color) {
   const int y = blockIdx.x;
   if (y < 2 || y >= h - 2) return;
   __shared__ int wsum[8];
@@ -407,7 +476,8 @@ __global__ void __launch_bounds__(256) k_dense_emit(const unsigned* __restrict__
   for (int x0 = 2; x0 < w - 2; x0 += 256) {
     const int x = x0 + threadIdx.x;
     const int i = x + y * w;
-    const bool take = x < w - 2 && dense_take(proj, idepth0, dense_only, i);
+    const int c = x < w - 2 ? s.cls(i) : 0;
+    const bool take = c == 1;
     const unsigned bal = __ballot_sync(0xffffffffu, take);
     if (lane == 0) wsum[warp] = __popc(bal);
     __syncthreads();
@@ -416,15 +486,79 @@ __global__ void __launch_bounds__(256) k_dense_emit(const unsigned* __restrict__
     for (int k = 0; k < 8; ++k) { before += k < warp ? wsum[k] : 0; all += wsum[k]; }
     if (take) {
       const int o = base + before + __popc(bal & ((1u << lane) - 1u));
-      pc_u[o] = (float)x;
-      pc_v[o] = (float)y;
-      pc_idepth[o] = __fdiv_rn(1.f, __uint_as_float(proj[i]));
-      pc_color[o] = gray[(size_t)i * gstride];
+      if (o < cap) s.emit(o, x, y, i, pc_u, pc_v, pc_idepth, pc_color);
     }
+    if (Sel::kStale && c == 2 && i == *stale && *total < cap) s.emit(*total, x, y, i, pc_u, pc_v, pc_idepth, pc_color);
+    if (Sel::kStale && x < w - 2) s.finish(i, c);
     __syncthreads();
     if (threadIdx.x == 0) base += all;
     __syncthreads();
   }
+}
+
+// ================================================================================================
+// n7 (SURVEY 8f): CoarseTracker::makeCoarseDepthL0 (CoarseTracker.cpp:148-374) on the device, every level, then n1's dense
+// append on level 0 (setCoarseTrackingRef, :633-733).  Every float operation is the reference's, correctly rounded.
+// ================================================================================================
+// Scatter (:155-182): the points arrive sorted by (pixel, input index) - a stable radix sort of the pixel keys - and each
+// pixel's run is summed sequentially in input order, so the sums do not depend on scheduling.  a = centerProjectedTo[2] or
+// ph->idepth, b = HdiF (monocular) or idepth_hessian (RGB-D).
+__global__ void k_coarse_scatter(const int* __restrict__ pix, const int* __restrict__ order, const float* __restrict__ a,
+                                 const float* __restrict__ b, int n, int rgbd, float* __restrict__ idepth, float* __restrict__ wsum) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n || (k > 0 && pix[k - 1] == pix[k])) return;
+  const int p = pix[k];
+  float s = 0.f, ws = 0.f;
+  for (int j = k; j < n && pix[j] == p; ++j) {
+    const int q = order[j];
+    // sqrtf(1e-3 / (HdiF + 1e-12)): double literals, so the quotient is a double narrowed to float for sqrtf
+    const float wt = rgbd ? b[q] : __fsqrt_rn(__double2float_rn(__ddiv_rn(1e-3, __dadd_rn((double)b[q], 1e-12))));
+    s = __fadd_rn(s, __fmul_rn(a[q], wt));
+    ws = __fadd_rn(ws, wt);
+  }
+  idepth[p] = s;
+  wsum[p] = ws;
+}
+// Sum pyramid (:222-243): level l from the un-dilated level l-1, a + b + c + d left to right.
+__global__ void k_coarse_sum(const float* __restrict__ id_lm, const float* __restrict__ ws_lm, int wlm1, float* __restrict__ id_l,
+                             float* __restrict__ ws_l, int wl, int hl) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= wl * hl) return;
+  const int y = i / wl, x = i - y * wl, b = 2 * x + 2 * y * wlm1;
+  id_l[i] = __fadd_rn(__fadd_rn(__fadd_rn(id_lm[b], id_lm[b + 1]), id_lm[b + wlm1]), id_lm[b + wlm1 + 1]);
+  ws_l[i] = __fadd_rn(__fadd_rn(__fadd_rn(ws_lm[b], ws_lm[b + 1]), ws_lm[b + wlm1]), ws_lm[b + wlm1 + 1]);
+}
+// Dilation (:246-322) over the flat range [w, w*h - w): a pixel without weight takes the mean of its weighted neighbours - the
+// 4 diagonal ones on levels 0 and 1, the 4 axis ones above - read from the pre-dilation weights wbak (so column 0 and w-1 see
+// the neighbouring rows).  idepth is updated in place (only pixels with wbak <= 0 are written, only pixels with wbak > 0 are
+// read), the weights go to wout.  On levels 0 / 1 the first and the last pixel of the range have one diagonal neighbour outside
+// the image (index -1 and w*h, the padding of the reference's allocation): it counts as unweighted.
+template <bool kDiag>
+__global__ void k_coarse_dilate(float* __restrict__ idepth, const float* __restrict__ wbak, float* __restrict__ wout, int w, int h) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int n = w * h;
+  if (i >= n) return;
+  float wi = wbak[i];
+  if (i >= w && i < n - w && wi <= 0.f) {
+    const int nb[4] = {kDiag ? i + 1 + w : i + 1, kDiag ? i - 1 - w : i - 1, kDiag ? i + w - 1 : i + w, kDiag ? i - w + 1 : i - w};
+    float sum = 0.f, num = 0.f, numn = 0.f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int j = nb[k];
+      if (j < 0 || j >= n) continue;
+      const float wj = wbak[j];
+      if (wj > 0.f) {
+        sum = __fadd_rn(sum, idepth[j]);
+        num = __fadd_rn(num, wj);
+        numn = __fadd_rn(numn, 1.f);
+      }
+    }
+    if (numn > 0.f) {
+      idepth[i] = __fdiv_rn(sum, numn);
+      wi = __fdiv_rn(num, numn);
+    }
+  }
+  wout[i] = wi;
 }
 
 // ================================================================================================
@@ -747,6 +881,7 @@ class TrackerImpl final : public TrackerIface {
     TDM_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
     TDM_CUDA(cudaStreamCreateWithPriority(&stream_, cudaStreamNonBlocking, hi));  // highest priority (cpp:72-74)
     TDM_CUDA(cudaMalloc(&d_pc_, (size_t)4 * n_max_ * 4));
+    TDM_CUDA(cudaMemset(d_pc_, 0, (size_t)4 * n_max_ * 4));   // like the reference's arrays, they persist across references
     TDM_CUDA(cudaMalloc(&d_warped_, (size_t)7 * n_max_ * 4));
     TDM_CUDA(cudaMemset(d_warped_, 0, (size_t)7 * n_max_ * 4));
     TDM_CUDA(cudaMalloc(&d_dI_, (size_t)3 * w * h * 4));
@@ -766,6 +901,9 @@ class TrackerImpl final : public TrackerIface {
     if (d_batch_) { cudaFree(d_batch_); cudaFreeHost(h_batch_); cudaFree(d_batch_partials_); cudaFree(d_batch_ticket_); cudaFreeHost(h_batch_out_); }
     cudaFree(d_proj_); cudaFree(d_depth_); cudaFree(d_idepth0_); cudaFree(d_gray_); cudaFree(d_rowcnt_); cudaFree(d_rowoff_);
     cudaFree(d_total_); cudaFree(d_lm_ctx_); cudaFree(d_lm_out_);
+    cudaFree(d_coarse_); cudaFree(d_rowlast_); cudaFree(d_coarse_cnt_); cudaFree(d_coarse_stale_); cudaFree(d_pts_); cudaFree(d_coarse_tmp_);
+    if (h_coarse_cnt_) cudaFreeHost(h_coarse_cnt_);
+    if (h_pts_) cudaFreeHost(h_pts_);
     if (lm_exec_) cudaGraphExecDestroy(lm_exec_);
     for (cudaEvent_t e : {lm_in_free_, lm_e0_, lm_e1_, ready_})
       if (e) cudaEventDestroy(e);
@@ -884,38 +1022,13 @@ class TrackerImpl final : public TrackerIface {
     } else if (a.gray_ready) {
       TDM_CUDA(cudaStreamWaitEvent(stream_, (cudaEvent_t)a.gray_ready, 0));
     }
-    // KRKi = (K R) Ki, Kt = K t in float, k = 0,1,2 (CoarseTracker.cpp:676-677)
-    DenseWarp m;
-    {
-      const float K[9] = {fx_, 0, cx_, 0, fy_, cy_, 0, 0, 1};
-      const float Ki[9] = {1.0f / fx_, 0, -cx_ / fx_, 0, 1.0f / fy_, -cy_ / fy_, 0, 0, 1};
-      float R[9], t[3], KR[9];
-      for (int r = 0; r < 3; ++r) {
-        for (int c = 0; c < 3; ++c) R[3 * r + c] = (float)a.T_depth_to_ref[4 * r + c];
-        t[r] = (float)a.T_depth_to_ref[4 * r + 3];
-      }
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) {
-          volatile float s = 0;
-          for (int k = 0; k < 3; ++k) { volatile float q = K[3 * r + k] * R[3 * k + c]; s = s + q; }
-          KR[3 * r + c] = s;
-        }
-      for (int r = 0; r < 3; ++r) {
-        for (int c = 0; c < 3; ++c) {
-          volatile float s = 0;
-          for (int k = 0; k < 3; ++k) { volatile float q = KR[3 * r + k] * Ki[3 * k + c]; s = s + q; }
-          m.KRKi[3 * r + c] = s;
-        }
-        volatile float s = 0;
-        for (int k = 0; k < 3; ++k) { volatile float q = K[3 * r + k] * t[k]; s = s + q; }
-        m.Kt[r] = s;
-      }
-    }
+    const DenseWarp m = dense_warp(a.T_depth_to_ref);
     TDM_CUDA(cudaMemsetAsync(d_proj_, 0xFF, 4 * npx, stream_));
     const int nx = (w_ + a.step - 1) / a.step, ny = (h_ + a.step - 1) / a.step;
     k_dense_warp<<<(nx * ny + 255) / 256, 256, 0, stream_>>>(d_depth, w_, h_, a.step, m, d_proj_);
-    k_dense_rowcount<<<h_, 256, 0, stream_>>>(d_proj_, d_id0, a.dense_only, w_, h_, d_rowcnt_);
-    k_dense_rowscan<<<1, 32, 0, stream_>>>(d_rowcnt_, h_, d_rowoff_, d_total_);
+    const DenseSel sel{d_proj_, d_id0, a.dense_only, d_gray, gstride};
+    k_compact_rowcount<<<h_, 256, 0, stream_>>>(sel, w_, h_, d_rowcnt_, nullptr);
+    k_compact_rowscan<<<1, 32, 0, stream_>>>(d_rowcnt_, nullptr, w_, h_, nullptr, d_rowoff_, d_total_, nullptr);
     TDM_CUDA(cudaMemcpyAsync(h_total_, d_total_, 4, cudaMemcpyDeviceToHost, stream_));
     TDM_CUDA(cudaGetLastError());
     TDM_CUDA(cudaStreamSynchronize(stream_));
@@ -932,8 +1045,8 @@ class TrackerImpl final : public TrackerIface {
         TDM_CUDA(cudaMemsetAsync(d_pc_ + k * nm, 0, 4, stream_));
       }
     }
-    k_dense_emit<<<h_, 256, 0, stream_>>>(d_proj_, d_id0, a.dense_only, w_, h_, d_rowoff_, d_gray, gstride, a.n_sparse + 1,
-                                          d_pc_, d_pc_ + nm, d_pc_ + 2 * nm, d_pc_ + 3 * nm);
+    k_compact_emit<<<h_, 256, 0, stream_>>>(sel, w_, h_, d_rowoff_, a.n_sparse + 1, n_max_, nullptr, nullptr,
+                                            d_pc_, d_pc_ + nm, d_pc_ + 2 * nm, d_pc_ + 3 * nm);
     TDM_CUDA(cudaGetLastError());
     n_ = a.n_sparse + total;      // the pre-increment quirk: the last appended point is not counted
     ref_exposure_ = a.ref_exposure;
@@ -1035,6 +1148,143 @@ class TrackerImpl final : public TrackerIface {
         tries[k].ok = t.ok; tries[k].aborted_level = t.aborted_level; tries[k].repeated_level = t.repeated_level;
       }
   }
+  // ---------------------------------------------------------------------------------------------- n7
+  void set_coarse_tracking_ref(TrackerIface* const* levels, const CoarseRefArgs& a, int pc_n[kMaxLevels]) override {
+    TDM_CHECK(levels && a.ref_pyramid && a.ref_aff && pc_n, "null argument");
+    TDM_CHECK(a.n_levels >= 1 && a.n_levels <= kMaxLevels, "n_levels must be in 1..5");
+    TDM_CHECK(a.n_points >= 0, "negative point count");
+    TDM_CHECK(a.n_points == 0 || (a.pt_u && a.pt_v && a.pt_idepth && a.pt_hessian), "point arrays missing");
+    TDM_CHECK(!a.depth || (a.T_depth_to_ref && a.step >= 1), "dense map without T_depth_to_ref, or bad tracking step");
+    const int L = a.n_levels;
+    TrackerImpl* lv[kMaxLevels] = {};
+    for (int l = 0; l < L; ++l) {
+      const std::string at = "set_coarse_tracking_ref level " + std::to_string(l) + ": ";
+      TDM_CHECK(levels[l], at + "null tracker");
+      lv[l] = dynamic_cast<TrackerImpl*>(levels[l]);
+      TDM_CHECK(lv[l], at + "not a tracker of this library");
+      TDM_CHECK(lv[l]->w_ == (w_ >> l) && lv[l]->h_ == (h_ >> l), at + "size must be level 0's size >> level");
+      TDM_CHECK(lv[l]->device_ == device_, at + "trackers live on different devices");
+    }
+    TDM_CHECK(have_k_, "set_coarse_tracking_ref level 0: setK missing (the dense part needs K[0])");
+    const PyramidIface& P = *a.ref_pyramid;
+    TDM_CHECK(P.levels() >= L && P.width(0) == w_ && P.height(0) == h_, "reference pyramid: too few levels or another level-0 size");
+    TDM_CHECK(P.device() == device_, "pyramid and tracker live on different devices");
+    TDM_CUDA(cudaSetDevice(device_));
+    ensure_front_buffers();
+    ensure_coarse_buffers(a.n_points);
+    // Pack (pixel, input index, value, weight input) and check the pixels: the reference would write outside idepth[0] there.
+    const int n = a.n_points;
+    const size_t cap = (size_t)coarse_cap_;
+    int* pk = reinterpret_cast<int*>(h_pts_);
+    for (int k = 0; k < n; ++k) {
+      int u, v;
+      if (a.rgbd_init) {   // int u = ph->u + 0.5 (double)
+        const double fu = (double)a.pt_u[k] + 0.5, fv = (double)a.pt_v[k] + 0.5;
+        TDM_CHECK(fu > -1.0 && fu < w_ && fv > -1.0 && fv < h_, "point " + std::to_string(k) + " rounds to a pixel outside the image");
+        u = (int)fu; v = (int)fv;
+      } else {             // int u = centerProjectedTo[0] + 0.5f (float)
+        const float fu = a.pt_u[k] + 0.5f, fv = a.pt_v[k] + 0.5f;
+        TDM_CHECK(fu > -1.f && fu < (float)w_ && fv > -1.f && fv < (float)h_, "point " + std::to_string(k) + " rounds to a pixel outside the image");
+        u = (int)fu; v = (int)fv;
+      }
+      pk[k] = u + w_ * v;
+      pk[cap + k] = k;
+    }
+    if (n) {
+      std::memcpy(h_pts_ + 2 * cap, a.pt_idepth, 4 * (size_t)n);
+      std::memcpy(h_pts_ + 3 * cap, a.pt_hessian, 4 * (size_t)n);
+    }
+    // Ordered after the pending work of every level (their references are overwritten), the pyramid and the dense map.
+    for (int l = 1; l < L; ++l) lv[l]->order_before(stream_);
+    TDM_CUDA(cudaStreamWaitEvent(stream_, (cudaEvent_t)P.ready_event(), 0));
+    if (a.depth && a.depth_on_device && a.depth_ready) TDM_CUDA(cudaStreamWaitEvent(stream_, (cudaEvent_t)a.depth_ready, 0));
+    size_t off[kMaxLevels + 1] = {0};
+    for (int l = 0; l < kMaxLevels; ++l) off[l + 1] = off[l] + (size_t)(w_ >> l) * (h_ >> l);
+    float *id = d_coarse_, *ws = d_coarse_ + off[kMaxLevels], *ws2 = d_coarse_ + 2 * off[kMaxLevels];
+    // 1. scatter (:150-182)
+    TDM_CUDA(cudaMemsetAsync(id, 0, 4 * off[1], stream_));
+    TDM_CUDA(cudaMemsetAsync(ws, 0, 4 * off[1], stream_));
+    if (n) {
+      int* d_pk = reinterpret_cast<int*>(d_pts_);
+      TDM_CUDA(cudaMemcpyAsync(d_pts_, h_pts_, 16 * cap, cudaMemcpyHostToDevice, stream_));
+      int bits = 1;
+      while ((1ll << bits) < (long long)w_ * h_) ++bits;
+      size_t tb = 0;
+      TDM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_pk, d_pk + 4 * cap, d_pk + cap, d_pk + 5 * cap, n, 0, bits, stream_));
+      if (tb > coarse_tmp_bytes_) {
+        TDM_CUDA(cudaStreamSynchronize(stream_));
+        cudaFree(d_coarse_tmp_);
+        d_coarse_tmp_ = nullptr; coarse_tmp_bytes_ = 0;
+        TDM_CUDA(cudaMalloc(&d_coarse_tmp_, tb));
+        coarse_tmp_bytes_ = tb;
+      }
+      TDM_CUDA(cub::DeviceRadixSort::SortPairs(d_coarse_tmp_, tb, d_pk, d_pk + 4 * cap, d_pk + cap, d_pk + 5 * cap, n, 0, bits, stream_));
+      k_coarse_scatter<<<(n + 255) / 256, 256, 0, stream_>>>(d_pk + 4 * cap, d_pk + 5 * cap, d_pts_ + 2 * cap, d_pts_ + 3 * cap, n,
+                                                             a.rgbd_init, id, ws);
+    }
+    // 2. sum pyramid from the un-dilated level below (:222-243)
+    for (int l = 1; l < L; ++l) {
+      const int wl = w_ >> l, hl = h_ >> l;
+      k_coarse_sum<<<(wl * hl + 255) / 256, 256, 0, stream_>>>(id + off[l - 1], ws + off[l - 1], w_ >> (l - 1), id + off[l], ws + off[l], wl, hl);
+    }
+    // 3. dilation (:246-322): diagonal neighbours on levels 0 / 1, axis neighbours above; weights ws -> ws2
+    for (int l = 0; l < L; ++l) {
+      const int wl = w_ >> l, hl = h_ >> l, g = (wl * hl + 255) / 256;
+      if (l < 2) k_coarse_dilate<true><<<g, 256, 0, stream_>>>(id + off[l], ws + off[l], ws2 + off[l], wl, hl);
+      else k_coarse_dilate<false><<<g, 256, 0, stream_>>>(id + off[l], ws + off[l], ws2 + off[l], wl, hl);
+    }
+    // 4. normalise and compact each level into its tracker's arrays (:325-370); counts in d_coarse_cnt_[l]
+    for (int l = 0; l < L; ++l) {
+      const int wl = w_ >> l, hl = h_ >> l;
+      const NormSel sel{id + off[l], ws2 + off[l], P.level_dI(l)};
+      const size_t nm = (size_t)lv[l]->n_max_;
+      float* pc = lv[l]->d_pc_;
+      k_compact_rowcount<<<hl, 256, 0, stream_>>>(sel, wl, hl, d_rowcnt_, d_rowlast_);
+      k_compact_rowscan<<<1, 32, 0, stream_>>>(d_rowcnt_, d_rowlast_, wl, hl, nullptr, d_rowoff_, d_coarse_cnt_ + l, d_coarse_stale_ + l);
+      k_compact_emit<<<hl, 256, 0, stream_>>>(sel, wl, hl, d_rowoff_, 0, lv[l]->n_max_, d_coarse_stale_ + l, d_coarse_cnt_ + l,
+                                              pc, pc + nm, pc + 2 * nm, pc + 3 * nm);
+    }
+    // 5. n1's dense append behind level 0's points, against the normalised idepth[0] (:655-732)
+    if (a.depth) {
+      const size_t npx = (size_t)w_ * h_, nm = (size_t)n_max_;
+      const float* d_depth = a.depth;
+      if (!a.depth_on_device) {
+        std::memcpy(h_front_, a.depth, 4 * npx);
+        TDM_CUDA(cudaMemcpyAsync(d_depth_, h_front_, 4 * npx, cudaMemcpyHostToDevice, stream_));
+        d_depth = d_depth_;
+      }
+      TDM_CUDA(cudaMemsetAsync(d_proj_, 0xFF, 4 * npx, stream_));
+      const int nx = (w_ + a.step - 1) / a.step, ny = (h_ + a.step - 1) / a.step;
+      k_dense_warp<<<(nx * ny + 255) / 256, 256, 0, stream_>>>(d_depth, w_, h_, a.step, dense_warp(a.T_depth_to_ref), d_proj_);
+      const DenseSel sel{d_proj_, id, a.dense_only, P.level_dI(0), 3};
+      k_compact_rowcount<<<h_, 256, 0, stream_>>>(sel, w_, h_, d_rowcnt_, nullptr);
+      k_compact_rowscan<<<1, 32, 0, stream_>>>(d_rowcnt_, nullptr, w_, h_, d_coarse_cnt_, d_rowoff_, d_coarse_cnt_ + kMaxLevels, nullptr);
+      k_compact_emit<<<h_, 256, 0, stream_>>>(sel, w_, h_, d_rowoff_, 1, n_max_, nullptr, nullptr,
+                                              d_pc_, d_pc_ + nm, d_pc_ + 2 * nm, d_pc_ + 3 * nm);
+    } else {
+      TDM_CUDA(cudaMemsetAsync(d_coarse_cnt_ + kMaxLevels, 0, 4, stream_));
+    }
+    TDM_CUDA(cudaGetLastError());
+    TDM_CUDA(cudaMemcpyAsync(h_coarse_cnt_, d_coarse_cnt_, 4 * (kMaxLevels + 1), cudaMemcpyDeviceToHost, stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_));
+    // Capacity: each level needs room for its count and the slot behind it; level 0 also for the dense points.
+    int cnt[kMaxLevels];
+    bool fits = true;
+    for (int l = 0; l < L; ++l) {
+      cnt[l] = h_coarse_cnt_[l] + (l == 0 ? h_coarse_cnt_[kMaxLevels] : 0);   // the `++pc_n` quirk: the last dense point is not counted
+      fits = fits && (long long)h_coarse_cnt_[l] + 1 + (l == 0 ? h_coarse_cnt_[kMaxLevels] : 0) <= lv[l]->n_max_;
+    }
+    for (int l = 0; l < L; ++l) {
+      TrackerImpl& t = *lv[l];
+      t.n_ = fits ? cnt[l] : 0;
+      t.have_ref_ = fits;
+      t.have_params_ = false;
+      t.ref_exposure_ = a.ref_exposure;
+      t.ref_aff_[0] = a.ref_aff[0]; t.ref_aff_[1] = a.ref_aff[1];
+    }
+    if (!fits) throw Error("set_coarse_tracking_ref: a level's n_max is too small for its points; every level's reference is now empty");
+    for (int l = 0; l < kMaxLevels; ++l) pc_n[l] = l < L ? cnt[l] : 0;
+  }
   void synchronize() override {
     TDM_CUDA(cudaSetDevice(device_));
     TDM_CUDA(cudaStreamSynchronize(stream_));
@@ -1065,6 +1315,59 @@ class TrackerImpl final : public TrackerIface {
     TDM_CUDA(cudaMalloc(&d_total_, 4));
     TDM_CUDA(cudaMallocHost(&h_front_, 3 * 4 * npx));
     TDM_CUDA(cudaMallocHost(&h_total_, 4));
+  }
+  // n7 scratch: idepth, weights and dilated weights of every level (levels concatenated), the packed points (pixel, index,
+  // value, weight input), their sorted copies (pixel, index) and the sort's temporary storage; grown to the largest point count
+  void ensure_coarse_buffers(int n) {
+    if (!d_coarse_) {
+      size_t tot = 0;
+      for (int l = 0; l < kMaxLevels; ++l) tot += (size_t)(w_ >> l) * (h_ >> l);
+      TDM_CUDA(cudaMalloc(&d_coarse_, 3 * 4 * tot));
+      TDM_CUDA(cudaMalloc(&d_rowlast_, 8 * (size_t)h_));
+      TDM_CUDA(cudaMalloc(&d_coarse_cnt_, 4 * (kMaxLevels + 1)));
+      TDM_CUDA(cudaMalloc(&d_coarse_stale_, 4 * kMaxLevels));
+      TDM_CUDA(cudaMallocHost(&h_coarse_cnt_, 4 * (kMaxLevels + 1)));
+    }
+    if (n > coarse_cap_) {
+      const int cap = n > 1024 ? n : 1024;
+      cudaFree(d_pts_); cudaFreeHost(h_pts_); cudaFree(d_coarse_tmp_);
+      d_pts_ = nullptr; h_pts_ = nullptr; d_coarse_tmp_ = nullptr; coarse_cap_ = 0;
+      TDM_CUDA(cudaMalloc(&d_pts_, 6 * 4 * (size_t)cap));
+      TDM_CUDA(cudaMallocHost(&h_pts_, 4 * 4 * (size_t)cap));
+      size_t tb = 0;
+      TDM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const int*)nullptr, (int*)nullptr, (const int*)nullptr, (int*)nullptr, cap));
+      TDM_CUDA(cudaMalloc(&d_coarse_tmp_, tb));
+      coarse_tmp_bytes_ = tb;
+      coarse_cap_ = cap;
+    }
+  }
+  // KRKi = (K R) Ki, Kt = K t in float, k = 0,1,2 (CoarseTracker.cpp:676-677)
+  DenseWarp dense_warp(const double* T) const {
+    DenseWarp m;
+    const float K[9] = {fx_, 0, cx_, 0, fy_, cy_, 0, 0, 1};
+    const float Ki[9] = {1.0f / fx_, 0, -cx_ / fx_, 0, 1.0f / fy_, -cy_ / fy_, 0, 0, 1};
+    float R[9], t[3], KR[9];
+    for (int r = 0; r < 3; ++r) {
+      for (int c = 0; c < 3; ++c) R[3 * r + c] = (float)T[4 * r + c];
+      t[r] = (float)T[4 * r + 3];
+    }
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) {
+        volatile float s = 0;
+        for (int k = 0; k < 3; ++k) { volatile float q = K[3 * r + k] * R[3 * k + c]; s = s + q; }
+        KR[3 * r + c] = s;
+      }
+    for (int r = 0; r < 3; ++r) {
+      for (int c = 0; c < 3; ++c) {
+        volatile float s = 0;
+        for (int k = 0; k < 3; ++k) { volatile float q = KR[3 * r + k] * Ki[3 * k + c]; s = s + q; }
+        m.KRKi[3 * r + c] = s;
+      }
+      volatile float s = 0;
+      for (int k = 0; k < 3; ++k) { volatile float q = K[3 * r + k] * t[k]; s = s + q; }
+      m.Kt[r] = s;
+    }
+    return m;
   }
   // The device LM loop as a graph, built once per tracker: k_lm_init, then WHILE (handle, default 1) { k_tracker<4> }.
   // Every parameter that changes between calls (levels, sizes, buffers, pose) travels in LmCtx::in, so the graph never
@@ -1340,6 +1643,13 @@ class TrackerImpl final : public TrackerIface {
   // n6 buffers
   RetrackIn* h_rt_in_ = nullptr;
   RetrackOut *h_rt_out_ = nullptr, *d_rt_out_ = nullptr;
+  // n7 buffers (ensure_coarse_buffers)
+  float *d_coarse_ = nullptr, *d_pts_ = nullptr, *h_pts_ = nullptr;
+  int2* d_rowlast_ = nullptr;
+  int *d_coarse_cnt_ = nullptr, *d_coarse_stale_ = nullptr, *h_coarse_cnt_ = nullptr;
+  void* d_coarse_tmp_ = nullptr;
+  size_t coarse_tmp_bytes_ = 0;
+  int coarse_cap_ = 0;
 };
 
 

@@ -4,6 +4,8 @@
 
 namespace tdm {
 
+class PyramidIface;
+
 class TrackerIface {
  public:
   virtual ~TrackerIface() = default;
@@ -106,6 +108,22 @@ class TrackerIface {
   };
   virtual void track_new_coarse(TrackerIface* const* levels, int coarsest, const NewCoarseArgs& a, NewCoarseResult* r,
                                 TryResult* tries /* r->tries entries, may be null */) = 0;
+  // n7: CoarseTracker::setCoarseTrackingRef with makeCoarseDepthL0 for levels[0..n_levels-1] (called on levels[0], which runs
+  // it on its stream); pc_n[l] receives each level's count
+  struct CoarseRefArgs {
+    int n_levels = 1, rgbd_init = 0;
+    int n_points = 0;
+    const float *pt_u = nullptr, *pt_v = nullptr, *pt_idepth = nullptr, *pt_hessian = nullptr;
+    const PyramidIface* ref_pyramid = nullptr;   // colours: level l's dIp[l][i][0]
+    const float* depth = nullptr;       // dense map (h*w, host or device), nullptr: none
+    bool depth_on_device = false;
+    void* depth_ready = nullptr;        // cudaEvent_t to wait for (device depth), may be null
+    const double* T_depth_to_ref = nullptr;
+    int step = 1, dense_only = 0;
+    float ref_exposure = 1.f;
+    const double* ref_aff = nullptr;
+  };
+  virtual void set_coarse_tracking_ref(TrackerIface* const* levels, const CoarseRefArgs& a, int pc_n[5]) = 0;
 };
 
 // FrameHessian::makeImages on the device (n2): all pyramid levels of (I, dx, dy) + absSquaredGrad.

@@ -243,3 +243,36 @@ def track_new_coarse(trackers, tries, aff_last_2_l, new_exposure, last_coarse_rm
     return dict(refToNew=np.array(r.ref_to_new, np.float64).reshape(4, 4), aff=np.array(r.aff_g2l, np.float64),
                 flow_vecs=np.array(r.flow_vecs, np.float64), achieved_res=np.array(r.achieved_res, np.float64),
                 have_one_good=bool(r.have_one_good), tries=r.tries, winner=r.winner, device_ms=r.device_ms, per_try=per_try)
+
+
+def set_coarse_tracking_ref(levels, points, ref_pyramid, depth=None, fusion=None, render_index=0, T_depth_to_ref=None,
+                            tracking_step=1, dense_only=False, rgbd_init=False, ref_exposure=1.0, ref_aff_g2l=(0.0, 0.0)):
+    """CoarseTracker::setCoarseTrackingRef with makeCoarseDepthL0 (CoarseTracker.cpp:148-374, :633-733) for every level in one
+    call on the device.  levels[l] is the CudaCoarseTracker of pyramid level l ((w >> l) x (h >> l)), levels[0] with setK.
+    points = (u, v, idepth, hessian) in the reference's order - monocular: centerProjectedTo[0..2] and efPoint->HdiF of the
+    points passing the lastResiduals[0] test; rgbd_init: ph->u, ph->v, ph->idepth, ph->idepth_hessian - or None for no points.
+    Colours come from ref_pyramid (an ImagePyramid of the reference keyframe).  The optional dense map is a host depth image or
+    the render_index-th render of a DrFusion, warped with T_depth_to_ref (4x4) and appended behind level 0's points.
+    Returns pc_n, one count per level; each level then holds its reference as after setReference."""
+    n_levels = len(levels)
+    hs = (ctypes.c_void_p * max(n_levels, 1))(*[t._h for t in levels])
+    keep = []
+
+    def ptr(a):
+        if a is None:
+            return None
+        a = _f(a)
+        keep.append(a)
+        return a.ctypes.data_as(_fp)
+
+    n = 0 if points is None else len(points[0])
+    pts = [None] * 4 if points is None else [ptr(a) for a in points]
+    assert points is None or all(len(a) == n for a in points)
+    T = None if T_depth_to_ref is None else np.ascontiguousarray(T_depth_to_ref, np.float64)
+    aff = np.ascontiguousarray(ref_aff_g2l, np.float64)
+    pc_n = np.zeros(5, np.int32)
+    check(lib().tdm_tracker_set_coarse_tracking_ref(
+        hs, n_levels, int(bool(rgbd_init)), n, pts[0], pts[1], pts[2], pts[3], ref_pyramid._h, ptr(depth),
+        None if fusion is None else fusion._h, int(render_index), None if T is None else T.ctypes.data_as(_dp), int(tracking_step),
+        int(bool(dense_only)), float(ref_exposure), aff.ctypes.data_as(_dp), pc_n.ctypes.data_as(ctypes.POINTER(ctypes.c_int))))
+    return [int(x) for x in pc_n[:n_levels]]
