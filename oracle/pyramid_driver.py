@@ -19,10 +19,11 @@ MAX_ITERATIONS = (10, 20, 50, 50, 50)   # CoarseTracker.cpp:751
 
 def track_pyramid(trackers_per_level, refToNew, aff, new_exposure, ref_exposure, ref_aff, coarse_cutoff=20.0,
                   max_iterations=MAX_ITERATIONS, lambda_extrapolation_limit=0.001, mode_a=0.0, mode_b=0.0,
-                  min_res_for_abort=None):
+                  min_res_for_abort=None, trace=None):
     """trackers_per_level[l] evaluates pyramid level l; len - 1 is the coarsest level.  Returns dict(ok, refToNew, aff,
     last_residuals (5,), last_flow_indicators (3,), aborted_level, repeated_level, iterations (5,), evaluations (5,),
-    cutoff_repeat (5,)) - the fields of tdm_track_pyramid_result."""
+    cutoff_repeat (5,)) - the fields of tdm_track_pyramid_result.  trace: as for oracle.lm_driver.track_level0, each record
+    with its level and pass (1 for the repeat of a level)."""
     T0, a0 = np.array(refToNew, np.float64), np.array(aff, np.float64)
     T, a = T0.copy(), a0.copy()
     min_res = np.full(5, np.nan) if min_res_for_abort is None else np.asarray(min_res_for_abort, np.float64)
@@ -31,9 +32,14 @@ def track_pyramid(trackers_per_level, refToNew, aff, new_exposure, ref_exposure,
     out = dict(last_residuals=last_res, iterations=its, evaluations=evs, cutoff_repeat=reps, aborted_level=-1, repeated_level=-1)
     lvl = len(trackers_per_level) - 1
     while lvl >= 0:
+        level_trace = None if trace is None else []
         r = track_level0(trackers_per_level[lvl], T, a, new_exposure, coarse_cutoff=coarse_cutoff,
                          max_iterations=max_iterations[lvl], lambda_extrapolation_limit=lambda_extrapolation_limit,
-                         fix_a=mode_a < 0, fix_b=mode_b < 0)
+                         fix_a=mode_a < 0, fix_b=mode_b < 0, trace=level_trace)
+        if trace is not None:
+            for rec in level_trace:
+                rec.update({"level": lvl, "pass": int(out["repeated_level"] == lvl)})
+            trace.extend(level_trace)
         T, a = r["refToNew"], r["aff"]
         its[lvl] += r["iterations"]
         evs[lvl] += r["evaluations"]

@@ -88,7 +88,8 @@ struct LmState {
   double T[16], aff[2];      // accepted
   double Tn[16], affn[2];    // candidate under evaluation
   double res_old[6], H[64], b[8];
-  double lambda, inc_norm;
+  float lambda;              // float as in the reference (CoarseTracker.cpp:798), like its extrapolation factor (:842)
+  double inc_norm;
   float repeat;
   int phase, iter, evals;    // of the current pass over the current level
 };
@@ -583,11 +584,12 @@ __device__ void lm_pose_from(const LmConfig& c, const double* T, const double* a
     }
   float eF = c.ref_exposure, eT = c.new_exposure;       // AffLight::fromToVecExposure, cuda_coarse_tracker.cpp:42-52
   if (eF == 0 || eT == 0) eT = eF = 1;
+  // rounded operations, no FMA contraction: the same bits as the host's prepare() computes for calcRes / calcResAndG
   const double a = exp(aff[0] - c.ref_aff[0]) * eT / eF;
-  const double bb = aff[1] - a * c.ref_aff[1];
+  const double bb = __dsub_rn(aff[1], __dmul_rn(a, c.ref_aff[1]));
   o->affa = (float)a; o->affb = (float)bb;
   o->cutoff = cutoff;
-  o->maxEnergy = 2 * c.huber * cutoff - c.huber * c.huber;
+  o->maxEnergy = __fsub_rn(__fmul_rn(__fmul_rn(2.f, c.huber), cutoff), __fmul_rn(c.huber, c.huber));
 }
 
 __device__ void lm_se3_exp(const double* xi, double* T) {   // Sophus convention (upsilon, omega)
@@ -618,14 +620,17 @@ __device__ void lm_next_candidate(const LmConfig& c, LmState* s, TrkPose* pose) 
     if (!((i == 6 && c.fix_a) || (i == 7 && c.fix_b))) idx[nf++] = i;
   double M[8][9];
   for (int r = 0; r < nf; ++r) {
-    for (int q = 0; q < nf; ++q) M[r][q] = s->H[8 * idx[r] + idx[q]] * (r == q ? 1.0 + s->lambda : 1.0);
+    for (int q = 0; q < nf; ++q) M[r][q] = s->H[8 * idx[r] + idx[q]] * (r == q ? (double)(1.f + s->lambda) : 1.0);
     M[r][nf] = -s->b[idx[r]];
   }
-  for (int k = 0; k < nf; ++k) {             // Gaussian elimination, partial pivoting
+  // Gaussian elimination, partial pivoting.  A column without a non-zero pivot (a parameter no point constrains: its row
+  // and column of the damped H are 0) gets increment 0, as Eigen's LDLT (CoarseTracker.cpp:815) treats a zero pivot.
+  for (int k = 0; k < nf; ++k) {
     int piv = k;
     for (int r = k + 1; r < nf; ++r) if (fabs(M[r][k]) > fabs(M[piv][k])) piv = r;
     if (piv != k) for (int q = 0; q <= nf; ++q) { const double t = M[k][q]; M[k][q] = M[piv][q]; M[piv][q] = t; }
     const double d = M[k][k];
+    if (d == 0) continue;
     for (int r = k + 1; r < nf; ++r) {
       const double f = M[r][k] / d;
       for (int q = k; q <= nf; ++q) M[r][q] -= f * M[k][q];
@@ -635,10 +640,10 @@ __device__ void lm_next_candidate(const LmConfig& c, LmState* s, TrkPose* pose) 
   for (int k = nf - 1; k >= 0; --k) {
     double v = M[k][nf];
     for (int q = k + 1; q < nf; ++q) v -= M[k][q] * inc[idx[q]];
-    inc[idx[k]] = v / M[k][k];
+    inc[idx[k]] = M[k][k] == 0 ? 0.0 : v / M[k][k];
   }
-  double extrap = 1.0;
-  if (s->lambda < c.lambda_limit) extrap = sqrt(sqrt((double)c.lambda_limit / s->lambda));
+  float extrap = 1.f;
+  if (s->lambda < c.lambda_limit) extrap = sqrtf(sqrtf(c.lambda_limit / s->lambda));
   double n2 = 0, sum = 0;
   const double scale[8] = {1.0, 1.0, 1.0, 0.5, 0.5, 0.5, 10.0, 1000.0};
   double sc[8];
@@ -672,7 +677,7 @@ __device__ void lm_begin_level(LmCtx* c, int lvl) {   // CoarseTracker.cpp:764,7
   c->lvl = lvl;
   for (int i = 0; i < 16; ++i) s->Tn[i] = s->T[i];
   s->affn[0] = s->aff[0]; s->affn[1] = s->aff[1];
-  s->lambda = 0.01; s->inc_norm = 0; s->repeat = 1.f; s->phase = 0; s->iter = 0; s->evals = 0;
+  s->lambda = 0.01f; s->inc_norm = 0; s->repeat = 1.f; s->phase = 0; s->iter = 0; s->evals = 0;
   lm_pose_from(cfg, s->T, s->aff, cfg.coarse_cutoff, &c->pose);
 }
 
@@ -740,7 +745,7 @@ __device__ void lm_finish_pyramid(LmCtx* ctx) {
     float eF = c0.ref_exposure, eT = c0.new_exposure;
     if (eF == 0 || eT == 0) eT = eF = 1;
     const double ra = exp(a - c0.ref_aff[0]) * eT / eF;
-    const double rb = b - ra * c0.ref_aff[1];
+    const double rb = __dsub_rn(b, __dmul_rn(ra, c0.ref_aff[1]));   // no FMA contraction, as on the host
     const float rel0 = (float)ra, rel1 = (float)rb;
     ok = !((ma == 0 && fabsf(logf(rel0)) > 1.5) || (mb == 0 && fabsf(rel1) > 200));
   }
@@ -827,9 +832,9 @@ __device__ __noinline__ void lm_step(LmCtx* ctx, const double* o /*kOut sums of 
       for (int i = 0; i < 6; ++i) s->res_old[i] = res[i];
       for (int i = 0; i < 16; ++i) s->T[i] = s->Tn[i];
       s->aff[0] = s->affn[0]; s->aff[1] = s->affn[1];
-      s->lambda *= 0.5;
+      s->lambda *= 0.5f;
     } else {
-      s->lambda *= 4;
+      s->lambda *= 4.f;
       if (s->lambda < c.lambda_limit) s->lambda = c.lambda_limit;
     }
     s->iter++;
