@@ -116,6 +116,17 @@ public:
                                                int render_index, Eigen::Matrix<double, 4, 4> const &T_depth_to_ref,
                                                int tracking_step, bool dense_only, float ref_exposure,
                                                Eigen::Vector2d const &ref_aff);
+  // Extension: the same, plus makeCoarseDepthL0's undilated level-0 cloud (pc_*_nodia, kept by levels[0]) and
+  // get_idepth_quantile(pc_n_nodia, pc_idepth_nodia, quantile_fraction) over it (tandem_backend.cpp:354-361), in the same call:
+  // *pc_n_nodia and *depth_quantile receive what FullSystem::deliverDrFrame reads for MVSNet's depth range (NaN when the
+  // cloud has no entry at the quantile's index).
+  static std::vector<int> setCoarseTrackingRef(std::vector<CudaCoarseTracker *> const &levels, bool rgbd_init, int n_points,
+                                               float const *pt_u, float const *pt_v, float const *pt_idepth,
+                                               float const *pt_hessian, tdm_pyramid *ref_pyramid, tdm_fusion *fusion,
+                                               int render_index, Eigen::Matrix<double, 4, 4> const &T_depth_to_ref,
+                                               int tracking_step, bool dense_only, float ref_exposure,
+                                               Eigen::Vector2d const &ref_aff, float quantile_fraction, int *pc_n_nodia,
+                                               float *depth_quantile);
 
   void synchronize();
 

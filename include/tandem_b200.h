@@ -429,6 +429,32 @@ int tdm_tracker_set_coarse_tracking_ref(tdm_tracker* const* levels, int n_levels
                                         const double T_depth_to_ref[16], int tracking_step, int dense_only, float ref_exposure,
                                         const double ref_aff_g2l[2], int pc_n[5]);
 
+/* n7 + nodia  tdm_tracker_set_coarse_tracking_ref, and in the same call on the same stream with the same host wait the rest of
+ *     makeCoarseDepthL0's level-0 output that FullSystem::deliverDrFrame reads for every MVSNet window (FullSystem.cpp:1175):
+ *     the undilated cloud pc_u/v/idepth/color_nodia (CoarseTracker.cpp:150-218) - candidates are the pixels of
+ *     [2,w-2) x [2,h-2) with a point, accepted when their colour is finite and their unweighted idepth sum > 0 (monocular;
+ *     RGB-D leaves the sums 0) - and get_idepth_quantile over it (tandem_backend.cpp:354-361): the idepth at index
+ *     (int)(quantile_fraction * (float)pc_n_nodia) in sorted order and 1.0f / it.  The cloud lives in levels[0] and persists
+ *     across calls like the reference's arrays: slot pc_n_nodia keeps the last rejected candidate behind the last accepted
+ *     one, or what it held before.  Plain tdm_tracker_set_coarse_tracking_ref calls leave it alone.  Both quantile values are
+ *     NaN when that index is not below pc_n_nodia (no accepted pixel, or quantile_fraction 1), where the reference reads
+ *     outside its vector.  quantile_fraction outside [0, 1] or not finite, or a null `out`, is an error and launches nothing;
+ *     everything else as tdm_tracker_set_coarse_tracking_ref.  `out` is filled even when a level's n_max turns out too small. */
+typedef struct tdm_coarse_nodia_result {
+  int pc_n_nodia;             /* CoarseTracker::pc_n_nodia */
+  float idepth_quantile;      /* the selected pc_idepth_nodia value */
+  float depth_quantile;       /* get_idepth_quantile's return value: MVSNet's depth_max is 3 * this (FullSystem.cpp:1180) */
+} tdm_coarse_nodia_result;
+int tdm_tracker_set_coarse_tracking_ref_nodia(tdm_tracker* const* levels, int n_levels, int rgbd_init, int n_points,
+                                              const float* pt_u, const float* pt_v, const float* pt_idepth, const float* pt_hessian,
+                                              tdm_pyramid* ref_pyramid, const float* depth, tdm_fusion* depth_from_fusion,
+                                              int render_index, const double T_depth_to_ref[16], int tracking_step, int dense_only,
+                                              float ref_exposure, const double ref_aff_g2l[2], float quantile_fraction, int pc_n[5],
+                                              tdm_coarse_nodia_result* out);
+/* Reads the first n entries (0..w*h) of level0's pc_u/v/idepth/color_nodia back (tests, dumps); any output pointer may be
+ * NULL.  An error before the first tdm_tracker_set_coarse_tracking_ref_nodia call with level0 as levels[0]. */
+int tdm_tracker_get_coarse_nodia(tdm_tracker* level0, int n, float* u, float* v, float* idepth, float* color);
+
 #ifdef __cplusplus
 }
 #endif

@@ -186,6 +186,27 @@ std::vector<int> CudaCoarseTracker::setCoarseTrackingRef(
   return std::vector<int>(pc_n, pc_n + (h.size() < 5 ? h.size() : 5));
 }
 
+std::vector<int> CudaCoarseTracker::setCoarseTrackingRef(
+    std::vector<CudaCoarseTracker*> const& levels, bool rgbd_init, int n_points, float const* pt_u, float const* pt_v,
+    float const* pt_idepth, float const* pt_hessian, tdm_pyramid* ref_pyramid, tdm_fusion* fusion, int render_index,
+    Eigen::Matrix<double, 4, 4> const& T_depth_to_ref, int tracking_step, bool dense_only, float ref_exposure,
+    Eigen::Vector2d const& ref_aff, float quantile_fraction, int* pc_n_nodia, float* depth_quantile) {
+  std::vector<tdm_tracker*> h;
+  for (CudaCoarseTracker* t : levels) h.push_back(t ? t->handle_ : nullptr);
+  double T[16];
+  to_row_major(T_depth_to_ref, T);
+  const double a[2] = {ref_aff(0), ref_aff(1)};
+  int pc_n[5] = {0, 0, 0, 0, 0};
+  tdm_coarse_nodia_result r;
+  chk(tdm_tracker_set_coarse_tracking_ref_nodia(h.data(), (int)h.size(), rgbd_init ? 1 : 0, n_points, pt_u, pt_v, pt_idepth,
+                                                pt_hessian, ref_pyramid, nullptr, fusion, render_index, T, tracking_step,
+                                                dense_only ? 1 : 0, ref_exposure, a, quantile_fraction, pc_n, &r),
+      "CudaCoarseTracker::setCoarseTrackingRef");
+  if (pc_n_nodia) *pc_n_nodia = r.pc_n_nodia;
+  if (depth_quantile) *depth_quantile = r.depth_quantile;
+  return std::vector<int>(pc_n, pc_n + (h.size() < 5 ? h.size() : 5));
+}
+
 CudaCoarseTracker::NewCoarseResult CudaCoarseTracker::trackNewCoarse(
     std::vector<CudaCoarseTracker*> const& levels, std::vector<Eigen::Matrix<double, 4, 4>> const& tries,
     Eigen::Vector2d const& aff_last_2_l, float new_exposure, float coarseCutoffTH, const int maxIterations[5],

@@ -80,6 +80,11 @@ class TrackTry(ctypes.Structure):
                 ("repeated_level", ctypes.c_int), ("evaluations", ctypes.c_int * 5)]
 
 
+class CoarseNodiaResult(ctypes.Structure):
+    """tdm_coarse_nodia_result (include/tandem_b200.h)."""
+    _fields_ = [("pc_n_nodia", ctypes.c_int), ("idepth_quantile", ctypes.c_float), ("depth_quantile", ctypes.c_float)]
+
+
 class TrackNewCoarseResult(ctypes.Structure):
     """tdm_track_new_coarse_result (include/tandem_b200.h)."""
     _fields_ = [("ref_to_new", ctypes.c_double * 16), ("aff_g2l", ctypes.c_double * 2), ("achieved_res", ctypes.c_double * 5),
@@ -165,6 +170,9 @@ def _declare(l):
         "tdm_tracker_track_pyramid": (i, [P(vp), i, dp, dp, f, f, ip, f, f, f, dp, P(TrackPyramidResult)]),
         "tdm_tracker_track_new_coarse": (i, [P(vp), i, dp, i, dp, f, f, ip, f, f, f, dp, f, P(TrackNewCoarseResult), P(TrackTry)]),
         "tdm_tracker_set_coarse_tracking_ref": (i, [P(vp), i, i, i, fp, fp, fp, fp, vp, fp, vp, i, dp, i, i, f, dp, ip]),
+        "tdm_tracker_set_coarse_tracking_ref_nodia": (i, [P(vp), i, i, i, fp, fp, fp, fp, vp, fp, vp, i, dp, i, i, f, dp, f, ip,
+                                                          P(CoarseNodiaResult)]),
+        "tdm_tracker_get_coarse_nodia": (i, [vp, i, fp, fp, fp, fp]),
     }
     missing = []
     for name, (res, args) in sigs.items():

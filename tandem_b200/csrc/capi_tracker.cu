@@ -1,4 +1,6 @@
 // extern "C" entry points for the coarse tracker (include/tandem_b200.h).
+#include <cmath>
+
 #include "../../include/tandem_b200.h"
 #include "capi_common.h"
 #include "common.cuh"
@@ -275,15 +277,19 @@ int tdm_tracker_track_new_coarse(tdm_tracker* const* levels, int coarsest_level,
 }
 
 /* ---- SURVEY 8(f) n7: CoarseTracker::setCoarseTrackingRef with makeCoarseDepthL0, every level on the device ---- */
-int tdm_tracker_set_coarse_tracking_ref(tdm_tracker* const* levels, int n_levels, int rgbd_init, int n_points, const float* pt_u,
-                                        const float* pt_v, const float* pt_idepth, const float* pt_hessian, tdm_pyramid* ref_pyramid,
-                                        const float* depth, tdm_fusion* depth_from_fusion, int render_index,
-                                        const double T_depth_to_ref[16], int tracking_step, int dense_only, float ref_exposure,
-                                        const double ref_aff_g2l[2], int pc_n[5]) {
-  TDM_API_BEGIN
+}  // extern "C"
+
+// n7's arguments, checked and passed to levels[0]; nodia (with its fraction) adds the undilated cloud and its quantile
+static void coarse_tracking_ref(tdm_tracker* const* levels, int n_levels, int rgbd_init, int n_points, const float* pt_u,
+                                const float* pt_v, const float* pt_idepth, const float* pt_hessian, tdm_pyramid* ref_pyramid,
+                                const float* depth, tdm_fusion* depth_from_fusion, int render_index, const double T_depth_to_ref[16],
+                                int tracking_step, int dense_only, float ref_exposure, const double ref_aff_g2l[2],
+                                float quantile_fraction, int pc_n[5], tdm::TrackerIface::CoarseNodiaResult* nodia) {
   TDM_CHECK(levels && ref_pyramid && ref_aff_g2l && pc_n, "null argument");
   TDM_CHECK(n_levels >= 1 && n_levels <= 5, "n_levels must be in 1..5");
   TDM_CHECK(!(depth && depth_from_fusion), "pass at most one of depth / depth_from_fusion");
+  TDM_CHECK(!nodia || (std::isfinite(quantile_fraction) && quantile_fraction >= 0.f && quantile_fraction <= 1.f),
+            "quantile_fraction must be finite and in [0, 1]");
   tdm::TrackerIface* impl[5] = {};
   for (int l = 0; l < n_levels; ++l) {
     TDM_CHECK(levels[l], "set_coarse_tracking_ref level " + std::to_string(l) + ": null tracker");
@@ -304,7 +310,51 @@ int tdm_tracker_set_coarse_tracking_ref(tdm_tracker* const* levels, int n_levels
   }
   a.T_depth_to_ref = T_depth_to_ref; a.step = tracking_step; a.dense_only = dense_only;
   a.ref_exposure = ref_exposure; a.ref_aff = ref_aff_g2l;
-  impl[0]->set_coarse_tracking_ref(impl, a, pc_n);
+  a.quantile_fraction = quantile_fraction;
+  impl[0]->set_coarse_tracking_ref(impl, a, pc_n, nodia);
+}
+
+extern "C" {
+
+int tdm_tracker_set_coarse_tracking_ref(tdm_tracker* const* levels, int n_levels, int rgbd_init, int n_points, const float* pt_u,
+                                        const float* pt_v, const float* pt_idepth, const float* pt_hessian, tdm_pyramid* ref_pyramid,
+                                        const float* depth, tdm_fusion* depth_from_fusion, int render_index,
+                                        const double T_depth_to_ref[16], int tracking_step, int dense_only, float ref_exposure,
+                                        const double ref_aff_g2l[2], int pc_n[5]) {
+  TDM_API_BEGIN
+  coarse_tracking_ref(levels, n_levels, rgbd_init, n_points, pt_u, pt_v, pt_idepth, pt_hessian, ref_pyramid, depth, depth_from_fusion,
+                      render_index, T_depth_to_ref, tracking_step, dense_only, ref_exposure, ref_aff_g2l, 0.f, pc_n, nullptr);
+  return TDM_OK;
+  TDM_API_END
+}
+
+/* ---- n7 + the undilated level-0 cloud and the MVSNet depth range's inverse-depth quantile over it ---- */
+int tdm_tracker_set_coarse_tracking_ref_nodia(tdm_tracker* const* levels, int n_levels, int rgbd_init, int n_points,
+                                              const float* pt_u, const float* pt_v, const float* pt_idepth, const float* pt_hessian,
+                                              tdm_pyramid* ref_pyramid, const float* depth, tdm_fusion* depth_from_fusion,
+                                              int render_index, const double T_depth_to_ref[16], int tracking_step, int dense_only,
+                                              float ref_exposure, const double ref_aff_g2l[2], float quantile_fraction, int pc_n[5],
+                                              tdm_coarse_nodia_result* out) {
+  TDM_API_BEGIN
+  TDM_CHECK(out, "null argument");
+  tdm::TrackerIface::CoarseNodiaResult r{};
+  const auto give = [&] { out->pc_n_nodia = r.pc_n_nodia; out->idepth_quantile = r.idepth_quantile; out->depth_quantile = r.depth_quantile; };
+  try {
+    coarse_tracking_ref(levels, n_levels, rgbd_init, n_points, pt_u, pt_v, pt_idepth, pt_hessian, ref_pyramid, depth,
+                        depth_from_fusion, render_index, T_depth_to_ref, tracking_step, dense_only, ref_exposure, ref_aff_g2l,
+                        quantile_fraction, pc_n, &r);
+  } catch (...) {   // a capacity error: the nodia outputs were computed
+    give();
+    throw;
+  }
+  give();
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_tracker_get_coarse_nodia(tdm_tracker* level0, int n, float* u, float* v, float* idepth, float* color) {
+  TDM_API_BEGIN
+  TDM_CHECK(level0, "null handle");
+  level0->impl->get_coarse_nodia(n, u, v, idepth, color);
   return TDM_OK;
   TDM_API_END
 }

@@ -411,6 +411,23 @@ struct NormSel {              // n7: CoarseTracker.cpp:346-370 on one level (ide
     idepth[i] = c == 1 ? __fdiv_rn(idepth[i], wsum[i]) : -1.f;
   }
 };
+struct NodiaSel {             // the undilated level-0 cloud, CoarseTracker.cpp:186-218 (pc_*_nodia)
+  static constexpr bool kStale = true;
+  const float* idepth_nodia;  // unweighted idepth sums
+  const float* wsum;          // level 0's weights before the dilation
+  const float* gray;          // level 0's (I, dx, dy) image
+  __device__ __forceinline__ int cls(int i) const {
+    if (!(wsum[i] > 0.f)) return 0;
+    return isfinite(gray[3 * (size_t)i]) && idepth_nodia[i] > 0.f ? 1 : 2;
+  }
+  __device__ __forceinline__ void emit(int o, int x, int y, int i, float* pc_u, float* pc_v, float* pc_idepth, float* pc_color) const {
+    pc_u[o] = (float)x;
+    pc_v[o] = (float)y;
+    pc_idepth[o] = idepth_nodia[i];
+    pc_color[o] = gray[3 * (size_t)i];
+  }
+  __device__ __forceinline__ void finish(int, int) const {}   // the -1 the reference writes back only marks the nodia image
+};
 // rowlast[y] = (last x of class 1, last x of class 2) in row y, -1 for none; only for selectors with kStale
 template <class Sel>
 __global__ void __launch_bounds__(256) k_compact_rowcount(Sel s, int w, int h, int* __restrict__ rowcnt, int2* __restrict__ rowlast) {
@@ -503,22 +520,46 @@ __global__ void __launch_bounds__(256) k_compact_emit(Sel s, int w, int h, const
 // ================================================================================================
 // Scatter (:155-182): the points arrive sorted by (pixel, input index) - a stable radix sort of the pixel keys - and each
 // pixel's run is summed sequentially in input order, so the sums do not depend on scheduling.  a = centerProjectedTo[2] or
-// ph->idepth, b = HdiF (monocular) or idepth_hessian (RGB-D).
+// ph->idepth, b = HdiF (monocular) or idepth_hessian (RGB-D).  kNodia also sums a unweighted into idepth_nodia (:167,
+// monocular only; in RGB-D mode it keeps the zeros it was cleared to).
+template <bool kNodia>
 __global__ void k_coarse_scatter(const int* __restrict__ pix, const int* __restrict__ order, const float* __restrict__ a,
-                                 const float* __restrict__ b, int n, int rgbd, float* __restrict__ idepth, float* __restrict__ wsum) {
+                                 const float* __restrict__ b, int n, int rgbd, float* __restrict__ idepth, float* __restrict__ wsum,
+                                 float* __restrict__ idepth_nodia) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n || (k > 0 && pix[k - 1] == pix[k])) return;
   const int p = pix[k];
-  float s = 0.f, ws = 0.f;
+  float s = 0.f, ws = 0.f, sn = 0.f;
   for (int j = k; j < n && pix[j] == p; ++j) {
     const int q = order[j];
     // sqrtf(1e-3 / (HdiF + 1e-12)): double literals, so the quotient is a double narrowed to float for sqrtf
     const float wt = rgbd ? b[q] : __fsqrt_rn(__double2float_rn(__ddiv_rn(1e-3, __dadd_rn((double)b[q], 1e-12))));
     s = __fadd_rn(s, __fmul_rn(a[q], wt));
     ws = __fadd_rn(ws, wt);
+    if (kNodia) sn = __fadd_rn(sn, a[q]);
   }
   idepth[p] = s;
   wsum[p] = ws;
+  if (kNodia && !rgbd) idepth_nodia[p] = sn;
+}
+// get_idepth_quantile (tandem_backend.cpp:354-361) on the first *count keys: keys[k] = pc_idepth_nodia[k] below the count, +inf
+// from there to n (the slot at *count, a rejected candidate, is not a key).  Accepted values are > 0, so +inf sorts behind them.
+__global__ void k_nodia_keys(const float* __restrict__ pc_idepth, const int* __restrict__ count, int n, float* __restrict__ keys) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) keys[k] = k < *count ? pc_idepth[k] : __int_as_float(0x7f800000);
+}
+// out[0] = the idepth at index (int)(fraction * (float)count) of the sorted keys, out[1] = 1.0f / it, both as float bits; NaN
+// when the index is not below the count (no keys at all, or fraction 1), where the reference reads outside its vector.
+__global__ void k_nodia_quantile(const float* __restrict__ sorted, const int* __restrict__ count, float fraction, int* __restrict__ out) {
+  const int m = *count;
+  const int k = __float2int_rz(__fmul_rn(fraction, __int2float_rn(m)));
+  float v = __int_as_float(0x7fc00000), d = v;
+  if (m > 0 && k < m) {
+    v = sorted[k];
+    d = __fdiv_rn(1.f, v);
+  }
+  out[0] = __float_as_int(v);
+  out[1] = __float_as_int(d);
 }
 // Sum pyramid (:222-243): level l from the un-dilated level l-1, a + b + c + d left to right.
 __global__ void k_coarse_sum(const float* __restrict__ id_lm, const float* __restrict__ ws_lm, int wlm1, float* __restrict__ id_l,
@@ -907,6 +948,7 @@ class TrackerImpl final : public TrackerIface {
     cudaFree(d_proj_); cudaFree(d_depth_); cudaFree(d_idepth0_); cudaFree(d_gray_); cudaFree(d_rowcnt_); cudaFree(d_rowoff_);
     cudaFree(d_total_); cudaFree(d_lm_ctx_); cudaFree(d_lm_out_);
     cudaFree(d_coarse_); cudaFree(d_rowlast_); cudaFree(d_coarse_cnt_); cudaFree(d_coarse_stale_); cudaFree(d_pts_); cudaFree(d_coarse_tmp_);
+    cudaFree(d_nodia_);
     if (h_coarse_cnt_) cudaFreeHost(h_coarse_cnt_);
     if (h_pts_) cudaFreeHost(h_pts_);
     if (lm_exec_) cudaGraphExecDestroy(lm_exec_);
@@ -1154,8 +1196,11 @@ class TrackerImpl final : public TrackerIface {
       }
   }
   // ---------------------------------------------------------------------------------------------- n7
-  void set_coarse_tracking_ref(TrackerIface* const* levels, const CoarseRefArgs& a, int pc_n[kMaxLevels]) override {
+  void set_coarse_tracking_ref(TrackerIface* const* levels, const CoarseRefArgs& a, int pc_n[kMaxLevels],
+                               CoarseNodiaResult* nodia) override {
     TDM_CHECK(levels && a.ref_pyramid && a.ref_aff && pc_n, "null argument");
+    TDM_CHECK(!nodia || (std::isfinite(a.quantile_fraction) && a.quantile_fraction >= 0.f && a.quantile_fraction <= 1.f),
+              "quantile_fraction must be finite and in [0, 1]");
     TDM_CHECK(a.n_levels >= 1 && a.n_levels <= kMaxLevels, "n_levels must be in 1..5");
     TDM_CHECK(a.n_points >= 0, "negative point count");
     TDM_CHECK(a.n_points == 0 || (a.pt_u && a.pt_v && a.pt_idepth && a.pt_hessian), "point arrays missing");
@@ -1177,6 +1222,7 @@ class TrackerImpl final : public TrackerIface {
     TDM_CUDA(cudaSetDevice(device_));
     ensure_front_buffers();
     ensure_coarse_buffers(a.n_points);
+    if (nodia) ensure_nodia_buffers();
     // Pack (pixel, input index, value, weight input) and check the pixels: the reference would write outside idepth[0] there.
     const int n = a.n_points;
     const size_t cap = (size_t)coarse_cap_;
@@ -1209,6 +1255,7 @@ class TrackerImpl final : public TrackerIface {
     // 1. scatter (:150-182)
     TDM_CUDA(cudaMemsetAsync(id, 0, 4 * off[1], stream_));
     TDM_CUDA(cudaMemsetAsync(ws, 0, 4 * off[1], stream_));
+    if (nodia) TDM_CUDA(cudaMemsetAsync(d_nodia_, 0, 4 * off[1], stream_));
     if (n) {
       int* d_pk = reinterpret_cast<int*>(d_pts_);
       TDM_CUDA(cudaMemcpyAsync(d_pts_, h_pts_, 16 * cap, cudaMemcpyHostToDevice, stream_));
@@ -1216,16 +1263,14 @@ class TrackerImpl final : public TrackerIface {
       while ((1ll << bits) < (long long)w_ * h_) ++bits;
       size_t tb = 0;
       TDM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_pk, d_pk + 4 * cap, d_pk + cap, d_pk + 5 * cap, n, 0, bits, stream_));
-      if (tb > coarse_tmp_bytes_) {
-        TDM_CUDA(cudaStreamSynchronize(stream_));
-        cudaFree(d_coarse_tmp_);
-        d_coarse_tmp_ = nullptr; coarse_tmp_bytes_ = 0;
-        TDM_CUDA(cudaMalloc(&d_coarse_tmp_, tb));
-        coarse_tmp_bytes_ = tb;
-      }
+      grow_coarse_tmp(tb);
       TDM_CUDA(cub::DeviceRadixSort::SortPairs(d_coarse_tmp_, tb, d_pk, d_pk + 4 * cap, d_pk + cap, d_pk + 5 * cap, n, 0, bits, stream_));
-      k_coarse_scatter<<<(n + 255) / 256, 256, 0, stream_>>>(d_pk + 4 * cap, d_pk + 5 * cap, d_pts_ + 2 * cap, d_pts_ + 3 * cap, n,
-                                                             a.rgbd_init, id, ws);
+      if (nodia)
+        k_coarse_scatter<true><<<(n + 255) / 256, 256, 0, stream_>>>(d_pk + 4 * cap, d_pk + 5 * cap, d_pts_ + 2 * cap, d_pts_ + 3 * cap,
+                                                                     n, a.rgbd_init, id, ws, d_nodia_);
+      else
+        k_coarse_scatter<false><<<(n + 255) / 256, 256, 0, stream_>>>(d_pk + 4 * cap, d_pk + 5 * cap, d_pts_ + 2 * cap, d_pts_ + 3 * cap,
+                                                                      n, a.rgbd_init, id, ws, nullptr);
     }
     // 2. sum pyramid from the un-dilated level below (:222-243)
     for (int l = 1; l < L; ++l) {
@@ -1269,9 +1314,39 @@ class TrackerImpl final : public TrackerIface {
     } else {
       TDM_CUDA(cudaMemsetAsync(d_coarse_cnt_ + kMaxLevels, 0, 4, stream_));
     }
+    if (nodia) {
+      // 6. the undilated level-0 cloud (:186-218) from ws[0], which the dilation left as it was, into the persistent nodia
+      //    arrays; count in d_coarse_cnt_[kMaxLevels + 1].  Slot pc_n_nodia < (w-4)(h-4) + 1 <= w*h always fits.
+      const size_t npx = (size_t)w_ * h_;
+      float* pc = d_nodia_ + npx;
+      int* cnt = d_coarse_cnt_ + kMaxLevels + 1;
+      const NodiaSel sel{d_nodia_, ws, P.level_dI(0)};
+      k_compact_rowcount<<<h_, 256, 0, stream_>>>(sel, w_, h_, d_rowcnt_, d_rowlast_);
+      k_compact_rowscan<<<1, 32, 0, stream_>>>(d_rowcnt_, d_rowlast_, w_, h_, nullptr, d_rowoff_, cnt, d_coarse_stale_ + kMaxLevels);
+      k_compact_emit<<<h_, 256, 0, stream_>>>(sel, w_, h_, d_rowoff_, 0, (int)npx, d_coarse_stale_ + kMaxLevels, cnt,
+                                              pc, pc + npx, pc + 2 * npx, pc + 3 * npx);
+      // 7. the quantile (tandem_backend.cpp:354-361) into d_coarse_cnt_[kMaxLevels + 2, + 3].  Every accepted pixel holds at
+      //    least one point, so pc_n_nodia <= n: n keys padded with +inf hold every value.  The packed points are dead by now,
+      //    their buffer holds the keys and their sorted copy.
+      float *keys = d_pts_, *sorted = d_pts_ + cap;
+      if (n) {
+        k_nodia_keys<<<(n + 255) / 256, 256, 0, stream_>>>(pc + 2 * npx, cnt, n, keys);
+        size_t tb = 0;
+        TDM_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, keys, sorted, n, 0, 32, stream_));
+        grow_coarse_tmp(tb);
+        TDM_CUDA(cub::DeviceRadixSort::SortKeys(d_coarse_tmp_, tb, keys, sorted, n, 0, 32, stream_));
+      }
+      k_nodia_quantile<<<1, 1, 0, stream_>>>(sorted, cnt, a.quantile_fraction, d_coarse_cnt_ + kMaxLevels + 2);
+    }
     TDM_CUDA(cudaGetLastError());
-    TDM_CUDA(cudaMemcpyAsync(h_coarse_cnt_, d_coarse_cnt_, 4 * (kMaxLevels + 1), cudaMemcpyDeviceToHost, stream_));
+    TDM_CUDA(cudaMemcpyAsync(h_coarse_cnt_, d_coarse_cnt_, 4 * (kMaxLevels + (nodia ? 4 : 1)), cudaMemcpyDeviceToHost, stream_));
     TDM_CUDA(cudaStreamSynchronize(stream_));
+    if (nodia) {   // written whether or not the levels fit below
+      nodia->pc_n_nodia = h_coarse_cnt_[kMaxLevels + 1];
+      std::memcpy(&nodia->idepth_quantile, h_coarse_cnt_ + kMaxLevels + 2, 4);
+      std::memcpy(&nodia->depth_quantile, h_coarse_cnt_ + kMaxLevels + 3, 4);
+      have_nodia_ = true;
+    }
     // Capacity: each level needs room for its count and the slot behind it; level 0 also for the dense points.
     int cnt[kMaxLevels];
     bool fits = true;
@@ -1289,6 +1364,16 @@ class TrackerImpl final : public TrackerIface {
     }
     if (!fits) throw Error("set_coarse_tracking_ref: a level's n_max is too small for its points; every level's reference is now empty");
     for (int l = 0; l < kMaxLevels; ++l) pc_n[l] = l < L ? cnt[l] : 0;
+  }
+  void get_coarse_nodia(int n, float* u, float* v, float* idepth, float* color) override {
+    TDM_CHECK(have_nodia_, "get_coarse_nodia before any set_coarse_tracking_ref call with the nodia outputs on this tracker");
+    const size_t npx = (size_t)w_ * h_;
+    TDM_CHECK(n >= 0 && (size_t)n <= npx, "get_coarse_nodia: bad n");
+    TDM_CUDA(cudaSetDevice(device_));
+    float* dst[4] = {u, v, idepth, color};
+    for (int k = 0; k < 4; ++k)
+      if (dst[k]) TDM_CUDA(cudaMemcpyAsync(dst[k], d_nodia_ + (k + 1) * npx, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_));
   }
   void synchronize() override {
     TDM_CUDA(cudaSetDevice(device_));
@@ -1329,9 +1414,10 @@ class TrackerImpl final : public TrackerIface {
       for (int l = 0; l < kMaxLevels; ++l) tot += (size_t)(w_ >> l) * (h_ >> l);
       TDM_CUDA(cudaMalloc(&d_coarse_, 3 * 4 * tot));
       TDM_CUDA(cudaMalloc(&d_rowlast_, 8 * (size_t)h_));
-      TDM_CUDA(cudaMalloc(&d_coarse_cnt_, 4 * (kMaxLevels + 1)));
-      TDM_CUDA(cudaMalloc(&d_coarse_stale_, 4 * kMaxLevels));
-      TDM_CUDA(cudaMallocHost(&h_coarse_cnt_, 4 * (kMaxLevels + 1)));
+      // counts per level, the dense count, then (nodia) pc_n_nodia and the quantile's idepth and depth bits
+      TDM_CUDA(cudaMalloc(&d_coarse_cnt_, 4 * (kMaxLevels + 4)));
+      TDM_CUDA(cudaMalloc(&d_coarse_stale_, 4 * (kMaxLevels + 1)));
+      TDM_CUDA(cudaMallocHost(&h_coarse_cnt_, 4 * (kMaxLevels + 4)));
     }
     if (n > coarse_cap_) {
       const int cap = n > 1024 ? n : 1024;
@@ -1345,6 +1431,22 @@ class TrackerImpl final : public TrackerIface {
       coarse_tmp_bytes_ = tb;
       coarse_cap_ = cap;
     }
+  }
+  void grow_coarse_tmp(size_t tb) {
+    if (tb <= coarse_tmp_bytes_) return;
+    TDM_CUDA(cudaStreamSynchronize(stream_));
+    cudaFree(d_coarse_tmp_);
+    d_coarse_tmp_ = nullptr; coarse_tmp_bytes_ = 0;
+    TDM_CUDA(cudaMalloc(&d_coarse_tmp_, tb));
+    coarse_tmp_bytes_ = tb;
+  }
+  // the nodia image (unweighted idepth sums of level 0) and the persistent pc_u/v/idepth/color_nodia, w*h floats each; the
+  // arrays start zeroed, so a slot nothing has written reads as 0
+  void ensure_nodia_buffers() {
+    if (d_nodia_) return;
+    const size_t npx = (size_t)w_ * h_;
+    TDM_CUDA(cudaMalloc(&d_nodia_, 5 * 4 * npx));
+    TDM_CUDA(cudaMemsetAsync(d_nodia_ + npx, 0, 4 * 4 * npx, stream_));
   }
   // KRKi = (K R) Ki, Kt = K t in float, k = 0,1,2 (CoarseTracker.cpp:676-677)
   DenseWarp dense_warp(const double* T) const {
@@ -1655,6 +1757,8 @@ class TrackerImpl final : public TrackerIface {
   void* d_coarse_tmp_ = nullptr;
   size_t coarse_tmp_bytes_ = 0;
   int coarse_cap_ = 0;
+  float* d_nodia_ = nullptr;   // ensure_nodia_buffers
+  bool have_nodia_ = false;
 };
 
 

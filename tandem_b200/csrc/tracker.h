@@ -122,8 +122,18 @@ class TrackerIface {
     int step = 1, dense_only = 0;
     float ref_exposure = 1.f;
     const double* ref_aff = nullptr;
+    float quantile_fraction = 0.f;      // with nodia: the fraction of get_idepth_quantile, in [0, 1]
   };
-  virtual void set_coarse_tracking_ref(TrackerIface* const* levels, const CoarseRefArgs& a, int pc_n[5]) = 0;
+  // With nodia also the undilated level-0 cloud pc_*_nodia (CoarseTracker.cpp:150-218, kept by levels[0] across calls) and
+  // the MVSNet depth range's inverse-depth quantile over it (FullSystem.cpp:1175, tandem_backend.cpp:354-361)
+  struct CoarseNodiaResult {
+    int pc_n_nodia;
+    float idepth_quantile, depth_quantile;   // NaN when the quantile's index is not below pc_n_nodia
+  };
+  virtual void set_coarse_tracking_ref(TrackerIface* const* levels, const CoarseRefArgs& a, int pc_n[5],
+                                       CoarseNodiaResult* nodia /* null: n7 alone */) = 0;
+  // the first n entries of levels[0]'s pc_u/v/idepth/color_nodia; an error before the first call with nodia
+  virtual void get_coarse_nodia(int n, float* u, float* v, float* idepth, float* color) = 0;
 };
 
 // FrameHessian::makeImages on the device (n2): all pyramid levels of (I, dx, dy) + absSquaredGrad.

@@ -5,7 +5,7 @@ import ctypes
 
 import numpy as np
 
-from ._lib import TrackNewCoarseResult, TrackPyramidResult, TrackResult, TrackTry, check, lib
+from ._lib import CoarseNodiaResult, TrackNewCoarseResult, TrackPyramidResult, TrackResult, TrackTry, check, lib
 
 _fp = ctypes.POINTER(ctypes.c_float)
 _dp = ctypes.POINTER(ctypes.c_double)
@@ -157,6 +157,13 @@ class CudaCoarseTracker:
         check(lib().tdm_tracker_get_reference(self._h, n, *[a.ctypes.data_as(_fp) for a in out]))
         return out
 
+    def getCoarseNodia(self, n):
+        """The first n entries of (pc_u, pc_v, pc_idepth, pc_color)_nodia, the undilated level-0 cloud this tracker holds as
+        levels[0] of set_coarse_tracking_ref_nodia (n = pc_n_nodia + 1 includes the slot behind the count)."""
+        out = [np.empty(n, np.float32) for _ in range(4)]
+        check(lib().tdm_tracker_get_coarse_nodia(self._h, n, *[a.ctypes.data_as(_fp) for a in out]))
+        return out
+
     def track(self, refToNew, aff_g2l, new_exposure, coarse_cutoff=20.0, max_iterations=10,
               lambda_extrapolation_limit=0.001, fix_a=False, fix_b=False):
         """One pyramid level of CoarseTracker::trackNewestCoarse (CoarseTracker.cpp:761-916) on the device."""
@@ -245,15 +252,9 @@ def track_new_coarse(trackers, tries, aff_last_2_l, new_exposure, last_coarse_rm
                 have_one_good=bool(r.have_one_good), tries=r.tries, winner=r.winner, device_ms=r.device_ms, per_try=per_try)
 
 
-def set_coarse_tracking_ref(levels, points, ref_pyramid, depth=None, fusion=None, render_index=0, T_depth_to_ref=None,
-                            tracking_step=1, dense_only=False, rgbd_init=False, ref_exposure=1.0, ref_aff_g2l=(0.0, 0.0)):
-    """CoarseTracker::setCoarseTrackingRef with makeCoarseDepthL0 (CoarseTracker.cpp:148-374, :633-733) for every level in one
-    call on the device.  levels[l] is the CudaCoarseTracker of pyramid level l ((w >> l) x (h >> l)), levels[0] with setK.
-    points = (u, v, idepth, hessian) in the reference's order - monocular: centerProjectedTo[0..2] and efPoint->HdiF of the
-    points passing the lastResiduals[0] test; rgbd_init: ph->u, ph->v, ph->idepth, ph->idepth_hessian - or None for no points.
-    Colours come from ref_pyramid (an ImagePyramid of the reference keyframe).  The optional dense map is a host depth image or
-    the render_index-th render of a DrFusion, warped with T_depth_to_ref (4x4) and appended behind level 0's points.
-    Returns pc_n, one count per level; each level then holds its reference as after setReference."""
+def _coarse_ref_call(levels, points, ref_pyramid, depth, fusion, render_index, T_depth_to_ref, tracking_step, dense_only, rgbd_init,
+                     ref_exposure, ref_aff_g2l, nodia=None):
+    """n7 (nodia None) or its nodia entry (nodia = (quantile_fraction, CoarseNodiaResult)); returns pc_n."""
     n_levels = len(levels)
     hs = (ctypes.c_void_p * max(n_levels, 1))(*[t._h for t in levels])
     keep = []
@@ -271,8 +272,38 @@ def set_coarse_tracking_ref(levels, points, ref_pyramid, depth=None, fusion=None
     T = None if T_depth_to_ref is None else np.ascontiguousarray(T_depth_to_ref, np.float64)
     aff = np.ascontiguousarray(ref_aff_g2l, np.float64)
     pc_n = np.zeros(5, np.int32)
-    check(lib().tdm_tracker_set_coarse_tracking_ref(
-        hs, n_levels, int(bool(rgbd_init)), n, pts[0], pts[1], pts[2], pts[3], ref_pyramid._h, ptr(depth),
-        None if fusion is None else fusion._h, int(render_index), None if T is None else T.ctypes.data_as(_dp), int(tracking_step),
-        int(bool(dense_only)), float(ref_exposure), aff.ctypes.data_as(_dp), pc_n.ctypes.data_as(ctypes.POINTER(ctypes.c_int))))
+    args = [hs, n_levels, int(bool(rgbd_init)), n, pts[0], pts[1], pts[2], pts[3], ref_pyramid._h, ptr(depth),
+            None if fusion is None else fusion._h, int(render_index), None if T is None else T.ctypes.data_as(_dp),
+            int(tracking_step), int(bool(dense_only)), float(ref_exposure), aff.ctypes.data_as(_dp)]
+    pc_n_p = pc_n.ctypes.data_as(ctypes.POINTER(ctypes.c_int))
+    if nodia is None:
+        check(lib().tdm_tracker_set_coarse_tracking_ref(*args, pc_n_p))
+    else:
+        check(lib().tdm_tracker_set_coarse_tracking_ref_nodia(*args, float(nodia[0]), pc_n_p, ctypes.byref(nodia[1])))
     return [int(x) for x in pc_n[:n_levels]]
+
+
+def set_coarse_tracking_ref(levels, points, ref_pyramid, depth=None, fusion=None, render_index=0, T_depth_to_ref=None,
+                            tracking_step=1, dense_only=False, rgbd_init=False, ref_exposure=1.0, ref_aff_g2l=(0.0, 0.0)):
+    """CoarseTracker::setCoarseTrackingRef with makeCoarseDepthL0 (CoarseTracker.cpp:148-374, :633-733) for every level in one
+    call on the device.  levels[l] is the CudaCoarseTracker of pyramid level l ((w >> l) x (h >> l)), levels[0] with setK.
+    points = (u, v, idepth, hessian) in the reference's order - monocular: centerProjectedTo[0..2] and efPoint->HdiF of the
+    points passing the lastResiduals[0] test; rgbd_init: ph->u, ph->v, ph->idepth, ph->idepth_hessian - or None for no points.
+    Colours come from ref_pyramid (an ImagePyramid of the reference keyframe).  The optional dense map is a host depth image or
+    the render_index-th render of a DrFusion, warped with T_depth_to_ref (4x4) and appended behind level 0's points.
+    Returns pc_n, one count per level; each level then holds its reference as after setReference."""
+    return _coarse_ref_call(levels, points, ref_pyramid, depth, fusion, render_index, T_depth_to_ref, tracking_step, dense_only,
+                            rgbd_init, ref_exposure, ref_aff_g2l)
+
+
+def set_coarse_tracking_ref_nodia(levels, points, ref_pyramid, quantile_fraction=0.2, depth=None, fusion=None, render_index=0,
+                                  T_depth_to_ref=None, tracking_step=1, dense_only=False, rgbd_init=False, ref_exposure=1.0,
+                                  ref_aff_g2l=(0.0, 0.0)):
+    """set_coarse_tracking_ref, plus in the same call the undilated level-0 cloud pc_*_nodia (CoarseTracker.cpp:150-218, held
+    by levels[0], see CudaCoarseTracker.getCoarseNodia) and get_idepth_quantile over it (tandem_backend.cpp:354-361), from
+    which FullSystem::deliverDrFrame takes MVSNet's depth range (depth_max = 3 * depth_quantile).
+    Returns (pc_n, pc_n_nodia, depth_quantile); depth_quantile is NaN when the cloud has no entry at the quantile's index."""
+    r = CoarseNodiaResult()
+    pc_n = _coarse_ref_call(levels, points, ref_pyramid, depth, fusion, render_index, T_depth_to_ref, tracking_step, dense_only,
+                            rgbd_init, ref_exposure, ref_aff_g2l, nodia=(quantile_fraction, r))
+    return pc_n, r.pc_n_nodia, r.depth_quantile
