@@ -184,20 +184,19 @@ int tdm_mvsnet_run_resident_multi(tdm_mvsnet* const* hs, int n, int iters_total,
   for (int j = 0; j < n; ++j) st[j] = (cudaStream_t)hs[j]->impl->resident_stream();
   hs[0]->impl->resident_launch(0);   // drains every engine's worker before the clock starts
   for (int j = 1; j < n; ++j) hs[j]->impl->resident_launch(0);
-  std::vector<cudaEvent_t> ev(n + 1);
-  for (auto& e : ev) TDM_CUDA(cudaEventCreate(&e));
-  TDM_CUDA(cudaEventRecord(ev[0], st[0]));
-  for (int j = 1; j < n; ++j) TDM_CUDA(cudaStreamWaitEvent(st[j], ev[0], 0));
+  std::vector<tdm::Event> ev(n + 1);
+  for (auto& e : ev) e = tdm::make_event();
+  TDM_CUDA(cudaEventRecord(ev[0].get(), st[0]));
+  for (int j = 1; j < n; ++j) TDM_CUDA(cudaStreamWaitEvent(st[j], ev[0].get(), 0));
   int nl = 0;
   for (int it = 0; it < iters_total; ++it) nl = hs[it % n]->impl->resident_launch(1);   // round robin, one stream per engine
   for (int j = 1; j < n; ++j) {
-    TDM_CUDA(cudaEventRecord(ev[j], st[j]));
-    TDM_CUDA(cudaStreamWaitEvent(st[0], ev[j], 0));
+    TDM_CUDA(cudaEventRecord(ev[j].get(), st[j]));
+    TDM_CUDA(cudaStreamWaitEvent(st[0], ev[j].get(), 0));
   }
-  TDM_CUDA(cudaEventRecord(ev[n], st[0]));
-  TDM_CUDA(cudaEventSynchronize(ev[n]));
-  TDM_CUDA(cudaEventElapsedTime(ms_total, ev[0], ev[n]));
-  for (auto& e : ev) cudaEventDestroy(e);
+  TDM_CUDA(cudaEventRecord(ev[n].get(), st[0]));
+  TDM_CUDA(cudaEventSynchronize(ev[n].get()));
+  TDM_CUDA(cudaEventElapsedTime(ms_total, ev[0].get(), ev[n].get()));
   if (launches) *launches = nl;
   return TDM_OK;
   TDM_API_END

@@ -5,8 +5,10 @@
 #include <cuda_fp16.h>
 #include <cstdint>
 #include <cstdio>
+#include <memory>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 
 namespace tdm {
 
@@ -27,6 +29,42 @@ struct Error : std::runtime_error {
   do {                                                                          \
     if (!(cond)) throw ::tdm::Error(std::string("check failed: ") + (msg));     \
   } while (0)
+
+// Owners of CUDA resources: each releases its resource when it goes out of scope, so a throw between two creations leaks
+// nothing and no class frees by hand.  The device alias of mapped host memory (cudaHostGetDevicePointer) is a plain pointer.
+struct DevFree { void operator()(void* p) const { cudaFree(p); } };
+struct HostFree { void operator()(void* p) const { cudaFreeHost(p); } };
+struct EventDestroy { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
+struct StreamDestroy { void operator()(cudaStream_t s) const { cudaStreamDestroy(s); } };
+struct GraphExecDestroy { void operator()(cudaGraphExec_t g) const { cudaGraphExecDestroy(g); } };
+struct GraphDestroy { void operator()(cudaGraph_t g) const { cudaGraphDestroy(g); } };
+
+template <typename T> using DevPtr = std::unique_ptr<T, DevFree>;
+template <typename T> using HostPtr = std::unique_ptr<T, HostFree>;   // cudaMallocHost and cudaHostAlloc memory
+using Event = std::unique_ptr<std::remove_pointer_t<cudaEvent_t>, EventDestroy>;
+using Stream = std::unique_ptr<std::remove_pointer_t<cudaStream_t>, StreamDestroy>;
+using GraphExec = std::unique_ptr<std::remove_pointer_t<cudaGraphExec_t>, GraphExecDestroy>;
+using Graph = std::unique_ptr<std::remove_pointer_t<cudaGraph_t>, GraphDestroy>;
+
+template <typename T = void> DevPtr<T> make_dev(size_t bytes) {
+  void* p = nullptr;
+  TDM_CUDA(cudaMalloc(&p, bytes));
+  return DevPtr<T>(static_cast<T*>(p));
+}
+// flags 0 is cudaMallocHost; cudaHostAllocMapped for memory the device reads and writes in place
+template <typename T = void> HostPtr<T> make_host(size_t bytes, unsigned flags = cudaHostAllocDefault) {
+  void* p = nullptr;
+  TDM_CUDA(cudaHostAlloc(&p, bytes, flags));
+  return HostPtr<T>(static_cast<T*>(p));
+}
+inline Event make_event(unsigned flags = cudaEventDefault) { cudaEvent_t e; TDM_CUDA(cudaEventCreateWithFlags(&e, flags)); return Event(e); }
+inline Stream make_stream(int priority) {   // non-blocking; priority 0 is the default
+  cudaStream_t s;
+  TDM_CUDA(cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, priority));
+  return Stream(s);
+}
+inline Graph make_graph() { cudaGraph_t g; TDM_CUDA(cudaGraphCreate(&g, 0)); return Graph(g); }
+inline GraphExec make_graph_exec(cudaGraph_t g) { cudaGraphExec_t x; TDM_CUDA(cudaGraphInstantiate(&x, g, 0)); return GraphExec(x); }
 
 inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 

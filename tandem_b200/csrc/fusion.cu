@@ -808,58 +808,47 @@ class FusionImpl final : public FusionIface {
     d_.mod_c32 = (unsigned)((1ull << 32) % (unsigned long long)o.num_buckets);
     int lo, hi;
     TDM_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    TDM_CUDA(cudaStreamCreateWithPriority(&stream_, cudaStreamNonBlocking, lo));  // low priority as tsdf_volume.cu:64-75
-    TDM_CUDA(cudaMalloc(&d_.keys, n_entries_ * 8));
-    TDM_CUDA(cudaMalloc(&d_.ptrs, n_entries_ * 4));
-    TDM_CUDA(cudaMalloc(&d_.voxels, (size_t)o.num_blocks * 512 * 8));
-    TDM_CUDA(cudaMalloc(&d_.list, (size_t)o.num_blocks * sizeof(int4)));
-    TDM_CUDA(cudaMalloc(&d_.counters, 8 * sizeof(int)));
-    TDM_CUDA(cudaMalloc(&d_.bbox, 6 * sizeof(int)));
+    stream_ = make_stream(lo);  // low priority as tsdf_volume.cu:64-75
+    keys_ = make_dev<unsigned long long>(n_entries_ * 8); d_.keys = keys_.get();
+    ptrs_ = make_dev<int>(n_entries_ * 4); d_.ptrs = ptrs_.get();
+    voxels_ = make_dev<uint2>((size_t)o.num_blocks * 512 * 8); d_.voxels = voxels_.get();
+    list_ = make_dev<int4>((size_t)o.num_blocks * sizeof(int4)); d_.list = list_.get();
+    counters_ = make_dev<int>(8 * sizeof(int)); d_.counters = counters_.get();
+    bbox_ = make_dev<int>(6 * sizeof(int)); d_.bbox = bbox_.get();
     {
       const int init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
       TDM_CUDA(cudaMemcpy(d_.bbox, init, sizeof(init), cudaMemcpyHostToDevice));
     }
-    TDM_CUDA(cudaMalloc(&d_vis_list_, (size_t)o.num_blocks * sizeof(int)));
-    TDM_CUDA(cudaMemsetAsync(d_.voxels, 0, (size_t)o.num_blocks * 512 * 8, stream_));
-    TDM_CUDA(cudaMemsetAsync(d_.counters, 0, 8 * sizeof(int), stream_));
-    k_fill_keys<<<cdiv(n_entries_, 256), 256, 0, stream_>>>(d_.keys, d_.ptrs, n_entries_);
+    d_vis_list_ = make_dev<int>((size_t)o.num_blocks * sizeof(int));
+    TDM_CUDA(cudaMemsetAsync(d_.voxels, 0, (size_t)o.num_blocks * 512 * 8, stream_.get()));
+    TDM_CUDA(cudaMemsetAsync(d_.counters, 0, 8 * sizeof(int), stream_.get()));
+    k_fill_keys<<<cdiv(n_entries_, 256), 256, 0, stream_.get()>>>(d_.keys, d_.ptrs, n_entries_);
     TDM_CUDA(cudaGetLastError());
     const size_t npx = (size_t)o.height * o.width;
-    TDM_CUDA(cudaMallocHost(&h_bgr_in_, npx * 3));
-    TDM_CUDA(cudaMallocHost(&h_depth_in_, npx * 4));
-    TDM_CUDA(cudaMalloc(&d_bgr_in_, npx * 3));
-    TDM_CUDA(cudaMalloc(&d_depth_in_, npx * 4));
+    h_bgr_in_ = make_host<unsigned char>(npx * 3);
+    h_depth_in_ = make_host<float>(npx * 4);
+    d_bgr_in_ = make_dev<unsigned char>(npx * 3);
+    d_depth_in_ = make_dev<float>(npx * 4);
     const int ns = std::max(1, o.num_render_streams);
     for (int half = 0; half < 2; ++half) {
-      TDM_CUDA(cudaMallocHost(&h_bgr_out_[half], npx * 3 * ns));
-      TDM_CUDA(cudaMallocHost(&h_depth_out_[half], npx * 4 * ns));
-      std::memset(h_bgr_out_[half], 0, npx * 3 * ns);     // "slab_exchange" mode never writes them: GetRenderResult then hands out
-      std::memset(h_depth_out_[half], 0, npx * 4 * ns);   // all-miss images rather than uninitialised memory
+      h_bgr_out_[half] = make_host<unsigned char>(npx * 3 * ns);
+      h_depth_out_[half] = make_host<float>(npx * 4 * ns);
+      std::memset(h_bgr_out_[half].get(), 0, npx * 3 * ns);     // "slab_exchange" mode never writes them: GetRenderResult then hands out
+      std::memset(h_depth_out_[half].get(), 0, npx * 4 * ns);   // all-miss images rather than uninitialised memory
     }
-    TDM_CUDA(cudaMalloc(&d_bgr_out_, npx * 3 * ns));
-    TDM_CUDA(cudaMalloc(&d_depth_out_, npx * 4 * ns));
-    TDM_CUDA(cudaMallocHost(&h_counters_, 8 * sizeof(int)));
-    TDM_CUDA(cudaEventCreateWithFlags(&ev_int_, cudaEventDisableTiming));
-    TDM_CUDA(cudaEventCreateWithFlags(&ev_render_, cudaEventDisableTiming));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    d_bgr_out_ = make_dev<unsigned char>(npx * 3 * ns);
+    d_depth_out_ = make_dev<float>(npx * 4 * ns);
+    h_counters_ = make_host<int>(8 * sizeof(int));
+    ev_int_ = make_event(cudaEventDisableTiming);
+    ev_render_ = make_event(cudaEventDisableTiming);
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
     render_poses_.resize(ns);
   }
 
   ~FusionImpl() override {
     cudaSetDevice(device_);
-    cudaStreamSynchronize(stream_);
+    cudaStreamSynchronize(stream_.get());
     for (void* q : ipc_opened_) cudaIpcCloseMemHandle(q);
-    cudaFree(d_.keys); cudaFree(d_.ptrs); cudaFree(d_.voxels); cudaFree(d_.list); cudaFree(d_.counters); cudaFree(d_.bbox); cudaFree(d_vis_list_);
-    cudaFreeHost(h_bgr_in_); cudaFreeHost(h_depth_in_); cudaFree(d_bgr_in_); cudaFree(d_depth_in_);
-    for (int half = 0; half < 2; ++half) { cudaFreeHost(h_bgr_out_[half]); cudaFreeHost(h_depth_out_[half]); }
-    cudaFree(d_bgr_out_); cudaFree(d_depth_out_); cudaFreeHost(h_counters_);
-    cudaEventDestroy(ev_int_); cudaEventDestroy(ev_render_);
-    cudaFree(d_hit_keys_); cudaFree(d_unpack_depth_); cudaFree(d_unpack_bgr_);
-    cudaFree(d_mesh_tables_); cudaFree(d_mesh_counts_); cudaFree(d_mesh_offsets_); cudaFree(d_mesh_total_);
-    cudaFree(d_mesh_vert_); cudaFree(d_mesh_cols_); cudaFreeHost(h_mesh_total_);
-    if (ev_mesh0_) cudaEventDestroy(ev_mesh0_);
-    if (ev_mesh1_) cudaEventDestroy(ev_mesh1_);
-    cudaStreamDestroy(stream_);
   }
 
   // IntegrateScanAsync, tsdf_volume.cu:515-598
@@ -878,20 +867,20 @@ class FusionImpl final : public FusionIface {
     if (page_locked(bgr) && page_locked(depth)) {
       // page-locked caller buffers: DMA straight from them; they are only ours during this call (tsdf_volume.cu:542-543
       // copies before returning), so wait for the two DMAs (2.15 MB, ~45 us) - cheaper than the staging memcpy it replaces
-      TDM_CUDA(cudaMemcpyAsync(d_bgr_in_, bgr, npx * 3, cudaMemcpyHostToDevice, stream_));
-      TDM_CUDA(cudaMemcpyAsync(d_depth_in_, depth, npx * 4, cudaMemcpyHostToDevice, stream_));
-      TDM_CUDA(cudaEventRecord(ev_int_, stream_));
+      TDM_CUDA(cudaMemcpyAsync(d_bgr_in_.get(), bgr, npx * 3, cudaMemcpyHostToDevice, stream_.get()));
+      TDM_CUDA(cudaMemcpyAsync(d_depth_in_.get(), depth, npx * 4, cudaMemcpyHostToDevice, stream_.get()));
+      TDM_CUDA(cudaEventRecord(ev_int_.get(), stream_.get()));
       launch_integrate();
-      TDM_CUDA(cudaEventSynchronize(ev_int_));
+      TDM_CUDA(cudaEventSynchronize(ev_int_.get()));
     } else {
-      TDM_CUDA(cudaEventSynchronize(ev_int_));  // previous scan has left the pinned staging buffers
-      std::memcpy(h_bgr_in_, bgr, npx * 3);
-      std::memcpy(h_depth_in_, depth, npx * 4);
-      TDM_CUDA(cudaMemcpyAsync(d_bgr_in_, h_bgr_in_, npx * 3, cudaMemcpyHostToDevice, stream_));
-      TDM_CUDA(cudaMemcpyAsync(d_depth_in_, h_depth_in_, npx * 4, cudaMemcpyHostToDevice, stream_));
+      TDM_CUDA(cudaEventSynchronize(ev_int_.get()));  // previous scan has left the pinned staging buffers
+      std::memcpy(h_bgr_in_.get(), bgr, npx * 3);
+      std::memcpy(h_depth_in_.get(), depth, npx * 4);
+      TDM_CUDA(cudaMemcpyAsync(d_bgr_in_.get(), h_bgr_in_.get(), npx * 3, cudaMemcpyHostToDevice, stream_.get()));
+      TDM_CUDA(cudaMemcpyAsync(d_depth_in_.get(), h_depth_in_.get(), npx * 4, cudaMemcpyHostToDevice, stream_.get()));
       launch_integrate();
     }
-    TDM_CUDA(cudaEventRecord(ev_int_, stream_));
+    TDM_CUDA(cudaEventRecord(ev_int_.get(), stream_.get()));
     have_scan_ = true;
     ++volume_epoch_;   // a pending mesh extracted before this scan no longer describes the volume
     next_ = kRender;
@@ -911,13 +900,13 @@ class FusionImpl final : public FusionIface {
     if (!inv4_f32(p.m, pinv.m)) throw Error("camera pose is singular");
     TDM_CUDA(cudaSetDevice(device_));
     const size_t npx = (size_t)d_.o.height * d_.o.width;
-    TDM_CUDA(cudaStreamWaitEvent(stream_, (cudaEvent_t)ready, 0));
-    TDM_CUDA(cudaMemcpyAsync(d_bgr_in_, bgr, npx * 3, cudaMemcpyDeviceToDevice, stream_));
-    TDM_CUDA(cudaMemcpyAsync(d_depth_in_, depth, npx * 4, cudaMemcpyDeviceToDevice, stream_));
+    TDM_CUDA(cudaStreamWaitEvent(stream_.get(), (cudaEvent_t)ready, 0));
+    TDM_CUDA(cudaMemcpyAsync(d_bgr_in_.get(), bgr, npx * 3, cudaMemcpyDeviceToDevice, stream_.get()));
+    TDM_CUDA(cudaMemcpyAsync(d_depth_in_.get(), depth, npx * 4, cudaMemcpyDeviceToDevice, stream_.get()));
     pose_ = p;
     pose_inv_ = pinv;
     launch_integrate();
-    TDM_CUDA(cudaEventRecord(ev_int_, stream_));
+    TDM_CUDA(cudaEventRecord(ev_int_.get(), stream_.get()));
     have_scan_ = true;
     ++volume_epoch_;
     next_ = kRender;
@@ -930,7 +919,7 @@ class FusionImpl final : public FusionIface {
     TDM_CUDA(cudaSetDevice(device_));
     for (int i = 0; i < n; ++i) std::memcpy(render_poses_[i].m, poses[i], 64);
     launch_render(n, true);
-    TDM_CUDA(cudaEventRecord(ev_render_, stream_));
+    TDM_CUDA(cudaEventRecord(ev_render_.get(), stream_.get()));
     n_rendered_ = n;
     next_ = kGet;
   }
@@ -940,11 +929,11 @@ class FusionImpl final : public FusionIface {
     if (next_ != kGet) throw Error("call order is IntegrateScanAsync -> RenderAsync -> GetRenderResult (tsdf_volume.cu:703-708)");
     if (n != n_rendered_) throw Error("GetRenderResult: wrong number of outputs");
     TDM_CUDA(cudaSetDevice(device_));
-    if (!slab_exchange_) TDM_CUDA(cudaEventSynchronize(ev_render_));   // exchange mode: nothing was copied back, nothing to wait for
+    if (!slab_exchange_) TDM_CUDA(cudaEventSynchronize(ev_render_.get()));   // exchange mode: nothing was copied back, nothing to wait for
     const size_t npx = (size_t)d_.o.height * d_.o.width;
     for (int i = 0; i < n; ++i) {
-      bgr[i] = h_bgr_out_[free_half_] + (size_t)i * npx * 3;
-      depth[i] = h_depth_out_[free_half_] + (size_t)i * npx;
+      bgr[i] = h_bgr_out_[free_half_].get() + (size_t)i * npx * 3;
+      depth[i] = h_depth_out_[free_half_].get() + (size_t)i * npx;
     }
     free_half_ ^= 1;  // the returned half stays valid until the next GetRenderResult (tsdf_volume.cu:719-732)
     next_ = kIntegrate;
@@ -1016,20 +1005,20 @@ class FusionImpl final : public FusionIface {
 
   void synchronize() override {
     TDM_CUDA(cudaSetDevice(device_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
   }
 
   void get_stats(tdm_fusion_stats* s) override {
     fetch_counters();
-    s->allocated_blocks = std::min(h_counters_[0], d_.o.num_blocks);
-    s->dropped_blocks = h_counters_[1];
-    s->visible_blocks = h_counters_[2];
-    s->candidate_blocks = h_counters_[3];
+    s->allocated_blocks = std::min(h_counters_.get()[0], d_.o.num_blocks);
+    s->dropped_blocks = h_counters_.get()[1];
+    s->visible_blocks = h_counters_.get()[2];
+    s->candidate_blocks = h_counters_.get()[3];
   }
 
   long long dump_blocks(int* coords, void* voxels, size_t cap) override {
     fetch_counters();
-    const long long n = std::min(h_counters_[0], d_.o.num_blocks);
+    const long long n = std::min(h_counters_.get()[0], d_.o.num_blocks);
     if (!coords) return n;
     std::vector<int4> list((size_t)n);
     TDM_CUDA(cudaMemcpy(list.data(), d_.list, (size_t)n * sizeof(int4), cudaMemcpyDeviceToHost));
@@ -1098,9 +1087,9 @@ class FusionImpl final : public FusionIface {
 
   const float* render_depth_device(int i, void** ready_event, int* device) override {
     TDM_CHECK(i >= 0 && i < n_rendered_, "render_depth_device: no such render");
-    if (ready_event) *ready_event = (void*)ev_render_;
+    if (ready_event) *ready_event = (void*)ev_render_.get();
     if (device) *device = device_;
-    return d_depth_out_ + (size_t)i * d_.o.height * d_.o.width;
+    return d_depth_out_.get() + (size_t)i * d_.o.height * d_.o.width;
   }
   // slab exchange step: device buffer of packed nearest-hit keys of render i (valid until the next call), stream synchronised
   long long* render_keys_device(int i) override {
@@ -1109,67 +1098,64 @@ class FusionImpl final : public FusionIface {
     const int npx = d_.o.height * d_.o.width;
     if (slab_exchange_) {   // the ray-cast wrote the keys itself; no extra kernel, no host sync: the caller's collective is
       TDM_CHECK(i == 0 && d_hit_keys_, "slab exchange mode packs render 0 only");   // enqueued on stream() behind it
-      return d_hit_keys_;
+      return d_hit_keys_.get();
     }
-    if (!d_hit_keys_) TDM_CUDA(cudaMalloc(&d_hit_keys_, (size_t)npx * sizeof(long long)));
-    k_pack_hits<<<cdiv(npx, 256), 256, 0, stream_>>>(d_depth_out_ + (size_t)i * npx, d_bgr_out_ + (size_t)i * npx * 3, d_hit_keys_, npx);
+    if (!d_hit_keys_) d_hit_keys_ = make_dev<long long>((size_t)npx * sizeof(long long));
+    k_pack_hits<<<cdiv(npx, 256), 256, 0, stream_.get()>>>(d_depth_out_.get() + (size_t)i * npx, d_bgr_out_.get() + (size_t)i * npx * 3, d_hit_keys_.get(), npx);
     TDM_CUDA(cudaGetLastError());
-    TDM_CUDA(cudaStreamSynchronize(stream_));
-    return d_hit_keys_;
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
+    return d_hit_keys_.get();
   }
-  void* stream() override { return (void*)stream_; }
+  void* stream() override { return (void*)stream_.get(); }
   void unpack_keys(const long long* keys_dev, float* depth_out, unsigned char* bgr_out) override {
     TDM_CUDA(cudaSetDevice(device_));
     const int npx = d_.o.height * d_.o.width;
-    if (!d_unpack_depth_) {
-      TDM_CUDA(cudaMalloc(&d_unpack_depth_, (size_t)npx * 4));
-      TDM_CUDA(cudaMalloc(&d_unpack_bgr_, (size_t)npx * 3));
+    if (!d_unpack_depth_) {   // set last: the pair is complete once it is
+      DevPtr<float> depth = make_dev<float>((size_t)npx * 4);
+      d_unpack_bgr_ = make_dev<unsigned char>((size_t)npx * 3);
+      d_unpack_depth_ = std::move(depth);
     }
-    k_unpack_hits<<<cdiv(npx, 256), 256, 0, stream_>>>(keys_dev, d_unpack_depth_, d_unpack_bgr_, npx);
+    k_unpack_hits<<<cdiv(npx, 256), 256, 0, stream_.get()>>>(keys_dev, d_unpack_depth_.get(), d_unpack_bgr_.get(), npx);
     TDM_CUDA(cudaGetLastError());
-    TDM_CUDA(cudaMemcpyAsync(depth_out, d_unpack_depth_, (size_t)npx * 4, cudaMemcpyDeviceToHost, stream_));
-    TDM_CUDA(cudaMemcpyAsync(bgr_out, d_unpack_bgr_, (size_t)npx * 3, cudaMemcpyDeviceToHost, stream_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    TDM_CUDA(cudaMemcpyAsync(depth_out, d_unpack_depth_.get(), (size_t)npx * 4, cudaMemcpyDeviceToHost, stream_.get()));
+    TDM_CUDA(cudaMemcpyAsync(bgr_out, d_unpack_bgr_.get(), (size_t)npx * 3, cudaMemcpyDeviceToHost, stream_.get()));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
   }
   void run_resident(int iters, float* ms_int, float* ms_render) override {
     TDM_CHECK(have_scan_, "run_resident: no scan submitted yet");
     TDM_CUDA(cudaSetDevice(device_));
-    cudaEvent_t e0, e1, e2;
-    TDM_CUDA(cudaEventCreate(&e0)); TDM_CUDA(cudaEventCreate(&e1)); TDM_CUDA(cudaEventCreate(&e2));
-    TDM_CUDA(cudaEventCreate(&ev_split_));
+    const Event e0 = make_event(), e1 = make_event(), e2 = make_event(), split = make_event();
     float ti = 0, tr = 0, ta = 0;
     const int n = std::max(1, d_.o.num_render_streams);
     if (render_poses_.empty()) render_poses_.resize(1);
     for (int it = 0; it < iters; ++it) {
-      TDM_CUDA(cudaEventRecord(e0, stream_));
-      launch_integrate();
-      TDM_CUDA(cudaEventRecord(e1, stream_));
+      TDM_CUDA(cudaEventRecord(e0.get(), stream_.get()));
+      launch_integrate(split.get());
+      TDM_CUDA(cudaEventRecord(e1.get(), stream_.get()));
       launch_render(n, false);
-      TDM_CUDA(cudaEventRecord(e2, stream_));
-      TDM_CUDA(cudaEventSynchronize(e2));
+      TDM_CUDA(cudaEventRecord(e2.get(), stream_.get()));
+      TDM_CUDA(cudaEventSynchronize(e2.get()));
       float a, b, c;
-      TDM_CUDA(cudaEventElapsedTime(&a, e0, e1));
-      TDM_CUDA(cudaEventElapsedTime(&b, e1, e2));
-      TDM_CUDA(cudaEventElapsedTime(&c, e0, ev_split_));
+      TDM_CUDA(cudaEventElapsedTime(&a, e0.get(), e1.get()));
+      TDM_CUDA(cudaEventElapsedTime(&b, e1.get(), e2.get()));
+      TDM_CUDA(cudaEventElapsedTime(&c, e0.get(), split.get()));
       ti += a; tr += b; ta += c;
     }
-    cudaEventDestroy(e0); cudaEventDestroy(e1); cudaEventDestroy(e2);
-    cudaEventDestroy(ev_split_);
-    ev_split_ = nullptr;
     *ms_int = ti; *ms_render = tr;
     last_alloc_ms_ = ta / std::max(iters, 1);
   }
 
  private:
-  void launch_integrate() {
+  // split (run_resident only) is recorded between the allocation and the visibility pass
+  void launch_integrate(cudaEvent_t split = nullptr) {
     const int npx = d_.o.height * d_.o.width;
-    TDM_CUDA(cudaMemsetAsync(d_.counters + 2, 0, 2 * sizeof(int), stream_));
-    k_allocate<<<cdiv(npx, 128), 128, 0, stream_>>>(d_, d_depth_in_, pose_);
+    TDM_CUDA(cudaMemsetAsync(d_.counters + 2, 0, 2 * sizeof(int), stream_.get()));
+    k_allocate<<<cdiv(npx, 128), 128, 0, stream_.get()>>>(d_, d_depth_in_.get(), pose_);
     TDM_CUDA(cudaGetLastError());
-    if (ev_split_) TDM_CUDA(cudaEventRecord(ev_split_, stream_));
-    k_visible<<<cdiv(d_.o.num_blocks, 256), 256, 0, stream_>>>(d_, pose_inv_, d_vis_list_);
+    if (split) TDM_CUDA(cudaEventRecord(split, stream_.get()));
+    k_visible<<<cdiv(d_.o.num_blocks, 256), 256, 0, stream_.get()>>>(d_, pose_inv_, d_vis_list_.get());
     TDM_CUDA(cudaGetLastError());
-    k_integrate_list<<<132 * 8, 256, 0, stream_>>>(d_, d_bgr_in_, d_depth_in_, pose_inv_, d_vis_list_);
+    k_integrate_list<<<132 * 8, 256, 0, stream_.get()>>>(d_, d_bgr_in_.get(), d_depth_in_.get(), pose_inv_, d_vis_list_.get());
     TDM_CUDA(cudaGetLastError());
   }
   void launch_render(int n, bool copy_back) {
@@ -1178,49 +1164,50 @@ class FusionImpl final : public FusionIface {
     const bool peer = d_.pr_world > 1;
     const bool slab = !peer && (d_.slab_lo != INT_MIN || d_.slab_hi != INT_MAX) && slab_clip_;
     for (int i = 0; i < n; ++i) {
-      unsigned char* bo = d_bgr_out_ + (size_t)i * npx * 3;
-      float* dout_i = d_depth_out_ + (size_t)i * npx;
+      unsigned char* bo = d_bgr_out_.get() + (size_t)i * npx * 3;
+      float* dout_i = d_depth_out_.get() + (size_t)i * npx;
       long long* keys = nullptr;
       if (slab_exchange_ && raycast_shared_ && i == 0) {   // k_raycast writes no keys
-        if (!d_hit_keys_) TDM_CUDA(cudaMalloc(&d_hit_keys_, npx * sizeof(long long)));
-        keys = d_hit_keys_;
+        if (!d_hit_keys_) d_hit_keys_ = make_dev<long long>(npx * sizeof(long long));
+        keys = d_hit_keys_.get();
       }
       const Mat4& T = render_poses_[i];
-      if (!raycast_shared_) k_raycast<<<dim3(cdiv(d_.o.width, 16), cdiv(d_.o.height, 16)), 256, 0, stream_>>>(d_, T, bo, dout_i);
-      else if (peer) k_raycast_shared<false, false, true><<<grid8, 64, 0, stream_>>>(d_, T, bo, dout_i, keys);
-      else if (slab && fast_div_) k_raycast_shared<true, true, false><<<grid8, 64, 0, stream_>>>(d_, T, bo, dout_i, keys);
-      else if (slab) k_raycast_shared<true, false, false><<<grid8, 64, 0, stream_>>>(d_, T, bo, dout_i, keys);
-      else if (fast_div_) k_raycast_shared<false, true, false><<<grid8, 64, 0, stream_>>>(d_, T, bo, dout_i, keys);
-      else k_raycast_shared<false, false, false><<<grid8, 64, 0, stream_>>>(d_, T, bo, dout_i, keys);
+      if (!raycast_shared_) k_raycast<<<dim3(cdiv(d_.o.width, 16), cdiv(d_.o.height, 16)), 256, 0, stream_.get()>>>(d_, T, bo, dout_i);
+      else if (peer) k_raycast_shared<false, false, true><<<grid8, 64, 0, stream_.get()>>>(d_, T, bo, dout_i, keys);
+      else if (slab && fast_div_) k_raycast_shared<true, true, false><<<grid8, 64, 0, stream_.get()>>>(d_, T, bo, dout_i, keys);
+      else if (slab) k_raycast_shared<true, false, false><<<grid8, 64, 0, stream_.get()>>>(d_, T, bo, dout_i, keys);
+      else if (fast_div_) k_raycast_shared<false, true, false><<<grid8, 64, 0, stream_.get()>>>(d_, T, bo, dout_i, keys);
+      else k_raycast_shared<false, false, false><<<grid8, 64, 0, stream_.get()>>>(d_, T, bo, dout_i, keys);
       TDM_CUDA(cudaGetLastError());
     }
     if (copy_back && !slab_exchange_) {   // slab exchange mode: the per-slab render is only an operand of the exchange step
-      TDM_CUDA(cudaMemcpyAsync(h_bgr_out_[free_half_], d_bgr_out_, npx * 3 * n, cudaMemcpyDeviceToHost, stream_));
-      TDM_CUDA(cudaMemcpyAsync(h_depth_out_[free_half_], d_depth_out_, npx * 4 * n, cudaMemcpyDeviceToHost, stream_));
+      TDM_CUDA(cudaMemcpyAsync(h_bgr_out_[free_half_].get(), d_bgr_out_.get(), npx * 3 * n, cudaMemcpyDeviceToHost, stream_.get()));
+      TDM_CUDA(cudaMemcpyAsync(h_depth_out_[free_half_].get(), d_depth_out_.get(), npx * 4 * n, cudaMemcpyDeviceToHost, stream_.get()));
     }
   }
   static constexpr int kMeshGrid = 132 * 8;   // 8 CTAs per SM of an H100 SXM
   // count + scan + emit + total on stream_ (no host sync)
   void launch_mesh_all() {
-    TDM_CUDA(cudaEventRecord(ev_mesh0_, stream_));
-    k_mesh<false><<<kMeshGrid, 256, 0, stream_>>>(d_, mesh_axes_, d_mesh_counts_, nullptr, 0, nullptr, nullptr);
+    TDM_CUDA(cudaEventRecord(ev_mesh0_.get(), stream_.get()));
+    k_mesh<false><<<kMeshGrid, 256, 0, stream_.get()>>>(d_, mesh_axes_, d_mesh_counts_.get(), nullptr, 0, nullptr, nullptr);
     TDM_CUDA(cudaGetLastError());
-    k_mesh_scan<<<1, 1024, 0, stream_>>>(d_mesh_counts_, d_mesh_offsets_, d_.counters, d_.o.num_blocks, d_mesh_total_);
+    k_mesh_scan<<<1, 1024, 0, stream_.get()>>>(d_mesh_counts_.get(), d_mesh_offsets_.get(), d_.counters, d_.o.num_blocks, d_mesh_total_.get());
     TDM_CUDA(cudaGetLastError());
     launch_mesh_emit();
-    TDM_CUDA(cudaMemcpyAsync(h_mesh_total_, d_mesh_total_, sizeof(int), cudaMemcpyDeviceToHost, stream_));
-    TDM_CUDA(cudaEventRecord(ev_mesh1_, stream_));
+    TDM_CUDA(cudaMemcpyAsync(h_mesh_total_.get(), d_mesh_total_.get(), sizeof(int), cudaMemcpyDeviceToHost, stream_.get()));
+    TDM_CUDA(cudaEventRecord(ev_mesh1_.get(), stream_.get()));
   }
   void start_mesh(const float* lower, const float* upper) {
     TDM_CUDA(cudaSetDevice(device_));
     const int nblk = d_.o.num_blocks;
-    if (!d_mesh_counts_) {
-      TDM_CUDA(cudaMalloc(&d_mesh_counts_, (size_t)nblk * sizeof(int)));
-      TDM_CUDA(cudaMalloc(&d_mesh_offsets_, (size_t)nblk * sizeof(int)));
-      TDM_CUDA(cudaMalloc(&d_mesh_total_, sizeof(int)));
-      TDM_CUDA(cudaMallocHost(&h_mesh_total_, sizeof(int)));
-      TDM_CUDA(cudaEventCreate(&ev_mesh0_));
-      TDM_CUDA(cudaEventCreate(&ev_mesh1_));
+    if (!d_mesh_counts_) {   // set last: the group is complete once it is
+      DevPtr<int> counts = make_dev<int>((size_t)nblk * sizeof(int));
+      d_mesh_offsets_ = make_dev<int>((size_t)nblk * sizeof(int));
+      d_mesh_total_ = make_dev<int>(sizeof(int));
+      h_mesh_total_ = make_host<int>(sizeof(int));
+      ev_mesh0_ = make_event();
+      ev_mesh1_ = make_event();
+      d_mesh_counts_ = std::move(counts);
     }
     // per-axis tables -> one device buffer: [cells x | cells y | cells z | ranges x | ranges y | ranges z]
     MeshAxisHost A[3];
@@ -1240,9 +1227,9 @@ class FusionImpl final : public FusionIface {
     *h_mesh_total_ = 0;
     if (empty) return;
     if (bytes > mesh_tables_cap_) {
-      cudaFree(d_mesh_tables_);
-      d_mesh_tables_ = nullptr;
-      TDM_CUDA(cudaMalloc(&d_mesh_tables_, bytes));
+      d_mesh_tables_.reset();
+      mesh_tables_cap_ = 0;
+      d_mesh_tables_ = make_dev<char>(bytes);
       mesh_tables_cap_ = bytes;
     }
     std::vector<char> host(bytes, 0);
@@ -1250,18 +1237,18 @@ class FusionImpl final : public FusionIface {
     for (int a = 0; a < 3; ++a) {
       const size_t nb = A[a].cells.size() * sizeof(MeshAxisCell);
       std::memcpy(host.data() + off, A[a].cells.data(), nb);
-      mesh_axes_.cells[a] = reinterpret_cast<const MeshAxisCell*>(d_mesh_tables_ + off);
+      mesh_axes_.cells[a] = reinterpret_cast<const MeshAxisCell*>(d_mesh_tables_.get() + off);
       off += (nb + 15) / 16 * 16;
     }
     for (int a = 0; a < 3; ++a) {
       const size_t nb = A[a].ranges.size() * sizeof(int2);
       std::memcpy(host.data() + off, A[a].ranges.data(), nb);
-      mesh_axes_.brange[a] = reinterpret_cast<const int2*>(d_mesh_tables_ + off);
+      mesh_axes_.brange[a] = reinterpret_cast<const int2*>(d_mesh_tables_.get() + off);
       off += (nb + 15) / 16 * 16;
       mesh_axes_.bmin[a] = A[a].bmin;
       mesh_axes_.nb[a] = A[a].nb;
     }
-    TDM_CUDA(cudaMemcpyAsync(d_mesh_tables_, host.data(), off, cudaMemcpyHostToDevice, stream_));  // pageable: staged before return
+    TDM_CUDA(cudaMemcpyAsync(d_mesh_tables_.get(), host.data(), off, cudaMemcpyHostToDevice, stream_.get()));  // pageable: staged before return
     if (!d_mesh_vert_) {   // first estimate (72 B per triangle, 2 M triangles = 151 MB); finish_mesh grows it when the count says so
       const char* init = getenv("TDM_MESH_INIT_TRIS");
       grow_mesh_buffers(init && atoll(init) > 0 ? atoll(init) : (1 << 21));
@@ -1272,8 +1259,8 @@ class FusionImpl final : public FusionIface {
   long long finish_mesh(float* vert, float* cols, size_t max_vertices, bool query_only) {
     if (mesh_empty_) { mesh_ms_ = 0.f; return 0; }
     TDM_CUDA(cudaSetDevice(device_));
-    TDM_CUDA(cudaEventSynchronize(ev_mesh1_));
-    TDM_CUDA(cudaEventElapsedTime(&mesh_ms_, ev_mesh0_, ev_mesh1_));
+    TDM_CUDA(cudaEventSynchronize(ev_mesh1_.get()));
+    TDM_CUDA(cudaEventElapsedTime(&mesh_ms_, ev_mesh0_.get(), ev_mesh1_.get()));
     long long ntri = *h_mesh_total_;
     // (also for a count-only query: the count handed out must be the count of the mesh the copy call will deliver)
     // First estimate too small: grow and run the extraction again.  The per-block counts / offsets of the first run are
@@ -1284,9 +1271,9 @@ class FusionImpl final : public FusionIface {
       TDM_CHECK(attempt < 4, "mesh output kept outgrowing its buffers");
       grow_mesh_buffers(ntri + ntri / 4);
       launch_mesh_all();
-      TDM_CUDA(cudaEventSynchronize(ev_mesh1_));
+      TDM_CUDA(cudaEventSynchronize(ev_mesh1_.get()));
       float again = 0.f;
-      TDM_CUDA(cudaEventElapsedTime(&again, ev_mesh0_, ev_mesh1_));
+      TDM_CUDA(cudaEventElapsedTime(&again, ev_mesh0_.get(), ev_mesh1_.get()));
       mesh_ms_ += again;
       ntri = *h_mesh_total_;
       mesh_epoch_ = volume_epoch_;
@@ -1297,42 +1284,47 @@ class FusionImpl final : public FusionIface {
       throw Error("Did not provide enough storage for mesh. (tsdf_volume.cu:796-799)");
     if (nv > 0) {
       TDM_CHECK(vert && cols, "null mesh output buffers");
-      TDM_CUDA(cudaMemcpy(vert, d_mesh_vert_, (size_t)nv * 3 * sizeof(float), cudaMemcpyDeviceToHost));
-      TDM_CUDA(cudaMemcpy(cols, d_mesh_cols_, (size_t)nv * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+      TDM_CUDA(cudaMemcpy(vert, d_mesh_vert_.get(), (size_t)nv * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+      TDM_CUDA(cudaMemcpy(cols, d_mesh_cols_.get(), (size_t)nv * 3 * sizeof(float), cudaMemcpyDeviceToHost));
     }
     return nv;
   }
   void grow_mesh_buffers(long long tris) {
-    cudaFree(d_mesh_vert_); cudaFree(d_mesh_cols_);
-    d_mesh_vert_ = d_mesh_cols_ = nullptr;
+    d_mesh_vert_.reset(); d_mesh_cols_.reset();
     mesh_cap_tris_ = 0;
-    TDM_CUDA(cudaMalloc(&d_mesh_vert_, (size_t)tris * 9 * sizeof(float)));
-    TDM_CUDA(cudaMalloc(&d_mesh_cols_, (size_t)tris * 9 * sizeof(float)));
+    d_mesh_vert_ = make_dev<float>((size_t)tris * 9 * sizeof(float));
+    d_mesh_cols_ = make_dev<float>((size_t)tris * 9 * sizeof(float));
     mesh_cap_tris_ = (int)std::min<long long>(tris, INT_MAX);
   }
   void launch_mesh_emit() {
-    k_mesh<true><<<kMeshGrid, 256, 0, stream_>>>(d_, mesh_axes_, d_mesh_counts_, d_mesh_offsets_, mesh_cap_tris_, d_mesh_vert_, d_mesh_cols_);
+    k_mesh<true><<<kMeshGrid, 256, 0, stream_.get()>>>(d_, mesh_axes_, d_mesh_counts_.get(), d_mesh_offsets_.get(), mesh_cap_tris_, d_mesh_vert_.get(), d_mesh_cols_.get());
     TDM_CUDA(cudaGetLastError());
   }
   void fetch_counters() {
     TDM_CUDA(cudaSetDevice(device_));
-    TDM_CUDA(cudaMemcpyAsync(h_counters_, d_.counters, 8 * sizeof(int), cudaMemcpyDeviceToHost, stream_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    TDM_CUDA(cudaMemcpyAsync(h_counters_.get(), d_.counters, 8 * sizeof(int), cudaMemcpyDeviceToHost, stream_.get()));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
   }
 
   enum Next { kIntegrate, kRender, kGet };
   int device_;
   FusionDev d_{};
   long long n_entries_ = 0;
-  cudaStream_t stream_ = nullptr;
-  cudaEvent_t ev_int_ = nullptr, ev_render_ = nullptr;
-  unsigned char *h_bgr_in_ = nullptr, *d_bgr_in_ = nullptr;
-  float *h_depth_in_ = nullptr, *d_depth_in_ = nullptr;
-  unsigned char* h_bgr_out_[2] = {nullptr, nullptr};
-  float* h_depth_out_[2] = {nullptr, nullptr};
-  unsigned char* d_bgr_out_ = nullptr;
-  float* d_depth_out_ = nullptr;
-  int* h_counters_ = nullptr;
+  Stream stream_;
+  DevPtr<unsigned long long> keys_;   // the hash table and voxel pool d_ points at
+  DevPtr<int> ptrs_, counters_, bbox_;
+  DevPtr<uint2> voxels_;
+  DevPtr<int4> list_;
+  Event ev_int_, ev_render_;
+  HostPtr<unsigned char> h_bgr_in_;
+  DevPtr<unsigned char> d_bgr_in_;
+  HostPtr<float> h_depth_in_;
+  DevPtr<float> d_depth_in_;
+  HostPtr<unsigned char> h_bgr_out_[2];
+  HostPtr<float> h_depth_out_[2];
+  DevPtr<unsigned char> d_bgr_out_;
+  DevPtr<float> d_depth_out_;
+  HostPtr<int> h_counters_;
   int free_half_ = 0;
   Mat4 pose_{}, pose_inv_{};
   std::vector<Mat4> render_poses_;
@@ -1345,20 +1337,20 @@ class FusionImpl final : public FusionIface {
   bool slab_clip_ = true;        // Z-slab volumes: rays are only sampled inside the slab's z range (bit-identical, see k_raycast_shared)
   bool slab_exchange_ = false;   // Z-slab volumes: the ray-cast emits packed nearest-hit keys for the exchange step, the per-slab
                                  // render is not copied back and GetRenderResult does not wait (tandem_b200.parallel)
-  int* d_vis_list_ = nullptr;
-  cudaEvent_t ev_split_ = nullptr;
+  DevPtr<int> d_vis_list_;
   float last_alloc_ms_ = 0.f;
-  long long* d_hit_keys_ = nullptr;
-  float* d_unpack_depth_ = nullptr;
-  unsigned char* d_unpack_bgr_ = nullptr;
+  DevPtr<long long> d_hit_keys_;
+  DevPtr<float> d_unpack_depth_;
+  DevPtr<unsigned char> d_unpack_bgr_;
   // mesh extraction state
-  char* d_mesh_tables_ = nullptr;
+  DevPtr<char> d_mesh_tables_;
   size_t mesh_tables_cap_ = 0;
   MeshAxes mesh_axes_{};
-  int *d_mesh_counts_ = nullptr, *d_mesh_offsets_ = nullptr, *d_mesh_total_ = nullptr, *h_mesh_total_ = nullptr;
-  float *d_mesh_vert_ = nullptr, *d_mesh_cols_ = nullptr;
+  DevPtr<int> d_mesh_counts_, d_mesh_offsets_, d_mesh_total_;
+  HostPtr<int> h_mesh_total_;
+  DevPtr<float> d_mesh_vert_, d_mesh_cols_;
   int mesh_cap_tris_ = 0;
-  cudaEvent_t ev_mesh0_ = nullptr, ev_mesh1_ = nullptr;
+  Event ev_mesh0_, ev_mesh1_;
   enum MeshKind { kMeshNone, kMeshAsync, kMeshBlocking };
   MeshKind mesh_kind_ = kMeshNone;   // who owns the extraction sitting in the device buffers
   bool mesh_empty_ = false;

@@ -36,16 +36,19 @@ namespace {
 
 std::mutex g_slot_mu;
 bool g_slot_used[kMaxEngines] = {};
-int acquire_slot() {
-  std::lock_guard<std::mutex> lk(g_slot_mu);
-  for (int i = 0; i < kMaxEngines; ++i)
-    if (!g_slot_used[i]) { g_slot_used[i] = true; return i; }
-  throw Error("too many DrMvsnet instances alive in this process (max 8)");
-}
-void release_slot(int i) {
-  std::lock_guard<std::mutex> lk(g_slot_mu);
-  if (i >= 0 && i < kMaxEngines) g_slot_used[i] = false;
-}
+// An engine's index into the constant banks (c_call_params, c_feat_slot, c_conv00), held for the engine's lifetime.
+struct EngineSlot {
+  int index = -1;
+  EngineSlot() {
+    std::lock_guard<std::mutex> lk(g_slot_mu);
+    for (index = 0; index < kMaxEngines; ++index)
+      if (!g_slot_used[index]) { g_slot_used[index] = true; return; }
+    throw Error("too many DrMvsnet instances alive in this process (max 8)");
+  }
+  ~EngineSlot() { std::lock_guard<std::mutex> lk(g_slot_mu); g_slot_used[index] = false; }
+  EngineSlot(const EngineSlot&) = delete;
+  EngineSlot& operator=(const EngineSlot&) = delete;
+};
 
 // ---- small host linear algebra (double) --------------------------------------------------------
 void mat4_mul(const double* a, const double* b, double* c) {
@@ -90,7 +93,7 @@ void world_to_pixel(const float* K, const float* c2w, double* P) {
 }
 
 struct DevBuf {
-  void* p = nullptr;
+  DevPtr<void> p;
   size_t bytes = 0;       // allocation size (with halos)
   size_t alg_bytes = 0;   // algorithmic size C*D*H*W*sizeof(element): what the roofline counts
   int C = 0, D = 0, H = 0, W = 0;
@@ -102,10 +105,10 @@ struct DevBuf {
 struct DevConv {
   int cin = 0, cout = 0, kd = 1, kh = 1, kw = 1;
   bool transposed = false;
-  float* w = nullptr;
-  float* bias = nullptr;
+  DevPtr<float> w;
+  DevPtr<float> bias;
   // tensor-core path (conv_tc.cuh): weights pre-arranged as the canonical K-major B image in the input's 16-bit type
-  void* bimg = nullptr;
+  DevPtr<void> bimg;
   int npad = 0;
   bool tc_ok = false;
   bool tc_deconv = false;  // transposed conv evaluated as a GEMM over the input grid (N = 8 parity classes x cout)
@@ -114,15 +117,15 @@ struct DevConv {
   bool tc_up2 = false;     // MODE 3: the fused FPN tail, conv3x3 of a nearest-x2 up-sampled map + conv3x3 of a fine map,
                            // on the coarse grid
   bool tc_s2 = false;      // stride-2 conv on the tensor-map (strided TMA) kernel, conv_tc_s2.cuh
-  void* bimg_s2 = nullptr;
+  DevPtr<void> bimg_s2;
   int npad_s2 = 0, nsplit_s2 = 1;
-  void* bimg_is = nullptr;  // input-stationary B image (conv_tc_is.cuh): 3x3x3 layers with 1 or 8 output channels
+  DevPtr<void> bimg_is;  // input-stationary B image (conv_tc_is.cuh): 3x3x3 layers with 1 or 8 output channels
 };
 
 struct LaunchRec {
   std::string name;
   double bytes = 0, flops = 0;
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  Event e0, e1;
   float ms = 0;
 };
 
@@ -139,13 +142,12 @@ class MvsnetEngine final : public MvsnetIface {
     va_ = wf_.view_aggregation;
     int lo, hi;
     TDM_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    TDM_CUDA(cudaStreamCreateWithPriority(&stream_, cudaStreamNonBlocking, lo));
-    TDM_CUDA(cudaStreamCreateWithPriority(&side_stream_, cudaStreamNonBlocking, lo));
-    TDM_CUDA(cudaEventCreateWithFlags(&ev_fork_, cudaEventDisableTiming));
-    TDM_CUDA(cudaEventCreateWithFlags(&ev_join_, cudaEventDisableTiming));
-    slot_ = acquire_slot();
-    for (auto& e : ev_out_) TDM_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    TDM_CUDA(cudaEventCreateWithFlags(&ev_in_, cudaEventDisableTiming));
+    stream_ = make_stream(lo);
+    side_stream_ = make_stream(lo);
+    ev_fork_ = make_event(cudaEventDisableTiming);
+    ev_join_ = make_event(cudaEventDisableTiming);
+    for (auto& e : ev_out_) e = make_event(cudaEventDisableTiming);
+    ev_in_ = make_event(cudaEventDisableTiming);
     upload_weights();
     worker_ = std::thread([this] { this->loop(); });
   }
@@ -160,32 +162,11 @@ class MvsnetEngine final : public MvsnetIface {
     if (worker_.joinable()) worker_.join();
     cudaSetDevice(device_);
     // consumers of the keyframe handoff may still be reading it: read_handoff returns once their reads are enqueued
-    cudaStreamSynchronize(stream_);
-    for (int i = 0; i < n_ho_release_; ++i) cudaEventSynchronize(ev_ho_release_[i]);
-    for (cudaEvent_t e : ev_ho_release_) cudaEventDestroy(e);
-    if (ev_ho_ready_) cudaEventDestroy(ev_ho_ready_);
-    cudaFree(d_ho_depth_); cudaFree(d_ho_bgr_);
-    free_plan();
-    for (auto& kv : convs_) { cudaFree(kv.second.w); cudaFree(kv.second.bias); cudaFree(kv.second.bimg); cudaFree(kv.second.bimg_s2); cudaFree(kv.second.bimg_is); }
-    if (d_cv_stats_) {
-      unsigned st[2] = {0, 0};
-      if (std::getenv("TDM_DEBUG_PLAN") && cudaMemcpy(st, d_cv_stats_, sizeof(st), cudaMemcpyDeviceToHost) == cudaSuccess)
-        fprintf(stderr, "[cv_tma] (CTA, view) pairs staged by TMA: %u, fallen back to global gathers: %u\n", st[0], st[1]);
-      cudaFree(d_cv_stats_);
-    }
-    if (select_state_) cudaFree(select_state_);
-    if (select2_) cudaFree(select2_);
-    release_slot(slot_);
-    if (d_bs3_) cudaFree(d_bs3_);
-    if (h_params_) cudaFreeHost(h_params_);
-    if (h_feat_slot_) cudaFreeHost(h_feat_slot_);
-    if (d_params_) cudaFree(d_params_);
-    for (auto& e : ev_out_) if (e) cudaEventDestroy(e);
-    if (ev_in_) cudaEventDestroy(ev_in_);
-    if (ev_fork_) cudaEventDestroy(ev_fork_);
-    if (ev_join_) cudaEventDestroy(ev_join_);
-    if (side_stream_) cudaStreamDestroy(side_stream_);
-    if (stream_) cudaStreamDestroy(stream_);
+    cudaStreamSynchronize(stream_.get());
+    for (int i = 0; i < n_ho_release_; ++i) cudaEventSynchronize(ev_ho_release_[i].get());
+    unsigned st[2] = {0, 0};
+    if (d_cv_stats_ && std::getenv("TDM_DEBUG_PLAN") && cudaMemcpy(st, d_cv_stats_.get(), sizeof(st), cudaMemcpyDeviceToHost) == cudaSuccess)
+      fprintf(stderr, "[cv_tma] (CTA, view) pairs staged by TMA: %u, fallen back to global gathers: %u\n", st[0], st[1]);
   }
 
   void set_option(const std::string& key, int value) override {
@@ -195,7 +176,7 @@ class MvsnetEngine final : public MvsnetIface {
       cv_done_.wait(lk, [this] { return !busy_; });
     }
     TDM_CUDA(cudaSetDevice(device_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
     if (key == "eager_d2h") { eager_d2h_ = value != 0; return; }   // not part of the captured launch sequence
     drop_graph();
     cache_valid_ = false;   // features computed under other options are not reused
@@ -350,24 +331,24 @@ class MvsnetEngine final : public MvsnetIface {
       // Page-locked result buffers: the four maps are DMA'd from the device straight into them (they stay on the device
       // until this handle's next forward, which cannot start before this call returns) - no staging copy.
       for (int k = 0; k < 4; ++k)
-        TDM_CUDA(cudaMemcpyAsync(dst[k], fbuf(names[k]), n * 4, cudaMemcpyDeviceToHost, stream_));
-      TDM_CUDA(cudaStreamSynchronize(stream_));
+        TDM_CUDA(cudaMemcpyAsync(dst[k], fbuf(names[k]), n * 4, cudaMemcpyDeviceToHost, stream_.get()));
+      TDM_CUDA(cudaStreamSynchronize(stream_.get()));
     } else {
       if (!eager_d2h_) {   // the worker did not copy back: do it now
         for (int k = 0; k < 4; ++k) {
-          TDM_CUDA(cudaMemcpyAsync(h_out_ + k * n, fbuf(names[k]), n * 4, cudaMemcpyDeviceToHost, stream_));
-          TDM_CUDA(cudaEventRecord(ev_out_[k], stream_));
+          TDM_CUDA(cudaMemcpyAsync(h_out_.get() + k * n, fbuf(names[k]), n * 4, cudaMemcpyDeviceToHost, stream_.get()));
+          TDM_CUDA(cudaEventRecord(ev_out_[k].get(), stream_.get()));
         }
       }
       // each map is copied to caller memory by the pool as soon as its D2H has landed
       std::vector<CopyPool::Job> jobs;
-      TDM_CUDA(cudaEventSynchronize(ev_out_[3]));   // 4.9 MB over PCIe: ~0.1 ms; simpler than per-map hand-off
+      TDM_CUDA(cudaEventSynchronize(ev_out_[3].get()));   // 4.9 MB over PCIe: ~0.1 ms; simpler than per-map hand-off
       constexpr int kSlices = 2;
       for (int k = 0; k < 4; ++k)
         if (dst[k])
           for (int sl = 0; sl < kSlices; ++sl) {
             const size_t e0 = n * sl / kSlices, e1 = n * (sl + 1) / kSlices;
-            jobs.push_back({dst[k] + e0, h_out_ + k * n + e0, (e1 - e0) * 4, nullptr});
+            jobs.push_back({dst[k] + e0, h_out_.get() + k * n + e0, (e1 - e0) * 4, nullptr});
           }
       CopyPool::shared().run(jobs);
     }
@@ -379,11 +360,11 @@ class MvsnetEngine final : public MvsnetIface {
     std::unique_lock<std::mutex> lk(mu_);
     if (!ho_valid_) throw Error("no MVSNet result to integrate: call GetResult first");
     Handoff h;
-    h.depth = d_ho_depth_;
-    h.bgr = d_ho_bgr_;
+    h.depth = d_ho_depth_.get();
+    h.bgr = d_ho_bgr_.get();
     std::memcpy(h.c2w, ho_c2w_, sizeof(ho_c2w_));
     h.H = ho_H_; h.W = ho_W_; h.device = device_;
-    h.ready = (void*)ev_ho_ready_;
+    h.ready = (void*)ev_ho_ready_.get();
     try {
       consume(h);
     } catch (...) {
@@ -404,7 +385,7 @@ class MvsnetEngine final : public MvsnetIface {
     if (it == bufs_.end()) throw Error("no such stage output: " + name);
     const size_t n = (size_t)it->second.H * it->second.W;
     TDM_CHECK(cap >= n, "stage_output: capacity too small");
-    TDM_CUDA(cudaMemcpy(out, it->second.p, n * 4, cudaMemcpyDeviceToHost));
+    TDM_CUDA(cudaMemcpy(out, it->second.p.get(), n * 4, cudaMemcpyDeviceToHost));
   }
 
   // FeatureNet intermediates ("f.*") are those of the last forward, over the views it computed (k planes after a cached call);
@@ -421,17 +402,15 @@ class MvsnetEngine final : public MvsnetIface {
     if (!out) return n;
     TDM_CHECK((long long)cap >= n, "debug_tensor: capacity too small");
     if (b.f32) {
-      TDM_CUDA(cudaMemcpy(out, b.p, n * 4, cudaMemcpyDeviceToHost));  // C==1 planar already
+      TDM_CUDA(cudaMemcpy(out, b.p.get(), n * 4, cudaMemcpyDeviceToHost));  // C==1 planar already
       return n;
     }
-    float* tmp = nullptr;
-    TDM_CUDA(cudaMalloc(&tmp, n * 4));
-    if (b.kind == 2) k_p8_to_planar_f32<TV><<<cdiv(n, 256), 256, 0, stream_>>>(p8<const TV>(b), tmp);
-    else k_p8_to_planar_f32<TA><<<cdiv(n, 256), 256, 0, stream_>>>(p8<const TA>(b), tmp);
+    const DevPtr<float> tmp = make_dev<float>(n * 4);
+    if (b.kind == 2) k_p8_to_planar_f32<TV><<<cdiv(n, 256), 256, 0, stream_.get()>>>(p8<const TV>(b), tmp.get());
+    else k_p8_to_planar_f32<TA><<<cdiv(n, 256), 256, 0, stream_.get()>>>(p8<const TA>(b), tmp.get());
     TDM_CUDA(cudaGetLastError());
-    TDM_CUDA(cudaMemcpyAsync(out, tmp, n * 4, cudaMemcpyDeviceToHost, stream_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
-    cudaFree(tmp);
+    TDM_CUDA(cudaMemcpyAsync(out, tmp.get(), n * 4, cudaMemcpyDeviceToHost, stream_.get()));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
     if (b.kind == 2 && kVolScale != 1.f)
       for (long long i = 0; i < n; ++i) out[i] *= 1.f / kVolScale;   // report the volume in its own units
     if ((name == "feat1" || name == "feat2" || name == "feat3") && !slots_identity()) {
@@ -454,20 +433,16 @@ class MvsnetEngine final : public MvsnetIface {
     int slots[kMaxSrc + 1];
     for (int j = 0; j < n_new; ++j) slots[j] = view_slot_[window_index(V_ - n_new + j, last_ref_index_)];
     if (n_new < V_) ensure_feature_scratch(n_new);
-    cudaEvent_t e0, e1;
-    TDM_CUDA(cudaEventCreate(&e0));
-    TDM_CUDA(cudaEventCreate(&e1));
-    TDM_CUDA(cudaEventRecord(e0, stream_));
+    const Event e0 = make_event(), e1 = make_event();
+    TDM_CUDA(cudaEventRecord(e0.get(), stream_.get()));
     for (int i = 0; i < iters; ++i) forward(n_new, slots, false);
-    TDM_CUDA(cudaEventRecord(e1, stream_));
-    TDM_CUDA(cudaEventSynchronize(e1));
-    TDM_CUDA(cudaEventElapsedTime(ms_total, e0, e1));
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
+    TDM_CUDA(cudaEventRecord(e1.get(), stream_.get()));
+    TDM_CUDA(cudaEventSynchronize(e1.get()));
+    TDM_CUDA(cudaEventElapsedTime(ms_total, e0.get(), e1.get()));
     if (launches) *launches = launches_per_forward_;
   }
 
-  void* resident_stream() override { return (void*)stream_; }
+  void* resident_stream() override { return (void*)stream_.get(); }
   int resident_device() const override { return device_; }
   int resident_launch(int iters) override {
     wait();
@@ -484,12 +459,10 @@ class MvsnetEngine final : public MvsnetIface {
     forward(V_, nullptr, false);  // warm
     recs_.clear();
     forward(V_, nullptr, true);
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
     std::ostringstream os;
     for (auto& r : recs_) {
-      cudaEventElapsedTime(&r.ms, r.e0, r.e1);
-      cudaEventDestroy(r.e0);
-      cudaEventDestroy(r.e1);
+      cudaEventElapsedTime(&r.ms, r.e0.get(), r.e1.get());
       os << r.name << " " << r.ms << " " << (long long)r.bytes << " " << (long long)r.flops << "\n";
     }
     recs_.clear();
@@ -504,11 +477,11 @@ class MvsnetEngine final : public MvsnetIface {
       for (auto& v : fc.w) v *= 1.f / kVolScale;   // the stage's conv0 reads the volume stored as value * kVolScale (exact power of two)
     DevConv dc;
     dc.cin = fc.cin; dc.cout = fc.cout; dc.kd = fc.kd; dc.kh = fc.kh; dc.kw = fc.kw; dc.transposed = fc.transposed;
-    TDM_CUDA(cudaMalloc(&dc.w, fc.w.size() * 4));
-    TDM_CUDA(cudaMemcpy(dc.w, fc.w.data(), fc.w.size() * 4, cudaMemcpyHostToDevice));
+    dc.w = make_dev<float>(fc.w.size() * 4);
+    TDM_CUDA(cudaMemcpy(dc.w.get(), fc.w.data(), fc.w.size() * 4, cudaMemcpyHostToDevice));
     if (!fc.bias.empty()) {
-      TDM_CUDA(cudaMalloc(&dc.bias, fc.bias.size() * 4));
-      TDM_CUDA(cudaMemcpy(dc.bias, fc.bias.data(), fc.bias.size() * 4, cudaMemcpyHostToDevice));
+      dc.bias = make_dev<float>(fc.bias.size() * 4);
+      TDM_CUDA(cudaMemcpy(dc.bias.get(), fc.bias.data(), fc.bias.size() * 4, cudaMemcpyHostToDevice));
     }
     if (key.size() == 7 && key.compare(2, 5, ".prob") == 0 && key[0] == 's' && fc.w.size() == 216) {
       TDM_CHECK(fc.cin == 8 && fc.cout == 1 && fc.kd == 3 && fc.kh == 3 && fc.kw == 3, "unexpected prob layer shape");
@@ -557,7 +530,7 @@ class MvsnetEngine final : public MvsnetIface {
         dc.bimg_s2 = upload(img);
       }
     }
-    convs_[key] = dc;
+    convs_[key] = std::move(dc);
   }
 
   // Algebraic fusion of the FPN tail for stage 3 (module.py:522-530): feat3 = out3(up2(i2) + skip3(c3) + b3) is linear,
@@ -599,16 +572,15 @@ class MvsnetEngine final : public MvsnetIface {
     dc.npad = 32;
     dc.hilo = dc.tc_ok = dc.tc_up2 = true;
     upload_bimgs<TA>(a, dc);
-    TDM_CUDA(cudaMalloc(&d_bs3_, 32 * 4));
-    TDM_CUDA(cudaMemcpy(d_bs3_, ws.bias.data(), 32 * 4, cudaMemcpyHostToDevice));
+    d_bs3_ = make_dev<float>(32 * 4);
+    TDM_CUDA(cudaMemcpy(d_bs3_.get(), ws.bias.data(), 32 * 4, cudaMemcpyHostToDevice));
     fused_fpn_ = true;
   }
 
   template <typename T>
-  static void* upload(const std::vector<T>& img) {
-    void* p = nullptr;
-    TDM_CUDA(cudaMalloc(&p, img.size() * sizeof(T)));
-    TDM_CUDA(cudaMemcpy(p, img.data(), img.size() * sizeof(T), cudaMemcpyHostToDevice));
+  static DevPtr<void> upload(const std::vector<T>& img) {
+    DevPtr<void> p = make_dev(img.size() * sizeof(T));
+    TDM_CUDA(cudaMemcpy(p.get(), img.data(), img.size() * sizeof(T), cudaMemcpyHostToDevice));
     return p;
   }
   // B images of the stride-1 kernel and, for the 3x3x3 layers with 1 or 8 output channels, of the input-stationary one
@@ -636,7 +608,7 @@ class MvsnetEngine final : public MvsnetIface {
         for (int ci = 0; ci < 3; ++ci)
           for (int co = 0; co < 8; ++co) cw.w[t * 3 + ci][co] = c3.w[((size_t)t * 3 + ci) * 8 + co];
       for (int co = 0; co < 8; ++co) cw.bias[co] = c3.bias[co];
-      TDM_CUDA(cudaMemcpyToSymbol(c_conv00, &cw, sizeof(cw), (size_t)slot_ * sizeof(Conv00Weights)));
+      TDM_CUDA(cudaMemcpyToSymbol(c_conv00, &cw, sizeof(cw), (size_t)slot_.index * sizeof(Conv00Weights)));
     }
     {
       FoldedConv c00 = fold_conv(wf_, f + "conv0.0.conv.weight", "", f + "conv0.0.bn", false, 8);
@@ -689,12 +661,12 @@ class MvsnetEngine final : public MvsnetIface {
         gt.b2 = (float)b2;
       }
     }
-    TDM_CUDA(cudaMalloc(&select_state_, sizeof(SelectState)));
-    TDM_CUDA(cudaMalloc(&select2_, sizeof(SelectState2)));
-    TDM_CUDA(cudaMemset(select2_, 0, sizeof(SelectState2)));
-    TDM_CUDA(cudaMallocHost(&h_params_, sizeof(CallParams)));
-    TDM_CUDA(cudaMalloc(&d_params_, sizeof(CallParams)));
-    TDM_CUDA(cudaMallocHost(&h_feat_slot_, sizeof(c_feat_slot[0])));
+    select_state_ = make_dev<SelectState>(sizeof(SelectState));
+    select2_ = make_dev<SelectState2>(sizeof(SelectState2));
+    TDM_CUDA(cudaMemset(select2_.get(), 0, sizeof(SelectState2)));
+    h_params_ = make_host<CallParams>(sizeof(CallParams));
+    d_params_ = make_dev<CallParams>(sizeof(CallParams));
+    h_feat_slot_ = make_host<int>(sizeof(c_feat_slot[0]));
     for (int v = 0; v <= kMaxSrc; ++v) view_slot_[v] = v;
   }
 
@@ -714,8 +686,8 @@ class MvsnetEngine final : public MvsnetIface {
       b.pd = pd3 ? 1 : 0;
       b.bytes = (size_t)(C / 8) * (D + 2 * b.pd) * (H + 2) * (W + 2) * 8 * es + 4096;  // + slack for tile over-reads
     }
-    TDM_CUDA(cudaMalloc(&b.p, b.bytes));
-    TDM_CUDA(cudaMemsetAsync(b.p, 0, b.bytes, stream_));  // halos stay zero forever: kernels only write the interior
+    b.p = make_dev(b.bytes);
+    TDM_CUDA(cudaMemsetAsync(b.p.get(), 0, b.bytes, stream_.get()));  // halos stay zero forever: kernels only write the interior
     if (debug_poison_) {
       // all-ones bytes are a NaN in fp32, fp16 and bf16: a position the forward should have stored but did not reads as
       // non-finite instead of as a plausible 0 (which a ReLU layer's true output often is).  The P8 interiors and the
@@ -726,19 +698,20 @@ class MvsnetEngine final : public MvsnetIface {
         for (int p = 0; p < (C / 8) * (D + 2 * b.pd); ++p) {
           const int d = p % (D + 2 * b.pd);
           if (d < b.pd || d >= D + b.pd) continue;
-          TDM_CUDA(cudaMemset2DAsync((uint8_t*)b.p + ((size_t)p * (H + 2) + 1) * row + 8 * es, row, 0xFF, (size_t)W * 8 * es, H, stream_));
+          TDM_CUDA(cudaMemset2DAsync((uint8_t*)b.p.get() + ((size_t)p * (H + 2) + 1) * row + 8 * es, row, 0xFF, (size_t)W * 8 * es, H, stream_.get()));
         }
       } else if (name.size() >= 6 && name.compare(name.size() - 6, 6, "logits") == 0) {
-        TDM_CUDA(cudaMemsetAsync(b.p, 0xFF, b.bytes, stream_));
+        TDM_CUDA(cudaMemsetAsync(b.p.get(), 0xFF, b.bytes, stream_.get()));
       }
     }
-    bufs_[name] = b;
-    return bufs_[name];
+    DevBuf& slot = bufs_[name];
+    slot = std::move(b);
+    return slot;
   }
   template <typename T>
   static P8<T> p8(const DevBuf& b) {
     P8<T> t;
-    t.p = (T*)b.p;
+    t.p = (T*)b.p.get();
     t.C = b.C; t.D = b.D; t.H = b.H; t.W = b.W; t.pd = b.pd;
     t.Hp = b.H + 2; t.Wp = b.W + 2;
     t.gs = (long long)(b.D + 2 * b.pd) * t.Hp * t.Wp * 8;
@@ -748,19 +721,16 @@ class MvsnetEngine final : public MvsnetIface {
     drop_graph();
     cv_tmap_ok_ = false;
     tc_cache_.clear();
-    for (auto& kv : bufs_) cudaFree(kv.second.p);
     bufs_.clear();
-    if (h_bgr_) cudaFreeHost(h_bgr_);
-    if (h_out_) cudaFreeHost(h_out_);
-    if (d_bgr_) cudaFree(d_bgr_);
-    h_bgr_ = nullptr; h_out_ = nullptr; d_bgr_ = nullptr;
+    h_bgr_.reset();
+    h_out_.reset();
+    d_bgr_.reset();
     cache_valid_ = false;
     for (int v = 0; v <= kMaxSrc; ++v) view_slot_[v] = v;
   }
   // FeatureNet's buffers over D views; sfx "" = the whole window (feat1..feat3 are then the feature pool), "@k" = the scratch
   // of a cached forward over k new views
-  void alloc_featurenet(int D, const std::string& sfx) {
-    const int H = H_, W = W_;
+  void alloc_featurenet(int D, const std::string& sfx, int H, int W) {
     alloc("f.img" + sfx, 8, D, H, W);
     alloc("f.c0_0" + sfx, 8, D, H, W);
     alloc("f.c3" + sfx, 8, D, H, W);
@@ -779,16 +749,16 @@ class MvsnetEngine final : public MvsnetIface {
   }
   // made once per k and plan (freed with the plan), outside any capture: the forward over k views then replays as its own graph
   void ensure_feature_scratch(int k) {
-    if (!bufs_.count("feat1@" + std::to_string(k))) alloc_featurenet(k, "@" + std::to_string(k));
+    if (!bufs_.count("feat1@" + std::to_string(k))) alloc_featurenet(k, "@" + std::to_string(k), H_, W_);
   }
   void ensure_plan(int V, int H, int W) {
     if (V == V_ && H == H_ && W == W_) return;
     free_plan();
-    V_ = V; H_ = H; W_ = W;
-    TDM_CUDA(cudaMallocHost(&h_bgr_, (size_t)V * H * W * 3));
-    TDM_CUDA(cudaMallocHost(&h_out_, (size_t)4 * H * W * sizeof(float)));
-    TDM_CUDA(cudaMalloc(&d_bgr_, (size_t)V * H * W * 3));
-    alloc_featurenet(V, "");
+    V_ = H_ = W_ = 0;   // no plan until every buffer below exists
+    h_bgr_ = make_host<unsigned char>((size_t)V * H * W * 3);
+    h_out_ = make_host<float>((size_t)4 * H * W * sizeof(float));
+    d_bgr_ = make_dev<unsigned char>((size_t)V * H * W * 3);
+    alloc_featurenet(V, "", H, W);
     for (int s = 1; s <= 3; ++s) {
       const std::string k = "s" + std::to_string(s) + ".";
       const int sc = 1 << (3 - s);
@@ -814,8 +784,9 @@ class MvsnetEngine final : public MvsnetIface {
         alloc(k + n, 1, 1, Hs, Ws, true);
     }
     alloc("thr", 1, 1, 1, 4, true);
+    V_ = V; H_ = H; W_ = W;
   }
-  float* fbuf(const std::string& n) { return (float*)bufs_.at(n).p; }
+  float* fbuf(const std::string& n) { return (float*)bufs_.at(n).p.get(); }
 
   // ---------------------------------------------------------------- launches
   void rec_begin(const std::string& name, double bytes, double flops) {
@@ -823,20 +794,18 @@ class MvsnetEngine final : public MvsnetIface {
     if (!profiling_) return;
     LaunchRec r;
     r.name = name; r.bytes = bytes; r.flops = flops;
-    cudaEventCreate(&r.e0);
-    cudaEventCreate(&r.e1);
-    cudaEventRecord(r.e0, stream_);
-    recs_.push_back(r);
+    r.e0 = make_event();
+    r.e1 = make_event();
+    cudaEventRecord(r.e0.get(), stream_.get());
+    recs_.push_back(std::move(r));
   }
   void rec_end() {
     if (!profiling_) return;
-    cudaEventRecord(recs_.back().e1, stream_);
+    cudaEventRecord(recs_.back().e1.get(), stream_.get());
   }
   void rec_cancel() {
     --launch_count_;
     if (!profiling_) return;
-    cudaEventDestroy(recs_.back().e0);
-    cudaEventDestroy(recs_.back().e1);
     recs_.pop_back();
   }
 
@@ -848,36 +817,36 @@ class MvsnetEngine final : public MvsnetIface {
     if (res) r = p8<const TOut>(*res);
     P8<TOut> o{}, ob{};
     float* plain = nullptr;
-    if constexpr (COUT == 1) plain = (float*)out.p; else o = p8<TOut>(out);
+    if constexpr (COUT == 1) plain = (float*)out.p.get(); else o = p8<TOut>(out);
     if constexpr (COUT != 1) {
       if (out_b) {
         ob = p8<TOut>(*out_b);
-        launch_k(k_conv_direct<TIn, TOut, CIN, COUT>, dim3(cdiv(npos, 128)), dim3(128), p8<const TIn>(in), c.w, c.bias, r, o, plain, g, ob, bias_b);
+        launch_k(k_conv_direct<TIn, TOut, CIN, COUT>, dim3(cdiv(npos, 128)), dim3(128), p8<const TIn>(in), c.w.get(), c.bias.get(), r, o, plain, g, ob, bias_b);
         return;
       }
     }
     if constexpr (COUT >= 16) {
       if (npos < 128ll * 592) {  // too few positions to fill the chip: split the output channels over blockIdx.y
         dim3 grid(cdiv(npos, 128), COUT / 8);
-        launch_k(k_conv_direct<TIn, TOut, CIN, COUT, 8>, grid, dim3(128), p8<const TIn>(in), c.w, c.bias, r, o, plain, g, P8<TOut>{}, (const float*)nullptr);
+        launch_k(k_conv_direct<TIn, TOut, CIN, COUT, 8>, grid, dim3(128), p8<const TIn>(in), c.w.get(), c.bias.get(), r, o, plain, g, P8<TOut>{}, (const float*)nullptr);
         return;
       }
     }
-    launch_k(k_conv_direct<TIn, TOut, CIN, COUT>, dim3(cdiv(npos, 128)), dim3(128), p8<const TIn>(in), c.w, c.bias, r, o, plain, g, P8<TOut>{}, (const float*)nullptr);
+    launch_k(k_conv_direct<TIn, TOut, CIN, COUT>, dim3(cdiv(npos, 128)), dim3(128), p8<const TIn>(in), c.w.get(), c.bias.get(), r, o, plain, g, P8<TOut>{}, (const float*)nullptr);
   }
 
   // the other kernels of the forward (all begin with grid_dep_sync()): with use_pdl = 2 they carry the attribute too
   template <typename... KArgs, typename... Args>
   void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, Args&&... args) {
     if (use_pdl_ < 2) {
-      kern<<<grid, block, 0, stream_>>>(static_cast<KArgs>(args)...);
+      kern<<<grid, block, 0, stream_.get()>>>(static_cast<KArgs>(args)...);
       return;
     }
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = 0;
-    cfg.stream = stream_;
+    cfg.stream = stream_.get();
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
@@ -908,7 +877,7 @@ class MvsnetEngine final : public MvsnetIface {
     // with PDL an early-launched dependent must not stack several CTAs on the few SMs its predecessor left idle (they would
     // compete for those SMs' issue slots while the rest of the GPU waits): ask for enough shared memory that one CTA fills an SM
     cfg.dynamicSmemBytes = use_pdl_ ? std::max(smem, (size_t)pdl_min_smem_kb_ * 1024) : smem;
-    cfg.stream = stream_;
+    cfg.stream = stream_.get();
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = use_pdl_ ? 1 : 0;
@@ -946,7 +915,7 @@ class MvsnetEngine final : public MvsnetIface {
     const cuuint32_t box[4] = {8, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
     const cuuint32_t es[4] = {1, (cuuint32_t)estr, (cuuint32_t)estr, 1};
     const CUtensorMapDataType dt = std::is_same<TIn, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-    const CUresult r = tc::encode_tiled_fn()(&tmap, dt, 4, in.p, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    const CUresult r = tc::encode_tiled_fn()(&tmap, dt, 4, in.p.get(), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     TDM_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed for " + wkey + " (" + std::to_string((int)r) + ")");
@@ -992,8 +961,8 @@ class MvsnetEngine final : public MvsnetIface {
     if (profiling_) recs_.back().name = wkey + "[tc-is]";   // the record conv() opened as "[tc]"
     constexpr int NWG = tc::conv_nwg(0, 3 * CPK, Tail::max_d);
     TDM_CHECK(pl.nwg == NWG, wkey + ": tile plan balanced for another warpgroup count than the kernel's");
-    launch_tc<tc::k_conv_tc_is<TIn, TA, CIN, CPK, PLAIN, Tail, NWG>>(dim3(pl.grid), pl.smem, tcx.tmap, (const TIn*)c.bimg_is, (const float*)c.bias,
-                                                               PLAIN ? (TA*)nullptr : (TA*)out.p, PLAIN ? (float*)out.p : (float*)nullptr, pl.g, tail);
+    launch_tc<tc::k_conv_tc_is<TIn, TA, CIN, CPK, PLAIN, Tail, NWG>>(dim3(pl.grid), pl.smem, tcx.tmap, (const TIn*)c.bimg_is.get(), (const float*)c.bias.get(),
+                                                               PLAIN ? (TA*)nullptr : (TA*)out.p.get(), PLAIN ? (float*)out.p.get() : (float*)nullptr, pl.g, tail);
   }
 
   template <typename TIn, typename TOut, int CIN, int NPAD, int KD, bool PLAIN, int MODE = 0, bool HILO = false, typename Tail = tc::NoTail>
@@ -1029,8 +998,8 @@ class MvsnetEngine final : public MvsnetIface {
     const tc::Plan& pl = tcx.plan;
     TOut* op = nullptr;
     float* plain = nullptr;
-    if constexpr (PLAIN) plain = (float*)out.p;
-    else op = (TOut*)out.p;
+    if constexpr (PLAIN) plain = (float*)out.p.get();
+    else op = (TOut*)out.p.get();
     constexpr int NWG = tc::conv_nwg(MODE, HILO ? 2 * NPAD : NPAD, Tail::max_d);
     TDM_CHECK(pl.nwg == NWG, wkey + ": tile plan balanced for another warpgroup count than the kernel's");
     // MODE 1: each N slice of NPAD columns is 8 classes x NPAD / 8 channels, whole output channel groups of the box;
@@ -1039,8 +1008,8 @@ class MvsnetEngine final : public MvsnetIface {
               (MODE != 3 || c.cout == 8), wkey + ": parity-class layer with an unexpected cout");
     TDM_CHECK(MODE != 1 || (out.pd == 1 && (!res || (res->D == out.D && res->H == out.H && res->W == out.W && res->C == out.C))),
               wkey + ": transposed conv skip / output shapes differ");
-    launch_tc<tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail, NWG>>(dim3(pl.grid, c.nsplit), pl.smem, tcx.tmap, tcx.tmap_res, tcx.tmap_out, (const TIn*)c.bimg,
-                                                                              (const float*)c.bias, op, plain, pl.g, tail);
+    launch_tc<tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail, NWG>>(dim3(pl.grid, c.nsplit), pl.smem, tcx.tmap, tcx.tmap_res, tcx.tmap_out, (const TIn*)c.bimg.get(),
+                                                                              (const float*)c.bias.get(), op, plain, pl.g, tail);
   }
 
   template <int CIN, int NPAD, int KD, int KS>
@@ -1064,8 +1033,8 @@ class MvsnetEngine final : public MvsnetIface {
     const tc::PlanS2& pl = tcx.plan_s2;
     constexpr int NWG = tc::conv_nwg(0, NPAD, 0);
     TDM_CHECK(pl.nwg == NWG, wkey + ": tile plan balanced for another warpgroup count than the kernel's");
-    launch_tc<tc::k_conv_tc_s2<TA, TA, CIN, NPAD, KD, KS, NWG>>(dim3(pl.grid, c.nsplit_s2), pl.smem, tcx.tmap, (const TA*)c.bimg_s2,
-                                                          (const float*)c.bias, (TA*)out.p, pl.g);
+    launch_tc<tc::k_conv_tc_s2<TA, TA, CIN, NPAD, KD, KS, NWG>>(dim3(pl.grid, c.nsplit_s2), pl.smem, tcx.tmap, (const TA*)c.bimg_s2.get(),
+                                                          (const float*)c.bias.get(), (TA*)out.p.get(), pl.g);
   }
 
   bool conv_tc_s2_dispatch(const std::string& wkey, const DevBuf& bi, const DevConv& c, const DevBuf& bo, bool relu) {
@@ -1198,7 +1167,7 @@ class MvsnetEngine final : public MvsnetIface {
           wkey.size() == 7 && wkey.compare(2, 5, ".prob") == 0) {
         rec_begin(wkey + "[direct]", bytes, 2.0 * macs);
         const long long nthr = (long long)bi.D * bi.H * (bi.W / 4);
-        k_prob_direct<4><<<cdiv(nthr, 128), 128, 0, stream_>>>(p8<const __half>(bi), (float*)bo.p, prob_w_[wkey[1] - '1']);
+        k_prob_direct<4><<<cdiv(nthr, 128), 128, 0, stream_.get()>>>(p8<const __half>(bi), (float*)bo.p.get(), prob_w_[wkey[1] - '1']);
         TDM_CUDA(cudaGetLastError());
         rec_end();
         return;
@@ -1298,11 +1267,11 @@ class MvsnetEngine final : public MvsnetIface {
       cutoff = std::max(0ll, std::min((long long)n - 1, cutoff));
       h_params_->cutoff[s - 1] = (unsigned)cutoff;
     }
-    TDM_CUDA(cudaMemcpyAsync(d_params_, h_params_, sizeof(CallParams), cudaMemcpyHostToDevice, stream_));
-    TDM_CUDA(cudaMemcpyToSymbolAsync(c_call_params, h_params_, sizeof(CallParams), (size_t)slot_ * sizeof(CallParams),
-                                     cudaMemcpyHostToDevice, stream_));
-    TDM_CUDA(cudaMemcpyToSymbolAsync(c_feat_slot, h_feat_slot_, sizeof(c_feat_slot[0]), (size_t)slot_ * sizeof(c_feat_slot[0]),
-                                     cudaMemcpyHostToDevice, stream_));
+    TDM_CUDA(cudaMemcpyAsync(d_params_.get(), h_params_.get(), sizeof(CallParams), cudaMemcpyHostToDevice, stream_.get()));
+    TDM_CUDA(cudaMemcpyToSymbolAsync(c_call_params, h_params_.get(), sizeof(CallParams), (size_t)slot_.index * sizeof(CallParams),
+                                     cudaMemcpyHostToDevice, stream_.get()));
+    TDM_CUDA(cudaMemcpyToSymbolAsync(c_feat_slot, h_feat_slot_.get(), sizeof(c_feat_slot[0]), (size_t)slot_.index * sizeof(c_feat_slot[0]),
+                                     cudaMemcpyHostToDevice, stream_.get()));
   }
 
   void cost_volume(int s) {
@@ -1324,14 +1293,18 @@ class MvsnetEngine final : public MvsnetIface {
           const cuuint64_t strides[3] = {16, (cuuint64_t)(fb.W + 2) * 16, (cuuint64_t)(fb.W + 2) * (fb.H + 2) * 16};
           const cuuint32_t box[4] = {8, (cuuint32_t)kCvBW, (cuuint32_t)kCvBH, 1};
           const cuuint32_t estr[4] = {1, 1, 1, 1};
-          const CUresult r = tc::encode_tiled_fn()(&cv_tmap_, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, fb.p, dims, strides, box, estr,
+          const CUresult r = tc::encode_tiled_fn()(&cv_tmap_, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, fb.p.get(), dims, strides, box, estr,
                                                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
                                                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
           TDM_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed for the cost-volume source tile");
-          if (!d_cv_stats_) { TDM_CUDA(cudaMalloc(&d_cv_stats_, 2 * sizeof(unsigned))); TDM_CUDA(cudaMemset(d_cv_stats_, 0, 2 * sizeof(unsigned))); }
+          if (!d_cv_stats_) {
+            DevPtr<unsigned> st = make_dev<unsigned>(2 * sizeof(unsigned));
+            TDM_CUDA(cudaMemset(st.get(), 0, 2 * sizeof(unsigned)));
+            d_cv_stats_ = std::move(st);
+          }
           cv_tmap_ok_ = true;
         }
-        k_cost_volume_va16_tma<TV, true><<<dim3(cdiv(vb.W, 16), cdiv(vb.H, 8)), 256, 0, stream_>>>(cv_tmap_, p8<const __half>(fb), dm, p8<TV>(vb), slot_, s - 1, d_cv_stats_);
+        k_cost_volume_va16_tma<TV, true><<<dim3(cdiv(vb.W, 16), cdiv(vb.H, 8)), 256, 0, stream_.get()>>>(cv_tmap_, p8<const __half>(fb), dm, p8<TV>(vb), slot_.index, s - 1, d_cv_stats_.get());
         TDM_CUDA(cudaGetLastError());
         rec_end();
         return;
@@ -1342,7 +1315,7 @@ class MvsnetEngine final : public MvsnetIface {
         const bool h16 = cv_variant_ >= 3;   // (variant 5 = variant 3 outside stage 3)
         const long long thr = (long long)cdiv(vb.D, nd) * vb.H * vb.W * (fb.C == 32 ? 2 : 1);
         const unsigned grid = (unsigned)cdiv(thr, 128);
-        auto go = [&](auto kern) { launch_k(kern, dim3(grid), dim3(128), p8<const __half>(fb), dm, p8<TV>(vb), slot_, s - 1); };
+        auto go = [&](auto kern) { launch_k(kern, dim3(grid), dim3(128), p8<const __half>(fb), dm, p8<TV>(vb), slot_.index, s - 1); };
         if (fb.C == 32) {
           if (nd == 2) { if (h16) go(k_cost_volume_va16<TV, 16, 2, 2, true>); else go(k_cost_volume_va16<TV, 16, 2, 2, false>); }
           else         { if (h16) go(k_cost_volume_va16<TV, 16, 2, 4, true>); else go(k_cost_volume_va16<TV, 16, 2, 4, false>); }
@@ -1357,9 +1330,9 @@ class MvsnetEngine final : public MvsnetIface {
       }
     }
     if (done) {}
-    else if (fb.C == 32) k_cost_volume<TA, TV, 16, 2><<<cdiv(2 * n, 128), 128, 0, stream_>>>(p8<const TA>(fb), dm, p8<TV>(vb), slot_, s - 1);
-    else if (fb.C == 16) k_cost_volume<TA, TV, 16><<<cdiv(n, 128), 128, 0, stream_>>>(p8<const TA>(fb), dm, p8<TV>(vb), slot_, s - 1);
-    else if (fb.C == 8) k_cost_volume<TA, TV, 8><<<cdiv(n, 128), 128, 0, stream_>>>(p8<const TA>(fb), dm, p8<TV>(vb), slot_, s - 1);
+    else if (fb.C == 32) k_cost_volume<TA, TV, 16, 2><<<cdiv(2 * n, 128), 128, 0, stream_.get()>>>(p8<const TA>(fb), dm, p8<TV>(vb), slot_.index, s - 1);
+    else if (fb.C == 16) k_cost_volume<TA, TV, 16><<<cdiv(n, 128), 128, 0, stream_.get()>>>(p8<const TA>(fb), dm, p8<TV>(vb), slot_.index, s - 1);
+    else if (fb.C == 8) k_cost_volume<TA, TV, 8><<<cdiv(n, 128), 128, 0, stream_.get()>>>(p8<const TA>(fb), dm, p8<TV>(vb), slot_.index, s - 1);
     else throw Error("unsupported feature channels");
     TDM_CUDA(cudaGetLastError());
     rec_end();
@@ -1373,7 +1346,7 @@ class MvsnetEngine final : public MvsnetIface {
     const std::string k = "s" + std::to_string(s) + ".";
     if (!inline_dmin_) { d.map = fbuf(k + "dmin"); return d; }
     const DevBuf& pd = bufs_.at("s" + std::to_string(s - 1) + ".depth_dense");
-    d.prev = (const float*)pd.p; d.ph = pd.H; d.pw = pd.W;
+    d.prev = (const float*)pd.p.get(); d.ph = pd.H; d.pw = pd.W;
     return d;
   }
 
@@ -1394,22 +1367,22 @@ class MvsnetEngine final : public MvsnetIface {
     const int n = d.H * d.W;
     if (fused_select_) {
       rec_begin(k + "edge_metric+select0", 8.0 * n, 0);
-      launch_k(k_edge_metric_select0, dim3(cdiv(n, 256)), dim3(256), fbuf(k + "depth_dense"), fbuf(k + "edge"), d.H, d.W, select2_, &d_params_->cutoff[s - 1]);
+      launch_k(k_edge_metric_select0, dim3(cdiv(n, 256)), dim3(256), fbuf(k + "depth_dense"), fbuf(k + "edge"), d.H, d.W, select2_.get(), &d_params_->cutoff[s - 1]);
       rec_end();
       rec_begin(k + "percentile", 8.0 * n, 0);
       for (int pass = 1; pass <= 2; ++pass)
-        launch_k(k_select_pass, dim3(std::min(cdiv(n, 256 * 8), 2 * kNumSm)), dim3(256), fbuf(k + "edge"), n, select2_, pass, fbuf("thr") + (s - 1));
+        launch_k(k_select_pass, dim3(std::min(cdiv(n, 256 * 8), 2 * kNumSm)), dim3(256), fbuf(k + "edge"), n, select2_.get(), pass, fbuf("thr") + (s - 1));
       launch_count_ += 1;
       rec_end();
     } else {
     rec_begin(k + "edge_metric", 8.0 * n, 0);
-    k_edge_metric<<<cdiv(n, 128), 128, 0, stream_>>>(fbuf(k + "depth_dense"), fbuf(k + "edge"), d.H, d.W);
+    k_edge_metric<<<cdiv(n, 128), 128, 0, stream_.get()>>>(fbuf(k + "depth_dense"), fbuf(k + "edge"), d.H, d.W);
     rec_end();
     rec_begin(k + "percentile", 12.0 * n, 0);
-    k_select_init<<<1, 256, 0, stream_>>>(select_state_, &d_params_->cutoff[s - 1]);
+    k_select_init<<<1, 256, 0, stream_.get()>>>(select_state_.get(), &d_params_->cutoff[s - 1]);
     for (int pass = 0; pass < 3; ++pass) {
-      k_select_hist<<<std::min(cdiv(n, 256 * 8), 592), 256, 0, stream_>>>(fbuf(k + "edge"), n, select_state_, pass);
-      k_select_scan<<<1, 1024, 0, stream_>>>(select_state_, pass, fbuf("thr") + (s - 1));
+      k_select_hist<<<std::min(cdiv(n, 256 * 8), 592), 256, 0, stream_.get()>>>(fbuf(k + "edge"), n, select_state_.get(), pass);
+      k_select_scan<<<1, 1024, 0, stream_.get()>>>(select_state_.get(), pass, fbuf("thr") + (s - 1));
     }
     launch_count_ += 6;
     rec_end();
@@ -1428,31 +1401,27 @@ class MvsnetEngine final : public MvsnetIface {
   // identity table) or, for the feature cache, the k views in slots fslots[0..k-1]; one graph per k, the slots are data.
   void forward(int k, const int* fslots, bool profiling) {
     fk_ = k;
-    for (int j = 0; j <= kMaxSrc; ++j) h_feat_slot_[j] = k == V_ || j >= k ? j : fslots[j];
+    for (int j = 0; j <= kMaxSrc; ++j) h_feat_slot_.get()[j] = k == V_ || j >= k ? j : fslots[j];
     upload_call_params();
     if (profiling || !use_graph_) { forward_launches(profiling); return; }
     FwdGraph& fg = graphs_[k];
-    if (fg.exec) { TDM_CUDA(cudaGraphLaunch(fg.exec, stream_)); return; }
+    if (fg.exec) { TDM_CUDA(cudaGraphLaunch(fg.exec.get(), stream_.get())); return; }
     if (!fg.warmed) { forward_launches(false); fg.warmed = true; return; }
-    cudaGraph_t graph = nullptr;
-    TDM_CUDA(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
+    cudaGraph_t captured = nullptr;
+    TDM_CUDA(cudaStreamBeginCapture(stream_.get(), cudaStreamCaptureModeThreadLocal));
     try {
       forward_launches(false);
     } catch (...) {
-      cudaStreamEndCapture(stream_, &graph);
-      if (graph) cudaGraphDestroy(graph);
+      cudaStreamEndCapture(stream_.get(), &captured);
+      Graph discarded(captured);
       throw;
     }
-    TDM_CUDA(cudaStreamEndCapture(stream_, &graph));
-    TDM_CUDA(cudaGraphInstantiate(&fg.exec, graph, 0));
-    cudaGraphDestroy(graph);
-    TDM_CUDA(cudaGraphLaunch(fg.exec, stream_));
+    TDM_CUDA(cudaStreamEndCapture(stream_.get(), &captured));
+    const Graph graph(captured);
+    fg.exec = make_graph_exec(graph.get());
+    TDM_CUDA(cudaGraphLaunch(fg.exec.get(), stream_.get()));
   }
-  void drop_graph() {
-    for (auto& kv : graphs_)
-      if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-    graphs_.clear();
-  }
+  void drop_graph() { graphs_.clear(); }
 
   // feature cache: FeatureNet output `name` over the fk_ computed views -> their pool slots (c_feat_slot) of `name` over V
   void scatter_features(const std::string& name) {
@@ -1462,8 +1431,8 @@ class MvsnetEngine final : public MvsnetIface {
     TDM_CHECK(src.pd == 0 && dst.pd == 0 && src.C == dst.C && src.H == dst.H && src.W == dst.W, "feature scatter: shape mismatch");
     const int plane_vec = (int)((size_t)(src.H + 2) * (src.W + 2) * 8 * sizeof(TA) / 16);
     rec_begin(name + "[scatter]", 2.0 * src.alg_bytes, 0);
-    launch_k(k_scatter_planes, dim3(cdiv(plane_vec, 256), (src.C / 8) * fk_), dim3(256), (const uint4*)src.p, (uint4*)dst.p,
-             plane_vec, fk_, V_, slot_);
+    launch_k(k_scatter_planes, dim3(cdiv(plane_vec, 256), (src.C / 8) * fk_), dim3(256), (const uint4*)src.p.get(), (uint4*)dst.p.get(),
+             plane_vec, fk_, V_, slot_.index);
     TDM_CUDA(cudaGetLastError());
     rec_end();
   }
@@ -1485,14 +1454,14 @@ class MvsnetEngine final : public MvsnetIface {
         if (direct_conv00_) {
           fused = true;
           rec_begin("f.conv0.0[u8-direct]", 3.0 * n + 8.0 * n * sizeof(TA), 2.0 * 27 * 8 * (double)n);
-          launch_k(k_conv00_u8<TA>, dim3(cdiv(W, 32), cdiv(H, 8), k), dim3(256), d_bgr_, p8<TA>(bufs_.at(fb("f.c0_0"))), H, W, slot_);
+          launch_k(k_conv00_u8<TA>, dim3(cdiv(W, 32), cdiv(H, 8), k), dim3(256), d_bgr_.get(), p8<TA>(bufs_.at(fb("f.c0_0"))), H, W, slot_.index);
           TDM_CUDA(cudaGetLastError());
           rec_end();
         }
       }
       if (!fused) {
         rec_begin("preprocess", 3.0 * n + 8.0 * n * sizeof(TA), 0);
-        k_preprocess_bgr<TA, kRawInput><<<cdiv(n, 256), 256, 0, stream_>>>(d_bgr_, p8<TA>(bufs_.at(fb("f.img"))), k, H * W, slot_);
+        k_preprocess_bgr<TA, kRawInput><<<cdiv(n, 256), 256, 0, stream_.get()>>>(d_bgr_.get(), p8<TA>(bufs_.at(fb("f.img"))), k, H * W, slot_.index);
         TDM_CUDA(cudaGetLastError());
         rec_end();
         conv("f.conv0.0", fb("f.img"), fb("f.c0_0"), 1, 1, 1, true);
@@ -1510,12 +1479,12 @@ class MvsnetEngine final : public MvsnetIface {
     // stage-2 cost volume (inside the captured graph these are two parallel branches).  Not while profiling: the per-kernel
     // events assume one stream.
     struct SwapBack {   // an exception inside the branch must not leave the engine on the side stream
-      cudaStream_t &a, &b; bool on;
+      Stream &a, &b; bool on;
       ~SwapBack() { if (on) std::swap(a, b); }
     } side{stream_, side_stream_, false};
     if (fork) {
-      TDM_CUDA(cudaEventRecord(ev_fork_, stream_));
-      TDM_CUDA(cudaStreamWaitEvent(side_stream_, ev_fork_, 0));
+      TDM_CUDA(cudaEventRecord(ev_fork_.get(), stream_.get()));
+      TDM_CUDA(cudaStreamWaitEvent(side_stream_.get(), ev_fork_.get(), 0));
       std::swap(stream_, side_stream_);
       side.on = true;
     } else {
@@ -1523,7 +1492,7 @@ class MvsnetEngine final : public MvsnetIface {
       scatter_features("feat1");
     }
     if (fused_fpn_ && use_tc_) {
-      conv("f.skip2", fb("f.c2"), fb("f.i2"), 1, 1, 1, false, 2, fb("f.c1"), fb("f.i2b"), d_bs3_);
+      conv("f.skip2", fb("f.c2"), fb("f.i2"), 1, 1, 1, false, 2, fb("f.c1"), fb("f.i2b"), d_bs3_.get());
       conv("f.out2", fb("f.i2"), fb("feat2"), 1, 1, 1, false);
       conv_fpn3("f.fpn3", fb("f.i2b"), fb("f.c3"), fb("feat3"));
     } else {
@@ -1535,7 +1504,7 @@ class MvsnetEngine final : public MvsnetIface {
     scatter_features("feat2");
     scatter_features("feat3");
     if (fork) {
-      TDM_CUDA(cudaEventRecord(ev_join_, stream_));      // stream_ is the side stream here
+      TDM_CUDA(cudaEventRecord(ev_join_.get(), stream_.get()));      // stream_ is the side stream here
       std::swap(stream_, side_stream_);
       side.on = false;
       conv("f.out1", fb("f.c1"), fb("feat1"), 1, 1, 1, false);
@@ -1547,11 +1516,11 @@ class MvsnetEngine final : public MvsnetIface {
       const std::string k = "s" + std::to_string(s) + ".";
       const HypSpec hs = hyp_spec(s);
       const DevBuf& dd = bufs_.at(k + "depth_dense");
-      if (s == 2 && fork) TDM_CUDA(cudaStreamWaitEvent(stream_, ev_join_, 0));
+      if (s == 2 && fork) TDM_CUDA(cudaStreamWaitEvent(stream_.get(), ev_join_.get(), 0));
       if (s > 1 && !inline_dmin_) {
         const DevBuf& pd = bufs_.at("s" + std::to_string(s - 1) + ".depth_dense");
         rec_begin(k + "adaptive_dmin", 4.0 * (pd.H * pd.W + dd.H * dd.W), 0);
-        k_adaptive_dmin<<<cdiv(dd.H * dd.W, 256), 256, 0, stream_>>>((const float*)pd.p, pd.H, pd.W, fbuf(k + "dmin"),
+        k_adaptive_dmin<<<cdiv(dd.H * dd.W, 256), 256, 0, stream_.get()>>>((const float*)pd.p.get(), pd.H, pd.W, fbuf(k + "dmin"),
                                                                     &d_params_->half_range[s - 1]);
         TDM_CUDA(cudaGetLastError());
         rec_end();
@@ -1611,13 +1580,13 @@ class MvsnetEngine final : public MvsnetIface {
         if (eager_d2h_) {
           const char* names[4] = {"s3.depth", "s3.confidence", "s3.depth_dense", "s3.confidence_dense"};
           for (int k = 0; k < 4; ++k) {
-            TDM_CUDA(cudaMemcpyAsync(h_out_ + k * n, fbuf(names[k]), n * 4, cudaMemcpyDeviceToHost, stream_));
-            TDM_CUDA(cudaEventRecord(ev_out_[k], stream_));
+            TDM_CUDA(cudaMemcpyAsync(h_out_.get() + k * n, fbuf(names[k]), n * 4, cudaMemcpyDeviceToHost, stream_.get()));
+            TDM_CUDA(cudaEventRecord(ev_out_[k].get(), stream_.get()));
           }
         } else {
-          TDM_CUDA(cudaEventRecord(ev_out_[0], stream_));   // GetResult copies back itself (page-locked caller buffers)
+          TDM_CUDA(cudaEventRecord(ev_out_[0].get(), stream_.get()));   // GetResult copies back itself (page-locked caller buffers)
         }
-        wait_event_politely(ev_out_[0]);   // result "ready" as soon as the first map is home; GetResult waits per map
+        wait_event_politely(ev_out_[0].get());   // result "ready" as soon as the first map is home; GetResult waits per map
       } catch (const std::exception& e) {
         err = e.what();
       }
@@ -1642,20 +1611,19 @@ class MvsnetEngine final : public MvsnetIface {
     const size_t n = (size_t)H_ * W_;
     ho_valid_ = false;
     if (ho_H_ != H_ || ho_W_ != W_) {
-      for (int i = 0; i < n_ho_release_; ++i) TDM_CUDA(cudaEventSynchronize(ev_ho_release_[i]));
+      for (int i = 0; i < n_ho_release_; ++i) TDM_CUDA(cudaEventSynchronize(ev_ho_release_[i].get()));
       n_ho_release_ = 0;
-      cudaFree(d_ho_depth_); cudaFree(d_ho_bgr_);
-      d_ho_depth_ = nullptr; d_ho_bgr_ = nullptr; ho_H_ = ho_W_ = 0;
-      TDM_CUDA(cudaMalloc(&d_ho_depth_, n * 4));
-      TDM_CUDA(cudaMalloc(&d_ho_bgr_, n * 3));
+      d_ho_depth_.reset(); d_ho_bgr_.reset(); ho_H_ = ho_W_ = 0;
+      d_ho_depth_ = make_dev<float>(n * 4);
+      d_ho_bgr_ = make_dev<unsigned char>(n * 3);
       ho_H_ = H_; ho_W_ = W_;
     }
-    if (!ev_ho_ready_) TDM_CUDA(cudaEventCreateWithFlags(&ev_ho_ready_, cudaEventDisableTiming));
-    for (int i = 0; i < n_ho_release_; ++i) TDM_CUDA(cudaStreamWaitEvent(stream_, ev_ho_release_[i], 0));
+    if (!ev_ho_ready_) ev_ho_ready_ = make_event(cudaEventDisableTiming);
+    for (int i = 0; i < n_ho_release_; ++i) TDM_CUDA(cudaStreamWaitEvent(stream_.get(), ev_ho_release_[i].get(), 0));
     n_ho_release_ = 0;
-    TDM_CUDA(cudaMemcpyAsync(d_ho_depth_, fbuf("s3.depth"), n * 4, cudaMemcpyDeviceToDevice, stream_));
-    TDM_CUDA(cudaMemcpyAsync(d_ho_bgr_, d_bgr_ + (size_t)view_slot_[0] * n * 3, n * 3, cudaMemcpyDeviceToDevice, stream_));
-    TDM_CUDA(cudaEventRecord(ev_ho_ready_, stream_));
+    TDM_CUDA(cudaMemcpyAsync(d_ho_depth_.get(), fbuf("s3.depth"), n * 4, cudaMemcpyDeviceToDevice, stream_.get()));
+    TDM_CUDA(cudaMemcpyAsync(d_ho_bgr_.get(), d_bgr_.get() + (size_t)view_slot_[0] * n * 3, n * 3, cudaMemcpyDeviceToDevice, stream_.get()));
+    TDM_CUDA(cudaEventRecord(ev_ho_ready_.get(), stream_.get()));
     std::memcpy(ho_c2w_, c2w_[0], sizeof(ho_c2w_));
     ho_valid_ = true;
   }
@@ -1664,9 +1632,9 @@ class MvsnetEngine final : public MvsnetIface {
     if (n_ho_release_ == (int)ev_ho_release_.size()) {
       cudaEvent_t e = nullptr;
       if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) return false;
-      ev_ho_release_.push_back(e);
+      ev_ho_release_.emplace_back(e);
     }
-    if (cudaEventRecord(ev_ho_release_[n_ho_release_], (cudaStream_t)stream) != cudaSuccess) return false;
+    if (cudaEventRecord(ev_ho_release_[n_ho_release_].get(), (cudaStream_t)stream) != cudaSuccess) return false;
     ++n_ho_release_;
     return true;
   }
@@ -1694,9 +1662,9 @@ class MvsnetEngine final : public MvsnetIface {
       // threads.  The caller owns them only during this call, so the call returns once the seven DMAs have landed
       // (6.45 MB over PCIe gen5: ~0.13 ms, less than the staging memcpy it replaces).
       for (int j = 0; j < n; ++j)
-        TDM_CUDA(cudaMemcpyAsync(d_bgr_ + (size_t)slots[j] * img, srcs[j], img, cudaMemcpyHostToDevice, stream_));
-      TDM_CUDA(cudaEventRecord(ev_in_, stream_));
-      TDM_CUDA(cudaEventSynchronize(ev_in_));
+        TDM_CUDA(cudaMemcpyAsync(d_bgr_.get() + (size_t)slots[j] * img, srcs[j], img, cudaMemcpyHostToDevice, stream_.get()));
+      TDM_CUDA(cudaEventRecord(ev_in_.get(), stream_.get()));
+      TDM_CUDA(cudaEventSynchronize(ev_in_.get()));
     } else {
       // Pageable caller memory: staged through pinned memory.  The staging copy of view v+1 overlaps the DMA of view v (the
       // worker is idle here, so this thread may enqueue on the engine's stream); each view is split into slices copied by the
@@ -1709,11 +1677,11 @@ class MvsnetEngine final : public MvsnetIface {
       for (int j = 0; j < n; ++j) {
         for (int sl = 0; sl < kSlices; ++sl) {
           const size_t b0 = img * sl / kSlices, b1 = img * (sl + 1) / kSlices;
-          unsigned char* hp = h_bgr_ + (size_t)slots[j] * img + b0;
-          unsigned char* dp = d_bgr_ + (size_t)slots[j] * img + b0;
+          unsigned char* hp = h_bgr_.get() + (size_t)slots[j] * img + b0;
+          unsigned char* dp = d_bgr_.get() + (size_t)slots[j] * img + b0;
           jobs.push_back({hp, srcs[j] + b0, b1 - b0, [this, hp, dp, b0, b1, &err_mu, &first_err] {
                             cudaSetDevice(device_);   // pool threads start on device 0
-                            const cudaError_t e = cudaMemcpyAsync(dp, hp, b1 - b0, cudaMemcpyHostToDevice, stream_);
+                            const cudaError_t e = cudaMemcpyAsync(dp, hp, b1 - b0, cudaMemcpyHostToDevice, stream_.get());
                             if (e != cudaSuccess) { std::lock_guard<std::mutex> lk(err_mu); first_err = e; }
                           }});
         }
@@ -1774,15 +1742,15 @@ class MvsnetEngine final : public MvsnetIface {
   static constexpr bool kRawInput = sizeof(TA) == 2;   // 16-bit engines: exact u8/256 input, 256/255 folded into f.conv0.0
 
   int device_ = 0;
-  cudaStream_t stream_ = nullptr;
+  Stream stream_;
   WeightFile wf_;
   int depth_num_[3];
   bool va_ = false;
   std::map<std::string, DevConv> convs_;
   Gate gates_[3];
   std::map<std::string, DevBuf> bufs_;
-  SelectState* select_state_ = nullptr;
-  SelectState2* select2_ = nullptr;
+  DevPtr<SelectState> select_state_;
+  DevPtr<SelectState2> select2_;
   bool inline_dmin_ = true;    // adaptive range's d_min computed where it is consumed (dmin_px) instead of by k_adaptive_dmin (A/B: 0)
   // softmax / soft-argmin / confidence in the epilogue of the tensor-core prob convolution (set_option("fused_regress", 1)):
   // bit-identical to k_regress and three launches fewer, but the consumer threads of a CTA finish their pixels after the last
@@ -1796,29 +1764,29 @@ class MvsnetEngine final : public MvsnetIface {
   int pdl_min_smem_kb_ = 120;
   bool fused_select_ = true;   // edge metric + pass 0 in one kernel, passes 1 / 2 with the scan in their last CTA (A/B: set_option("fused_select", 0))
   int V_ = 0, H_ = 0, W_ = 0;
-  unsigned char* h_bgr_ = nullptr;
-  unsigned char* d_bgr_ = nullptr;
-  float* h_out_ = nullptr;
-  cudaEvent_t ev_out_[4] = {nullptr, nullptr, nullptr, nullptr};
-  cudaEvent_t ev_in_ = nullptr;
+  HostPtr<unsigned char> h_bgr_;
+  DevPtr<unsigned char> d_bgr_;
+  HostPtr<float> h_out_;
+  Event ev_out_[4];
+  Event ev_in_;
   bool eager_d2h_ = true;   // worker copies the four maps into pinned staging right behind the forward (pageable callers);
                             // 0: GetResult copies back itself - for callers that pass page-locked result buffers
   float c2w_[kMaxSrc + 1][16];
   // keyframe handoff (fill_handoff / read_handoff): the last fetched result, kept until the next GetResult
-  float* d_ho_depth_ = nullptr;
-  unsigned char* d_ho_bgr_ = nullptr;
+  DevPtr<float> d_ho_depth_;
+  DevPtr<unsigned char> d_ho_bgr_;
   float ho_c2w_[16];
   int ho_H_ = 0, ho_W_ = 0;
   bool ho_valid_ = false;
-  cudaEvent_t ev_ho_ready_ = nullptr;
-  std::vector<cudaEvent_t> ev_ho_release_;   // pool; the first n_ho_release_ were recorded by consumers since the last fill
+  Event ev_ho_ready_;
+  std::vector<Event> ev_ho_release_;   // pool; the first n_ho_release_ were recorded by consumers since the last fill
   int n_ho_release_ = 0;
   float K_[27];
   float dmin_ = 0, dmax_ = 0, discard_ = 0;
-  float* d_bs3_ = nullptr;
-  CallParams* h_params_ = nullptr;   // pinned
-  CallParams* d_params_ = nullptr;
-  int* h_feat_slot_ = nullptr;       // pinned [kMaxSrc + 1]: the table c_feat_slot[slot_] the next forward uses
+  DevPtr<float> d_bs3_;
+  HostPtr<CallParams> h_params_;   // pinned
+  DevPtr<CallParams> d_params_;
+  HostPtr<int> h_feat_slot_;       // pinned [kMaxSrc + 1]: the table c_feat_slot[slot_] the next forward uses
   // feature cache (call_async_ids): slot s of d_bgr_ / feat1..3 holds the view with id slot_id_[s] when cache_valid_; view vi of
   // the last window (reference first) is in slot view_slot_[vi] (the identity after a plain call_async)
   long long slot_id_[kMaxSrc + 1] = {};
@@ -1828,17 +1796,17 @@ class MvsnetEngine final : public MvsnetIface {
   int n_computed_ = 0;                                 // views FeatureNet computed for the last call
   int call_k_ = 0, call_slots_[kMaxSrc + 1] = {};      // the submitted window's FeatureNet views, for the worker
   int fk_ = 0;                                         // views FeatureNet computes in the forward being enqueued / last enqueued
-  struct FwdGraph { cudaGraphExec_t exec = nullptr; bool warmed = false; };
+  struct FwdGraph { GraphExec exec; bool warmed = false; };
   std::map<int, FwdGraph> graphs_;   // one captured forward per FeatureNet view count
   CUtensorMap cv_tmap_{};      // cv_variant 5 (A/B): tiled view of feat3 for the TMA-staged cost volume
   bool cv_tmap_ok_ = false;
-  unsigned* d_cv_stats_ = nullptr;
+  DevPtr<unsigned> d_cv_stats_;
   int cv_variant_ = 3;   // 0: generic cost-volume kernel; 1-4: k_cost_volume_va16 (ND 2/2/4 | 4/4/4, fp32 | fp16 accumulate)
   // Programmatic dependent launch of the tensor-core kernels: the trigger sits after griddepcontrol.wait (a trigger before it
   // lets the whole chain of later kernels become resident early), and pdl_min_smem_kb_ = 120 keeps one tensor-core CTA per SM.
   bool use_graph_ = true;
   int use_pdl_ = 1;   // 2: the FMA-pipe kernels (cost volume, soft-argmin, edge filter ...) are launched with the attribute as well
-  int slot_ = 0;           // index into c_call_params
+  EngineSlot slot_;
   int tc_smem_kb_ = 225;   // shared-memory budget of the tile planner (<= 113 lets two CTAs share an SM)
   bool fused_fpn_ = false;
   bool prob_direct_ = false;  // `prob` (8 -> 1 channels) on the FMA pipes (k_prob_direct) instead of the tensor-core tile; an A/B option and an independent check
@@ -1846,8 +1814,8 @@ class MvsnetEngine final : public MvsnetIface {
   ProbWeights prob_w_[3] = {};
   bool direct_conv00_ = true; // 16-bit engines: pre-processing + conv0.0 fused on the FMA pipes (k_conv00_u8); 0 = preprocess + tensor-core conv
   bool fork_fpn_ = true;      // FPN tail on a second stream / graph branch (A/B: set_option("fork_fpn", 0))
-  cudaStream_t side_stream_ = nullptr;
-  cudaEvent_t ev_fork_ = nullptr, ev_join_ = nullptr;
+  Stream side_stream_;
+  Event ev_fork_, ev_join_;
   bool filter_all_ = false, keep_ = true, use_tc_ = (sizeof(TA) == 2);  // tensor-core convs are the default on 16-bit engines
   bool debug_poison_ = false;  // set_option("debug_poison", 1): activation interiors start as NaN (alloc), for the layer tests
   bool profiling_ = false;

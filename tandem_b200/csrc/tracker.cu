@@ -925,42 +925,23 @@ class TrackerImpl final : public TrackerIface {
     TDM_CUDA(cudaSetDevice(device_));
     int lo, hi;
     TDM_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    TDM_CUDA(cudaStreamCreateWithPriority(&stream_, cudaStreamNonBlocking, hi));  // highest priority (cpp:72-74)
-    TDM_CUDA(cudaMalloc(&d_pc_, (size_t)4 * n_max_ * 4));
-    TDM_CUDA(cudaMemset(d_pc_, 0, (size_t)4 * n_max_ * 4));   // like the reference's arrays, they persist across references
-    TDM_CUDA(cudaMalloc(&d_warped_, (size_t)7 * n_max_ * 4));
-    TDM_CUDA(cudaMemset(d_warped_, 0, (size_t)7 * n_max_ * 4));
-    TDM_CUDA(cudaMalloc(&d_dI_, (size_t)3 * w * h * 4));
-    TDM_CUDA(cudaMalloc(&d_partials_, (size_t)kBlocks * kOut * 8));
-    TDM_CUDA(cudaMalloc(&d_ticket_, 4));
-    TDM_CUDA(cudaMemset(d_ticket_, 0, 4));
-    TDM_CUDA(cudaMallocHost(&h_pc_, (size_t)4 * n_max_ * 4));
-    TDM_CUDA(cudaMallocHost(&h_dI_, (size_t)3 * w * h * 4));
-    TDM_CUDA(cudaHostAlloc(&h_out_, kOut * 8, cudaHostAllocMapped));
-    TDM_CUDA(cudaHostGetDevicePointer(&d_out_, h_out_, 0));
+    stream_ = make_stream(hi);  // highest priority (cpp:72-74)
+    d_pc_ = make_dev<float>((size_t)4 * n_max_ * 4);
+    TDM_CUDA(cudaMemset(d_pc_.get(), 0, (size_t)4 * n_max_ * 4));   // like the reference's arrays, they persist across references
+    d_warped_ = make_dev<float>((size_t)7 * n_max_ * 4);
+    TDM_CUDA(cudaMemset(d_warped_.get(), 0, (size_t)7 * n_max_ * 4));
+    d_dI_ = make_dev<float>((size_t)3 * w * h * 4);
+    d_partials_ = make_dev<double>((size_t)kBlocks * kOut * 8);
+    d_ticket_ = make_dev<unsigned>(4);
+    TDM_CUDA(cudaMemset(d_ticket_.get(), 0, 4));
+    h_pc_ = make_host<float>((size_t)4 * n_max_ * 4);
+    h_dI_ = make_host<float>((size_t)3 * w * h * 4);
+    h_out_ = make_host<double>(kOut * 8, cudaHostAllocMapped);
+    TDM_CUDA(cudaHostGetDevicePointer(&d_out_, h_out_.get(), 0));
   }
   ~TrackerImpl() override {
     cudaSetDevice(device_);
-    cudaStreamSynchronize(stream_);
-    cudaFree(d_pc_); cudaFree(d_warped_); cudaFree(d_dI_); cudaFree(d_partials_); cudaFree(d_ticket_);
-    cudaFreeHost(h_pc_); cudaFreeHost(h_dI_); cudaFreeHost(h_out_);
-    if (d_batch_) { cudaFree(d_batch_); cudaFreeHost(h_batch_); cudaFree(d_batch_partials_); cudaFree(d_batch_ticket_); cudaFreeHost(h_batch_out_); }
-    cudaFree(d_proj_); cudaFree(d_depth_); cudaFree(d_idepth0_); cudaFree(d_gray_); cudaFree(d_rowcnt_); cudaFree(d_rowoff_);
-    cudaFree(d_total_); cudaFree(d_lm_ctx_); cudaFree(d_lm_out_);
-    cudaFree(d_coarse_); cudaFree(d_rowlast_); cudaFree(d_coarse_cnt_); cudaFree(d_coarse_stale_); cudaFree(d_pts_); cudaFree(d_coarse_tmp_);
-    cudaFree(d_nodia_);
-    if (h_coarse_cnt_) cudaFreeHost(h_coarse_cnt_);
-    if (h_pts_) cudaFreeHost(h_pts_);
-    if (lm_exec_) cudaGraphExecDestroy(lm_exec_);
-    for (cudaEvent_t e : {lm_in_free_, lm_e0_, lm_e1_, ready_})
-      if (e) cudaEventDestroy(e);
-    if (h_front_) cudaFreeHost(h_front_);
-    if (h_total_) cudaFreeHost(h_total_);
-    if (h_lm_in_) cudaFreeHost(h_lm_in_);
-    if (h_lm_res_) cudaFreeHost(h_lm_res_);
-    if (h_rt_in_) cudaFreeHost(h_rt_in_);
-    if (h_rt_out_) cudaFreeHost(h_rt_out_);
-    cudaStreamDestroy(stream_);
+    cudaStreamSynchronize(stream_.get());
   }
 
   void set_k(int w, int h, float fx, float fy, float cx, float cy) override {
@@ -976,15 +957,15 @@ class TrackerImpl final : public TrackerIface {
                      const double ref_aff[2]) override {
     if (n > n_max_) throw Error("Called CudaCoarseTracker::setReference with n > n_max points. (cuda_coarse_tracker.cpp:82)");
     TDM_CUDA(cudaSetDevice(device_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));  // pinned staging may still be in flight
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));  // pinned staging may still be in flight
     n_ = n;
     const size_t nm = (size_t)n_max_;
-    std::memcpy(h_pc_, u, 4 * (size_t)n);
-    std::memcpy(h_pc_ + nm, v, 4 * (size_t)n);
-    std::memcpy(h_pc_ + 2 * nm, idepth, 4 * (size_t)n);
-    std::memcpy(h_pc_ + 3 * nm, color, 4 * (size_t)n);
+    std::memcpy(h_pc_.get(), u, 4 * (size_t)n);
+    std::memcpy(h_pc_.get() + nm, v, 4 * (size_t)n);
+    std::memcpy(h_pc_.get() + 2 * nm, idepth, 4 * (size_t)n);
+    std::memcpy(h_pc_.get() + 3 * nm, color, 4 * (size_t)n);
     for (int a = 0; a < 4; ++a)
-      TDM_CUDA(cudaMemcpyAsync(d_pc_ + a * nm, h_pc_ + a * nm, 4 * (size_t)n, cudaMemcpyHostToDevice, stream_));
+      TDM_CUDA(cudaMemcpyAsync(d_pc_.get() + a * nm, h_pc_.get() + a * nm, 4 * (size_t)n, cudaMemcpyHostToDevice, stream_.get()));
     ref_exposure_ = ref_exposure;
     ref_aff_[0] = ref_aff[0]; ref_aff_[1] = ref_aff[1];
     have_ref_ = true;
@@ -993,9 +974,9 @@ class TrackerImpl final : public TrackerIface {
 
   void set_new(const float* dI) override {
     TDM_CUDA(cudaSetDevice(device_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
-    std::memcpy(h_dI_, dI, (size_t)3 * w_ * h_ * 4);
-    TDM_CUDA(cudaMemcpyAsync(d_dI_, h_dI_, (size_t)3 * w_ * h_ * 4, cudaMemcpyHostToDevice, stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
+    std::memcpy(h_dI_.get(), dI, (size_t)3 * w_ * h_ * 4);
+    TDM_CUDA(cudaMemcpyAsync(d_dI_.get(), h_dI_.get(), (size_t)3 * w_ * h_ * 4, cudaMemcpyHostToDevice, stream_.get()));
     have_new_ = true;
     have_params_ = false;   // calcG is only defined on the buffers of a calcRes against THIS image (cuda_coarse_tracker.cpp:277-281)
   }
@@ -1003,14 +984,14 @@ class TrackerImpl final : public TrackerIface {
   void calc_res(const double* refToNew, float new_exposure, const double aff[2], float cutoffTH, double res6[6]) override {
     prepare(refToNew, new_exposure, aff, cutoffTH);
     launch(0);
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
     finish_res(res6);
   }
   void calc_g(float new_exposure, const double aff[2], double H[64], double b[8]) override {
     TDM_CHECK(have_params_, "calcG before calcRes (or the reference / new image changed since the last calcRes)");
     set_aff(new_exposure, aff);
     launch(1);
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
     finish_g(H, b);
   }
   // The fused path writes no warped buffers, so what a later calc_g refers to - the parameters and count of the last
@@ -1023,7 +1004,7 @@ class TrackerImpl final : public TrackerIface {
     try {
       prepare(refToNew, new_exposure, aff, cutoffTH);
       launch(2);
-      TDM_CUDA(cudaStreamSynchronize(stream_));
+      TDM_CUDA(cudaStreamSynchronize(stream_.get()));
       finish_res(res6);
       finish_g(H, b);
     } catch (...) {
@@ -1040,45 +1021,45 @@ class TrackerImpl final : public TrackerIface {
     TDM_CHECK(a.step >= 1 && a.n_sparse >= 0, "bad tracking step / sparse count");
     TDM_CHECK(a.n_sparse == 0 || (a.pc_u && a.pc_v && a.pc_idepth && a.pc_color), "sparse arrays missing");
     TDM_CUDA(cudaSetDevice(device_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
     const size_t npx = (size_t)w_ * h_, nm = (size_t)n_max_;
     ensure_front_buffers();
     const int ns1 = a.n_sparse + 1;
     if ((long long)ns1 > n_max_) throw Error("setReferenceDense: more sparse points than n_max");
     const float* d_depth = a.depth;
     if (!a.depth_on_device) {
-      std::memcpy(h_front_, a.depth, 4 * npx);
-      TDM_CUDA(cudaMemcpyAsync(d_depth_, h_front_, 4 * npx, cudaMemcpyHostToDevice, stream_));
-      d_depth = d_depth_;
+      std::memcpy(h_front_.get(), a.depth, 4 * npx);
+      TDM_CUDA(cudaMemcpyAsync(d_depth_.get(), h_front_.get(), 4 * npx, cudaMemcpyHostToDevice, stream_.get()));
+      d_depth = d_depth_.get();
     } else if (a.depth_ready) {
-      TDM_CUDA(cudaStreamWaitEvent(stream_, (cudaEvent_t)a.depth_ready, 0));
+      TDM_CUDA(cudaStreamWaitEvent(stream_.get(), (cudaEvent_t)a.depth_ready, 0));
     }
     const float* d_id0 = nullptr;
     if (a.idepth0) {
-      std::memcpy(h_front_ + npx, a.idepth0, 4 * npx);
-      TDM_CUDA(cudaMemcpyAsync(d_idepth0_, h_front_ + npx, 4 * npx, cudaMemcpyHostToDevice, stream_));
-      d_id0 = d_idepth0_;
+      std::memcpy(h_front_.get() + npx, a.idepth0, 4 * npx);
+      TDM_CUDA(cudaMemcpyAsync(d_idepth0_.get(), h_front_.get() + npx, 4 * npx, cudaMemcpyHostToDevice, stream_.get()));
+      d_id0 = d_idepth0_.get();
     }
     const float* d_gray = a.ref_gray;
     int gstride = a.gray_stride;
     if (!a.gray_on_device) {
-      std::memcpy(h_front_ + 2 * npx, a.ref_gray, 4 * npx);
-      TDM_CUDA(cudaMemcpyAsync(d_gray_, h_front_ + 2 * npx, 4 * npx, cudaMemcpyHostToDevice, stream_));
-      d_gray = d_gray_;
+      std::memcpy(h_front_.get() + 2 * npx, a.ref_gray, 4 * npx);
+      TDM_CUDA(cudaMemcpyAsync(d_gray_.get(), h_front_.get() + 2 * npx, 4 * npx, cudaMemcpyHostToDevice, stream_.get()));
+      d_gray = d_gray_.get();
       gstride = 1;
     } else if (a.gray_ready) {
-      TDM_CUDA(cudaStreamWaitEvent(stream_, (cudaEvent_t)a.gray_ready, 0));
+      TDM_CUDA(cudaStreamWaitEvent(stream_.get(), (cudaEvent_t)a.gray_ready, 0));
     }
     const DenseWarp m = dense_warp(a.T_depth_to_ref);
-    TDM_CUDA(cudaMemsetAsync(d_proj_, 0xFF, 4 * npx, stream_));
+    TDM_CUDA(cudaMemsetAsync(d_proj_.get(), 0xFF, 4 * npx, stream_.get()));
     const int nx = (w_ + a.step - 1) / a.step, ny = (h_ + a.step - 1) / a.step;
-    k_dense_warp<<<(nx * ny + 255) / 256, 256, 0, stream_>>>(d_depth, w_, h_, a.step, m, d_proj_);
-    const DenseSel sel{d_proj_, d_id0, a.dense_only, d_gray, gstride};
-    k_compact_rowcount<<<h_, 256, 0, stream_>>>(sel, w_, h_, d_rowcnt_, nullptr);
-    k_compact_rowscan<<<1, 32, 0, stream_>>>(d_rowcnt_, nullptr, w_, h_, nullptr, d_rowoff_, d_total_, nullptr);
-    TDM_CUDA(cudaMemcpyAsync(h_total_, d_total_, 4, cudaMemcpyDeviceToHost, stream_));
+    k_dense_warp<<<(nx * ny + 255) / 256, 256, 0, stream_.get()>>>(d_depth, w_, h_, a.step, m, d_proj_.get());
+    const DenseSel sel{d_proj_.get(), d_id0, a.dense_only, d_gray, gstride};
+    k_compact_rowcount<<<h_, 256, 0, stream_.get()>>>(sel, w_, h_, d_rowcnt_.get(), nullptr);
+    k_compact_rowscan<<<1, 32, 0, stream_.get()>>>(d_rowcnt_.get(), nullptr, w_, h_, nullptr, d_rowoff_.get(), d_total_.get(), nullptr);
+    TDM_CUDA(cudaMemcpyAsync(h_total_.get(), d_total_.get(), 4, cudaMemcpyDeviceToHost, stream_.get()));
     TDM_CUDA(cudaGetLastError());
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
     const int total = *h_total_;
     if ((long long)a.n_sparse + 1 + total > n_max_) throw Error("setReferenceDense: n_max too small for the dense points");
     // Only now is the current reference overwritten, so that a call refused above leaves it as it was.
@@ -1086,14 +1067,14 @@ class TrackerImpl final : public TrackerIface {
     const float* src[4] = {a.pc_u, a.pc_v, a.pc_idepth, a.pc_color};
     for (int k = 0; k < 4; ++k) {
       if (src[k]) {
-        std::memcpy(h_pc_ + k * nm, src[k], 4 * (size_t)ns1);
-        TDM_CUDA(cudaMemcpyAsync(d_pc_ + k * nm, h_pc_ + k * nm, 4 * (size_t)ns1, cudaMemcpyHostToDevice, stream_));
+        std::memcpy(h_pc_.get() + k * nm, src[k], 4 * (size_t)ns1);
+        TDM_CUDA(cudaMemcpyAsync(d_pc_.get() + k * nm, h_pc_.get() + k * nm, 4 * (size_t)ns1, cudaMemcpyHostToDevice, stream_.get()));
       } else {
-        TDM_CUDA(cudaMemsetAsync(d_pc_ + k * nm, 0, 4, stream_));
+        TDM_CUDA(cudaMemsetAsync(d_pc_.get() + k * nm, 0, 4, stream_.get()));
       }
     }
-    k_compact_emit<<<h_, 256, 0, stream_>>>(sel, w_, h_, d_rowoff_, a.n_sparse + 1, n_max_, nullptr, nullptr,
-                                            d_pc_, d_pc_ + nm, d_pc_ + 2 * nm, d_pc_ + 3 * nm);
+    k_compact_emit<<<h_, 256, 0, stream_.get()>>>(sel, w_, h_, d_rowoff_.get(), a.n_sparse + 1, n_max_, nullptr, nullptr,
+                                            d_pc_.get(), d_pc_.get() + nm, d_pc_.get() + 2 * nm, d_pc_.get() + 3 * nm);
     TDM_CUDA(cudaGetLastError());
     n_ = a.n_sparse + total;      // the pre-increment quirk: the last appended point is not counted
     ref_exposure_ = a.ref_exposure;
@@ -1111,21 +1092,21 @@ class TrackerImpl final : public TrackerIface {
     const size_t nm = (size_t)n_max_;
     float* dst[4] = {u, v, idepth, color};
     for (int k = 0; k < 4; ++k)
-      if (dst[k]) TDM_CUDA(cudaMemcpyAsync(dst[k], d_pc_ + k * nm, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+      if (dst[k]) TDM_CUDA(cudaMemcpyAsync(dst[k], d_pc_.get() + k * nm, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream_.get()));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
   }
   void get_warped(int n, float* out) override {
     TDM_CHECK(n >= 0 && n <= n_max_, "get_warped: bad n");
     TDM_CUDA(cudaSetDevice(device_));
     for (int k = 0; k < 7; ++k)
-      TDM_CUDA(cudaMemcpyAsync(out + (size_t)k * n, d_warped_ + (size_t)k * n_max_, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+      TDM_CUDA(cudaMemcpyAsync(out + (size_t)k * n, d_warped_.get() + (size_t)k * n_max_, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream_.get()));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
   }
   // ---------------------------------------------------------------------------------------------- n2
   void set_new_device(const float* d_dI, void* ready_event) override {
     TDM_CUDA(cudaSetDevice(device_));
-    if (ready_event) TDM_CUDA(cudaStreamWaitEvent(stream_, (cudaEvent_t)ready_event, 0));
-    TDM_CUDA(cudaMemcpyAsync(d_dI_, d_dI, (size_t)3 * w_ * h_ * 4, cudaMemcpyDeviceToDevice, stream_));
+    if (ready_event) TDM_CUDA(cudaStreamWaitEvent(stream_.get(), (cudaEvent_t)ready_event, 0));
+    TDM_CUDA(cudaMemcpyAsync(d_dI_.get(), d_dI, (size_t)3 * w_ * h_ * 4, cudaMemcpyDeviceToDevice, stream_.get()));
     have_new_ = true;
     have_params_ = false;   // calcG is only defined on the buffers of a calcRes against THIS image (cuda_coarse_tracker.cpp:277-281)
   }
@@ -1182,7 +1163,7 @@ class TrackerImpl final : public TrackerIface {
     q.n_tries = a.n_tries;
     std::memcpy(q.tries, a.tries, (size_t)a.n_tries * 16 * sizeof(double));
     run_lm(a.tries, a.aff_last_2_l, &r->device_ms, &h_rt_out_->done, offsetof(RetrackIn, tries) + (size_t)a.n_tries * 16 * sizeof(double));
-    const volatile RetrackOut* o = h_rt_out_;
+    const volatile RetrackOut* o = h_rt_out_.get();
     for (int i = 0; i < 16; ++i) r->refToNew[i] = o->T[i];
     for (int i = 0; i < 2; ++i) r->aff[i] = o->aff[i];
     for (int l = 0; l < kMaxLevels; ++l) r->achieved_res[l] = o->achieved[l];
@@ -1226,7 +1207,7 @@ class TrackerImpl final : public TrackerIface {
     // Pack (pixel, input index, value, weight input) and check the pixels: the reference would write outside idepth[0] there.
     const int n = a.n_points;
     const size_t cap = (size_t)coarse_cap_;
-    int* pk = reinterpret_cast<int*>(h_pts_);
+    int* pk = reinterpret_cast<int*>(h_pts_.get());
     for (int k = 0; k < n; ++k) {
       int u, v;
       if (a.rgbd_init) {   // int u = ph->u + 0.5 (double)
@@ -1242,56 +1223,56 @@ class TrackerImpl final : public TrackerIface {
       pk[cap + k] = k;
     }
     if (n) {
-      std::memcpy(h_pts_ + 2 * cap, a.pt_idepth, 4 * (size_t)n);
-      std::memcpy(h_pts_ + 3 * cap, a.pt_hessian, 4 * (size_t)n);
+      std::memcpy(h_pts_.get() + 2 * cap, a.pt_idepth, 4 * (size_t)n);
+      std::memcpy(h_pts_.get() + 3 * cap, a.pt_hessian, 4 * (size_t)n);
     }
     // Ordered after the pending work of every level (their references are overwritten), the pyramid and the dense map.
-    for (int l = 1; l < L; ++l) lv[l]->order_before(stream_);
-    TDM_CUDA(cudaStreamWaitEvent(stream_, (cudaEvent_t)P.ready_event(), 0));
-    if (a.depth && a.depth_on_device && a.depth_ready) TDM_CUDA(cudaStreamWaitEvent(stream_, (cudaEvent_t)a.depth_ready, 0));
+    for (int l = 1; l < L; ++l) lv[l]->order_before(stream_.get());
+    TDM_CUDA(cudaStreamWaitEvent(stream_.get(), (cudaEvent_t)P.ready_event(), 0));
+    if (a.depth && a.depth_on_device && a.depth_ready) TDM_CUDA(cudaStreamWaitEvent(stream_.get(), (cudaEvent_t)a.depth_ready, 0));
     size_t off[kMaxLevels + 1] = {0};
     for (int l = 0; l < kMaxLevels; ++l) off[l + 1] = off[l] + (size_t)(w_ >> l) * (h_ >> l);
-    float *id = d_coarse_, *ws = d_coarse_ + off[kMaxLevels], *ws2 = d_coarse_ + 2 * off[kMaxLevels];
+    float *id = d_coarse_.get(), *ws = d_coarse_.get() + off[kMaxLevels], *ws2 = d_coarse_.get() + 2 * off[kMaxLevels];
     // 1. scatter (:150-182)
-    TDM_CUDA(cudaMemsetAsync(id, 0, 4 * off[1], stream_));
-    TDM_CUDA(cudaMemsetAsync(ws, 0, 4 * off[1], stream_));
-    if (nodia) TDM_CUDA(cudaMemsetAsync(d_nodia_, 0, 4 * off[1], stream_));
+    TDM_CUDA(cudaMemsetAsync(id, 0, 4 * off[1], stream_.get()));
+    TDM_CUDA(cudaMemsetAsync(ws, 0, 4 * off[1], stream_.get()));
+    if (nodia) TDM_CUDA(cudaMemsetAsync(d_nodia_.get(), 0, 4 * off[1], stream_.get()));
     if (n) {
-      int* d_pk = reinterpret_cast<int*>(d_pts_);
-      TDM_CUDA(cudaMemcpyAsync(d_pts_, h_pts_, 16 * cap, cudaMemcpyHostToDevice, stream_));
+      int* d_pk = reinterpret_cast<int*>(d_pts_.get());
+      TDM_CUDA(cudaMemcpyAsync(d_pts_.get(), h_pts_.get(), 16 * cap, cudaMemcpyHostToDevice, stream_.get()));
       int bits = 1;
       while ((1ll << bits) < (long long)w_ * h_) ++bits;
       size_t tb = 0;
-      TDM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_pk, d_pk + 4 * cap, d_pk + cap, d_pk + 5 * cap, n, 0, bits, stream_));
+      TDM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_pk, d_pk + 4 * cap, d_pk + cap, d_pk + 5 * cap, n, 0, bits, stream_.get()));
       grow_coarse_tmp(tb);
-      TDM_CUDA(cub::DeviceRadixSort::SortPairs(d_coarse_tmp_, tb, d_pk, d_pk + 4 * cap, d_pk + cap, d_pk + 5 * cap, n, 0, bits, stream_));
+      TDM_CUDA(cub::DeviceRadixSort::SortPairs(d_coarse_tmp_.get(), tb, d_pk, d_pk + 4 * cap, d_pk + cap, d_pk + 5 * cap, n, 0, bits, stream_.get()));
       if (nodia)
-        k_coarse_scatter<true><<<(n + 255) / 256, 256, 0, stream_>>>(d_pk + 4 * cap, d_pk + 5 * cap, d_pts_ + 2 * cap, d_pts_ + 3 * cap,
-                                                                     n, a.rgbd_init, id, ws, d_nodia_);
+        k_coarse_scatter<true><<<(n + 255) / 256, 256, 0, stream_.get()>>>(d_pk + 4 * cap, d_pk + 5 * cap, d_pts_.get() + 2 * cap, d_pts_.get() + 3 * cap,
+                                                                     n, a.rgbd_init, id, ws, d_nodia_.get());
       else
-        k_coarse_scatter<false><<<(n + 255) / 256, 256, 0, stream_>>>(d_pk + 4 * cap, d_pk + 5 * cap, d_pts_ + 2 * cap, d_pts_ + 3 * cap,
+        k_coarse_scatter<false><<<(n + 255) / 256, 256, 0, stream_.get()>>>(d_pk + 4 * cap, d_pk + 5 * cap, d_pts_.get() + 2 * cap, d_pts_.get() + 3 * cap,
                                                                       n, a.rgbd_init, id, ws, nullptr);
     }
     // 2. sum pyramid from the un-dilated level below (:222-243)
     for (int l = 1; l < L; ++l) {
       const int wl = w_ >> l, hl = h_ >> l;
-      k_coarse_sum<<<(wl * hl + 255) / 256, 256, 0, stream_>>>(id + off[l - 1], ws + off[l - 1], w_ >> (l - 1), id + off[l], ws + off[l], wl, hl);
+      k_coarse_sum<<<(wl * hl + 255) / 256, 256, 0, stream_.get()>>>(id + off[l - 1], ws + off[l - 1], w_ >> (l - 1), id + off[l], ws + off[l], wl, hl);
     }
     // 3. dilation (:246-322): diagonal neighbours on levels 0 / 1, axis neighbours above; weights ws -> ws2
     for (int l = 0; l < L; ++l) {
       const int wl = w_ >> l, hl = h_ >> l, g = (wl * hl + 255) / 256;
-      if (l < 2) k_coarse_dilate<true><<<g, 256, 0, stream_>>>(id + off[l], ws + off[l], ws2 + off[l], wl, hl);
-      else k_coarse_dilate<false><<<g, 256, 0, stream_>>>(id + off[l], ws + off[l], ws2 + off[l], wl, hl);
+      if (l < 2) k_coarse_dilate<true><<<g, 256, 0, stream_.get()>>>(id + off[l], ws + off[l], ws2 + off[l], wl, hl);
+      else k_coarse_dilate<false><<<g, 256, 0, stream_.get()>>>(id + off[l], ws + off[l], ws2 + off[l], wl, hl);
     }
     // 4. normalise and compact each level into its tracker's arrays (:325-370); counts in d_coarse_cnt_[l]
     for (int l = 0; l < L; ++l) {
       const int wl = w_ >> l, hl = h_ >> l;
       const NormSel sel{id + off[l], ws2 + off[l], P.level_dI(l)};
       const size_t nm = (size_t)lv[l]->n_max_;
-      float* pc = lv[l]->d_pc_;
-      k_compact_rowcount<<<hl, 256, 0, stream_>>>(sel, wl, hl, d_rowcnt_, d_rowlast_);
-      k_compact_rowscan<<<1, 32, 0, stream_>>>(d_rowcnt_, d_rowlast_, wl, hl, nullptr, d_rowoff_, d_coarse_cnt_ + l, d_coarse_stale_ + l);
-      k_compact_emit<<<hl, 256, 0, stream_>>>(sel, wl, hl, d_rowoff_, 0, lv[l]->n_max_, d_coarse_stale_ + l, d_coarse_cnt_ + l,
+      float* pc = lv[l]->d_pc_.get();
+      k_compact_rowcount<<<hl, 256, 0, stream_.get()>>>(sel, wl, hl, d_rowcnt_.get(), d_rowlast_.get());
+      k_compact_rowscan<<<1, 32, 0, stream_.get()>>>(d_rowcnt_.get(), d_rowlast_.get(), wl, hl, nullptr, d_rowoff_.get(), d_coarse_cnt_.get() + l, d_coarse_stale_.get() + l);
+      k_compact_emit<<<hl, 256, 0, stream_.get()>>>(sel, wl, hl, d_rowoff_.get(), 0, lv[l]->n_max_, d_coarse_stale_.get() + l, d_coarse_cnt_.get() + l,
                                               pc, pc + nm, pc + 2 * nm, pc + 3 * nm);
     }
     // 5. n1's dense append behind level 0's points, against the normalised idepth[0] (:655-732)
@@ -1299,60 +1280,60 @@ class TrackerImpl final : public TrackerIface {
       const size_t npx = (size_t)w_ * h_, nm = (size_t)n_max_;
       const float* d_depth = a.depth;
       if (!a.depth_on_device) {
-        std::memcpy(h_front_, a.depth, 4 * npx);
-        TDM_CUDA(cudaMemcpyAsync(d_depth_, h_front_, 4 * npx, cudaMemcpyHostToDevice, stream_));
-        d_depth = d_depth_;
+        std::memcpy(h_front_.get(), a.depth, 4 * npx);
+        TDM_CUDA(cudaMemcpyAsync(d_depth_.get(), h_front_.get(), 4 * npx, cudaMemcpyHostToDevice, stream_.get()));
+        d_depth = d_depth_.get();
       }
-      TDM_CUDA(cudaMemsetAsync(d_proj_, 0xFF, 4 * npx, stream_));
+      TDM_CUDA(cudaMemsetAsync(d_proj_.get(), 0xFF, 4 * npx, stream_.get()));
       const int nx = (w_ + a.step - 1) / a.step, ny = (h_ + a.step - 1) / a.step;
-      k_dense_warp<<<(nx * ny + 255) / 256, 256, 0, stream_>>>(d_depth, w_, h_, a.step, dense_warp(a.T_depth_to_ref), d_proj_);
-      const DenseSel sel{d_proj_, id, a.dense_only, P.level_dI(0), 3};
-      k_compact_rowcount<<<h_, 256, 0, stream_>>>(sel, w_, h_, d_rowcnt_, nullptr);
-      k_compact_rowscan<<<1, 32, 0, stream_>>>(d_rowcnt_, nullptr, w_, h_, d_coarse_cnt_, d_rowoff_, d_coarse_cnt_ + kMaxLevels, nullptr);
-      k_compact_emit<<<h_, 256, 0, stream_>>>(sel, w_, h_, d_rowoff_, 1, n_max_, nullptr, nullptr,
-                                              d_pc_, d_pc_ + nm, d_pc_ + 2 * nm, d_pc_ + 3 * nm);
+      k_dense_warp<<<(nx * ny + 255) / 256, 256, 0, stream_.get()>>>(d_depth, w_, h_, a.step, dense_warp(a.T_depth_to_ref), d_proj_.get());
+      const DenseSel sel{d_proj_.get(), id, a.dense_only, P.level_dI(0), 3};
+      k_compact_rowcount<<<h_, 256, 0, stream_.get()>>>(sel, w_, h_, d_rowcnt_.get(), nullptr);
+      k_compact_rowscan<<<1, 32, 0, stream_.get()>>>(d_rowcnt_.get(), nullptr, w_, h_, d_coarse_cnt_.get(), d_rowoff_.get(), d_coarse_cnt_.get() + kMaxLevels, nullptr);
+      k_compact_emit<<<h_, 256, 0, stream_.get()>>>(sel, w_, h_, d_rowoff_.get(), 1, n_max_, nullptr, nullptr,
+                                              d_pc_.get(), d_pc_.get() + nm, d_pc_.get() + 2 * nm, d_pc_.get() + 3 * nm);
     } else {
-      TDM_CUDA(cudaMemsetAsync(d_coarse_cnt_ + kMaxLevels, 0, 4, stream_));
+      TDM_CUDA(cudaMemsetAsync(d_coarse_cnt_.get() + kMaxLevels, 0, 4, stream_.get()));
     }
     if (nodia) {
       // 6. the undilated level-0 cloud (:186-218) from ws[0], which the dilation left as it was, into the persistent nodia
       //    arrays; count in d_coarse_cnt_[kMaxLevels + 1].  Slot pc_n_nodia < (w-4)(h-4) + 1 <= w*h always fits.
       const size_t npx = (size_t)w_ * h_;
-      float* pc = d_nodia_ + npx;
-      int* cnt = d_coarse_cnt_ + kMaxLevels + 1;
-      const NodiaSel sel{d_nodia_, ws, P.level_dI(0)};
-      k_compact_rowcount<<<h_, 256, 0, stream_>>>(sel, w_, h_, d_rowcnt_, d_rowlast_);
-      k_compact_rowscan<<<1, 32, 0, stream_>>>(d_rowcnt_, d_rowlast_, w_, h_, nullptr, d_rowoff_, cnt, d_coarse_stale_ + kMaxLevels);
-      k_compact_emit<<<h_, 256, 0, stream_>>>(sel, w_, h_, d_rowoff_, 0, (int)npx, d_coarse_stale_ + kMaxLevels, cnt,
+      float* pc = d_nodia_.get() + npx;
+      int* cnt = d_coarse_cnt_.get() + kMaxLevels + 1;
+      const NodiaSel sel{d_nodia_.get(), ws, P.level_dI(0)};
+      k_compact_rowcount<<<h_, 256, 0, stream_.get()>>>(sel, w_, h_, d_rowcnt_.get(), d_rowlast_.get());
+      k_compact_rowscan<<<1, 32, 0, stream_.get()>>>(d_rowcnt_.get(), d_rowlast_.get(), w_, h_, nullptr, d_rowoff_.get(), cnt, d_coarse_stale_.get() + kMaxLevels);
+      k_compact_emit<<<h_, 256, 0, stream_.get()>>>(sel, w_, h_, d_rowoff_.get(), 0, (int)npx, d_coarse_stale_.get() + kMaxLevels, cnt,
                                               pc, pc + npx, pc + 2 * npx, pc + 3 * npx);
       // 7. the quantile (tandem_backend.cpp:354-361) into d_coarse_cnt_[kMaxLevels + 2, + 3].  Every accepted pixel holds at
       //    least one point, so pc_n_nodia <= n: n keys padded with +inf hold every value.  The packed points are dead by now,
       //    their buffer holds the keys and their sorted copy.
-      float *keys = d_pts_, *sorted = d_pts_ + cap;
+      float *keys = d_pts_.get(), *sorted = d_pts_.get() + cap;
       if (n) {
-        k_nodia_keys<<<(n + 255) / 256, 256, 0, stream_>>>(pc + 2 * npx, cnt, n, keys);
+        k_nodia_keys<<<(n + 255) / 256, 256, 0, stream_.get()>>>(pc + 2 * npx, cnt, n, keys);
         size_t tb = 0;
-        TDM_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, keys, sorted, n, 0, 32, stream_));
+        TDM_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, keys, sorted, n, 0, 32, stream_.get()));
         grow_coarse_tmp(tb);
-        TDM_CUDA(cub::DeviceRadixSort::SortKeys(d_coarse_tmp_, tb, keys, sorted, n, 0, 32, stream_));
+        TDM_CUDA(cub::DeviceRadixSort::SortKeys(d_coarse_tmp_.get(), tb, keys, sorted, n, 0, 32, stream_.get()));
       }
-      k_nodia_quantile<<<1, 1, 0, stream_>>>(sorted, cnt, a.quantile_fraction, d_coarse_cnt_ + kMaxLevels + 2);
+      k_nodia_quantile<<<1, 1, 0, stream_.get()>>>(sorted, cnt, a.quantile_fraction, d_coarse_cnt_.get() + kMaxLevels + 2);
     }
     TDM_CUDA(cudaGetLastError());
-    TDM_CUDA(cudaMemcpyAsync(h_coarse_cnt_, d_coarse_cnt_, 4 * (kMaxLevels + (nodia ? 4 : 1)), cudaMemcpyDeviceToHost, stream_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    TDM_CUDA(cudaMemcpyAsync(h_coarse_cnt_.get(), d_coarse_cnt_.get(), 4 * (kMaxLevels + (nodia ? 4 : 1)), cudaMemcpyDeviceToHost, stream_.get()));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
     if (nodia) {   // written whether or not the levels fit below
-      nodia->pc_n_nodia = h_coarse_cnt_[kMaxLevels + 1];
-      std::memcpy(&nodia->idepth_quantile, h_coarse_cnt_ + kMaxLevels + 2, 4);
-      std::memcpy(&nodia->depth_quantile, h_coarse_cnt_ + kMaxLevels + 3, 4);
+      nodia->pc_n_nodia = h_coarse_cnt_.get()[kMaxLevels + 1];
+      std::memcpy(&nodia->idepth_quantile, h_coarse_cnt_.get() + kMaxLevels + 2, 4);
+      std::memcpy(&nodia->depth_quantile, h_coarse_cnt_.get() + kMaxLevels + 3, 4);
       have_nodia_ = true;
     }
     // Capacity: each level needs room for its count and the slot behind it; level 0 also for the dense points.
     int cnt[kMaxLevels];
     bool fits = true;
     for (int l = 0; l < L; ++l) {
-      cnt[l] = h_coarse_cnt_[l] + (l == 0 ? h_coarse_cnt_[kMaxLevels] : 0);   // the `++pc_n` quirk: the last dense point is not counted
-      fits = fits && (long long)h_coarse_cnt_[l] + 1 + (l == 0 ? h_coarse_cnt_[kMaxLevels] : 0) <= lv[l]->n_max_;
+      cnt[l] = h_coarse_cnt_.get()[l] + (l == 0 ? h_coarse_cnt_.get()[kMaxLevels] : 0);   // the `++pc_n` quirk: the last dense point is not counted
+      fits = fits && (long long)h_coarse_cnt_.get()[l] + 1 + (l == 0 ? h_coarse_cnt_.get()[kMaxLevels] : 0) <= lv[l]->n_max_;
     }
     for (int l = 0; l < L; ++l) {
       TrackerImpl& t = *lv[l];
@@ -1372,39 +1353,38 @@ class TrackerImpl final : public TrackerIface {
     TDM_CUDA(cudaSetDevice(device_));
     float* dst[4] = {u, v, idepth, color};
     for (int k = 0; k < 4; ++k)
-      if (dst[k]) TDM_CUDA(cudaMemcpyAsync(dst[k], d_nodia_ + (k + 1) * npx, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+      if (dst[k]) TDM_CUDA(cudaMemcpyAsync(dst[k], d_nodia_.get() + (k + 1) * npx, 4 * (size_t)n, cudaMemcpyDeviceToHost, stream_.get()));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
   }
   void synchronize() override {
     TDM_CUDA(cudaSetDevice(device_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
   }
   void run_resident(int iters, float* ms) override {
     TDM_CHECK(have_params_, "run_resident before calcRes");
     TDM_CUDA(cudaSetDevice(device_));
-    cudaEvent_t e0, e1;
-    TDM_CUDA(cudaEventCreate(&e0)); TDM_CUDA(cudaEventCreate(&e1));
-    TDM_CUDA(cudaEventRecord(e0, stream_));
+    const Event e0 = make_event(), e1 = make_event();
+    TDM_CUDA(cudaEventRecord(e0.get(), stream_.get()));
     for (int i = 0; i < iters; ++i) launch(2);
-    TDM_CUDA(cudaEventRecord(e1, stream_));
-    TDM_CUDA(cudaEventSynchronize(e1));
-    TDM_CUDA(cudaEventElapsedTime(ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    TDM_CUDA(cudaEventRecord(e1.get(), stream_.get()));
+    TDM_CUDA(cudaEventSynchronize(e1.get()));
+    TDM_CUDA(cudaEventElapsedTime(ms, e0.get(), e1.get()));
   }
 
  private:
+  // Each lazy group below is made in locals and kept only once all of it exists, so its guard means "complete".
   void ensure_front_buffers() {
     if (d_proj_) return;
     const size_t npx = (size_t)w_ * h_;
-    TDM_CUDA(cudaMalloc(&d_proj_, 4 * npx));
-    TDM_CUDA(cudaMalloc(&d_depth_, 4 * npx));
-    TDM_CUDA(cudaMalloc(&d_idepth0_, 4 * npx));
-    TDM_CUDA(cudaMalloc(&d_gray_, 4 * npx));
-    TDM_CUDA(cudaMalloc(&d_rowcnt_, 4 * (size_t)h_));
-    TDM_CUDA(cudaMalloc(&d_rowoff_, 4 * (size_t)h_));
-    TDM_CUDA(cudaMalloc(&d_total_, 4));
-    TDM_CUDA(cudaMallocHost(&h_front_, 3 * 4 * npx));
-    TDM_CUDA(cudaMallocHost(&h_total_, 4));
+    DevPtr<unsigned> proj = make_dev<unsigned>(4 * npx);
+    DevPtr<float> depth = make_dev<float>(4 * npx), idepth0 = make_dev<float>(4 * npx), gray = make_dev<float>(4 * npx);
+    DevPtr<int> rowcnt = make_dev<int>(4 * (size_t)h_), rowoff = make_dev<int>(4 * (size_t)h_), total = make_dev<int>(4);
+    HostPtr<float> front = make_host<float>(3 * 4 * npx);
+    HostPtr<int> htotal = make_host<int>(4);
+    d_depth_ = std::move(depth); d_idepth0_ = std::move(idepth0); d_gray_ = std::move(gray);
+    d_rowcnt_ = std::move(rowcnt); d_rowoff_ = std::move(rowoff); d_total_ = std::move(total);
+    h_front_ = std::move(front); h_total_ = std::move(htotal);
+    d_proj_ = std::move(proj);
   }
   // n7 scratch: idepth, weights and dilated weights of every level (levels concatenated), the packed points (pixel, index,
   // value, weight input), their sorted copies (pixel, index) and the sort's temporary storage; grown to the largest point count
@@ -1412,32 +1392,32 @@ class TrackerImpl final : public TrackerIface {
     if (!d_coarse_) {
       size_t tot = 0;
       for (int l = 0; l < kMaxLevels; ++l) tot += (size_t)(w_ >> l) * (h_ >> l);
-      TDM_CUDA(cudaMalloc(&d_coarse_, 3 * 4 * tot));
-      TDM_CUDA(cudaMalloc(&d_rowlast_, 8 * (size_t)h_));
+      DevPtr<float> coarse = make_dev<float>(3 * 4 * tot);
+      DevPtr<int2> rowlast = make_dev<int2>(8 * (size_t)h_);
       // counts per level, the dense count, then (nodia) pc_n_nodia and the quantile's idepth and depth bits
-      TDM_CUDA(cudaMalloc(&d_coarse_cnt_, 4 * (kMaxLevels + 4)));
-      TDM_CUDA(cudaMalloc(&d_coarse_stale_, 4 * (kMaxLevels + 1)));
-      TDM_CUDA(cudaMallocHost(&h_coarse_cnt_, 4 * (kMaxLevels + 4)));
+      DevPtr<int> cnt = make_dev<int>(4 * (kMaxLevels + 4)), stale = make_dev<int>(4 * (kMaxLevels + 1));
+      HostPtr<int> hcnt = make_host<int>(4 * (kMaxLevels + 4));
+      d_rowlast_ = std::move(rowlast); d_coarse_cnt_ = std::move(cnt); d_coarse_stale_ = std::move(stale);
+      h_coarse_cnt_ = std::move(hcnt);
+      d_coarse_ = std::move(coarse);
     }
-    if (n > coarse_cap_) {
+    if (n > coarse_cap_) {   // the old set is freed first; coarse_cap_ is 0 until the new one is complete
       const int cap = n > 1024 ? n : 1024;
-      cudaFree(d_pts_); cudaFreeHost(h_pts_); cudaFree(d_coarse_tmp_);
-      d_pts_ = nullptr; h_pts_ = nullptr; d_coarse_tmp_ = nullptr; coarse_cap_ = 0;
-      TDM_CUDA(cudaMalloc(&d_pts_, 6 * 4 * (size_t)cap));
-      TDM_CUDA(cudaMallocHost(&h_pts_, 4 * 4 * (size_t)cap));
+      d_pts_.reset(); h_pts_.reset(); d_coarse_tmp_.reset(); coarse_tmp_bytes_ = 0; coarse_cap_ = 0;
+      d_pts_ = make_dev<float>(6 * 4 * (size_t)cap);
+      h_pts_ = make_host<float>(4 * 4 * (size_t)cap);
       size_t tb = 0;
       TDM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const int*)nullptr, (int*)nullptr, (const int*)nullptr, (int*)nullptr, cap));
-      TDM_CUDA(cudaMalloc(&d_coarse_tmp_, tb));
+      d_coarse_tmp_ = make_dev(tb);
       coarse_tmp_bytes_ = tb;
       coarse_cap_ = cap;
     }
   }
   void grow_coarse_tmp(size_t tb) {
     if (tb <= coarse_tmp_bytes_) return;
-    TDM_CUDA(cudaStreamSynchronize(stream_));
-    cudaFree(d_coarse_tmp_);
-    d_coarse_tmp_ = nullptr; coarse_tmp_bytes_ = 0;
-    TDM_CUDA(cudaMalloc(&d_coarse_tmp_, tb));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
+    d_coarse_tmp_.reset(); coarse_tmp_bytes_ = 0;
+    d_coarse_tmp_ = make_dev(tb);
     coarse_tmp_bytes_ = tb;
   }
   // the nodia image (unweighted idepth sums of level 0) and the persistent pc_u/v/idepth/color_nodia, w*h floats each; the
@@ -1445,8 +1425,9 @@ class TrackerImpl final : public TrackerIface {
   void ensure_nodia_buffers() {
     if (d_nodia_) return;
     const size_t npx = (size_t)w_ * h_;
-    TDM_CUDA(cudaMalloc(&d_nodia_, 5 * 4 * npx));
-    TDM_CUDA(cudaMemsetAsync(d_nodia_ + npx, 0, 4 * 4 * npx, stream_));
+    DevPtr<float> nodia = make_dev<float>(5 * 4 * npx);
+    TDM_CUDA(cudaMemsetAsync(nodia.get() + npx, 0, 4 * 4 * npx, stream_.get()));
+    d_nodia_ = std::move(nodia);
   }
   // KRKi = (K R) Ki, Kt = K t in float, k = 0,1,2 (CoarseTracker.cpp:676-677)
   DenseWarp dense_warp(const double* T) const {
@@ -1481,53 +1462,50 @@ class TrackerImpl final : public TrackerIface {
   // needs an update.
   void ensure_lm_buffers() {
     if (lm_exec_) return;
-    TDM_CUDA(cudaMalloc(&d_lm_ctx_, sizeof(LmCtx)));
-    TDM_CUDA(cudaMalloc(&d_lm_out_, kOut * 8));
-    TDM_CUDA(cudaMallocHost(&h_lm_in_, sizeof(LmIn)));
-    TDM_CUDA(cudaHostAlloc(&h_lm_res_, sizeof(LmResult), cudaHostAllocMapped));
-    TDM_CUDA(cudaHostGetDevicePointer(&d_lm_res_, h_lm_res_, 0));
-    TDM_CUDA(cudaEventCreateWithFlags(&lm_in_free_, cudaEventDisableTiming));
-    TDM_CUDA(cudaEventCreate(&lm_e0_));
-    TDM_CUDA(cudaEventCreate(&lm_e1_));
-    cudaGraph_t g = nullptr;
-    TDM_CUDA(cudaGraphCreate(&g, 0));
-    try {
-      cudaGraphConditionalHandle loop;
-      TDM_CUDA(cudaGraphConditionalHandleCreate(&loop, g, 1, cudaGraphCondAssignDefault));
-      cudaKernelNodeParams kp = {};
-      void* init_args[] = {&d_lm_ctx_, &d_lm_res_, &loop};
-      kp.func = (void*)k_lm_init;
-      kp.gridDim = dim3(1); kp.blockDim = dim3(32);
-      kp.kernelParams = init_args;
-      cudaGraphNode_t init;
-      TDM_CUDA(cudaGraphAddKernelNode(&init, g, nullptr, 0, &kp));
-      cudaGraphNodeParams cp = {};
-      cp.type = cudaGraphNodeTypeConditional;
-      cp.conditional.handle = loop;
-      cp.conditional.type = cudaGraphCondTypeWhile;
-      cp.conditional.size = 1;
-      cudaGraphNode_t while_node;
-      TDM_CUDA(cudaGraphAddNode(&while_node, g, &init, 1, &cp));
-      TrkParams p{};                                 // unused: the kernel reads the level's parameters from LmCtx
-      TrkBufs b{};
-      b.lm = d_lm_ctx_; b.partials = d_partials_; b.ticket = d_ticket_; b.out = d_lm_out_;
-      void* eval_args[] = {&p, &b};
-      kp.func = (void*)k_tracker<4>;
-      kp.gridDim = dim3(kBlocks); kp.blockDim = dim3(kThreads);
-      kp.kernelParams = eval_args;
-      cudaGraphNode_t eval;
-      TDM_CUDA(cudaGraphAddKernelNode(&eval, cp.conditional.phGraph_out[0], nullptr, 0, &kp));
-      TDM_CUDA(cudaGraphInstantiate(&lm_exec_, g, 0));
-    } catch (...) {
-      cudaGraphDestroy(g);
-      throw;
-    }
-    cudaGraphDestroy(g);
+    DevPtr<LmCtx> ctx = make_dev<LmCtx>(sizeof(LmCtx));
+    DevPtr<double> out = make_dev<double>(kOut * 8);
+    HostPtr<LmIn> in = make_host<LmIn>(sizeof(LmIn));
+    HostPtr<LmResult> res = make_host<LmResult>(sizeof(LmResult), cudaHostAllocMapped);
+    LmResult* d_res = nullptr;
+    TDM_CUDA(cudaHostGetDevicePointer(&d_res, res.get(), 0));
+    Event in_free = make_event(cudaEventDisableTiming), e0 = make_event(), e1 = make_event();
+    const Graph g = make_graph();
+    cudaGraphConditionalHandle loop;
+    TDM_CUDA(cudaGraphConditionalHandleCreate(&loop, g.get(), 1, cudaGraphCondAssignDefault));
+    cudaKernelNodeParams kp = {};
+    LmCtx* d_ctx = ctx.get();
+    void* init_args[] = {&d_ctx, &d_res, &loop};
+    kp.func = (void*)k_lm_init;
+    kp.gridDim = dim3(1); kp.blockDim = dim3(32);
+    kp.kernelParams = init_args;
+    cudaGraphNode_t init;
+    TDM_CUDA(cudaGraphAddKernelNode(&init, g.get(), nullptr, 0, &kp));
+    cudaGraphNodeParams cp = {};
+    cp.type = cudaGraphNodeTypeConditional;
+    cp.conditional.handle = loop;
+    cp.conditional.type = cudaGraphCondTypeWhile;
+    cp.conditional.size = 1;
+    cudaGraphNode_t while_node;
+    TDM_CUDA(cudaGraphAddNode(&while_node, g.get(), &init, 1, &cp));
+    TrkParams p{};                                 // unused: the kernel reads the level's parameters from LmCtx
+    TrkBufs b{};
+    b.lm = d_ctx; b.partials = d_partials_.get(); b.ticket = d_ticket_.get(); b.out = out.get();
+    void* eval_args[] = {&p, &b};
+    kp.func = (void*)k_tracker<4>;
+    kp.gridDim = dim3(kBlocks); kp.blockDim = dim3(kThreads);
+    kp.kernelParams = eval_args;
+    cudaGraphNode_t eval;
+    TDM_CUDA(cudaGraphAddKernelNode(&eval, cp.conditional.phGraph_out[0], nullptr, 0, &kp));
+    GraphExec exec = make_graph_exec(g.get());
+    d_lm_ctx_ = std::move(ctx); d_lm_out_ = std::move(out); h_lm_in_ = std::move(in); h_lm_res_ = std::move(res);
+    d_lm_res_ = d_res;
+    lm_in_free_ = std::move(in_free); lm_e0_ = std::move(e0); lm_e1_ = std::move(e1);
+    lm_exec_ = std::move(exec);
   }
   // the staging of LmCtx::in; free once the previous call's upload has completed (normally long since)
   LmIn& lm_in() {
     ensure_lm_buffers();
-    TDM_CUDA(cudaEventSynchronize(lm_in_free_));
+    TDM_CUDA(cudaEventSynchronize(lm_in_free_.get()));
     return *h_lm_in_;
   }
   // Checks the levels of an n5 / n6 call and fills LmCtx::in's staging with them (everything but min_res and the mode); an
@@ -1554,7 +1532,7 @@ class TrackerImpl final : public TrackerIface {
     for (int l = 0; l <= coarsest; ++l) {
       lv[l]->fill_level(&in.lv[l], new_exposure, coarse_cutoff, max_iterations[l], lambda_limit, mode_a < 0, mode_b < 0);
       in.max_evals += 2 * (1 + 6 + max_iterations[l]);   // a level may run twice (the repeat rule)
-      if (l > 0) lv[l]->order_before(stream_);           // reference upload, setNewFromPyramid copy of that tracker
+      if (l > 0) lv[l]->order_before(stream_.get());           // reference upload, setNewFromPyramid copy of that tracker
     }
     in.mode_a = mode_a; in.mode_b = mode_b;
     in.coarsest = coarsest;
@@ -1568,7 +1546,7 @@ class TrackerImpl final : public TrackerIface {
     for (int i = 0; i < 9; ++i) L->p.Ki[i] = Ki_[i];
     L->p.huber = huber_; L->p.ref_b = (float)ref_aff_[1];
     const size_t nm = (size_t)n_max_;
-    L->pc_u = d_pc_; L->pc_v = d_pc_ + nm; L->pc_idepth = d_pc_ + 2 * nm; L->pc_color = d_pc_ + 3 * nm; L->dInew = d_dI_;
+    L->pc_u = d_pc_.get(); L->pc_v = d_pc_.get() + nm; L->pc_idepth = d_pc_.get() + 2 * nm; L->pc_color = d_pc_.get() + 3 * nm; L->dInew = d_dI_.get();
     LmConfig& c = L->cfg;
     for (int i = 0; i < 9; ++i) c.Ki[i] = Ki_[i];
     c.ref_exposure = ref_exposure_; c.new_exposure = new_exposure;
@@ -1578,9 +1556,9 @@ class TrackerImpl final : public TrackerIface {
   }
   // orders this tracker's pending stream work before work enqueued later on `other`
   void order_before(cudaStream_t other) {
-    if (!ready_) TDM_CUDA(cudaEventCreateWithFlags(&ready_, cudaEventDisableTiming));
-    TDM_CUDA(cudaEventRecord(ready_, stream_));
-    TDM_CUDA(cudaStreamWaitEvent(other, ready_, 0));
+    if (!ready_) ready_ = make_event(cudaEventDisableTiming);
+    TDM_CUDA(cudaEventRecord(ready_.get(), stream_.get()));
+    TDM_CUDA(cudaStreamWaitEvent(other, ready_.get(), 0));
   }
   // Runs the graph on h_lm_in_ (filled by the caller) with one host wait; returns the mapped result.  n6 passes its own mapped
   // completion flag and the first rt_bytes of h_rt_in_ to upload next to LmIn.
@@ -1590,23 +1568,25 @@ class TrackerImpl final : public TrackerIface {
     in.aff0[0] = aff0[0]; in.aff0[1] = aff0[1];
     if (!done) done = &h_lm_res_->done;
     *done = 0;
-    TDM_CUDA(cudaEventRecord(lm_e0_, stream_));
-    TDM_CUDA(cudaMemcpyAsync(&d_lm_ctx_->in, h_lm_in_, sizeof(LmIn), cudaMemcpyHostToDevice, stream_));
-    if (rt_bytes) TDM_CUDA(cudaMemcpyAsync(&d_lm_ctx_->rin, h_rt_in_, rt_bytes, cudaMemcpyHostToDevice, stream_));
-    TDM_CUDA(cudaEventRecord(lm_in_free_, stream_));
-    TDM_CUDA(cudaGraphLaunch(lm_exec_, stream_));
-    TDM_CUDA(cudaEventRecord(lm_e1_, stream_));
-    TDM_CUDA(cudaEventSynchronize(lm_e1_));
-    TDM_CUDA(cudaEventElapsedTime(device_ms, lm_e0_, lm_e1_));
+    TDM_CUDA(cudaEventRecord(lm_e0_.get(), stream_.get()));
+    TDM_CUDA(cudaMemcpyAsync(&d_lm_ctx_->in, h_lm_in_.get(), sizeof(LmIn), cudaMemcpyHostToDevice, stream_.get()));
+    if (rt_bytes) TDM_CUDA(cudaMemcpyAsync(&d_lm_ctx_->rin, h_rt_in_.get(), rt_bytes, cudaMemcpyHostToDevice, stream_.get()));
+    TDM_CUDA(cudaEventRecord(lm_in_free_.get(), stream_.get()));
+    TDM_CUDA(cudaGraphLaunch(lm_exec_.get(), stream_.get()));
+    TDM_CUDA(cudaEventRecord(lm_e1_.get(), stream_.get()));
+    TDM_CUDA(cudaEventSynchronize(lm_e1_.get()));
+    TDM_CUDA(cudaEventElapsedTime(device_ms, lm_e0_.get(), lm_e1_.get()));
     if (*done != 1) throw Error("track: the device loop did not finish (internal error)");
-    return h_lm_res_;
+    return h_lm_res_.get();
   }
   // n6: the try list's pinned staging (guarded like LmCtx::in's, by lm_in_free_) and the mapped result with the per-try records
   void ensure_rt_buffers() {
     if (h_rt_in_) return;
-    TDM_CUDA(cudaMallocHost(&h_rt_in_, sizeof(RetrackIn)));
-    TDM_CUDA(cudaHostAlloc(&h_rt_out_, sizeof(RetrackOut), cudaHostAllocMapped));
-    TDM_CUDA(cudaHostGetDevicePointer(&d_rt_out_, h_rt_out_, 0));
+    HostPtr<RetrackIn> in = make_host<RetrackIn>(sizeof(RetrackIn));
+    HostPtr<RetrackOut> out = make_host<RetrackOut>(sizeof(RetrackOut), cudaHostAllocMapped);
+    TDM_CUDA(cudaHostGetDevicePointer(&d_rt_out_, out.get(), 0));
+    h_rt_out_ = std::move(out);
+    h_rt_in_ = std::move(in);
   }
   void set_aff(float new_exposure, const double aff[2]) {  // AffLight::fromToVecExposure, cpp:42-52
     float eF = ref_exposure_, eT = new_exposure;
@@ -1643,12 +1623,12 @@ class TrackerImpl final : public TrackerIface {
     TrkBufs b;
     const size_t nm = (size_t)n_max_;
     b.lm = nullptr;
-    b.pc_u = d_pc_; b.pc_v = d_pc_ + nm; b.pc_idepth = d_pc_ + 2 * nm; b.pc_color = d_pc_ + 3 * nm;
-    b.dInew = d_dI_; b.warped = d_warped_; b.n_max = n_max_;
-    b.partials = d_partials_; b.ticket = d_ticket_; b.out = d_out_; b.batch = nullptr;
-    if (mode == 0) k_tracker<0><<<kBlocks, kThreads, 0, stream_>>>(p_, b);
-    else if (mode == 1) k_tracker<1><<<kBlocks, kThreads, 0, stream_>>>(p_, b);
-    else k_tracker<2><<<kBlocks, kThreads, 0, stream_>>>(p_, b);
+    b.pc_u = d_pc_.get(); b.pc_v = d_pc_.get() + nm; b.pc_idepth = d_pc_.get() + 2 * nm; b.pc_color = d_pc_.get() + 3 * nm;
+    b.dInew = d_dI_.get(); b.warped = d_warped_.get(); b.n_max = n_max_;
+    b.partials = d_partials_.get(); b.ticket = d_ticket_.get(); b.out = d_out_; b.batch = nullptr;
+    if (mode == 0) k_tracker<0><<<kBlocks, kThreads, 0, stream_.get()>>>(p_, b);
+    else if (mode == 1) k_tracker<1><<<kBlocks, kThreads, 0, stream_.get()>>>(p_, b);
+    else k_tracker<2><<<kBlocks, kThreads, 0, stream_.get()>>>(p_, b);
     TDM_CUDA(cudaGetLastError());
   }
   // Batched calcRes over n_hyp poses (motion hypotheses of FullSystem::trackNewCoarse, FullSystem.cpp:437-530) in ONE launch and
@@ -1659,20 +1639,23 @@ class TrackerImpl final : public TrackerIface {
     TDM_CHECK(have_k_ && have_new_, "calcResBatch before setK / setNew");
     TDM_CUDA(cudaSetDevice(device_));
     if (!d_batch_) {
-      TDM_CUDA(cudaMalloc(&d_batch_, kMaxHyp * sizeof(TrkPose)));
-      TDM_CUDA(cudaMallocHost(&h_batch_, kMaxHyp * sizeof(TrkPose)));
-      TDM_CUDA(cudaMalloc(&d_batch_partials_, (size_t)kMaxHyp * kBlocks * kOut * 8));
-      TDM_CUDA(cudaMalloc(&d_batch_ticket_, kMaxHyp * 4));
-      TDM_CUDA(cudaMemset(d_batch_ticket_, 0, kMaxHyp * 4));
-      TDM_CUDA(cudaHostAlloc(&h_batch_out_, (size_t)kMaxHyp * kOut * 8, cudaHostAllocMapped));
-      TDM_CUDA(cudaHostGetDevicePointer(&d_batch_out_, h_batch_out_, 0));
+      DevPtr<TrkPose> batch = make_dev<TrkPose>(kMaxHyp * sizeof(TrkPose));
+      HostPtr<TrkPose> hbatch = make_host<TrkPose>(kMaxHyp * sizeof(TrkPose));
+      DevPtr<double> partials = make_dev<double>((size_t)kMaxHyp * kBlocks * kOut * 8);
+      DevPtr<unsigned> ticket = make_dev<unsigned>(kMaxHyp * 4);
+      TDM_CUDA(cudaMemset(ticket.get(), 0, kMaxHyp * 4));
+      HostPtr<double> out = make_host<double>((size_t)kMaxHyp * kOut * 8, cudaHostAllocMapped);
+      TDM_CUDA(cudaHostGetDevicePointer(&d_batch_out_, out.get(), 0));
+      h_batch_ = std::move(hbatch); d_batch_partials_ = std::move(partials); d_batch_ticket_ = std::move(ticket);
+      h_batch_out_ = std::move(out);
+      d_batch_ = std::move(batch);
     }
-    TDM_CUDA(cudaStreamSynchronize(stream_));   // the pinned pose staging may still be in flight from the previous batch
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));   // the pinned pose staging may still be in flight from the previous batch
     const TrkParams saved = p_;
     const bool saved_have = have_params_;
     for (int k = 0; k < n_hyp; ++k) {
       prepare(refToNew + 16 * k, new_exposure, aff + 2 * k, cutoffTH);   // the exact host arithmetic of calcRes, per pose
-      TrkPose& q = h_batch_[k];
+      TrkPose& q = h_batch_.get()[k];
       for (int i = 0; i < 9; ++i) q.RKi[i] = p_.RKi[i];
       for (int i = 0; i < 3; ++i) q.t[i] = p_.t[i];
       q.affa = p_.affa; q.affb = p_.affb; q.cutoff = p_.cutoff; q.maxEnergy = p_.maxEnergy;
@@ -1680,31 +1663,31 @@ class TrackerImpl final : public TrackerIface {
     TrkParams pb = p_;
     p_ = saved;                                   // calcG keeps referring to the last plain calcRes
     have_params_ = saved_have;
-    TDM_CUDA(cudaMemcpyAsync(d_batch_, h_batch_, n_hyp * sizeof(TrkPose), cudaMemcpyHostToDevice, stream_));
+    TDM_CUDA(cudaMemcpyAsync(d_batch_.get(), h_batch_.get(), n_hyp * sizeof(TrkPose), cudaMemcpyHostToDevice, stream_.get()));
     TrkBufs b;
     const size_t nm = (size_t)n_max_;
     b.lm = nullptr;
-    b.pc_u = d_pc_; b.pc_v = d_pc_ + nm; b.pc_idepth = d_pc_ + 2 * nm; b.pc_color = d_pc_ + 3 * nm;
-    b.dInew = d_dI_; b.warped = nullptr; b.n_max = n_max_;
-    b.partials = d_batch_partials_; b.ticket = d_batch_ticket_; b.out = d_batch_out_; b.batch = d_batch_;
-    k_tracker<3><<<dim3(kBlocks, n_hyp), kThreads, 0, stream_>>>(pb, b);
+    b.pc_u = d_pc_.get(); b.pc_v = d_pc_.get() + nm; b.pc_idepth = d_pc_.get() + 2 * nm; b.pc_color = d_pc_.get() + 3 * nm;
+    b.dInew = d_dI_.get(); b.warped = nullptr; b.n_max = n_max_;
+    b.partials = d_batch_partials_.get(); b.ticket = d_batch_ticket_.get(); b.out = d_batch_out_; b.batch = d_batch_.get();
+    k_tracker<3><<<dim3(kBlocks, n_hyp), kThreads, 0, stream_.get()>>>(pb, b);
     TDM_CUDA(cudaGetLastError());
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
     for (int k = 0; k < n_hyp; ++k) {
-      const volatile double* o = h_batch_out_ + (size_t)k * kOut;
+      const volatile double* o = h_batch_out_.get() + (size_t)k * kOut;
       double* r = res6 + 6 * k;
       r[0] = o[0]; r[1] = o[1]; r[2] = o[4] / o[6]; r[3] = 0; r[4] = o[5] / o[6]; r[5] = o[3] / o[1];
     }
   }
   void finish_res(double res6[6]) {  // cpp:264-272
-    const volatile double* o = h_out_;
+    const volatile double* o = h_out_.get();
     res6[0] = o[0]; res6[1] = o[1];
     res6[2] = o[4] / o[6]; res6[3] = 0; res6[4] = o[5] / o[6];
     res6[5] = o[3] / o[1];
     num_warped_ = (int)o[2];
   }
   void finish_g(double H[64], double b[8]) {  // cpp:335-355
-    const volatile double* o = h_out_ + kRes;
+    const volatile double* o = h_out_.get() + kRes;
     const double factor = 1.0 / num_warped_;
     static const double scale[8] = {1.0, 1.0, 1.0, 0.5, 0.5, 0.5, 10.0, 1000.0};
     for (int r = 0; r < 8; ++r) {
@@ -1725,39 +1708,51 @@ class TrackerImpl final : public TrackerIface {
   static constexpr int kMaxIterations = 200;
   float ref_exposure_ = 1.f;
   double ref_aff_[2] = {0, 0};
-  cudaStream_t stream_ = nullptr;
-  float *d_pc_ = nullptr, *d_warped_ = nullptr, *d_dI_ = nullptr, *h_pc_ = nullptr, *h_dI_ = nullptr;
+  Stream stream_;
+  DevPtr<float> d_pc_, d_warped_, d_dI_;
+  HostPtr<float> h_pc_, h_dI_;
   static constexpr int kMaxHyp = 64;
-  TrkPose *d_batch_ = nullptr, *h_batch_ = nullptr;
-  double *d_batch_partials_ = nullptr, *h_batch_out_ = nullptr, *d_batch_out_ = nullptr;
-  unsigned* d_batch_ticket_ = nullptr;
-  double *d_partials_ = nullptr, *h_out_ = nullptr, *d_out_ = nullptr;
-  unsigned* d_ticket_ = nullptr;
+  DevPtr<TrkPose> d_batch_;
+  HostPtr<TrkPose> h_batch_;
+  DevPtr<double> d_batch_partials_;
+  HostPtr<double> h_batch_out_;
+  double* d_batch_out_ = nullptr;
+  DevPtr<unsigned> d_batch_ticket_;
+  DevPtr<double> d_partials_;
+  HostPtr<double> h_out_;
+  double* d_out_ = nullptr;
+  DevPtr<unsigned> d_ticket_;
   TrkParams p_{};
   int num_warped_ = 0;
   // n1 buffers
-  unsigned* d_proj_ = nullptr;
-  float *d_depth_ = nullptr, *d_idepth0_ = nullptr, *d_gray_ = nullptr, *h_front_ = nullptr;
-  int *d_rowcnt_ = nullptr, *d_rowoff_ = nullptr, *d_total_ = nullptr, *h_total_ = nullptr;
+  DevPtr<unsigned> d_proj_;
+  DevPtr<float> d_depth_, d_idepth0_, d_gray_;
+  HostPtr<float> h_front_;
+  DevPtr<int> d_rowcnt_, d_rowoff_, d_total_;
+  HostPtr<int> h_total_;
   // n3 buffers
-  LmCtx* d_lm_ctx_ = nullptr;
-  double* d_lm_out_ = nullptr;
-  LmIn* h_lm_in_ = nullptr;
-  LmResult *h_lm_res_ = nullptr, *d_lm_res_ = nullptr;
-  cudaGraphExec_t lm_exec_ = nullptr;
-  cudaEvent_t lm_in_free_ = nullptr, lm_e0_ = nullptr, lm_e1_ = nullptr;
-  cudaEvent_t ready_ = nullptr;   // order_before
+  DevPtr<LmCtx> d_lm_ctx_;
+  DevPtr<double> d_lm_out_;
+  HostPtr<LmIn> h_lm_in_;
+  HostPtr<LmResult> h_lm_res_;
+  LmResult* d_lm_res_ = nullptr;
+  GraphExec lm_exec_;
+  Event lm_in_free_, lm_e0_, lm_e1_;
+  Event ready_;   // order_before
   // n6 buffers
-  RetrackIn* h_rt_in_ = nullptr;
-  RetrackOut *h_rt_out_ = nullptr, *d_rt_out_ = nullptr;
+  HostPtr<RetrackIn> h_rt_in_;
+  HostPtr<RetrackOut> h_rt_out_;
+  RetrackOut* d_rt_out_ = nullptr;
   // n7 buffers (ensure_coarse_buffers)
-  float *d_coarse_ = nullptr, *d_pts_ = nullptr, *h_pts_ = nullptr;
-  int2* d_rowlast_ = nullptr;
-  int *d_coarse_cnt_ = nullptr, *d_coarse_stale_ = nullptr, *h_coarse_cnt_ = nullptr;
-  void* d_coarse_tmp_ = nullptr;
+  DevPtr<float> d_coarse_, d_pts_;
+  HostPtr<float> h_pts_;
+  DevPtr<int2> d_rowlast_;
+  DevPtr<int> d_coarse_cnt_, d_coarse_stale_;
+  HostPtr<int> h_coarse_cnt_;
+  DevPtr<void> d_coarse_tmp_;
   size_t coarse_tmp_bytes_ = 0;
   int coarse_cap_ = 0;
-  float* d_nodia_ = nullptr;   // ensure_nodia_buffers
+  DevPtr<float> d_nodia_;   // ensure_nodia_buffers
   bool have_nodia_ = false;
 };
 
@@ -1771,47 +1766,45 @@ class PyramidImpl final : public PyramidIface {
       throw Error("tandem_b200: no CUDA device visible - this library has no CPU fallback");
     TDM_CHECK(w > 0 && h > 0 && levels >= 1 && levels <= 8 && (w >> (levels - 1)) >= 3 && (h >> (levels - 1)) >= 3, "bad pyramid shape");
     TDM_CUDA(cudaSetDevice(device_));
-    TDM_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-    TDM_CUDA(cudaEventCreateWithFlags(&ready_, cudaEventDisableTiming));
+    stream_ = make_stream(0);
+    ready_ = make_event(cudaEventDisableTiming);
     size_t tot = 0;
     for (int l = 0; l < levels; ++l) { off_.push_back(tot); tot += (size_t)(w >> l) * (h >> l); }
-    TDM_CUDA(cudaMalloc(&d_dI_, 3 * 4 * tot));
-    TDM_CUDA(cudaMalloc(&d_abs_, 4 * tot));
-    TDM_CUDA(cudaMalloc(&d_gray_, 4 * (size_t)w * h));
-    TDM_CUDA(cudaMalloc(&d_in_, 4 * (size_t)w * h));
-    TDM_CUDA(cudaMallocHost(&h_in_, 4 * (size_t)w * h));
+    d_dI_ = make_dev<float>(3 * 4 * tot);
+    d_abs_ = make_dev<float>(4 * tot);
+    d_gray_ = make_dev<float>(4 * (size_t)w * h);
+    d_in_ = make_dev<float>(4 * (size_t)w * h);
+    h_in_ = make_host<float>(4 * (size_t)w * h);
   }
   ~PyramidImpl() override {
     cudaSetDevice(device_);
-    cudaStreamSynchronize(stream_);
-    cudaFree(d_dI_); cudaFree(d_abs_); cudaFree(d_gray_); cudaFree(d_in_); cudaFreeHost(h_in_);
-    cudaEventDestroy(ready_); cudaStreamDestroy(stream_);
+    cudaStreamSynchronize(stream_.get());
   }
   void build(const float* gray_host) override {
     TDM_CHECK(gray_host, "null argument");
     TDM_CUDA(cudaSetDevice(device_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
-    std::memcpy(h_in_, gray_host, 4 * (size_t)w_ * h_);
-    TDM_CUDA(cudaMemcpyAsync(d_in_, h_in_, 4 * (size_t)w_ * h_, cudaMemcpyHostToDevice, stream_));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
+    std::memcpy(h_in_.get(), gray_host, 4 * (size_t)w_ * h_);
+    TDM_CUDA(cudaMemcpyAsync(d_in_.get(), h_in_.get(), 4 * (size_t)w_ * h_, cudaMemcpyHostToDevice, stream_.get()));
     for (int l = 0; l < levels_; ++l) {
       const int wl = w_ >> l, hl = h_ >> l, n = wl * hl;
-      const float* src = l == 0 ? d_in_ : d_dI_ + 3 * off_[l - 1];
-      k_pyr_level<<<(n + 255) / 256, 256, 0, stream_>>>(src, l > 0, l > 0 ? (w_ >> (l - 1)) : 0, d_gray_, wl, hl);
-      k_pyr_grad<<<(n + 255) / 256, 256, 0, stream_>>>(d_gray_, d_dI_ + 3 * off_[l], d_abs_ + off_[l], wl, hl);
+      const float* src = l == 0 ? d_in_.get() : d_dI_.get() + 3 * off_[l - 1];
+      k_pyr_level<<<(n + 255) / 256, 256, 0, stream_.get()>>>(src, l > 0, l > 0 ? (w_ >> (l - 1)) : 0, d_gray_.get(), wl, hl);
+      k_pyr_grad<<<(n + 255) / 256, 256, 0, stream_.get()>>>(d_gray_.get(), d_dI_.get() + 3 * off_[l], d_abs_.get() + off_[l], wl, hl);
     }
     TDM_CUDA(cudaGetLastError());
-    TDM_CUDA(cudaEventRecord(ready_, stream_));
+    TDM_CUDA(cudaEventRecord(ready_.get(), stream_.get()));
   }
   void get_level(int lvl, float* dI_host, float* absgrad_host) override {
     TDM_CHECK(lvl >= 0 && lvl < levels_, "bad level");
     TDM_CUDA(cudaSetDevice(device_));
     const size_t n = (size_t)(w_ >> lvl) * (h_ >> lvl);
-    if (dI_host) TDM_CUDA(cudaMemcpyAsync(dI_host, d_dI_ + 3 * off_[lvl], 12 * n, cudaMemcpyDeviceToHost, stream_));
-    if (absgrad_host) TDM_CUDA(cudaMemcpyAsync(absgrad_host, d_abs_ + off_[lvl], 4 * n, cudaMemcpyDeviceToHost, stream_));
-    TDM_CUDA(cudaStreamSynchronize(stream_));
+    if (dI_host) TDM_CUDA(cudaMemcpyAsync(dI_host, d_dI_.get() + 3 * off_[lvl], 12 * n, cudaMemcpyDeviceToHost, stream_.get()));
+    if (absgrad_host) TDM_CUDA(cudaMemcpyAsync(absgrad_host, d_abs_.get() + off_[lvl], 4 * n, cudaMemcpyDeviceToHost, stream_.get()));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
   }
-  const float* level_dI(int lvl) const override { return d_dI_ + 3 * off_.at(lvl); }
-  void* ready_event() const override { return (void*)ready_; }
+  const float* level_dI(int lvl) const override { return d_dI_.get() + 3 * off_.at(lvl); }
+  void* ready_event() const override { return (void*)ready_.get(); }
   int width(int lvl) const override { return w_ >> lvl; }
   int height(int lvl) const override { return h_ >> lvl; }
   int levels() const override { return levels_; }
@@ -1819,10 +1812,11 @@ class PyramidImpl final : public PyramidIface {
 
  private:
   int w_, h_, levels_, device_;
-  cudaStream_t stream_ = nullptr;
-  cudaEvent_t ready_ = nullptr;
+  Stream stream_;
+  Event ready_;
   std::vector<size_t> off_;
-  float *d_dI_ = nullptr, *d_abs_ = nullptr, *d_gray_ = nullptr, *d_in_ = nullptr, *h_in_ = nullptr;
+  DevPtr<float> d_dI_, d_abs_, d_gray_, d_in_;
+  HostPtr<float> h_in_;
 };
 
 PyramidIface* make_pyramid(int w, int h, int levels, int device) { return new PyramidImpl(w, h, levels, device); }

@@ -5,7 +5,7 @@ import torch
 
 from oracle import mvsnet_oracle as O
 from tandem_b200 import DrMvsnet, default_weights
-from tandem_b200.weights_io import load_tdmw
+from tandem_b200.weights_io import load_tdmw, save_tdmw
 
 pytestmark = pytest.mark.gpu
 
@@ -279,6 +279,23 @@ def test_argument_errors_and_two_handles():
         a.CallAsync(96, 128, 3, 1, win["bgrs"], win["K"], win["c2ws"], 0.5, 5.0, 10.0)
     ra, rb = a.GetResult(), b.GetResult()
     assert np.array_equal(ra.depth_dense, rb.depth_dense) and np.array_equal(ra.confidence, rb.confidence)
+
+
+def test_failed_construction_releases_its_engine_slot(tmp_path, golden_small):
+    """A DrMvsnet whose weight file lacks a tensor fails with that tensor's name and gives back everything it took, its engine
+    slot included: more failures in a row than there are slots (8) still name the tensor, and an intact handle then works."""
+    from tandem_b200 import TandemError
+    w, dn, va = load_tdmw(default_weights("abl04_fewer_depth_planes"))
+    missing = "cost_regularization_net.stage2.conv3.conv.weight"
+    del w[missing]
+    broken = str(tmp_path / "missing_tensor.tdmw")
+    save_tdmw(broken, w, dn, va)
+    for _ in range(9):
+        with pytest.raises(TandemError, match=missing):
+            DrMvsnet(broken, precision="mixed16")
+    m, out = _run(golden_small, "abl04_fewer_depth_planes", "mixed16", filter_all=False)
+    assert float(np.mean(np.abs(out.depth - golden_small["abl04_stage3_depth"]))) < 1e-2
+    assert float(np.mean(np.abs(out.confidence - golden_small["abl04_stage3_confidence"]))) < 1e-2
 
 
 @pytest.mark.parametrize("which", ["full", "small"])
