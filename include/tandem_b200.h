@@ -73,7 +73,7 @@ int tdm_mvsnet_call_async_k(tdm_mvsnet* h, int height, int width, int view_num, 
  * bgrs[i] of a held id is ignored (the id wins: the cached image and features are used).  intrinsics: the 3x3
  * full-resolution K as in tdm_mvsnet_call_async, or with stage_k != 0 the 27 floats of tdm_mvsnet_call_async_k.
  * Errors, with nothing launched and the cache unchanged: a NULL image for an id the handle does not hold (every id, when
- * the size or view_num differs from the last call's), the same id twice, cv_variant 5, and every tdm_mvsnet_call_async
+ * the size or view_num differs from the last call's), the same id twice, and every tdm_mvsnet_call_async
  * error.  tdm_mvsnet_call_async / _call_async_k, a new size or view_num and any tdm_mvsnet_set_option except eager_d2h
  * empty the cache. */
 int tdm_mvsnet_call_async_ids(tdm_mvsnet* h, int height, int width, int view_num, int ref_index, const long long* view_ids,

@@ -609,14 +609,14 @@ def homography64(K, c2w_ref, c2w_src):
 
 @dataclass
 class CvArith:
-    """Error constants of a cost-volume kernel (mvsnet_kernels.cuh k_cost_volume / k_cost_volume_va16, cost_volume_tma.cuh):
+    """Error constants of a cost-volume kernel (mvsnet_kernels.cuh k_cost_volume / k_cost_volume_va16):
       u_bil    relative rounding of the bilinear sample: fp16 weights (2^-11) and four fp16 partial roundings (HFMA2 chain), or
                fp32 weights and FFMA (a few 2^-24) for the bf16 engine
       ref_chain  the chain starts from -ref / 64 (va16: the difference is formed in fp16); else warped - ref in fp32
       a_diff   absolute error of fp16 subnormals in the chain (true units)
       u_sq, a_sq  rounding of the square (fp16 x 2^-12 in va16: subnormal grid 2^-25 * 4096), fp32 otherwise
       u_dot, dot_steps  gate weights in fp16 (2^-11) and C/2 HFMA2 partial roundings (va16), or fp32 FFMA over C channels
-      u_acc    rounding of the accumulation over views per view: fp16 (ACC16) or fp32
+      u_acc    rounding of the accumulation over views per view: fp16 (va16) or fp32
       a_acc    subnormal grid of the fp16 accumulator in true units (2^-25 * 4096)
       u_out, a_out  the stored volume: fp16 x 2^-5 (subnormal grid 2^-25 * 32), bf16, or fp32 (0: the division by the view
                count is the last rounding and is counted below)
@@ -638,18 +638,19 @@ class CvArith:
 
 
 def cv_arith(precision: str, cv_variant: int, C: int, D: int) -> CvArith:
+    """cv_variant: the engine's set_option("cv_variant") value, 3 (default) or 4; it selects how many depths a thread of
+    k_cost_volume_va16 owns, which leaves the arithmetic of every entry unchanged."""
+    if cv_variant not in (3, 4):
+        raise ValueError(f"cv_variant {cv_variant}: the engine has variants 3 and 4 only")
     u, h = U_FP32, 2.0 ** -11
     if precision == "fp32":        # generic kernel, fp32 features / math / volume: bilinear weights (1 - ax)(1 - ay) carry 3
         # roundings, the 4-tap FMA chain 4 more
         return CvArith(7 * u, False, 0.0, u, 0.0, u, C, u, 0.0, 0.0, 0.0, "generic, fp32 math, fp32 volume", grid_sample=True)
     if precision == "bf16":        # generic kernel, fp32 arithmetic on bf16 features, bf16 volume
         return CvArith(6 * u, False, 0.0, u, 0.0, u, C, u, 0.0, 2.0 ** -8, 0.0, "generic, fp32 math, bf16 volume")
-    a_out = 2.0 ** -25 * 32.0
-    if cv_variant == 0:             # generic kernel: fp16 HFMA2 bilinear (weights rounded to fp16), fp32 from the difference on
-        return CvArith(5 * h, False, 4 * 2.0 ** -25, u, 0.0, u, C, u, 0.0, h, a_out, "generic, fp16 bilinear")
-    acc16 = cv_variant >= 3         # variants 3 / 4 / 5 accumulate over views in fp16 (5: the TMA kernel at stage 3, else 3)
-    return CvArith(5 * h, True, 5 * 2.0 ** -25 * 64, h, 2.0 ** -25 * 4096, h, C // 2 + 2, h if acc16 else u,
-                   2.0 ** -25 * 4096 if acc16 else 0.0, h, a_out, "va16, fp16 " + ("ACC16" if acc16 else "fp32 accumulate"))
+    # mixed16: k_cost_volume_va16, fp16 from the bilinear chain to the accumulation over views
+    return CvArith(5 * h, True, 5 * 2.0 ** -25 * 64, h, 2.0 ** -25 * 4096, h, C // 2 + 2, h, 2.0 ** -25 * 4096, h,
+                   2.0 ** -25 * 32.0, "va16, fp16 accumulate")
 
 
 def cost_volume_reference(w, s: int, feats: np.ndarray, hyps: np.ndarray, K, c2ws, ar: CvArith, interval: float):

@@ -27,7 +27,6 @@
 #include "conv_tc.cuh"
 #include "conv_tc_is.cuh"
 #include "conv_tc_s2.cuh"
-#include "cost_volume_tma.cuh"
 #include "weights.h"
 
 namespace tdm {
@@ -164,9 +163,6 @@ class MvsnetEngine final : public MvsnetIface {
     // consumers of the keyframe handoff may still be reading it: read_handoff returns once their reads are enqueued
     cudaStreamSynchronize(stream_.get());
     for (int i = 0; i < n_ho_release_; ++i) cudaEventSynchronize(ev_ho_release_[i].get());
-    unsigned st[2] = {0, 0};
-    if (d_cv_stats_ && std::getenv("TDM_DEBUG_PLAN") && cudaMemcpy(st, d_cv_stats_.get(), sizeof(st), cudaMemcpyDeviceToHost) == cudaSuccess)
-      fprintf(stderr, "[cv_tma] (CTA, view) pairs staged by TMA: %u, fallen back to global gathers: %u\n", st[0], st[1]);
   }
 
   void set_option(const std::string& key, int value) override {
@@ -184,7 +180,7 @@ class MvsnetEngine final : public MvsnetIface {
     else if (key == "use_graph") use_graph_ = value != 0;
     else if (key == "use_pdl") { TDM_CHECK(value >= 0 && value <= 2, "use_pdl: 0 off, 1 tensor-core kernels, 2 every kernel of the forward"); use_pdl_ = value; }
     else if (key == "pdl_min_smem_kb") { TDM_CHECK(value >= 0 && value <= 225, "pdl_min_smem_kb out of range"); pdl_min_smem_kb_ = value; }
-    else if (key == "cv_variant") { TDM_CHECK(value >= 0 && value <= 5, "cv_variant out of range"); cv_variant_ = value; }
+    else if (key == "cv_variant") { TDM_CHECK(value == 3 || value == 4, "cv_variant: 3 (default) or 4"); cv_variant_ = value; }
     else if (key == "tc_smem_kb") { TDM_CHECK(value >= 48 && value <= 225, "tc_smem_kb out of range"); tc_smem_kb_ = value; tc_cache_.clear(); }
     else if ((key.rfind("depth_num_stage", 0) == 0 && key.size() == 16 && key[15] >= '1' && key[15] <= '3') || key == "debug_poison") {
       // depth_num_stageN: override the checkpoint's MODEL.DEPTH_NUM for one stage (BASELINE.json configs[0] uses 32 stage-1
@@ -207,9 +203,7 @@ class MvsnetEngine final : public MvsnetIface {
     else if (key == "fork_fpn") fork_fpn_ = value != 0;
     else if (key == "prob_direct") prob_direct_ = value != 0;
     else if (key == "direct_conv00") direct_conv00_ = value != 0;
-    else if (key == "fused_select") fused_select_ = value != 0;
     else if (key == "fused_regress") fused_regress_ = value != 0;
-    else if (key == "inline_dmin") inline_dmin_ = value != 0;
     else throw Error("unknown option " + key);
   }
 
@@ -253,7 +247,6 @@ class MvsnetEngine final : public MvsnetIface {
       }
     std::unique_lock<std::mutex> lk(mu_);
     wait_idle_for_call(lk);
-    TDM_CHECK(cv_variant_ != 5, "CallAsyncIds: cv_variant 5 reads the views in window order and cannot use the feature cache");
     // everything below the checks changes state: decide first which views are held (a re-plan empties the pools)
     const bool same_plan = V == V_ && H == H_ && W == W_;
     int held_slot[kMaxSrc + 1];
@@ -662,8 +655,7 @@ class MvsnetEngine final : public MvsnetIface {
       }
     }
     select_state_ = make_dev<SelectState>(sizeof(SelectState));
-    select2_ = make_dev<SelectState2>(sizeof(SelectState2));
-    TDM_CUDA(cudaMemset(select2_.get(), 0, sizeof(SelectState2)));
+    TDM_CUDA(cudaMemset(select_state_.get(), 0, sizeof(SelectState)));
     h_params_ = make_host<CallParams>(sizeof(CallParams));
     d_params_ = make_dev<CallParams>(sizeof(CallParams));
     h_feat_slot_ = make_host<int>(sizeof(c_feat_slot[0]));
@@ -692,7 +684,7 @@ class MvsnetEngine final : public MvsnetIface {
       // all-ones bytes are a NaN in fp32, fp16 and bf16: a position the forward should have stored but did not reads as
       // non-finite instead of as a plausible 0 (which a ReLU layer's true output often is).  The P8 interiors and the
       // logits are poisoned; the other fp32 maps are not all written by every forward (depth / confidence / edge of the
-      // stages the edge filter skips, dmin with inline_dmin, thr's spare entry) and keep their zeros.
+      // stages the edge filter skips, thr's spare entry) and keep their zeros.
       if (!f32) {
         const size_t row = (size_t)(W + 2) * 8 * es;
         for (int p = 0; p < (C / 8) * (D + 2 * b.pd); ++p) {
@@ -719,7 +711,6 @@ class MvsnetEngine final : public MvsnetIface {
   }
   void free_plan() {
     drop_graph();
-    cv_tmap_ok_ = false;
     tc_cache_.clear();
     bufs_.clear();
     h_bgr_.reset();
@@ -779,7 +770,6 @@ class MvsnetEngine final : public MvsnetIface {
       alloc(k + "x9", 16, D1, Hs / 2, Ws / 2, false, false, true);
       alloc(k + "x11", 8, D, Hs, Ws, false, false, true);
       alloc(k + "logits", 1, D, Hs, Ws, true);
-      alloc(k + "dmin", 1, 1, Hs, Ws, true);
       for (const char* n : {"depth_dense", "confidence_dense", "depth", "confidence", "edge"})
         alloc(k + n, 1, 1, Hs, Ws, true);
     }
@@ -1283,54 +1273,24 @@ class MvsnetEngine final : public MvsnetIface {
     rec_begin(k + "cost_volume", (double)fb.alg_bytes + (double)vb.alg_bytes + (s > 1 ? 4.0 * vb.H * vb.W : 0.0),
               (double)n * nsrc * fb.C * 12.0);
     const DminSrc dm = dmin_src(s);
-    bool done = false;
     if constexpr (std::is_same<TA, __half>::value) {
-      if (va_ && cv_variant_ == 5 && fb.C == 8 && vb.D == 8) {
-        // A/B: source-view tiles staged in shared memory by TMA (cost_volume_tma.cuh); other stages run variant 3
-        TDM_CHECK(slots_identity(), "cv_variant 5 reads the views in window order, not through the feature pool's slots");
-        if (!cv_tmap_ok_) {
-          const cuuint64_t dims[4] = {8, (cuuint64_t)(fb.W + 2), (cuuint64_t)(fb.H + 2), (cuuint64_t)(fb.D + 2 * fb.pd)};
-          const cuuint64_t strides[3] = {16, (cuuint64_t)(fb.W + 2) * 16, (cuuint64_t)(fb.W + 2) * (fb.H + 2) * 16};
-          const cuuint32_t box[4] = {8, (cuuint32_t)kCvBW, (cuuint32_t)kCvBH, 1};
-          const cuuint32_t estr[4] = {1, 1, 1, 1};
-          const CUresult r = tc::encode_tiled_fn()(&cv_tmap_, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, fb.p.get(), dims, strides, box, estr,
-                                                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                                                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-          TDM_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed for the cost-volume source tile");
-          if (!d_cv_stats_) {
-            DevPtr<unsigned> st = make_dev<unsigned>(2 * sizeof(unsigned));
-            TDM_CUDA(cudaMemset(st.get(), 0, 2 * sizeof(unsigned)));
-            d_cv_stats_ = std::move(st);
-          }
-          cv_tmap_ok_ = true;
-        }
-        k_cost_volume_va16_tma<TV, true><<<dim3(cdiv(vb.W, 16), cdiv(vb.H, 8)), 256, 0, stream_.get()>>>(cv_tmap_, p8<const __half>(fb), dm, p8<TV>(vb), slot_.index, s - 1, d_cv_stats_.get());
+      if (va_) {
+        // depth hypotheses per thread: two, four at the 8-channel stage (variant 4: four at every stage); the 32 channels of
+        // stage 1 split over two lanes
+        const int nd = (cv_variant_ == 4 || fb.C == 8) ? 4 : 2;
+        const long long thr = (long long)cdiv(vb.D, nd) * vb.H * vb.W * (fb.C == 32 ? 2 : 1);
+        const unsigned grid = (unsigned)cdiv(thr, 128);
+        auto go = [&](auto kern) { launch_k(kern, dim3(grid), dim3(128), p8<const __half>(fb), dm, p8<TV>(vb), slot_.index, s - 1); };
+        if (fb.C == 32) { if (nd == 2) go(k_cost_volume_va16<TV, 16, 2, 2>); else go(k_cost_volume_va16<TV, 16, 2, 4>); }
+        else if (fb.C == 16) { if (nd == 2) go(k_cost_volume_va16<TV, 16, 1, 2>); else go(k_cost_volume_va16<TV, 16, 1, 4>); }
+        else if (fb.C == 8) go(k_cost_volume_va16<TV, 8, 1, 4>);
+        else throw Error("unsupported feature channels");
         TDM_CUDA(cudaGetLastError());
         rec_end();
         return;
       }
-      if (va_ && cv_variant_ > 0) {
-        done = true;
-        const int nd = (cv_variant_ == 2 || cv_variant_ == 4) ? 4 : (fb.C == 8 ? 4 : 2);
-        const bool h16 = cv_variant_ >= 3;   // (variant 5 = variant 3 outside stage 3)
-        const long long thr = (long long)cdiv(vb.D, nd) * vb.H * vb.W * (fb.C == 32 ? 2 : 1);
-        const unsigned grid = (unsigned)cdiv(thr, 128);
-        auto go = [&](auto kern) { launch_k(kern, dim3(grid), dim3(128), p8<const __half>(fb), dm, p8<TV>(vb), slot_.index, s - 1); };
-        if (fb.C == 32) {
-          if (nd == 2) { if (h16) go(k_cost_volume_va16<TV, 16, 2, 2, true>); else go(k_cost_volume_va16<TV, 16, 2, 2, false>); }
-          else         { if (h16) go(k_cost_volume_va16<TV, 16, 2, 4, true>); else go(k_cost_volume_va16<TV, 16, 2, 4, false>); }
-        } else if (fb.C == 16) {
-          if (nd == 2) { if (h16) go(k_cost_volume_va16<TV, 16, 1, 2, true>); else go(k_cost_volume_va16<TV, 16, 1, 2, false>); }
-          else         { if (h16) go(k_cost_volume_va16<TV, 16, 1, 4, true>); else go(k_cost_volume_va16<TV, 16, 1, 4, false>); }
-        } else if (fb.C == 8) {
-          if (h16) go(k_cost_volume_va16<TV, 8, 1, 4, true>); else go(k_cost_volume_va16<TV, 8, 1, 4, false>);
-        } else {
-          throw Error("unsupported feature channels");
-        }
-      }
     }
-    if (done) {}
-    else if (fb.C == 32) k_cost_volume<TA, TV, 16, 2><<<cdiv(2 * n, 128), 128, 0, stream_.get()>>>(p8<const TA>(fb), dm, p8<TV>(vb), slot_.index, s - 1);
+    if (fb.C == 32) k_cost_volume<TA, TV, 16, 2><<<cdiv(2 * n, 128), 128, 0, stream_.get()>>>(p8<const TA>(fb), dm, p8<TV>(vb), slot_.index, s - 1);
     else if (fb.C == 16) k_cost_volume<TA, TV, 16><<<cdiv(n, 128), 128, 0, stream_.get()>>>(p8<const TA>(fb), dm, p8<TV>(vb), slot_.index, s - 1);
     else if (fb.C == 8) k_cost_volume<TA, TV, 8><<<cdiv(n, 128), 128, 0, stream_.get()>>>(p8<const TA>(fb), dm, p8<TV>(vb), slot_.index, s - 1);
     else throw Error("unsupported feature channels");
@@ -1338,13 +1298,10 @@ class MvsnetEngine final : public MvsnetIface {
     rec_end();
   }
 
-  // where stage s takes the lower end of its hypothesis range from: computed in place from the previous stage's depth
-  // (inline_dmin_, default) or read from the map k_adaptive_dmin materialised
+  // the previous stage's depth map, from which stage s computes the lower end of its hypothesis range where it is consumed
   DminSrc dmin_src(int s) {
-    DminSrc d{nullptr, nullptr, 0, 0};
+    DminSrc d{nullptr, 0, 0};
     if (s <= 1) return d;
-    const std::string k = "s" + std::to_string(s) + ".";
-    if (!inline_dmin_) { d.map = fbuf(k + "dmin"); return d; }
     const DevBuf& pd = bufs_.at("s" + std::to_string(s - 1) + ".depth_dense");
     d.prev = (const float*)pd.p.get(); d.ph = pd.H; d.pw = pd.W;
     return d;
@@ -1365,28 +1322,14 @@ class MvsnetEngine final : public MvsnetIface {
     const std::string k = "s" + std::to_string(s) + ".";
     const DevBuf& d = bufs_.at(k + "depth_dense");
     const int n = d.H * d.W;
-    if (fused_select_) {
-      rec_begin(k + "edge_metric+select0", 8.0 * n, 0);
-      launch_k(k_edge_metric_select0, dim3(cdiv(n, 256)), dim3(256), fbuf(k + "depth_dense"), fbuf(k + "edge"), d.H, d.W, select2_.get(), &d_params_->cutoff[s - 1]);
-      rec_end();
-      rec_begin(k + "percentile", 8.0 * n, 0);
-      for (int pass = 1; pass <= 2; ++pass)
-        launch_k(k_select_pass, dim3(std::min(cdiv(n, 256 * 8), 2 * kNumSm)), dim3(256), fbuf(k + "edge"), n, select2_.get(), pass, fbuf("thr") + (s - 1));
-      launch_count_ += 1;
-      rec_end();
-    } else {
-    rec_begin(k + "edge_metric", 8.0 * n, 0);
-    k_edge_metric<<<cdiv(n, 128), 128, 0, stream_.get()>>>(fbuf(k + "depth_dense"), fbuf(k + "edge"), d.H, d.W);
+    rec_begin(k + "edge_metric+select0", 8.0 * n, 0);
+    launch_k(k_edge_metric_select0, dim3(cdiv(n, 256)), dim3(256), fbuf(k + "depth_dense"), fbuf(k + "edge"), d.H, d.W, select_state_.get(), &d_params_->cutoff[s - 1]);
     rec_end();
-    rec_begin(k + "percentile", 12.0 * n, 0);
-    k_select_init<<<1, 256, 0, stream_.get()>>>(select_state_.get(), &d_params_->cutoff[s - 1]);
-    for (int pass = 0; pass < 3; ++pass) {
-      k_select_hist<<<std::min(cdiv(n, 256 * 8), 592), 256, 0, stream_.get()>>>(fbuf(k + "edge"), n, select_state_.get(), pass);
-      k_select_scan<<<1, 1024, 0, stream_.get()>>>(select_state_.get(), pass, fbuf("thr") + (s - 1));
-    }
-    launch_count_ += 6;
+    rec_begin(k + "percentile", 8.0 * n, 0);
+    for (int pass = 1; pass <= 2; ++pass)
+      launch_k(k_select_pass, dim3(std::min(cdiv(n, 256 * 8), 2 * kNumSm)), dim3(256), fbuf(k + "edge"), n, select_state_.get(), pass, fbuf("thr") + (s - 1));
+    launch_count_ += 1;
     rec_end();
-    }
     rec_begin(k + "apply_mask", 20.0 * n, 0);
     launch_k(k_apply_edge_mask, dim3(cdiv(n, 256)), dim3(256), fbuf(k + "edge"), fbuf("thr") + (s - 1), fbuf(k + "depth_dense"),
                                                        fbuf(k + "confidence_dense"), fbuf(k + "depth"),
@@ -1517,14 +1460,6 @@ class MvsnetEngine final : public MvsnetIface {
       const HypSpec hs = hyp_spec(s);
       const DevBuf& dd = bufs_.at(k + "depth_dense");
       if (s == 2 && fork) TDM_CUDA(cudaStreamWaitEvent(stream_.get(), ev_join_.get(), 0));
-      if (s > 1 && !inline_dmin_) {
-        const DevBuf& pd = bufs_.at("s" + std::to_string(s - 1) + ".depth_dense");
-        rec_begin(k + "adaptive_dmin", 4.0 * (pd.H * pd.W + dd.H * dd.W), 0);
-        k_adaptive_dmin<<<cdiv(dd.H * dd.W, 256), 256, 0, stream_.get()>>>((const float*)pd.p.get(), pd.H, pd.W, fbuf(k + "dmin"),
-                                                                    &d_params_->half_range[s - 1]);
-        TDM_CUDA(cudaGetLastError());
-        rec_end();
-      }
       cost_volume(s);
       const bool four = hs.D == 4;
       const int s5 = four ? 1 : 2;
@@ -1750,8 +1685,6 @@ class MvsnetEngine final : public MvsnetIface {
   Gate gates_[3];
   std::map<std::string, DevBuf> bufs_;
   DevPtr<SelectState> select_state_;
-  DevPtr<SelectState2> select2_;
-  bool inline_dmin_ = true;    // adaptive range's d_min computed where it is consumed (dmin_px) instead of by k_adaptive_dmin (A/B: 0)
   // softmax / soft-argmin / confidence in the epilogue of the tensor-core prob convolution (set_option("fused_regress", 1)):
   // bit-identical to k_regress and three launches fewer, but the consumer threads of a CTA finish their pixels after the last
   // plane with nothing left to overlap, where the stand-alone kernel spreads the same work over 2048 threads per SM. Off.
@@ -1762,7 +1695,6 @@ class MvsnetEngine final : public MvsnetIface {
   struct TailReq { int stage; int D; DminSrc dsrc; float* depth; float* conf; const HypSpec* hyp; const float* half_range; bool done; };
   TailReq tail_req_{};
   int pdl_min_smem_kb_ = 120;
-  bool fused_select_ = true;   // edge metric + pass 0 in one kernel, passes 1 / 2 with the scan in their last CTA (A/B: set_option("fused_select", 0))
   int V_ = 0, H_ = 0, W_ = 0;
   HostPtr<unsigned char> h_bgr_;
   DevPtr<unsigned char> d_bgr_;
@@ -1798,10 +1730,9 @@ class MvsnetEngine final : public MvsnetIface {
   int fk_ = 0;                                         // views FeatureNet computes in the forward being enqueued / last enqueued
   struct FwdGraph { GraphExec exec; bool warmed = false; };
   std::map<int, FwdGraph> graphs_;   // one captured forward per FeatureNet view count
-  CUtensorMap cv_tmap_{};      // cv_variant 5 (A/B): tiled view of feat3 for the TMA-staged cost volume
-  bool cv_tmap_ok_ = false;
-  DevPtr<unsigned> d_cv_stats_;
-  int cv_variant_ = 3;   // 0: generic cost-volume kernel; 1-4: k_cost_volume_va16 (ND 2/2/4 | 4/4/4, fp32 | fp16 accumulate)
+  // 4: four depth hypotheses per thread of k_cost_volume_va16 at every stage.  Measured faster than the default 3 on an H100
+  // 80GB HBM3 at 700 W (DESIGN.md, "MVSNet variants removed"); off until a change of its own turns it on
+  int cv_variant_ = 3;
   // Programmatic dependent launch of the tensor-core kernels: the trigger sits after griddepcontrol.wait (a trigger before it
   // lets the whole chain of later kernels become resident early), and pdl_min_smem_kb_ = 120 keeps one tensor-core CTA per SM.
   bool use_graph_ = true;

@@ -359,15 +359,12 @@ __device__ __forceinline__ float hyp_value(const HypSpec& h, float dmin_px, int 
 // a4 without a kernel of its own (round 2): the lower end of a pixel's adaptive hypothesis range, d_min = max(up2(depth_prev) -
 // half_range, 1e-3) with up2 = bilinear x2, align_corners=False (cva_mvsnet.py:143-147, module.py:1503-1565), evaluated where it
 // is consumed - the cost-volume kernel's prologue and the regression - from the previous stage's depth map (4 L2-resident
-// loads).  Explicit fma / mul intrinsics: every consumer must see bit-identical hypotheses.  map != nullptr reads the
-// materialised map instead (k_adaptive_dmin, kept for the A/B and the fp32 parity engine's layer-wise tests).
+// loads).  Explicit fma / mul intrinsics: every consumer must see bit-identical hypotheses.
 struct DminSrc {
-  const float* map;    // [H][W] or null
   const float* prev;   // [ph][pw] depth of the previous stage
   int ph, pw;
 };
-__device__ __forceinline__ float dmin_px(const DminSrc& s, int pix, int x, int y, float half_range) {
-  if (s.map) return s.map[pix];
+__device__ __forceinline__ float dmin_px(const DminSrc& s, int x, int y, float half_range) {
   const float sy = fmaxf(__fmaf_rn(0.5f, (float)y + 0.5f, -0.5f), 0.f), sx = fmaxf(__fmaf_rn(0.5f, (float)x + 0.5f, -0.5f), 0.f);
   const int y0 = (int)sy, x0 = (int)sx;
   const int y1 = min(y0 + 1, s.ph - 1), x1 = min(x0 + 1, s.pw - 1);
@@ -377,24 +374,6 @@ __device__ __forceinline__ float dmin_px(const DminSrc& s, int pix, int x, int y
   const float t1 = __fmaf_rn(lx, s.prev[y1 * s.pw + x1], __fmul_rn(hx, s.prev[y1 * s.pw + x0]));
   const float up = __fmaf_rn(ly, t1, __fmul_rn(hy, t0));
   return fmaxf(up - half_range, 0.001f);
-}
-
-__global__ void k_adaptive_dmin(const float* __restrict__ prev /*[h][w]*/, int h, int w,
-                                float* __restrict__ dmin /*[2h][2w]*/, const float* __restrict__ half_range_p) {
-  const float half_range = *half_range_p;
-  const int H = 2 * h, W = 2 * w;
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= H * W) return;
-  const int y = i / W, x = i - y * W;
-  float sy = fmaxf(0.5f * ((float)y + 0.5f) - 0.5f, 0.f);
-  float sx = fmaxf(0.5f * ((float)x + 0.5f) - 0.5f, 0.f);
-  int y0 = (int)sy, x0 = (int)sx;
-  int y1 = min(y0 + 1, h - 1), x1 = min(x0 + 1, w - 1);
-  float ly = sy - (float)y0, lx = sx - (float)x0;
-  float hy = 1.f - ly, hx = 1.f - lx;
-  float up = hy * (hx * prev[y0 * w + x0] + lx * prev[y0 * w + x1]) +
-             ly * (hx * prev[y1 * w + x0] + lx * prev[y1 * w + x1]);
-  dmin[i] = fmaxf(up - half_range, 0.001f);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -459,7 +438,7 @@ k_cost_volume(P8<const T> feats /*views on the D axis, view v on plane p.plane[v
   const int x = (int)(i % p.W);
   const int y = (int)((i / p.W) % p.H);
   const int d = (int)(i / ((long long)p.W * p.H));
-  const float depth = hyp_value(p.hyp, p.hyp.adaptive ? dmin_px(dsrc, y * p.W + x, x, y, c_call_params[slot].half_range[stage]) : 0.f, d);
+  const float depth = hyp_value(p.hyp, p.hyp.adaptive ? dmin_px(dsrc, x, y, c_call_params[slot].half_range[stage]) : 0.f, d);
 
   float ref[C];
   {
@@ -627,7 +606,7 @@ k_cost_volume(P8<const T> feats /*views on the D axis, view v on plane p.plane[v
 //    directly; all fp16 operands carry a 1/64 scale (weights and ref; exact, a power of two) so the square, scaled by
 //    1/4096, cannot overflow before |warped - ref| = 16376 (features are fp16 themselves; max seen 115);
 //  * the gate's dot product runs in HFMA2 against a normalised fp16 copy of gw1 and is un-scaled in fp32;
-//  * accumulation over views stays fp32 (ACC16 = false) as packed FFMA2, or fp16 (ACC16 = true, study variant);
+//  * the gated squares are accumulated over views in fp16 (HFMA2) and widened to fp32 only for the store;
 //  * rcp.approx instead of the IEEE reciprocal, 32-bit element offsets.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float rcp_approx(float x) {
@@ -635,10 +614,8 @@ __device__ __forceinline__ float rcp_approx(float x) {
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
   return r;
 }
-// two independent correctly rounded FMAs (Hopper has no paired fp32 FMA instruction)
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
-template <typename TV, int C /*channels of one thread*/, int CSPLIT, int ND, bool ACC16>
+template <typename TV, int C /*channels of one thread*/, int CSPLIT, int ND>
 __global__ void __launch_bounds__(128)
 k_cost_volume_va16(P8<const __half> feats, const DminSrc dsrc, P8<TV> vol, int slot, int stage) {
   grid_dep_sync();
@@ -674,16 +651,15 @@ k_cost_volume_va16(P8<const __half> feats, const DminSrc dsrc, P8<TV> vol, int s
   }
   float depth[ND];
   {
-    const float dmn = p.hyp.adaptive ? dmin_px(dsrc, pix, x, y, c_call_params[slot].half_range[stage]) : 0.f;
+    const float dmn = p.hyp.adaptive ? dmin_px(dsrc, x, y, c_call_params[slot].half_range[stage]) : 0.f;
 #pragma unroll
     for (int k = 0; k < ND; ++k) depth[k] = hyp_value(p.hyp, dmn, min(d0 + k, p.D - 1));
   }
-  float2 acc[ND][C / 2];
-  __half2 acch[ND][C / 2];
+  __half2 acc[ND][C / 2];
 #pragma unroll
   for (int k = 0; k < ND; ++k)
 #pragma unroll
-    for (int c = 0; c < C / 2; ++c) { acc[k][c] = make_float2(0.f, 0.f); acch[k][c] = __float2half2_rn(0.f); }
+    for (int c = 0; c < C / 2; ++c) acc[k][c] = __float2half2_rn(0.f);
 
   const float fx = (float)x, fy = (float)y, Wf = (float)p.W, Hf = (float)p.H;
   const int row = feats.Wp * 8;
@@ -736,15 +712,9 @@ k_cost_volume_va16(P8<const __half> feats, const DminSrc dsrc, P8<TV> vol, int s
       if constexpr (CSPLIT == 2) dot += __shfl_xor_sync(0xffffffffu, dot, 1);
       const float h1 = fmaxf(fmaf(dot, p.dot_unscale, p.gb1), 0.f);
       const float g = fmaxf(fmaf(p.gw2, h1, p.gb2), 0.f) + 1.f;
-      if constexpr (ACC16) {
-        const __half2 gh = __float2half2_rn(g);
+      const __half2 gh = __float2half2_rn(g);
 #pragma unroll
-        for (int c = 0; c < C / 2; ++c) acch[k][c] = __hfma2(df[c], gh, acch[k][c]);
-      } else {
-        const float2 g2 = make_float2(g, g);
-#pragma unroll
-        for (int c = 0; c < C / 2; ++c) acc[k][c] = ffma2(__half22float2(df[c]), g2, acc[k][c]);
-      }
+      for (int c = 0; c < C / 2; ++c) acc[k][c] = __hfma2(df[c], gh, acc[k][c]);
     }
   }
   if (active) {
@@ -759,7 +729,7 @@ k_cost_volume_va16(P8<const __half> feats, const DminSrc dsrc, P8<TV> vol, int s
           float o8[8];
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
-            const float2 v = ACC16 ? __half22float2(acch[k][c0 / 2 + j]) : acc[k][c0 / 2 + j];
+            const float2 v = __half22float2(acc[k][c0 / 2 + j]);
             o8[2 * j] = vol_store<TV>(v.x * sc);
             o8[2 * j + 1] = vol_store<TV>(v.y * sc);
           }
@@ -787,7 +757,7 @@ __device__ __forceinline__ void regress_px(const float* __restrict__ logits /*[D
 #pragma unroll
   for (int j = 0; j < MAXD; ++j)
     if (j < D) { l[j] = expf(l[j] - m); s += l[j]; }
-  const float dm = hyp.adaptive ? dmin_px(dsrc, i, x, y, half_range) : 0.f;
+  const float dm = hyp.adaptive ? dmin_px(dsrc, x, y, half_range) : 0.f;
   float dsum = 0.f, isum = 0.f;
 #pragma unroll
   for (int j = 0; j < MAXD; ++j)
@@ -837,108 +807,18 @@ struct RegressTail {
 // float bit patterns (all values >= 0 so the unsigned order equals the float order);
 // (3) zero depth/confidence where edge > threshold.
 // ------------------------------------------------------------------------------------------------
-__global__ void k_edge_metric(const float* __restrict__ depth, float* __restrict__ edge, int H, int W) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= H * W) return;
-  const int y = i / W, x = i - y * W;
-  const float c = depth[i];
-  float e[25];
-#pragma unroll
-  for (int dy = -2; dy <= 2; ++dy)
-#pragma unroll
-    for (int dx = -2; dx <= 2; ++dx) {
-      const int yy = y + dy, xx = x + dx;
-      const float v = (yy >= 0 && yy < H && xx >= 0 && xx < W) ? depth[yy * W + xx] : 0.f;
-      e[(dy + 2) * 5 + dx + 2] = fabsf(v - c);
-    }
-  // partial selection: after pass k the k smallest are in e[0..k]
-#pragma unroll
-  for (int k = 0; k < 15; ++k) {
-#pragma unroll
-    for (int j = k + 1; j < 25; ++j) {
-      const float a = e[k], b = e[j];
-      e[k] = fminf(a, b);
-      e[j] = fmaxf(a, b);
-    }
-  }
-  edge[i] = e[14];
-}
-
+// The select's passes take 11 + 11 + 10 bits, one launch each: the CTAs histogram their share into shared memory, merge into the
+// global histogram, and the LAST CTA to finish (ticket) scans the 2048 bins, narrows (prefix, k) for the next pass and re-zeroes
+// the histogram.  Pass 0 rides on the edge-metric kernel itself (the values are in registers there).  State between passes lives
+// in SelectState; its histogram and ticket are zero whenever no select is in flight (zeroed at allocation and by every pass'
+// last CTA).
 struct SelectState {
-  unsigned prefix;   // bits decided so far (high bits)
-  unsigned k;        // remaining rank inside the current prefix bucket
-  unsigned hist[2048];
-};
-
-__global__ void k_select_init(SelectState* st, const unsigned* __restrict__ k) {
-  for (int i = threadIdx.x; i < 2048; i += blockDim.x) st->hist[i] = 0;
-  if (threadIdx.x == 0) { st->prefix = 0; st->k = *k; }
-}
-
-// pass p: 0 -> bits 31..21 (11), 1 -> bits 20..10 (11), 2 -> bits 9..0 (10)
-__global__ void k_select_hist(const float* __restrict__ v, int n, SelectState* st, int pass) {
-  __shared__ unsigned h[2048];
-  for (int i = threadIdx.x; i < 2048; i += blockDim.x) h[i] = 0;
-  __syncthreads();
-  const unsigned prefix = st->prefix;
-  const int shift = pass == 0 ? 21 : (pass == 1 ? 10 : 0);
-  const unsigned hi_mask = pass == 0 ? 0u : (pass == 1 ? 0xFFE00000u : 0xFFFFFC00u);
-  const unsigned bmask = pass == 2 ? 0x3FFu : 0x7FFu;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const unsigned b = __float_as_uint(v[i]);
-    if ((b & hi_mask) == prefix) atomicAdd(&h[(b >> shift) & bmask], 1u);
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < 2048; i += blockDim.x)
-    if (h[i]) atomicAdd(&st->hist[i], h[i]);
-}
-
-// one block of 1024 threads: parallel prefix over the 2048 bins, the thread whose bin pair contains rank k publishes
-__global__ void __launch_bounds__(1024) k_select_scan(SelectState* st, int pass, float* thr_out) {
-  __shared__ unsigned wsum[32];
-  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
-  const int shift = pass == 0 ? 21 : (pass == 1 ? 10 : 0);
-  const unsigned a = st->hist[2 * t], b = st->hist[2 * t + 1];
-  const unsigned k = st->k, prefix = st->prefix;
-  unsigned incl = a + b;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const unsigned n = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += n;
-  }
-  if (lane == 31) wsum[w] = incl;
-  __syncthreads();
-  unsigned off = 0;
-  for (int i = 0; i < w; ++i) off += wsum[i];
-  const unsigned excl = off + incl - (a + b);
-  __syncthreads();   // everybody has read st->hist / st->k before they are overwritten
-  st->hist[2 * t] = 0;
-  st->hist[2 * t + 1] = 0;
-  int bin = -1;
-  unsigned nk = 0;
-  if (k >= excl && k < excl + a) { bin = 2 * t; nk = k - excl; }
-  else if (k >= excl + a && k < excl + a + b) { bin = 2 * t + 1; nk = k - excl - a; }
-  if (bin >= 0) {
-    const unsigned np = prefix | ((unsigned)bin << shift);
-    st->k = nk;
-    st->prefix = np;
-    if (pass == 2) *thr_out = __uint_as_float(np);
-  }
-}
-
-// ---- fused percentile select (round 2): 4 launches instead of 9 --------------------------------------------------------
-// The exact k-th order statistic of the edge map is still a 3-pass radix select over the float bit patterns (11 + 11 + 10
-// bits), but every pass is ONE launch: the CTAs histogram their share into shared memory, merge into the global histogram,
-// and the LAST CTA to finish (ticket) scans the 2048 bins, narrows (prefix, k) for the next pass and re-zeroes the histogram.
-// Pass 0 rides on the edge-metric kernel itself (the values are in registers there).  State between passes lives in SelectState;
-// its histogram and ticket are zero whenever no select is in flight (zeroed at allocation and by every pass' last CTA).
-struct SelectState2 {
   unsigned prefix, k, ticket, pad;
   unsigned hist[2048];
 };
 
 // blockDim.x == 256.  Called by every thread of the last CTA of pass `pass`.
-__device__ __forceinline__ void select_scan_last_cta(SelectState2* st, int pass, unsigned k_in, unsigned prefix_in, float* thr_out) {
+__device__ __forceinline__ void select_scan_last_cta(SelectState* st, int pass, unsigned k_in, unsigned prefix_in, float* thr_out) {
   __shared__ unsigned wsum[8];
   const int t = threadIdx.x, lane = t & 31, w = t >> 5;
   const int shift = pass == 0 ? 21 : (pass == 1 ? 10 : 0);
@@ -975,7 +855,7 @@ __device__ __forceinline__ void select_scan_last_cta(SelectState2* st, int pass,
 }
 
 // shared by the three passes: merge the CTA's shared-memory histogram, elect the last CTA, let it scan
-__device__ __forceinline__ void select_finish_pass(SelectState2* st, unsigned* h /*shared [2048]*/, int pass, unsigned k_in, unsigned prefix_in,
+__device__ __forceinline__ void select_finish_pass(SelectState* st, unsigned* h /*shared [2048]*/, int pass, unsigned k_in, unsigned prefix_in,
                                                    float* thr_out) {
   __shared__ bool is_last;
   __syncthreads();
@@ -993,7 +873,7 @@ __device__ __forceinline__ void select_finish_pass(SelectState2* st, unsigned* h
 
 // a9 edge metric + pass 0 of the percentile select (bits 31..21)
 __global__ void __launch_bounds__(256) k_edge_metric_select0(const float* __restrict__ depth, float* __restrict__ edge, int H, int W,
-                                                             SelectState2* st, const unsigned* __restrict__ cutoff) {
+                                                             SelectState* st, const unsigned* __restrict__ cutoff) {
   grid_dep_sync();
   __shared__ unsigned h[2048];
   for (int i = threadIdx.x; i < 2048; i += blockDim.x) h[i] = 0;
@@ -1027,7 +907,7 @@ __global__ void __launch_bounds__(256) k_edge_metric_select0(const float* __rest
 }
 
 // passes 1 (bits 20..10) and 2 (bits 9..0)
-__global__ void __launch_bounds__(256) k_select_pass(const float* __restrict__ v, int n, SelectState2* st, int pass, float* thr_out) {
+__global__ void __launch_bounds__(256) k_select_pass(const float* __restrict__ v, int n, SelectState* st, int pass, float* thr_out) {
   grid_dep_sync();
   __shared__ unsigned h[2048];
   for (int i = threadIdx.x; i < 2048; i += blockDim.x) h[i] = 0;

@@ -288,7 +288,7 @@ def test_layers_four_depth_planes(golden_small, precision):
 
 
 OPTIONS = [dict(use_is=0), dict(use_tc=0), dict(prob_direct=1, fused_regress=1, direct_conv00=0), dict(fused_regress=1),
-           dict(tc_smem_kb=113), dict(fork_fpn=0, use_pdl=2), dict(cv_variant=0), dict(cv_variant=4), dict(cv_variant=5)]
+           dict(tc_smem_kb=113), dict(fork_fpn=0, use_pdl=2), dict(cv_variant=4)]
 
 
 def _run_options(opts, precision, **extra):
@@ -367,17 +367,16 @@ def test_layers_smem_113_at_view_maximum():
     check_forward(m, win, "abl03_view_aggregation", "mixed16", dn, dict(tc_smem_kb=113), "288x224v16 smem113", REPORT)
 
 
-@pytest.mark.parametrize("fused_select", [1, 0])
-def test_edge_filter_bit_exact(fused_select):
+def test_edge_filter_bit_exact():
     """filter_all_stages: the same select state serves three stages per forward and every discard percentage,
     including 0 % (nothing masked) and 100 % (everything above the minimum masked)."""
     win = _synthetic(3, 96, 128, seed=1)
-    m = _engine("abl03_view_aggregation", "mixed16", None, filter_all_stages=1, fused_select=fused_select)
+    m = _engine("abl03_view_aggregation", "mixed16", None, filter_all_stages=1)
     for discard in (0.0, 2.5, 10.0, 37.3, 100.0, 10.0):
         win["discard"] = discard
         _submit(m, win)
         outs, edges = _outputs(m, (1, 2, 3))
-        check_filter(outs, discard, (1, 2, 3), f"fused_select={fused_select} discard={discard}", edges)
+        check_filter(outs, discard, (1, 2, 3), f"discard={discard}", edges)
 
 
 def test_replays_are_bit_identical():
