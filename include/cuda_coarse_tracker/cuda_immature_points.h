@@ -1,0 +1,46 @@
+// The immature points of DSO's active keyframes on the device (n8, include/tandem_b200.h): FullSystem::traceNewCoarse
+// (tandem/src/FullSystem/FullSystem.cpp:650-691) becomes one trace() call per frame.  Host slot = the keyframe's index among
+// the active ones (0..7); INTEGRATION.md shows the call sites.  Owns one tdm_immature handle; not copyable.
+#ifndef TDM_CUDA_IMMATURE_POINTS_H
+#define TDM_CUDA_IMMATURE_POINTS_H
+
+#include <Eigen/Dense>
+
+#include <vector>
+
+struct tdm_immature;   // include/tandem_b200.h
+struct tdm_pyramid;
+
+class CudaImmaturePoints {
+ public:
+  // the reference's defaults (util/settings.cpp:84-148) for every trace setting
+  CudaImmaturePoints(int w, int h, int capacity_per_host, int device = 0);
+  ~CudaImmaturePoints();
+  CudaImmaturePoints(const CudaImmaturePoints &) = delete;
+  CudaImmaturePoints &operator=(const CudaImmaturePoints &) = delete;
+
+  // makeNewTraces (FullSystem.cpp:1629-1646): the constructor for the selected pixels of the new keyframe; returns how many
+  // points were kept (those with a finite energyTH, in input order)
+  int add(int host_slot, tdm_pyramid *host_pyramid, std::vector<int> const &u, std::vector<int> const &v,
+          std::vector<float> const &type);
+  // traceNewCoarse: traceOn of every point of the given hosts into the new frame, with KRKi, Kt and aff per host as
+  // traceNewCoarse computes them (:655-669).  Asynchronous; get() waits for it.
+  void trace(tdm_pyramid *frame_pyramid, std::vector<int> const &host_slots, std::vector<tdm_pyramid *> const &host_pyramids,
+             std::vector<Eigen::Matrix<float, 3, 3>> const &KRKi, std::vector<Eigen::Matrix<float, 3, 1>> const &Kt,
+             std::vector<Eigen::Matrix<float, 2, 1>> const &aff);
+  // the fields activatePointsMT reads (FullSystem.cpp:760-775, 792) of every point of a slot
+  struct State {
+    std::vector<float> u, v, idepth_min, idepth_max, quality, interval;
+    std::vector<int> status;
+  };
+  State get(int host_slot);
+  // after activatePointsMT's compaction (:849-856), with the indices the host set to null
+  void remove(int host_slot, std::vector<int> const &indices);
+  // the keyframe was marginalised
+  void dropHost(int host_slot);
+
+ private:
+  tdm_immature *handle_ = nullptr;
+};
+
+#endif

@@ -455,6 +455,61 @@ int tdm_tracker_set_coarse_tracking_ref_nodia(tdm_tracker* const* levels, int n_
  * NULL.  An error before the first tdm_tracker_set_coarse_tracking_ref_nodia call with level0 as levels[0]. */
 int tdm_tracker_get_coarse_nodia(tdm_tracker* level0, int n, float* u, float* v, float* idepth, float* color);
 
+/* n8  FullSystem::traceNewCoarse (tandem/src/FullSystem/FullSystem.cpp:650-691) on the device: the immature points of the
+ *     active keyframes live in device memory, one set per camera, in up to 8 host slots (0..7) of capacity_per_host points
+ *     each, stored field by field.  Every float operation is the reference's, correctly rounded and in its order.
+ *     settings: the reference's constants (util/settings.cpp:84-148); NULL takes the defaults below.
+ *     The one definitional difference: where a sample's 2x2 footprint leaves the image (the reference reads outside its
+ *     array), that sample counts as a non-finite hit (energy += 1e5). */
+typedef struct tdm_trace_settings {
+  float max_pix_search;              /* setting_maxPixSearch, 0.027 (of w + h) */
+  float trace_stepsize;              /* 1 */
+  float trace_gn_threshold;          /* 0.1 */
+  float trace_extra_slack_on_th;     /* 1.2 */
+  float trace_slack_interval;        /* 1.5 */
+  float trace_min_improvement_factor;   /* 2 */
+  float huber_th;                    /* setting_huberTH, 9 */
+  float outlier_th;                  /* setting_outlierTH, 144 */
+  float outlier_th_sum_component;    /* 2500 */
+  float overall_energy_th_weight;    /* 1 */
+  int min_trace_test_radius;         /* 2 */
+  int trace_gn_iterations;           /* 3 */
+} tdm_trace_settings;
+/* ImmaturePoint::lastTraceStatus values (ImmaturePoint.h:46-52) */
+enum { TDM_IPS_GOOD = 0, TDM_IPS_OOB, TDM_IPS_OUTLIER, TDM_IPS_SKIPPED, TDM_IPS_BADCONDITION, TDM_IPS_UNINITIALIZED };
+typedef struct tdm_immature tdm_immature;
+int tdm_immature_create(int w, int h, int capacity_per_host, const tdm_trace_settings* settings, int device, tdm_immature** out);
+/* Waits for the set's pending work. */
+void tdm_immature_destroy(tdm_immature* s);
+/* The constructor (ImmaturePoint.cpp:32-61) for n pixels (u, v) of host_pyramid's level 0, appended to host_slot in input
+ *     order; like makeNewTraces (FullSystem.cpp:1639-1644) only the points whose energyTH is finite are kept.  New points
+ *     have idepth_min 0, idepth_max NaN, quality 10000, status TDM_IPS_UNINITIALIZED.  Blocking (one host wait), ordered
+ *     after the pyramid's build; *n_added receives the number kept.  Invalid input (null handles or arrays, a slot outside
+ *     0..7, a pyramid of another level-0 size or device, a pixel outside [2, w-4] x [2, h-4], more than the slot's free
+ *     capacity in candidates) is an error and launches nothing. */
+int tdm_immature_add(tdm_immature* s, int host_slot, tdm_pyramid* host_pyramid, int n, const int* u, const int* v,
+                     const float* type, int* n_added);
+/* ImmaturePoint::traceOn (ImmaturePoint.cpp:75-414) of every point of the n_hosts slots host_slots[] into level 0 of
+ *     frame_pyramid, in one launch: KRKi9 (n_hosts x 9, row-major), Kt3 (n_hosts x 3) and aff2 (n_hosts x 2) per host as
+ *     traceNewCoarse computes them (:655-669).  host_pyramids (NULL, or n_hosts entries that may be NULL) are the hosts'
+ *     pyramids.  Asynchronous on the set's stream, after the build of every pyramid given; a later tdm_pyramid_build or
+ *     tdm_pyramid_destroy of any of them waits for the trace.  Invalid input (null handles or arrays, n_hosts outside 0..8,
+ *     a slot outside 0..7 or given twice, pyramids of another level-0 size or device) is an error and launches nothing. */
+int tdm_immature_trace(tdm_immature* s, tdm_pyramid* frame_pyramid, int n_hosts, const int* host_slots,
+                       tdm_pyramid* const* host_pyramids, const float* KRKi9, const float* Kt3, const float* aff2);
+/* Points first..first+n-1 of a slot (synchronises): *count receives the slot's number of points; any output may be NULL.
+ *     color and weights hold 8 floats per point, grad_h 4 (row-major gradH), uv 2 (lastTraceUV).  first + n beyond the
+ *     count is an error. */
+int tdm_immature_get(tdm_immature* s, int host_slot, int first, int n, int* count, float* u, float* v, float* type,
+                     float* energy_th, float* color, float* weights, float* grad_h, float* idepth_min, float* idepth_max,
+                     float* quality, int* status, float* uv, float* interval);
+/* Removes points of a slot the way activatePointsMT compacts host->immaturePoints (FullSystem.cpp:849-856): walking up
+ *     from index 0, a removed entry takes the last entry, which is popped, and is looked at again - so the set's indices
+ *     stay those of the host's vector after the same removals.  Duplicate or out-of-range indices are an error. */
+int tdm_immature_remove(tdm_immature* s, int host_slot, int n_removed, const int* indices);
+/* Empties a slot (its keyframe was marginalised). */
+int tdm_immature_drop_host(tdm_immature* s, int host_slot);
+
 #ifdef __cplusplus
 }
 #endif

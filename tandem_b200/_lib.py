@@ -35,6 +35,15 @@ def check(rc):
 
 #: the values tdm_debug_conv_plan_n writes, in order (include/tandem_b200.h; tdm_debug_conv_plan writes the first 12); nwg
 #: is the consumer-warpgroup count of the kernel the plan is made for
+class TraceSettings(ctypes.Structure):
+    """tdm_trace_settings (include/tandem_b200.h): the reference's constants of ImmaturePoint::traceOn."""
+    _fields_ = [("max_pix_search", ctypes.c_float), ("trace_stepsize", ctypes.c_float), ("trace_gn_threshold", ctypes.c_float),
+                ("trace_extra_slack_on_th", ctypes.c_float), ("trace_slack_interval", ctypes.c_float),
+                ("trace_min_improvement_factor", ctypes.c_float), ("huber_th", ctypes.c_float), ("outlier_th", ctypes.c_float),
+                ("outlier_th_sum_component", ctypes.c_float), ("overall_energy_th_weight", ctypes.c_float),
+                ("min_trace_test_radius", ctypes.c_int), ("trace_gn_iterations", ctypes.c_int)]
+
+
 CONV_PLAN_KEYS = ("S", "R", "TW", "P", "DR", "nch", "slot_pos", "tiles_w", "tiles_h", "tiles_d", "grid", "smem", "nwg")
 
 
@@ -173,6 +182,13 @@ def _declare(l):
         "tdm_tracker_set_coarse_tracking_ref_nodia": (i, [P(vp), i, i, i, fp, fp, fp, fp, vp, fp, vp, i, dp, i, i, f, dp, f, ip,
                                                           P(CoarseNodiaResult)]),
         "tdm_tracker_get_coarse_nodia": (i, [vp, i, fp, fp, fp, fp]),
+        "tdm_immature_create": (i, [i, i, i, P(TraceSettings), i, P(vp)]),
+        "tdm_immature_destroy": (None, [vp]),
+        "tdm_immature_add": (i, [vp, i, vp, i, ip, ip, fp, ip]),
+        "tdm_immature_trace": (i, [vp, vp, i, ip, P(vp), fp, fp, fp]),
+        "tdm_immature_get": (i, [vp, i, i, i, ip, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, ip, fp, fp]),
+        "tdm_immature_remove": (i, [vp, i, i, ip]),
+        "tdm_immature_drop_host": (i, [vp, i]),
     }
     missing = []
     for name, (res, args) in sigs.items():

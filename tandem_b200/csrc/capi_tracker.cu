@@ -1,5 +1,7 @@
 // extern "C" entry points for the coarse tracker (include/tandem_b200.h).
 #include <cmath>
+#include <cstring>
+#include <vector>
 
 #include "../../include/tandem_b200.h"
 #include "capi_common.h"
@@ -12,6 +14,9 @@ struct tdm_tracker {
 };
 struct tdm_pyramid {
   tdm::PyramidIface* impl;
+};
+struct tdm_immature {
+  tdm::ImmatureIface* impl;
 };
 struct tdm_fusion {   // same layout as in capi_fusion.cu (one pointer)
   tdm::FusionIface* impl;
@@ -355,6 +360,86 @@ int tdm_tracker_get_coarse_nodia(tdm_tracker* level0, int n, float* u, float* v,
   TDM_API_BEGIN
   TDM_CHECK(level0, "null handle");
   level0->impl->get_coarse_nodia(n, u, v, idepth, color);
+  return TDM_OK;
+  TDM_API_END
+}
+
+/* ---- SURVEY 8(f) n8: immature points traced on the device ---- */
+int tdm_immature_create(int w, int h, int capacity_per_host, const tdm_trace_settings* settings, int device, tdm_immature** out) {
+  TDM_API_BEGIN
+  TDM_CHECK(out, "null argument");
+  static const tdm_trace_settings defaults = {0.027f, 1.f, 0.1f, 1.2f, 1.5f, 2.f, 9.f, 144.f, 2500.f, 1.f, 2, 3};
+  *out = new tdm_immature{tdm::make_immature(w, h, capacity_per_host, (const float*)(settings ? settings : &defaults), device)};
+  return TDM_OK;
+  TDM_API_END
+}
+void tdm_immature_destroy(tdm_immature* s) {
+  if (!s) return;
+  try { delete s->impl; } catch (...) {}
+  delete s;
+}
+int tdm_immature_add(tdm_immature* s, int host_slot, tdm_pyramid* host_pyramid, int n, const int* u, const int* v,
+                     const float* type, int* n_added) {
+  TDM_API_BEGIN
+  TDM_CHECK(s && host_pyramid && n_added, "null argument");
+  *n_added = s->impl->add(host_slot, *host_pyramid->impl, n, u, v, type);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_immature_trace(tdm_immature* s, tdm_pyramid* frame_pyramid, int n_hosts, const int* host_slots,
+                       tdm_pyramid* const* host_pyramids, const float* KRKi9, const float* Kt3, const float* aff2) {
+  TDM_API_BEGIN
+  TDM_CHECK(s && frame_pyramid, "null argument");
+  TDM_CHECK(n_hosts >= 0 && n_hosts <= 8, "n_hosts outside 0..8");
+  const tdm::PyramidIface* hp[8] = {};
+  if (host_pyramids)
+    for (int j = 0; j < n_hosts; ++j) hp[j] = host_pyramids[j] ? host_pyramids[j]->impl : nullptr;
+  s->impl->trace(*frame_pyramid->impl, n_hosts, host_slots, hp, KRKi9, Kt3, aff2);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_immature_get(tdm_immature* s, int host_slot, int first, int n, int* count, float* u, float* v, float* type,
+                     float* energy_th, float* color, float* weights, float* grad_h, float* idepth_min, float* idepth_max,
+                     float* quality, int* status, float* uv, float* interval) {
+  TDM_API_BEGIN
+  TDM_CHECK(s, "null handle");
+  using namespace tdm;
+  const bool any = u || v || type || energy_th || color || weights || grad_h || idepth_min || idepth_max || quality || status ||
+                   uv || interval;
+  std::vector<float> rows(any ? (size_t)IM_ROWS * (n > 0 ? n : 0) : 0);
+  float* r[IM_ROWS] = {};
+  if (any)
+    for (int k = 0; k < IM_ROWS; ++k) r[k] = rows.data() + (size_t)k * n;
+  s->impl->get(host_slot, first, n, r);
+  if (count) *count = s->impl->count(host_slot);
+  if (!any) return TDM_OK;
+  auto plain = [&](int row, float* out) { if (out) std::memcpy(out, r[row], 4ull * n); };
+  plain(IM_U, u); plain(IM_V, v); plain(IM_TYPE, type); plain(IM_ETH, energy_th); plain(IM_IDMIN, idepth_min);
+  plain(IM_IDMAX, idepth_max); plain(IM_QUALITY, quality); plain(IM_INTERVAL, interval);
+  if (status) std::memcpy(status, r[IM_STATUS], 4ull * n);
+  for (int i = 0; i < n; ++i) {
+    for (int k = 0; k < 8; ++k) {
+      if (color) color[8 * i + k] = r[IM_COLOR + k][i];
+      if (weights) weights[8 * i + k] = r[IM_WEIGHTS + k][i];
+    }
+    for (int k = 0; k < 4; ++k)
+      if (grad_h) grad_h[4 * i + k] = r[IM_GRADH + k][i];
+    if (uv) { uv[2 * i] = r[IM_UVX][i]; uv[2 * i + 1] = r[IM_UVY][i]; }
+  }
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_immature_remove(tdm_immature* s, int host_slot, int n_removed, const int* indices) {
+  TDM_API_BEGIN
+  TDM_CHECK(s, "null handle");
+  s->impl->remove(host_slot, n_removed, indices);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_immature_drop_host(tdm_immature* s, int host_slot) {
+  TDM_API_BEGIN
+  TDM_CHECK(s, "null handle");
+  s->impl->drop_host(host_slot);
   return TDM_OK;
   TDM_API_END
 }

@@ -1805,6 +1805,10 @@ class PyramidImpl final : public PyramidIface {
   }
   const float* level_dI(int lvl) const override { return d_dI_.get() + 3 * off_.at(lvl); }
   void* ready_event() const override { return (void*)ready_.get(); }
+  void wait_for(void* event) const override {
+    TDM_CUDA(cudaSetDevice(device_));
+    TDM_CUDA(cudaStreamWaitEvent(stream_.get(), (cudaEvent_t)event, 0));
+  }
   int width(int lvl) const override { return w_ >> lvl; }
   int height(int lvl) const override { return h_ >> lvl; }
   int levels() const override { return levels_; }

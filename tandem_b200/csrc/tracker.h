@@ -144,12 +144,39 @@ class PyramidIface {
   virtual void get_level(int lvl, float* dI_host, float* absgrad_host) = 0;
   virtual const float* level_dI(int lvl) const = 0;   // device pointer, float3 per pixel
   virtual void* ready_event() const = 0;              // cudaEvent_t recorded after build()
+  // orders the next build() (and the destructor) after `event` (a cudaEvent_t a reader recorded behind its reads)
+  virtual void wait_for(void* event) const = 0;
   virtual int width(int lvl) const = 0;
   virtual int height(int lvl) const = 0;
   virtual int levels() const = 0;
   virtual int device() const = 0;
 };
 PyramidIface* make_pyramid(int w, int h, int levels, int device);
+
+// n8 (immature.cu): the immature points of up to 8 host keyframes (slots) and their trace into new frames.  Each field is a
+// row of 32-bit words, one per point; status is an int, the others floats.
+enum ImmatureRow { IM_U = 0, IM_V, IM_TYPE, IM_ETH, IM_IDMIN, IM_IDMAX, IM_QUALITY, IM_STATUS, IM_UVX, IM_UVY, IM_INTERVAL,
+                   IM_COLOR, IM_WEIGHTS = IM_COLOR + 8, IM_GRADH = IM_WEIGHTS + 8, IM_ROWS = IM_GRADH + 4 };
+class ImmatureIface {
+ public:
+  virtual ~ImmatureIface() = default;
+  // constructor for n candidate pixels of `host`'s level 0; appends the points with a finite energyTH, returns their number
+  virtual int add(int slot, const PyramidIface& host, int n, const int* u, const int* v, const float* type) = 0;
+  // traceOn of every point of the given slots into frame's level 0 (asynchronous); KRKi 9, Kt 3, aff 2 per host;
+  // host_pyramids (may be null, or hold nulls) are the hosts' pyramids the trace is ordered after and keeps alive
+  virtual void trace(const PyramidIface& frame, int n_hosts, const int* slots, const PyramidIface* const* host_pyramids,
+                     const float* KRKi, const float* Kt, const float* aff) = 0;
+  virtual int count(int slot) = 0;
+  // points first..first+n-1 of a slot, one output per ImmatureRow (null: not wanted); synchronises
+  virtual void get(int slot, int first, int n, float* const* rows) = 0;
+  virtual void remove(int slot, int n_removed, const int* indices) = 0;
+  virtual void drop_host(int slot) = 0;
+  virtual void synchronize() = 0;
+  virtual int width() const = 0;
+  virtual int height() const = 0;
+  virtual int device() const = 0;
+};
+ImmatureIface* make_immature(int w, int h, int capacity_per_host, const float* settings /* tdm_trace_settings */, int device);
 
 TrackerIface* make_tracker(int w, int h, float huber, float cutoff, int n_max, int device);
 

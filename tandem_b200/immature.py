@@ -1,0 +1,97 @@
+"""n8: DSO's immature points of the active keyframes kept in device memory and traced into each new frame
+(FullSystem::traceNewCoarse, FullSystem.cpp:650-691; ImmaturePoint::traceOn, ImmaturePoint.cpp:75-414) over the C ABI
+(include/tandem_b200.h, block n8)."""
+import ctypes
+
+import numpy as np
+
+from ._lib import TraceSettings, check, lib
+
+_fp = ctypes.POINTER(ctypes.c_float)
+_ip = ctypes.POINTER(ctypes.c_int)
+
+#: util/settings.cpp:84-148
+TRACE_DEFAULTS = dict(max_pix_search=0.027, trace_stepsize=1.0, trace_gn_threshold=0.1, trace_extra_slack_on_th=1.2,
+                      trace_slack_interval=1.5, trace_min_improvement_factor=2.0, huber_th=9.0, outlier_th=144.0,
+                      outlier_th_sum_component=2500.0, overall_energy_th_weight=1.0, min_trace_test_radius=2,
+                      trace_gn_iterations=3)
+#: ImmaturePoint::lastTraceStatus
+IPS_GOOD, IPS_OOB, IPS_OUTLIER, IPS_SKIPPED, IPS_BADCONDITION, IPS_UNINITIALIZED = range(6)
+FIELDS = {"u": (), "v": (), "type": (), "energy_th": (), "color": (8,), "weights": (8,), "grad_h": (4,), "idepth_min": (),
+          "idepth_max": (), "quality": (), "status": (), "uv": (2,), "interval": ()}
+
+
+def _p(a, t=_fp):
+    return None if a is None else a.ctypes.data_as(t)
+
+
+class ImmaturePoints:
+    """The immature points of up to 8 host keyframes (slots 0..7, capacity_per_host each) of one w x h camera."""
+
+    def __init__(self, w, h, capacity_per_host, device=0, **settings):
+        unknown = set(settings) - set(TRACE_DEFAULTS)
+        if unknown:
+            raise TypeError(f"unknown trace settings {sorted(unknown)}")
+        self.w, self.h = w, h
+        self.settings = dict(TRACE_DEFAULTS, **settings)
+        st = TraceSettings(**self.settings)
+        self._h = ctypes.c_void_p()
+        check(lib().tdm_immature_create(w, h, capacity_per_host, ctypes.byref(st), device, ctypes.byref(self._h)))
+
+    def close(self):
+        if self._h is not None:
+            lib().tdm_immature_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def add(self, slot, host_pyramid, u, v, type=None):
+        """The constructor for the pixels (u, v) of host_pyramid's level 0; returns how many points were kept."""
+        u = np.ascontiguousarray(u, np.int32)
+        v = np.ascontiguousarray(v, np.int32)
+        t = np.ones(len(u), np.float32) if type is None else np.ascontiguousarray(type, np.float32)
+        if not (len(u) == len(v) == len(t)):
+            raise ValueError("u, v and type differ in length")
+        n = ctypes.c_int()
+        check(lib().tdm_immature_add(self._h, slot, host_pyramid._h, len(u), _p(u, _ip), _p(v, _ip), _p(t), ctypes.byref(n)))
+        return n.value
+
+    def trace(self, frame_pyramid, slots, KRKi, Kt, aff, host_pyramids=None):
+        """traceOn of every point of `slots` into frame_pyramid's level 0 (asynchronous).  KRKi (n, 3, 3), Kt (n, 3) and
+        aff (n, 2) per slot."""
+        slots = np.ascontiguousarray(slots, np.int32).ravel()
+        n = len(slots)
+        K = np.ascontiguousarray(KRKi, np.float32).reshape(n, 9)
+        t = np.ascontiguousarray(Kt, np.float32).reshape(n, 3)
+        a = np.ascontiguousarray(aff, np.float32).reshape(n, 2)
+        hp = None
+        if host_pyramids is not None:
+            hp = (ctypes.c_void_p * n)(*[None if p is None else p._h.value for p in host_pyramids])
+        check(lib().tdm_immature_trace(self._h, frame_pyramid._h, n, _p(slots, _ip), hp, _p(K), _p(t), _p(a)))
+
+    def count(self, slot):
+        c = ctypes.c_int()
+        check(lib().tdm_immature_get(self._h, slot, 0, 0, ctypes.byref(c), *([None] * 13)))
+        return c.value
+
+    def get(self, slot, first=0, n=None):
+        """dict of every field (FIELDS) of points first..first+n-1 of a slot (all of them by default); synchronises."""
+        if n is None:
+            n = self.count(slot) - first
+        out = {k: np.empty((n,) + s, np.int32 if k == "status" else np.float32) for k, s in FIELDS.items()}
+        c = ctypes.c_int()
+        check(lib().tdm_immature_get(self._h, slot, first, n, ctypes.byref(c), *[
+            _p(out[k], _ip if k == "status" else _fp) for k in FIELDS]))
+        return out
+
+    def remove(self, slot, indices):
+        """Removes points the way activatePointsMT compacts host->immaturePoints (FullSystem.cpp:849-856)."""
+        idx = np.ascontiguousarray(indices, np.int32).ravel()
+        check(lib().tdm_immature_remove(self._h, slot, len(idx), _p(idx, _ip)))
+
+    def drop_host(self, slot):
+        check(lib().tdm_immature_drop_host(self._h, slot))

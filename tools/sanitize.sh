@@ -22,3 +22,4 @@ leg new_coarse_race $T2 racecheck tests/test_track_new_coarse_gpu.py -k "host_lo
 leg conv_is_mem $T1 memcheck tests/test_conv_is_gpu.py -k "abl04"
 leg feature_cache_mem $T1 memcheck tests/test_mvsnet_feature_cache_gpu.py -k "handoff or golden"
 leg feature_cache_race $T2 racecheck tests/test_mvsnet_feature_cache_gpu.py -k "handoff"
+leg trace_mem $T1 memcheck tests/test_trace_gpu.py -k "not shim and not random and not 2560"
