@@ -1,6 +1,6 @@
 // The immature points of DSO's active keyframes on the device (n8, include/tandem_b200.h): FullSystem::traceNewCoarse
 // (tandem/src/FullSystem/FullSystem.cpp:650-691) becomes one trace() call per frame.  Host slot = the keyframe's index among
-// the active ones (0..7); INTEGRATION.md shows the call sites.  Owns one tdm_immature handle; not copyable.
+// the active ones (0..7); INTEGRATION.md shows the call sites.  activatePointsMT's solve (n9) becomes one activate() call.  Owns one tdm_immature handle; not copyable.
 #ifndef TDM_CUDA_IMMATURE_POINTS_H
 #define TDM_CUDA_IMMATURE_POINTS_H
 
@@ -38,6 +38,30 @@ class CudaImmaturePoints {
   void remove(int host_slot, std::vector<int> const &indices);
   // the keyframe was marginalised
   void dropHost(int host_slot);
+
+  // n9: host->targetPrecalc[target]'s members that optimizeImmaturePoint reads (FrameFramePrecalc::set)
+  struct Precalc {
+    Eigen::Matrix<float, 3, 3> PRE_RTll;
+    Eigen::Matrix<float, 3, 1> PRE_tTll;
+    Eigen::Matrix<float, 2, 1> PRE_aff_mode;
+  };
+  // result[k] 1 / 0 / -1 as optimizeImmaturePoint returns a PointHessian / 0 / -1, idepth[k] its final currentIdepth,
+  // res_state / res_energy[k * n_frames + f] the residual to frame f's state_state / state_energy (-1 / NaN: the host)
+  struct Activation {
+    int n_frames = 0;
+    std::vector<int> result;
+    std::vector<float> idepth;
+    std::vector<signed char> res_state;
+    std::vector<float> res_energy;
+  };
+  // activatePointsMT_Reductor (FullSystem.cpp:694-703, 819-825) for the toOptimize list: frames are frameHessians in order
+  // (frame_slots[f] the frame's slot, -1 for the newest keyframe), precalc holds n_frames * n_frames entries
+  // [host * n_frames + target] (the diagonal is not read), (fxl, fyl, cxl, cyl) is Hcalib's.  Candidate k is point
+  // cand_index[k] of frame cand_frame[k]'s slot.  Blocking; the set is not changed.
+  Activation activate(std::vector<int> const &frame_slots, std::vector<tdm_pyramid *> const &frame_pyramids,
+                      std::vector<Precalc> const &precalc, float fxl, float fyl, float cxl, float cyl,
+                      std::vector<int> const &cand_frame, std::vector<int> const &cand_index, float min_idepth_h_act = 100.f,
+                      int gn_iterations = 3, int min_obs = 1);
 
  private:
   tdm_immature *handle_ = nullptr;

@@ -510,6 +510,38 @@ int tdm_immature_remove(tdm_immature* s, int host_slot, int n_removed, const int
 /* Empties a slot (its keyframe was marginalised). */
 int tdm_immature_drop_host(tdm_immature* s, int host_slot);
 
+/* n9  FullSystem::activatePointsMT's solve on the device: FullSystem::optimizeImmaturePoint (FullSystemOptPoint.cpp:51-205,
+ *     with ImmaturePoint::linearizeResidual, ImmaturePoint.cpp:476-543) for every candidate in one launch.  Every float
+ *     operation is the reference's, correctly rounded and in its order; the reference's double operations (the step, the
+ *     stop test, the lambda updates, lastEnergy's double increments) are done in double. */
+typedef struct tdm_activate_settings {
+  float min_idepth_h_act;   /* setting_minIdepthH_act, 100 */
+  int gn_iterations;        /* setting_GNItsOnPointActivation, 3 */
+  int min_obs;              /* activatePointsMT_Reductor's minObs, 1 */
+} tdm_activate_settings;
+/* The frames are frameHessians in order (n_frames, 1..8, the new keyframe included): frame_slots[f] is frame f's slot in the
+ *     set or -1 (a frame without points, such as the newest keyframe), frame_pyramids[f] its pyramid (level 0 is read).
+ *     precalc is n_frames x n_frames x 14 floats, [host][target] = host->targetPrecalc[target]'s PRE_RTll (row-major 3x3),
+ *     PRE_tTll (3) and PRE_aff_mode (2); the diagonal is not read.  calib4 = fxl, fyl, cxl, cyl (fxli = 1.0f / fxl, as
+ *     CalibHessian::setValueScaled sets it).  The Huber threshold is the set's huber_th.  Candidate k is point cand_index[k]
+ *     of slot frame_slots[cand_frame[k]] (activatePointsMT's toOptimize, FullSystem.cpp:742-810, in its order); its
+ *     residuals go to every other frame in frame order.
+ *     Outputs (any may be NULL): result[k] 1 (a PointHessian is made), 0 (optimizeImmaturePoint returned 0: the point stays
+ *     immature) or -1 (it returned (PointHessian*)-1); idepth[k] the final currentIdepth; res_state[k * n_frames + f] and
+ *     res_energy[...] the state_state (IN 0, OOB 1, OUTLIER 2) and state_energy of the residual to frame f, -1 and NaN in
+ *     the host's own column.  With these the host rebuilds the PointHessian and its IN residuals exactly as
+ *     optimizeImmaturePoint does (:180-199).
+ *     The set is not changed.  Blocking (one host wait), on the set's stream after its pending work and after the build of
+ *     every pyramid given; a later tdm_pyramid_build or tdm_pyramid_destroy of any of them waits for it.  n_cand 0 is a
+ *     no-op.  Invalid input (null handles or needed arrays, n_frames outside 1..8, a slot outside -1..7 or given twice, a
+ *     pyramid of another level-0 size or device, a candidate frame out of range or without a slot, an index at or beyond
+ *     its slot's count, a candidate given twice, gn_iterations outside 0..100, min_obs < 0) is an error and launches
+ *     nothing.  settings NULL: the defaults above. */
+int tdm_immature_activate(tdm_immature* s, int n_frames, const int* frame_slots, tdm_pyramid* const* frame_pyramids,
+                          const float* precalc, const float calib4[4], const tdm_activate_settings* settings, int n_cand,
+                          const int* cand_frame, const int* cand_index, int* result, float* idepth, signed char* res_state,
+                          float* res_energy);
+
 #ifdef __cplusplus
 }
 #endif

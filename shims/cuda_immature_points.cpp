@@ -65,3 +65,37 @@ void CudaImmaturePoints::remove(int host_slot, std::vector<int> const &indices) 
 }
 
 void CudaImmaturePoints::dropHost(int host_slot) { chk(tdm_immature_drop_host(handle_, host_slot), "CudaImmaturePoints::dropHost"); }
+
+CudaImmaturePoints::Activation CudaImmaturePoints::activate(std::vector<int> const &frame_slots,
+                                                            std::vector<tdm_pyramid *> const &frame_pyramids,
+                                                            std::vector<Precalc> const &precalc, float fxl, float fyl, float cxl,
+                                                            float cyl, std::vector<int> const &cand_frame,
+                                                            std::vector<int> const &cand_index, float min_idepth_h_act,
+                                                            int gn_iterations, int min_obs) {
+  const size_t n = frame_slots.size(), k = cand_frame.size();
+  if (frame_pyramids.size() != n || precalc.size() != n * n || cand_index.size() != k)
+    throw std::runtime_error("CudaImmaturePoints::activate: sizes differ");
+  std::vector<float> pc(14 * n * n);
+  for (size_t e = 0; e < n * n; ++e) {
+    float *o = pc.data() + 14 * e;
+    for (int r = 0; r < 3; ++r) {
+      for (int c = 0; c < 3; ++c) o[3 * r + c] = precalc[e].PRE_RTll(r, c);
+      o[9 + r] = precalc[e].PRE_tTll(r);
+    }
+    o[12] = precalc[e].PRE_aff_mode(0);
+    o[13] = precalc[e].PRE_aff_mode(1);
+  }
+  const float calib[4] = {fxl, fyl, cxl, cyl};
+  const tdm_activate_settings st = {min_idepth_h_act, gn_iterations, min_obs};
+  Activation a;
+  a.n_frames = (int)n;
+  a.result.resize(k);
+  a.idepth.resize(k);
+  a.res_state.resize(k * n);
+  a.res_energy.resize(k * n);
+  chk(tdm_immature_activate(handle_, (int)n, frame_slots.data(), frame_pyramids.data(), pc.data(), calib, &st, (int)k,
+                            cand_frame.data(), cand_index.data(), a.result.data(), a.idepth.data(), a.res_state.data(),
+                            a.res_energy.data()),
+      "CudaImmaturePoints::activate");
+  return a;
+}

@@ -44,6 +44,11 @@ class TraceSettings(ctypes.Structure):
                 ("min_trace_test_radius", ctypes.c_int), ("trace_gn_iterations", ctypes.c_int)]
 
 
+class ActivateSettings(ctypes.Structure):
+    """tdm_activate_settings (include/tandem_b200.h): the reference's constants of optimizeImmaturePoint."""
+    _fields_ = [("min_idepth_h_act", ctypes.c_float), ("gn_iterations", ctypes.c_int), ("min_obs", ctypes.c_int)]
+
+
 CONV_PLAN_KEYS = ("S", "R", "TW", "P", "DR", "nch", "slot_pos", "tiles_w", "tiles_h", "tiles_d", "grid", "smem", "nwg")
 
 
@@ -189,6 +194,8 @@ def _declare(l):
         "tdm_immature_get": (i, [vp, i, i, i, ip, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, ip, fp, fp]),
         "tdm_immature_remove": (i, [vp, i, i, ip]),
         "tdm_immature_drop_host": (i, [vp, i]),
+        "tdm_immature_activate": (i, [vp, i, ip, P(vp), fp, fp, P(ActivateSettings), i, ip, ip, ip, fp,
+                                      ctypes.POINTER(ctypes.c_byte), fp]),
     }
     missing = []
     for name, (res, args) in sigs.items():

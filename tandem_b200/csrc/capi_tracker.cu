@@ -444,4 +444,25 @@ int tdm_immature_drop_host(tdm_immature* s, int host_slot) {
   TDM_API_END
 }
 
+/* ---- n9: activatePointsMT's optimizeImmaturePoint on the device ---- */
+int tdm_immature_activate(tdm_immature* s, int n_frames, const int* frame_slots, tdm_pyramid* const* frame_pyramids,
+                          const float* precalc, const float calib4[4], const tdm_activate_settings* settings, int n_cand,
+                          const int* cand_frame, const int* cand_index, int* result, float* idepth, signed char* res_state,
+                          float* res_energy) {
+  TDM_API_BEGIN
+  TDM_CHECK(s && frame_slots && frame_pyramids, "null argument");
+  TDM_CHECK(n_frames >= 1 && n_frames <= 8, "n_frames outside 1..8");
+  static const tdm_activate_settings defaults = {100.f, 3, 1};
+  const tdm_activate_settings& st = settings ? *settings : defaults;
+  const tdm::PyramidIface* fp[8] = {};
+  for (int f = 0; f < n_frames; ++f) {
+    TDM_CHECK(frame_pyramids[f], "null argument");
+    fp[f] = frame_pyramids[f]->impl;
+  }
+  s->impl->activate(n_frames, frame_slots, fp, precalc, calib4, st.min_idepth_h_act, st.gn_iterations, st.min_obs, n_cand,
+                    cand_frame, cand_index, result, idepth, res_state, res_energy);
+  return TDM_OK;
+  TDM_API_END
+}
+
 }  // extern "C"

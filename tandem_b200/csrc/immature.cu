@@ -8,6 +8,7 @@
 // - the same values, so every branch is warp-uniform - the lanes share the discrete search (lane l takes steps l, l+32, ...,
 // rebuilding ptx / pty by the reference's chain of additions), a shuffle reduction picks the best step (first index on ties,
 // as the strict < does) and the second best outside its radius, and every lane runs the Gauss-Newton steps; lane 0 stores.
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <string>
@@ -365,6 +366,182 @@ __global__ void k_scatter_back(uint32_t* __restrict__ st, const uint32_t* __rest
   st[(size_t)r * kSlots * cap + (size_t)slot * cap + j] = scratch[(size_t)r * cap + j];
 }
 
+// ---- n9: activation (FullSystem::optimizeImmaturePoint, FullSystemOptPoint.cpp:51-205, with
+// ImmaturePoint::linearizeResidual, ImmaturePoint.cpp:476-543, and the 5-argument projectPoint / derive_idepth,
+// ResidualProjections.h:36-87) for every candidate of activatePointsMT in one launch.
+//
+// Shape (DESIGN.md, n9): one warp per candidate.  Residual r (to frame r, or r + 1 past the host) and pattern index i form
+// pair q = 8 r + i; lane l evaluates pairs l and l + 32 (so its pattern index is l & 7) at the current inverse depth and
+// leaves (in image, energy term, Hdd term, bd term) in shared memory.  Every lane then runs the reference's three serial
+// chains - the residual's energy, Hdd / bd across (residual, pattern index), lastEnergy across residuals - over the 56 slots
+// in the reference's order, so every lane holds the same state and every branch is warp-uniform; lane 0 stores.
+constexpr int kActThreads = 128, kActWarps = kActThreads / 32, kActPairs = 64;
+enum { RS_IN = 0, RS_OOB = 1, RS_OUTLIER = 2 };   // ResState
+struct ActivateLaunch {
+  const float* dI[kSlots];          // level 0 of frame f
+  float pc[kSlots][kSlots][14];     // [host][target]: PRE_RTll row-major, PRE_tTll, PRE_aff_mode
+  int slot[kSlots];
+  int n_frames, n_cand, w, h, cap, gn_its, min_obs;
+  float fxl, fyl, cxl, cyl, fxli, fyli, huber, min_h;
+};
+
+struct ActPair {
+  float e, hdd, bd;
+  int ok;
+};
+
+// linearizeResidual of every residual at `idepth` with `slack`, in the reference's order: *energy (lastEnergy / newEnergy)
+// is a float increased by each residual's double return; ns / nE receive state_NewState / state_NewEnergy
+__device__ __forceinline__ void act_linearize(const ActivateLaunch& L, ActPair* sm, int lane, int hf, float u, float v, float eth,
+                                              float col, float wt, float idepth, float slack, const int (&ss)[kSlots - 1],
+                                              const float (&se)[kSlots - 1], int (&ns)[kSlots - 1], float (&nE)[kSlots - 1],
+                                              float* energy, float* Hdd, float* bd) {
+  const int nres = L.n_frames - 1, i = lane & 7;
+  const float wM3G = (float)(L.w - 3), hM3G = (float)(L.h - 3);
+  __syncwarp();   // the previous evaluation's slots have been read
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int q = lane + 32 * half, r = q >> 3;
+    if (r >= nres) continue;
+    const int t = r < hf ? r : r + 1;
+    const float* P = L.pc[hf][t];
+    ActPair a{0.f, 0.f, 0.f, 0};
+    // projectPoint, 5-argument form
+    const float K0 = fm(fs(fa(u, (float)c_pattern[i][0]), L.cxl), L.fxli), K1 = fm(fs(fa(v, (float)c_pattern[i][1]), L.cyl), L.fyli);
+    const float p0 = fa(fa(fa(fm(P[0], K0), fm(P[1], K1)), fm(P[2], 1.f)), fm(P[9], idepth));
+    const float p1 = fa(fa(fa(fm(P[3], K0), fm(P[4], K1)), fm(P[5], 1.f)), fm(P[10], idepth));
+    const float p2 = fa(fa(fa(fm(P[6], K0), fm(P[7], K1)), fm(P[8], 1.f)), fm(P[11], idepth));
+    const float drescale = fd(1.0f, p2);
+    if (drescale > 0) {
+      const float pu = fm(p0, drescale), pv = fm(p1, drescale);
+      const float Ku = fa(fm(pu, L.fxl), L.cxl), Kv = fa(fm(pv, L.fyl), L.cyl);
+      if (Ku > 1.1f && Kv > 1.1f && Ku < wM3G && Kv < hM3G) {
+        float hit[3];
+        interp<3>(L.dI[t], Ku, Kv, L.w, hit);
+        if (isfinite(hit[0])) {
+          const float residual = fs(hit[0], fa(fm(P[12], col), P[13]));
+          float hw = fabsf(residual) < L.huber ? 1.f : fd(L.huber, fabsf(residual));
+          a.e = fm(fm(fm(fm(fm(wt, wt), hw), residual), residual), fs(2.f, hw));
+          const float dxInterp = fm(hit[1], L.fxl), dyInterp = fm(hit[2], L.fyl);
+          // derive_idepth; SCALE_IDEPTH is 1
+          const float d_idepth = fa(fm(fm(dxInterp, drescale), fs(P[9], fm(P[11], pu))),
+                                    fm(fm(dyInterp, drescale), fs(P[10], fm(P[11], pv))));
+          hw = fm(hw, fm(wt, wt));
+          a.hdd = fm(fm(hw, d_idepth), d_idepth);
+          a.bd = fm(fm(hw, residual), d_idepth);
+          a.ok = 1;
+        }
+      }
+    }
+    sm[q] = a;
+  }
+  __syncwarp();
+  const float th = fm(eth, slack);
+#pragma unroll
+  for (int r = 0; r < kSlots - 1; ++r) {
+    if (r >= nres) break;
+    double ret;
+    if (ss[r] == RS_OOB) {   // sticky
+      ns[r] = RS_OOB;
+      ret = (double)se[r];
+    } else {
+      float el = 0.f;
+      bool oob = false;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const ActPair a = sm[8 * r + k];
+        if (!a.ok) { oob = true; break; }   // the Hdd / bd of pattern indices 0..k-1 stay added
+        el = fa(el, a.e);
+        *Hdd = fa(*Hdd, a.hdd);
+        *bd = fa(*bd, a.bd);
+      }
+      if (oob) {
+        ns[r] = RS_OOB;
+        ret = (double)se[r];
+      } else {
+        if (el > th) { el = th; ns[r] = RS_OUTLIER; } else { ns[r] = RS_IN; }
+        nE[r] = el;
+        ret = (double)el;
+      }
+    }
+    *energy = __double2float_rn(__dadd_rn((double)*energy, ret));
+  }
+}
+
+__global__ void __launch_bounds__(kActThreads) k_activate(ActivateLaunch L, const uint32_t* __restrict__ st,
+                                                          const int* __restrict__ cand, int* __restrict__ result,
+                                                          float* __restrict__ out_idepth, float* __restrict__ out_energy,
+                                                          signed char* __restrict__ out_state) {
+  __shared__ ActPair smem[kActWarps][kActPairs];
+  const int k = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (k >= L.n_cand) return;   // warp-uniform
+  ActPair* sm = smem[threadIdx.x >> 5];
+  const int hf = cand[k];
+  const size_t stride = (size_t)kSlots * L.cap, p = (size_t)L.slot[hf] * L.cap + cand[L.n_cand + k];
+  const float* f = reinterpret_cast<const float*>(st);
+  const float u = f[IM_U * stride + p], v = f[IM_V * stride + p], eth = f[IM_ETH * stride + p];
+  const float idmin = f[IM_IDMIN * stride + p], idmax = f[IM_IDMAX * stride + p];
+  const float col = f[(IM_COLOR + (lane & 7)) * stride + p], wt = f[(IM_WEIGHTS + (lane & 7)) * stride + p];
+  const int nres = L.n_frames - 1;
+
+  int ss[kSlots - 1], ns[kSlots - 1];
+  float se[kSlots - 1], nE[kSlots - 1];
+#pragma unroll
+  for (int r = 0; r < kSlots - 1; ++r) { ss[r] = RS_IN; ns[r] = RS_OUTLIER; se[r] = 0.f; nE[r] = 0.f; }
+  float lastEnergy = 0.f, lastHdd = 0.f, lastbd = 0.f;
+  float currentIdepth = fm(fa(idmax, idmin), 0.5f);
+  act_linearize(L, sm, lane, hf, u, v, eth, col, wt, currentIdepth, 1000.f, ss, se, ns, nE, &lastEnergy, &lastHdd, &lastbd);
+#pragma unroll
+  for (int r = 0; r < kSlots - 1; ++r) { ss[r] = ns[r]; se[r] = nE[r]; }
+  int res;
+  if (!isfinite(lastEnergy) || lastHdd < L.min_h) {
+    res = 0;
+  } else {
+    res = 1;
+    float lambda = 0.1f;
+    for (int it = 0; it < L.gn_its; it++) {
+      const float H = fm(lastHdd, fa(1.f, lambda));
+      const float step = __double2float_rn(__dmul_rn(__ddiv_rn(1.0, (double)H), (double)lastbd));
+      const float newIdepth = fs(currentIdepth, step);
+      float newHdd = 0.f, newbd = 0.f, newEnergy = 0.f;
+      act_linearize(L, sm, lane, hf, u, v, eth, col, wt, newIdepth, 1.f, ss, se, ns, nE, &newEnergy, &newHdd, &newbd);
+      if (!isfinite(lastEnergy) || newHdd < L.min_h) { res = 0; break; }
+      if (newEnergy < lastEnergy) {
+        currentIdepth = newIdepth;
+        lastHdd = newHdd;
+        lastbd = newbd;
+        lastEnergy = newEnergy;
+#pragma unroll
+        for (int r = 0; r < kSlots - 1; ++r) { ss[r] = ns[r]; se[r] = nE[r]; }
+        lambda = __double2float_rn(__dmul_rn((double)lambda, 0.5));
+      } else {
+        lambda = __double2float_rn(__dmul_rn((double)lambda, 5.0));
+      }
+      if ((double)fabsf(step) < __dmul_rn(0.0001, (double)currentIdepth)) break;
+    }
+    if (res) {
+      int good = 0;
+#pragma unroll
+      for (int r = 0; r < kSlots - 1; ++r) good += r < nres && ss[r] == RS_IN;
+      if (!isfinite(currentIdepth) || good < L.min_obs || !isfinite(eth)) res = -1;
+    }
+  }
+  if (lane == 0) {
+    result[k] = res;
+    out_idepth[k] = currentIdepth;
+    const size_t o = (size_t)k * L.n_frames;
+    out_state[o + hf] = -1;
+    out_energy[o + hf] = __int_as_float(0x7fc00000);
+#pragma unroll
+    for (int r = 0; r < kSlots - 1; ++r) {
+      if (r >= nres) break;
+      const int t = r < hf ? r : r + 1;
+      out_state[o + t] = (signed char)ss[r];
+      out_energy[o + t] = se[r];
+    }
+  }
+}
+
 class ImmatureImpl final : public ImmatureIface {
  public:
   ImmatureImpl(int w, int h, int cap, const float* settings, int device) : w_(w), h_(h), cap_(cap), device_(device) {
@@ -450,6 +627,66 @@ class ImmatureImpl final : public ImmatureIface {
       if (host_pyramids && host_pyramids[j]) host_pyramids[j]->wait_for(done_.get());
   }
 
+  void activate(int n_frames, const int* frame_slots, const PyramidIface* const* frame_pyramids, const float* precalc,
+                const float* calib4, float min_idepth_h_act, int gn_iterations, int min_obs, int n_cand, const int* cand_frame,
+                const int* cand_index, int* result, float* idepth, signed char* res_state, float* res_energy) override {
+    TDM_CHECK(n_frames >= 1 && n_frames <= kSlots, "n_frames outside 1..8");
+    TDM_CHECK(frame_slots && frame_pyramids && precalc && calib4, "null argument");
+    TDM_CHECK(gn_iterations >= 0 && gn_iterations <= 100 && min_obs >= 0, "bad activation settings");
+    TDM_CHECK(n_cand >= 0 && (n_cand == 0 || (cand_frame && cand_index)), "null argument");
+    ActivateLaunch L{};
+    L.n_frames = n_frames; L.n_cand = n_cand; L.w = w_; L.h = h_; L.cap = cap_; L.gn_its = gn_iterations; L.min_obs = min_obs;
+    for (int f = 0; f < n_frames; ++f) {
+      TDM_CHECK(frame_slots[f] >= -1 && frame_slots[f] < kSlots, "frame slot outside -1..7");
+      for (int q = 0; q < f; ++q) TDM_CHECK(frame_slots[f] < 0 || frame_slots[q] != frame_slots[f], "a frame slot appears twice");
+      TDM_CHECK(frame_pyramids[f], "null argument");
+      check_pyramid(*frame_pyramids[f]);
+      L.dI[f] = frame_pyramids[f]->level_dI(0);
+      L.slot[f] = frame_slots[f];
+      for (int t = 0; t < n_frames; ++t) std::memcpy(L.pc[f][t], precalc + 14 * ((size_t)f * n_frames + t), sizeof L.pc[f][t]);
+    }
+    std::vector<std::vector<char>> seen(n_frames);
+    for (int k = 0; k < n_cand; ++k) {
+      const int f = cand_frame[k];
+      TDM_CHECK(f >= 0 && f < n_frames && frame_slots[f] >= 0, "candidate frame outside the frames with a slot");
+      const int n = count_[frame_slots[f]];
+      TDM_CHECK(cand_index[k] >= 0 && cand_index[k] < n, "candidate index outside its slot's points");
+      seen[f].resize(n, 0);
+      TDM_CHECK(!seen[f][cand_index[k]], "a candidate appears twice");
+      seen[f][cand_index[k]] = 1;
+    }
+    if (n_cand == 0) return;
+    L.fxl = calib4[0]; L.fyl = calib4[1]; L.cxl = calib4[2]; L.cyl = calib4[3];
+    L.fxli = 1.0f / L.fxl; L.fyli = 1.0f / L.fyl;   // CalibHessian::setValueScaled (HessianBlocks.h:435-436)
+    L.huber = s_.huber; L.min_h = min_idepth_h_act;
+    TDM_CUDA(cudaSetDevice(device_));
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));   // the staging buffers are free
+    reserve_activate(n_cand);
+    int* hc = h_act_cand_.get();
+    std::memcpy(hc, cand_frame, 4ull * n_cand);
+    std::memcpy(hc + n_cand, cand_index, 4ull * n_cand);
+    TDM_CUDA(cudaMemcpyAsync(d_act_cand_.get(), hc, 8ull * n_cand, cudaMemcpyHostToDevice, stream_.get()));
+    for (int f = 0; f < n_frames; ++f)
+      TDM_CUDA(cudaStreamWaitEvent(stream_.get(), (cudaEvent_t)frame_pyramids[f]->ready_event(), 0));
+    // output layout: result int[n], idepth float[n], energy float[n * n_frames], state int8[n * n_frames]
+    char* d = d_act_out_.get();
+    const size_t nn = (size_t)n_cand * n_frames, bytes = 8ull * n_cand + 5ull * nn;
+    k_activate<<<cdiv(n_cand, kActWarps), kActThreads, 0, stream_.get()>>>(
+        L, st_.get(), d_act_cand_.get(), reinterpret_cast<int*>(d), reinterpret_cast<float*>(d + 4ull * n_cand),
+        reinterpret_cast<float*>(d + 8ull * n_cand), reinterpret_cast<signed char*>(d + 8ull * n_cand + 4 * nn));
+    TDM_CUDA(cudaGetLastError());
+    TDM_CUDA(cudaMemcpyAsync(h_act_out_.get(), d, bytes, cudaMemcpyDeviceToHost, stream_.get()));
+    // a later build or destroy of a pyramid read here waits for the activation
+    TDM_CUDA(cudaEventRecord(done_.get(), stream_.get()));
+    for (int f = 0; f < n_frames; ++f) frame_pyramids[f]->wait_for(done_.get());
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
+    const char* h = h_act_out_.get();
+    if (result) std::memcpy(result, h, 4ull * n_cand);
+    if (idepth) std::memcpy(idepth, h + 4ull * n_cand, 4ull * n_cand);
+    if (res_energy) std::memcpy(res_energy, h + 8ull * n_cand, 4 * nn);
+    if (res_state) std::memcpy(res_state, h + 8ull * n_cand + 4 * nn, nn);
+  }
+
   int count(int slot) override { check_slot(slot); return count_[slot]; }
 
   void get(int slot, int first, int n, float* const* rows) override {
@@ -511,6 +748,19 @@ class ImmatureImpl final : public ImmatureIface {
     TDM_CHECK(p.width(0) == w_ && p.height(0) == h_, "pyramid level 0 is not the set's image size");
     TDM_CHECK(p.device() == device_, "pyramid and immature-point set live on different devices");
   }
+  // the activation's candidate and output buffers, made on first use for at least n candidates (at most every point of
+  // every slot); kept only once all of them exist.  The stream is idle when this runs.
+  void reserve_activate(int n) {
+    if (n <= act_cap_) return;
+    const int c = (int)std::min<long long>(std::max<long long>(n, 2ll * act_cap_), (long long)kSlots * cap_);
+    const size_t out = 8ull * c + 5ull * c * kSlots;
+    DevPtr<int> dc = make_dev<int>(8ull * c);
+    HostPtr<int> hc = make_host<int>(8ull * c);
+    DevPtr<char> dout = make_dev<char>(out);
+    HostPtr<char> hout = make_host<char>(out);
+    d_act_cand_ = std::move(dc); h_act_cand_ = std::move(hc); d_act_out_ = std::move(dout); h_act_out_ = std::move(hout);
+    act_cap_ = c;
+  }
   int w_, h_, cap_, device_;
   Settings s_;
   int count_[kSlots] = {};
@@ -520,6 +770,11 @@ class ImmatureImpl final : public ImmatureIface {
   DevPtr<int> d_cand_, d_added_;
   HostPtr<int> h_cand_, h_added_;
   HostPtr<float> h_rows_;
+  int act_cap_ = 0;
+  DevPtr<int> d_act_cand_;
+  HostPtr<int> h_act_cand_;
+  DevPtr<char> d_act_out_;
+  HostPtr<char> h_act_out_;
 };
 
 }  // namespace

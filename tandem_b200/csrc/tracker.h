@@ -166,6 +166,12 @@ class ImmatureIface {
   // host_pyramids (may be null, or hold nulls) are the hosts' pyramids the trace is ordered after and keeps alive
   virtual void trace(const PyramidIface& frame, int n_hosts, const int* slots, const PyramidIface* const* host_pyramids,
                      const float* KRKi, const float* Kt, const float* aff) = 0;
+  // n9: optimizeImmaturePoint for every candidate (cand_frame / cand_index) over the frames' level 0 (blocking, one host
+  // wait); frame_slots[f] is frame f's slot or -1, precalc n_frames x n_frames x 14, calib4 fxl fyl cxl cyl; outputs may be null
+  virtual void activate(int n_frames, const int* frame_slots, const PyramidIface* const* frame_pyramids, const float* precalc,
+                        const float* calib4, float min_idepth_h_act, int gn_iterations, int min_obs, int n_cand,
+                        const int* cand_frame, const int* cand_index, int* result, float* idepth, signed char* res_state,
+                        float* res_energy) = 0;
   virtual int count(int slot) = 0;
   // points first..first+n-1 of a slot, one output per ImmatureRow (null: not wanted); synchronises
   virtual void get(int slot, int first, int n, float* const* rows) = 0;

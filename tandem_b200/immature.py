@@ -1,11 +1,12 @@
 """n8: DSO's immature points of the active keyframes kept in device memory and traced into each new frame
 (FullSystem::traceNewCoarse, FullSystem.cpp:650-691; ImmaturePoint::traceOn, ImmaturePoint.cpp:75-414) over the C ABI
-(include/tandem_b200.h, block n8)."""
+(include/tandem_b200.h, block n8); n9: their activation solve (FullSystem::optimizeImmaturePoint,
+FullSystemOptPoint.cpp:51-205, for activatePointsMT's candidates)."""
 import ctypes
 
 import numpy as np
 
-from ._lib import TraceSettings, check, lib
+from ._lib import ActivateSettings, TraceSettings, check, lib
 
 _fp = ctypes.POINTER(ctypes.c_float)
 _ip = ctypes.POINTER(ctypes.c_int)
@@ -15,6 +16,8 @@ TRACE_DEFAULTS = dict(max_pix_search=0.027, trace_stepsize=1.0, trace_gn_thresho
                       trace_slack_interval=1.5, trace_min_improvement_factor=2.0, huber_th=9.0, outlier_th=144.0,
                       outlier_th_sum_component=2500.0, overall_energy_th_weight=1.0, min_trace_test_radius=2,
                       trace_gn_iterations=3)
+#: util/settings.cpp:62, 142 and activatePointsMT_Reductor's minObs
+ACTIVATE_DEFAULTS = dict(min_idepth_h_act=100.0, gn_iterations=3, min_obs=1)
 #: ImmaturePoint::lastTraceStatus
 IPS_GOOD, IPS_OOB, IPS_OUTLIER, IPS_SKIPPED, IPS_BADCONDITION, IPS_UNINITIALIZED = range(6)
 FIELDS = {"u": (), "v": (), "type": (), "energy_th": (), "color": (8,), "weights": (8,), "grad_h": (4,), "idepth_min": (),
@@ -95,3 +98,34 @@ class ImmaturePoints:
 
     def drop_host(self, slot):
         check(lib().tdm_immature_drop_host(self._h, slot))
+
+    def activate(self, frame_slots, frame_pyramids, precalc, calib, cand_frame, cand_index, min_idepth_h_act=100.0,
+                 gn_iterations=3, min_obs=1):
+        """optimizeImmaturePoint for every candidate (point cand_index[k] of frame cand_frame[k]'s slot) over the frames of
+        frameHessians: frame_slots[f] is frame f's slot or -1, frame_pyramids[f] its pyramid, precalc (n, n, 14) holds
+        [host][target] PRE_RTll (row-major), PRE_tTll and PRE_aff_mode, calib (fxl, fyl, cxl, cyl).  Blocking.  Returns
+        dict(result (n_cand,) int32 1 / 0 / -1, idepth (n_cand,) float32, res_state (n_cand, n_frames) int8 with -1 in the
+        host's column, res_energy (n_cand, n_frames) float32 with NaN there)."""
+        slots = np.ascontiguousarray(frame_slots, np.int32).ravel()
+        n = len(slots)
+        if len(frame_pyramids) != n:
+            raise ValueError("frame_slots and frame_pyramids differ in length")
+        pc = np.ascontiguousarray(precalc, np.float32)
+        if pc.size != n * n * 14:
+            raise ValueError("precalc must hold n_frames x n_frames x 14 floats")
+        cal = np.ascontiguousarray(calib, np.float32).ravel()
+        if cal.size != 4:
+            raise ValueError("calib must hold fxl, fyl, cxl, cyl")
+        cf = np.ascontiguousarray(cand_frame, np.int32).ravel()
+        ci = np.ascontiguousarray(cand_index, np.int32).ravel()
+        if len(cf) != len(ci):
+            raise ValueError("cand_frame and cand_index differ in length")
+        k = len(cf)
+        out = dict(result=np.empty(k, np.int32), idepth=np.empty(k, np.float32), res_state=np.empty((k, n), np.int8),
+                   res_energy=np.empty((k, n), np.float32))
+        fp = (ctypes.c_void_p * max(n, 1))(*[None if p is None else p._h.value for p in frame_pyramids])
+        st = ActivateSettings(min_idepth_h_act=min_idepth_h_act, gn_iterations=gn_iterations, min_obs=min_obs)
+        check(lib().tdm_immature_activate(self._h, n, _p(slots, _ip), fp, _p(pc), _p(cal), ctypes.byref(st), k, _p(cf, _ip),
+                                          _p(ci, _ip), _p(out["result"], _ip), _p(out["idepth"]),
+                                          _p(out["res_state"], ctypes.POINTER(ctypes.c_byte)), _p(out["res_energy"])))
+        return out

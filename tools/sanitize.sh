@@ -23,3 +23,4 @@ leg conv_is_mem $T1 memcheck tests/test_conv_is_gpu.py -k "abl04"
 leg feature_cache_mem $T1 memcheck tests/test_mvsnet_feature_cache_gpu.py -k "handoff or golden"
 leg feature_cache_race $T2 racecheck tests/test_mvsnet_feature_cache_gpu.py -k "handoff"
 leg trace_mem $T1 memcheck tests/test_trace_gpu.py -k "not shim and not random and not 2560"
+leg activate_mem $T1 memcheck tests/test_activate_gpu.py -k "not shim and not random"
