@@ -1,6 +1,6 @@
 // The immature points of DSO's active keyframes on the device (n8, include/tandem_b200.h): FullSystem::traceNewCoarse
 // (tandem/src/FullSystem/FullSystem.cpp:650-691) becomes one trace() call per frame.  Host slot = the keyframe's index among
-// the active ones (0..7); INTEGRATION.md shows the call sites.  activatePointsMT's solve (n9) becomes one activate() call.  Owns one tdm_immature handle; not copyable.
+// the active ones (0..7); INTEGRATION.md shows the call sites.  activatePointsMT's solve (n9) becomes one activate() call, makeNewTraces (n10) one makeNewTraces() call.  Owns one tdm_immature handle; not copyable.
 #ifndef TDM_CUDA_IMMATURE_POINTS_H
 #define TDM_CUDA_IMMATURE_POINTS_H
 
@@ -10,6 +10,7 @@
 
 struct tdm_immature;   // include/tandem_b200.h
 struct tdm_pyramid;
+class CudaPixelSelector;   // cuda_pixel_selector.h
 
 class CudaImmaturePoints {
  public:
@@ -23,6 +24,11 @@ class CudaImmaturePoints {
   // points were kept (those with a finite energyTH, in input order)
   int add(int host_slot, tdm_pyramid *host_pyramid, std::vector<int> const &u, std::vector<int> const &v,
           std::vector<float> const &type);
+  // n10: makeNewTraces (FullSystem.cpp:1623-1647) on the device: selector.makeMaps(fh, .., density) and the constructor for
+  // every selected pixel, appended in raster order; the map stays on the device.  u / v / type (may be null) receive the
+  // kept points.  Returns how many were kept.  Blocking.
+  int makeNewTraces(int host_slot, CudaPixelSelector &selector, tdm_pyramid *pyramid, float density, std::vector<int> *u = nullptr,
+                    std::vector<int> *v = nullptr, std::vector<float> *type = nullptr);
   // traceNewCoarse: traceOn of every point of the given hosts into the new frame, with KRKi, Kt and aff per host as
   // traceNewCoarse computes them (:655-669).  Asynchronous; get() waits for it.
   void trace(tdm_pyramid *frame_pyramid, std::vector<int> const &host_slots, std::vector<tdm_pyramid *> const &host_pyramids,
@@ -65,6 +71,7 @@ class CudaImmaturePoints {
 
  private:
   tdm_immature *handle_ = nullptr;
+  int capacity_ = 0;
 };
 
 #endif

@@ -542,6 +542,66 @@ int tdm_immature_activate(tdm_immature* s, int n_frames, const int* frame_slots,
                           const int* cand_frame, const int* cand_index, int* result, float* idepth, signed char* res_state,
                           float* res_energy);
 
+/* n10  DSO's pixel selection on the device: PixelSelector (tandem/src/FullSystem/PixelSelector2.cpp:41-438) - makeHists
+ *     (:78-141), select (:295-438) and makeMaps (:142-291) - on a tdm_pyramid's levels 0..2, and FullSystem::makeNewTraces
+ *     (FullSystem.cpp:1623-1647) into a set slot.  Every float operation is the reference's, correctly rounded and in its
+ *     order; the random pattern is glibc's rand() & 0xFF after srand(3141592), as the constructor makes it (:43-45), computed
+ *     without touching the process's rand state.  The selection reads absSquaredGrad without gamma weights: the reference's
+ *     setting_gammaWeightsPixelSelect 1 multiplies it by gw * gw (HessianBlocks.cpp:184-188), which is exactly 1 for a linear
+ *     response (B[i] = i, no photometric calibration), the contract here.
+ *     The two definitional differences, reads of memory the reference never writes:
+ *     - select reads level 2's last row at yf == h - 4 for every h; makeImages writes only rows 1..h2-2
+ *       (HessianBlocks.cpp:169).  The pyramid holds 0 there, and that 0 is read.
+ *     - thsSmoothed flat indices at or beyond w32 * h32 are uninitialised in the reference (`new float[...]`); select reaches
+ *       them iff w % 32 >= 6 or h % 32 >= 4 (752 x 480 does, 640 x 480 does not).  They read 0.  Indices inside the array
+ *       that wrap to the next row ((xf >> 5) == w32) are the reference's. */
+typedef struct tdm_select_settings {
+  float min_grad_hist_cut;            /* setting_minGradHistCut, 0.5; at most 0.99 */
+  float min_grad_hist_add;            /* setting_minGradHistAdd, 7 */
+  float grad_downweight_per_level;    /* setting_gradDownweightPerLevel, 0.75 */
+  int select_direction_distribution;  /* setting_selectDirectionDistribution, 1 (0 or 1) */
+} tdm_select_settings;
+typedef struct tdm_select_result {
+  int num_selected;     /* makeMaps' return value: the selected pixels after the subsample */
+  int n2, n3, n4;       /* the final select's counts of type 1, 2 and 4 (before the subsample) */
+  int potential_used;   /* the potential the final select ran with */
+  int potential_after;  /* currentPotential after the call */
+  int reselected;       /* 1 when makeMaps selected again with another potential (:198-228) */
+  int nonuniform_cells; /* cells of the final select whose level-2 selection depends on their direction (DESIGN.md, n10) */
+} tdm_select_result;
+typedef struct tdm_selector tdm_selector;
+/* One PixelSelector of a w x h camera (w / 32 and h / 32 at least 1); currentPotential starts at 3.  settings NULL: the
+ *     defaults above.  Invalid settings are an error. */
+int tdm_selector_create(int w, int h, const tdm_select_settings* settings, int device, tdm_selector** out);
+/* Waits for the selector's pending work. */
+void tdm_selector_destroy(tdm_selector* s);
+/* currentPotential (PixelSelector2.h:47); CoarseInitializer::setFirst sets it to 3 (CoarseInitializer.cpp:781).  A potential
+ *     below 1 is an error. */
+int tdm_selector_get_potential(tdm_selector* s, int* potential);
+int tdm_selector_set_potential(tdm_selector* s, int potential);
+/* PixelSelector::makeMaps(fh, map_out, density, recursions_left, false, th_factor) on pyramid's levels 0..2: select with the
+ *     current potential, re-select with a smaller one (quotia = density / selected > 1.25, potential > 1) or a larger one
+ *     (quotia < 0.25) while recursions are left, subsample to quotia below 0.95 with the pattern, and set currentPotential to
+ *     the ideal one.  The re-selection decision is made on the device.  map_out (NULL or a host w*h float map) receives
+ *     0 / 1 / 2 / 4 per pixel; *out (may be NULL) the counts and potentials.  Blocking (one host wait), after the pyramid's
+ *     build; a later tdm_pyramid_build or tdm_pyramid_destroy waits for it.  Invalid input (null handles, a pyramid with
+ *     fewer than 3 levels or of another level-0 size or device, a density negative or not finite, recursions_left outside
+ *     0..16, th_factor not finite or <= 0) is an error and launches nothing. */
+int tdm_selector_make_maps(tdm_selector* s, tdm_pyramid* pyramid, float density, int recursions_left, float th_factor,
+                           float* map_out, tdm_select_result* out);
+/* FullSystem::makeNewTraces (FullSystem.cpp:1623-1647) without the RGB-D gtDepth branch: makeMaps (recursions 1, thFactor 1)
+ *     and the ImmaturePoint constructor (as tdm_immature_add) for every selected pixel of [3, w-4) x [3, h-4) in raster
+ *     order with type = its map value; the points with a finite energyTH are appended to host_slot behind its points, in
+ *     that order.  The map never leaves the device.  *out and *n_added (may be NULL) receive the selection and the number
+ *     kept; u / v / type (NULL, or the slot's free capacity before the call) the kept points, so the host can build its own
+ *     ImmaturePoints.  Blocking (one host wait), on the set's stream after its pending work and the pyramid's build; a later
+ *     tdm_pyramid_build or tdm_pyramid_destroy waits for it.  Invalid input (what tdm_selector_make_maps rejects, a slot
+ *     outside 0..7, a selector or pyramid of another size or device than the set) is an error and launches nothing.  Kept
+ *     points beyond the slot's free capacity are an error found after the launch: the set and the potential are then
+ *     unchanged. */
+int tdm_immature_make_new_traces(tdm_immature* set, int host_slot, tdm_selector* sel, tdm_pyramid* pyramid, float density,
+                                 tdm_select_result* out, int* n_added, int* u, int* v, float* type);
+
 #ifdef __cplusplus
 }
 #endif

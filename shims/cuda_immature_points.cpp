@@ -1,5 +1,6 @@
 // CudaImmaturePoints over the tandem_b200 C ABI.  Errors throw std::runtime_error, as the tracker shim's do.
 #include "cuda_coarse_tracker/cuda_immature_points.h"
+#include "cuda_coarse_tracker/cuda_pixel_selector.h"
 
 #include <stdexcept>
 #include <string>
@@ -10,7 +11,7 @@ static void chk(int rc, const char *where) {
   if (rc != TDM_OK) throw std::runtime_error(std::string(where) + ": " + tdm_last_error());
 }
 
-CudaImmaturePoints::CudaImmaturePoints(int w, int h, int capacity_per_host, int device) {
+CudaImmaturePoints::CudaImmaturePoints(int w, int h, int capacity_per_host, int device) : capacity_(capacity_per_host) {
   chk(tdm_immature_create(w, h, capacity_per_host, nullptr, device, &handle_), "CudaImmaturePoints");
 }
 
@@ -22,6 +23,25 @@ int CudaImmaturePoints::add(int host_slot, tdm_pyramid *host_pyramid, std::vecto
   int n = 0;
   chk(tdm_immature_add(handle_, host_slot, host_pyramid, (int)u.size(), u.data(), v.data(), type.data(), &n),
       "CudaImmaturePoints::add");
+  return n;
+}
+
+int CudaImmaturePoints::makeNewTraces(int host_slot, CudaPixelSelector &selector, tdm_pyramid *pyramid, float density,
+                                      std::vector<int> *u, std::vector<int> *v, std::vector<float> *type) {
+  int free = 0, count = 0;
+  chk(tdm_immature_get(handle_, host_slot, 0, 0, &count, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                       nullptr, nullptr, nullptr, nullptr, nullptr),
+      "CudaImmaturePoints::makeNewTraces");
+  free = capacity_ - count;
+  std::vector<int> uu(free > 0 ? free : 0), vv(uu.size());
+  std::vector<float> tt(uu.size());
+  int n = 0;
+  chk(tdm_immature_make_new_traces(handle_, host_slot, selector.handle(), pyramid, density, nullptr, &n, uu.data(), vv.data(),
+                                   tt.data()),
+      "CudaImmaturePoints::makeNewTraces");
+  if (u) u->assign(uu.begin(), uu.begin() + n);
+  if (v) v->assign(vv.begin(), vv.begin() + n);
+  if (type) type->assign(tt.begin(), tt.begin() + n);
   return n;
 }
 

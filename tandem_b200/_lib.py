@@ -49,6 +49,18 @@ class ActivateSettings(ctypes.Structure):
     _fields_ = [("min_idepth_h_act", ctypes.c_float), ("gn_iterations", ctypes.c_int), ("min_obs", ctypes.c_int)]
 
 
+class SelectSettings(ctypes.Structure):
+    """tdm_select_settings (include/tandem_b200.h): the reference's constants of PixelSelector."""
+    _fields_ = [("min_grad_hist_cut", ctypes.c_float), ("min_grad_hist_add", ctypes.c_float),
+                ("grad_downweight_per_level", ctypes.c_float), ("select_direction_distribution", ctypes.c_int)]
+
+
+class SelectResult(ctypes.Structure):
+    """tdm_select_result (include/tandem_b200.h)."""
+    _fields_ = [(k, ctypes.c_int) for k in ("num_selected", "n2", "n3", "n4", "potential_used", "potential_after", "reselected",
+                                            "nonuniform_cells")]
+
+
 CONV_PLAN_KEYS = ("S", "R", "TW", "P", "DR", "nch", "slot_pos", "tiles_w", "tiles_h", "tiles_d", "grid", "smem", "nwg")
 
 
@@ -196,6 +208,12 @@ def _declare(l):
         "tdm_immature_drop_host": (i, [vp, i]),
         "tdm_immature_activate": (i, [vp, i, ip, P(vp), fp, fp, P(ActivateSettings), i, ip, ip, ip, fp,
                                       ctypes.POINTER(ctypes.c_byte), fp]),
+        "tdm_selector_create": (i, [i, i, P(SelectSettings), i, P(vp)]),
+        "tdm_selector_destroy": (None, [vp]),
+        "tdm_selector_get_potential": (i, [vp, ip]),
+        "tdm_selector_set_potential": (i, [vp, i]),
+        "tdm_selector_make_maps": (i, [vp, vp, f, i, f, fp, P(SelectResult)]),
+        "tdm_immature_make_new_traces": (i, [vp, i, vp, vp, f, P(SelectResult), ip, ip, ip, fp]),
     }
     missing = []
     for name, (res, args) in sigs.items():

@@ -9,6 +9,9 @@
 #include "fusion.h"
 #include "tracker.h"
 
+static_assert(sizeof(tdm_select_result) == sizeof(tdm::SelectResult), "tdm_select_result layout");
+static_assert(sizeof(tdm_select_settings) == 16, "tdm_select_settings layout");
+
 struct tdm_tracker {
   tdm::TrackerIface* impl;
 };
@@ -17,6 +20,9 @@ struct tdm_pyramid {
 };
 struct tdm_immature {
   tdm::ImmatureIface* impl;
+};
+struct tdm_selector {
+  tdm::SelectorIface* impl;
 };
 struct tdm_fusion {   // same layout as in capi_fusion.cu (one pointer)
   tdm::FusionIface* impl;
@@ -461,6 +467,53 @@ int tdm_immature_activate(tdm_immature* s, int n_frames, const int* frame_slots,
   }
   s->impl->activate(n_frames, frame_slots, fp, precalc, calib4, st.min_idepth_h_act, st.gn_iterations, st.min_obs, n_cand,
                     cand_frame, cand_index, result, idepth, res_state, res_energy);
+  return TDM_OK;
+  TDM_API_END
+}
+
+/* ---- n10: PixelSelector::makeMaps and makeNewTraces on the device ---- */
+int tdm_selector_create(int w, int h, const tdm_select_settings* settings, int device, tdm_selector** out) {
+  TDM_API_BEGIN
+  TDM_CHECK(out, "null argument");
+  static const tdm_select_settings defaults = {0.5f, 7.f, 0.75f, 1};
+  *out = new tdm_selector{tdm::make_selector(w, h, (const float*)(settings ? settings : &defaults), device)};
+  return TDM_OK;
+  TDM_API_END
+}
+void tdm_selector_destroy(tdm_selector* s) {
+  if (!s) return;
+  try { delete s->impl; } catch (...) {}
+  delete s;
+}
+int tdm_selector_get_potential(tdm_selector* s, int* potential) {
+  TDM_API_BEGIN
+  TDM_CHECK(s && potential, "null argument");
+  *potential = s->impl->potential();
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_selector_set_potential(tdm_selector* s, int potential) {
+  TDM_API_BEGIN
+  TDM_CHECK(s, "null handle");
+  s->impl->set_potential(potential);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_selector_make_maps(tdm_selector* s, tdm_pyramid* pyramid, float density, int recursions_left, float th_factor,
+                           float* map_out, tdm_select_result* out) {
+  TDM_API_BEGIN
+  TDM_CHECK(s && pyramid, "null argument");
+  s->impl->make_maps(*pyramid->impl, density, recursions_left, th_factor, map_out, reinterpret_cast<tdm::SelectResult*>(out));
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_immature_make_new_traces(tdm_immature* set, int host_slot, tdm_selector* sel, tdm_pyramid* pyramid, float density,
+                                 tdm_select_result* out, int* n_added, int* u, int* v, float* type) {
+  TDM_API_BEGIN
+  TDM_CHECK(set && sel && pyramid, "null argument");
+  const int n = set->impl->make_new_traces(host_slot, *sel->impl, *pyramid->impl, density,
+                                           reinterpret_cast<tdm::SelectResult*>(out), u, v, type);
+  if (n_added) *n_added = n;
   return TDM_OK;
   TDM_API_END
 }

@@ -294,16 +294,19 @@ __global__ void __launch_bounds__(128) k_trace(TraceLaunch L, uint32_t* __restri
   }
 }
 
-// The constructor for n candidate pixels of one slot; the points with a finite energyTH are appended in input order
-// behind the slot's `count` points, and *added receives their number.  One block.
+// The constructor for n candidate pixels of one slot (u at cand[c], v at cand[cs + c], the type's bits at cand[2 cs + c];
+// n read from n_dev when it is given); the points with a finite energyTH are appended in input order behind the slot's
+// `count` points, up to the slot's capacity, and *added receives the number kept, those beyond the capacity included.
+// One block.
 constexpr int kAddThreads = 256;
 __global__ void __launch_bounds__(kAddThreads) k_add(Settings S, uint32_t* __restrict__ st, int cap, int slot, int count,
-                                                     const float* __restrict__ dI, int w, int n, const int* __restrict__ cand,
-                                                     int* __restrict__ added) {
+                                                     const float* __restrict__ dI, int w, int n, const int* __restrict__ n_dev,
+                                                     int cs, const int* __restrict__ cand, int* __restrict__ added) {
   using Scan = cub::BlockScan<int, kAddThreads>;
   __shared__ typename Scan::TempStorage tmp;
   const size_t stride = (size_t)kSlots * cap;
   float* f = reinterpret_cast<float*>(st);
+  if (n_dev) n = *n_dev;
   int base = count;
   for (int c0 = 0; c0 < n; c0 += kAddThreads) {
     const int c = c0 + threadIdx.x;
@@ -311,7 +314,7 @@ __global__ void __launch_bounds__(kAddThreads) k_add(Settings S, uint32_t* __res
     int ok = 0, u = 0, v = 0;
     float type = 0.f;
     if (c < n) {
-      u = cand[c]; v = cand[n + c]; type = __int_as_float(cand[2 * n + c]);
+      u = cand[c]; v = cand[cs + c]; type = __int_as_float(cand[2 * cs + c]);
       ok = 1;
       for (int k = 0; k < 8; ++k) {
         // getInterpolatedElement33BiLin (globalFuncs.h:166-188) at integer coordinates
@@ -333,7 +336,7 @@ __global__ void __launch_bounds__(kAddThreads) k_add(Settings S, uint32_t* __res
     }
     int pos, tot;
     Scan(tmp).ExclusiveSum(ok, pos, tot);
-    if (ok) {
+    if (ok && base + pos < cap) {
       const size_t p = (size_t)slot * cap + base + pos;
       float eth = fm(8.f, S.outlier_th);
       eth = fm(eth, fm(S.overall_energy_th_weight, S.overall_energy_th_weight));
@@ -584,8 +587,8 @@ class ImmatureImpl final : public ImmatureIface {
     std::memcpy(h_cand_.get() + 2 * n, type, 4ull * n);
     TDM_CUDA(cudaMemcpyAsync(d_cand_.get(), h_cand_.get(), 12ull * n, cudaMemcpyHostToDevice, stream_.get()));
     TDM_CUDA(cudaStreamWaitEvent(stream_.get(), (cudaEvent_t)host.ready_event(), 0));
-    k_add<<<1, kAddThreads, 0, stream_.get()>>>(s_, st_.get(), cap_, slot, count_[slot], host.level_dI(0), w_, n, d_cand_.get(),
-                                                d_added_.get());
+    k_add<<<1, kAddThreads, 0, stream_.get()>>>(s_, st_.get(), cap_, slot, count_[slot], host.level_dI(0), w_, n, nullptr, n,
+                                                d_cand_.get(), d_added_.get());
     TDM_CUDA(cudaGetLastError());
     TDM_CUDA(cudaMemcpyAsync(h_added_.get(), d_added_.get(), 4, cudaMemcpyDeviceToHost, stream_.get()));
     TDM_CUDA(cudaStreamSynchronize(stream_.get()));
@@ -685,6 +688,43 @@ class ImmatureImpl final : public ImmatureIface {
     if (idepth) std::memcpy(idepth, h + 4ull * n_cand, 4ull * n_cand);
     if (res_energy) std::memcpy(res_energy, h + 8ull * n_cand, 4 * nn);
     if (res_state) std::memcpy(res_state, h + 8ull * n_cand + 4 * nn, nn);
+  }
+
+  int make_new_traces(int slot, SelectorIface& sel, const PyramidIface& p, float density, SelectResult* r, int* u, int* v,
+                      float* type) override {
+    check_slot(slot);
+    check_pyramid(p);
+    TDM_CHECK(sel.width() == w_ && sel.height() == h_, "pixel selector and immature-point set differ in image size");
+    TDM_CHECK(sel.device() == device_, "pixel selector and immature-point set live on different devices");
+    sel.check(p, density, 1, 1.f);
+    TDM_CUDA(cudaSetDevice(device_));
+    const int count = count_[slot], free = cap_ - count;
+    sel.enqueue(stream_.get(), p, density, 1, 1.f, true);
+    const SelectorIface::Candidates c = sel.candidates();
+    k_add<<<1, kAddThreads, 0, stream_.get()>>>(s_, st_.get(), cap_, slot, count, p.level_dI(0), w_, 0, c.count, c.stride, c.cand,
+                                                d_added_.get());
+    TDM_CUDA(cudaGetLastError());
+    TDM_CUDA(cudaMemcpyAsync(h_added_.get(), d_added_.get(), 4, cudaMemcpyDeviceToHost, stream_.get()));
+    // rows IM_U, IM_V, IM_TYPE of the slot's free part
+    if ((u || v || type) && free > 0)
+      TDM_CUDA(cudaMemcpy2DAsync(h_rows_.get(), 4ull * free, st_.get() + (size_t)slot * cap_ + count, 4ull * kSlots * cap_, 4ull * free,
+                                 3, cudaMemcpyDeviceToHost, stream_.get()));
+    // a later build or destroy of the pyramid waits for the call
+    TDM_CUDA(cudaEventRecord(done_.get(), stream_.get()));
+    p.wait_for(done_.get());
+    TDM_CUDA(cudaStreamSynchronize(stream_.get()));
+    const int added = *h_added_;
+    TDM_CHECK(added <= free, "make_new_traces: the slot's free capacity cannot hold the kept points");
+    SelectResult tmp;
+    sel.result(r ? r : &tmp, true);
+    count_[slot] += added;
+    const float* rows = h_rows_.get();
+    for (int i = 0; i < added; ++i) {
+      if (u) u[i] = (int)rows[i];
+      if (v) v[i] = (int)rows[free + i];
+      if (type) type[i] = rows[2 * free + i];
+    }
+    return added;
   }
 
   int count(int slot) override { check_slot(slot); return count_[slot]; }

@@ -1804,6 +1804,7 @@ class PyramidImpl final : public PyramidIface {
     TDM_CUDA(cudaStreamSynchronize(stream_.get()));
   }
   const float* level_dI(int lvl) const override { return d_dI_.get() + 3 * off_.at(lvl); }
+  const float* level_abs(int lvl) const override { return d_abs_.get() + off_.at(lvl); }
   void* ready_event() const override { return (void*)ready_.get(); }
   void wait_for(void* event) const override {
     TDM_CUDA(cudaSetDevice(device_));

@@ -143,6 +143,7 @@ class PyramidIface {
   virtual void build(const float* gray_host) = 0;
   virtual void get_level(int lvl, float* dI_host, float* absgrad_host) = 0;
   virtual const float* level_dI(int lvl) const = 0;   // device pointer, float3 per pixel
+  virtual const float* level_abs(int lvl) const = 0;  // device pointer, absSquaredGrad
   virtual void* ready_event() const = 0;              // cudaEvent_t recorded after build()
   // orders the next build() (and the destructor) after `event` (a cudaEvent_t a reader recorded behind its reads)
   virtual void wait_for(void* event) const = 0;
@@ -152,6 +153,37 @@ class PyramidIface {
   virtual int device() const = 0;
 };
 PyramidIface* make_pyramid(int w, int h, int levels, int device);
+
+// n10 (pixsel.cu): PixelSelector::makeMaps on a pyramid's levels 0..2 (tdm_select_result's layout)
+struct SelectResult {
+  int num_selected, n2, n3, n4, potential_used, potential_after, reselected, nonuniform_cells;
+};
+class SelectorIface {
+ public:
+  virtual ~SelectorIface() = default;
+  virtual int potential() const = 0;
+  virtual void set_potential(int p) = 0;
+  // blocking makeMaps; map_out (host, w*h) may be null
+  virtual void make_maps(const PyramidIface& p, float density, int recursions_left, float th_factor, float* map_out,
+                         SelectResult* r) = 0;
+  // what make_maps and enqueue reject
+  virtual void check(const PyramidIface& p, float density, int recursions_left, float th_factor) const = 0;
+  // makeMaps on `stream` (a cudaStream_t) after the pyramid's build, the map kept on the device; with emit also
+  // makeNewTraces' candidates (candidates()).  The result is copied to host memory that result() reads once the stream has
+  // been synchronised; result(commit) then sets the potential to the call's.
+  virtual void enqueue(void* stream, const PyramidIface& p, float density, int recursions_left, float th_factor, bool emit) = 0;
+  struct Candidates {
+    const int* cand;    // u at cand[k], v at cand[stride + k], the type's float bits at cand[2 stride + k]
+    int stride;
+    const int* count;   // device
+  };
+  virtual Candidates candidates() const = 0;
+  virtual void result(SelectResult* r, bool commit) = 0;
+  virtual int width() const = 0;
+  virtual int height() const = 0;
+  virtual int device() const = 0;
+};
+SelectorIface* make_selector(int w, int h, const float* settings /* tdm_select_settings */, int device);
 
 // n8 (immature.cu): the immature points of up to 8 host keyframes (slots) and their trace into new frames.  Each field is a
 // row of 32-bit words, one per point; status is an int, the others floats.
@@ -172,6 +204,11 @@ class ImmatureIface {
                         const float* calib4, float min_idepth_h_act, int gn_iterations, int min_obs, int n_cand,
                         const int* cand_frame, const int* cand_index, int* result, float* idepth, signed char* res_state,
                         float* res_energy) = 0;
+  // n10: makeNewTraces - makeMaps (recursions 1, thFactor 1) and the constructor for every selected pixel of
+  // [3, w-4) x [3, h-4), appended to the slot in raster order (blocking, one host wait); u / v / type (may be null) receive
+  // the kept points.  Kept points beyond the slot's free capacity are an error; the set and the potential are then unchanged.
+  virtual int make_new_traces(int slot, SelectorIface& sel, const PyramidIface& p, float density, SelectResult* r, int* u, int* v,
+                              float* type) = 0;
   virtual int count(int slot) = 0;
   // points first..first+n-1 of a slot, one output per ImmatureRow (null: not wanted); synchronises
   virtual void get(int slot, int first, int n, float* const* rows) = 0;

@@ -1,12 +1,13 @@
 """n8: DSO's immature points of the active keyframes kept in device memory and traced into each new frame
 (FullSystem::traceNewCoarse, FullSystem.cpp:650-691; ImmaturePoint::traceOn, ImmaturePoint.cpp:75-414) over the C ABI
 (include/tandem_b200.h, block n8); n9: their activation solve (FullSystem::optimizeImmaturePoint,
-FullSystemOptPoint.cpp:51-205, for activatePointsMT's candidates)."""
+FullSystemOptPoint.cpp:51-205, for activatePointsMT's candidates); n10: a new keyframe's points selected and constructed on the
+device (FullSystem::makeNewTraces, FullSystem.cpp:1623-1647)."""
 import ctypes
 
 import numpy as np
 
-from ._lib import ActivateSettings, TraceSettings, check, lib
+from ._lib import ActivateSettings, SelectResult, TraceSettings, check, lib
 
 _fp = ctypes.POINTER(ctypes.c_float)
 _ip = ctypes.POINTER(ctypes.c_int)
@@ -36,6 +37,7 @@ class ImmaturePoints:
         if unknown:
             raise TypeError(f"unknown trace settings {sorted(unknown)}")
         self.w, self.h = w, h
+        self._capacity = capacity_per_host
         self.settings = dict(TRACE_DEFAULTS, **settings)
         st = TraceSettings(**self.settings)
         self._h = ctypes.c_void_p()
@@ -75,6 +77,20 @@ class ImmaturePoints:
         if host_pyramids is not None:
             hp = (ctypes.c_void_p * n)(*[None if p is None else p._h.value for p in host_pyramids])
         check(lib().tdm_immature_trace(self._h, frame_pyramid._h, n, _p(slots, _ip), hp, _p(K), _p(t), _p(a)))
+
+    def make_new_traces(self, slot, selector, pyramid, density=1500.0):
+        """makeNewTraces: selector.make_maps on pyramid (recursions 1, thFactor 1) and the constructor for every selected pixel
+        of [3, w-4) x [3, h-4), appended to the slot in raster order; the map stays on the device.  Blocking.  Returns
+        dict(n_added, u, v, type (the kept points), result (PixelSelector.make_maps' dict))."""
+        free = self._capacity - self.count(slot)
+        u, v = np.empty(max(free, 0), np.int32), np.empty(max(free, 0), np.int32)
+        t = np.empty(max(free, 0), np.float32)
+        r, n = SelectResult(), ctypes.c_int()
+        check(lib().tdm_immature_make_new_traces(self._h, slot, selector._h, pyramid._h, density, ctypes.byref(r), ctypes.byref(n),
+                                                 _p(u, _ip), _p(v, _ip), _p(t)))
+        k = n.value
+        return dict(n_added=k, u=u[:k].copy(), v=v[:k].copy(), type=t[:k].copy(),
+                    result={f: getattr(r, f) for f, _ in SelectResult._fields_})
 
     def count(self, slot):
         c = ctypes.c_int()
