@@ -239,6 +239,10 @@ int tdm_debug_mesh_axis_table(float lower, float upper, float voxel_size, int* i
  * remainder (precomputed ceil(2^64 / num_buckets)) - and, in *reference_expression when non-NULL, the reference's expression
  * ((x * 73856093) ^ (y * 19349669) ^ (z * 83492791)) % num_buckets, + num_buckets when negative (hash_table.cu:157-168). */
 int tdm_debug_hash_slot(int x, int y, int z, int num_buckets, int* reference_expression);
+/* Host-only introspection (no GPU needed): 1 when the option "fast_div" takes effect for these divisors, 0 when the host keeps
+ * the IEEE division (a divisor with an all-ones significand, or one so small or large that an intermediate could under- or
+ * overflow, is not correctly rounded by the constant-divisor sequence). */
+int tdm_debug_fast_div_eligible(float voxel_size, float fx, float fy);
 /* Device time (CUDA events) of the last extraction: classify + scan + emit. */
 int tdm_fusion_last_mesh_ms(tdm_fusion* h, float* ms);
 /* Introspection for parity tests and the roofline: counters of the last integrate / render. */

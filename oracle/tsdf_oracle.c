@@ -17,7 +17,8 @@
  * decisions (pixel indices, voxel indices, weights) are bit-identical.
  * Deviations from the letter of the reference, all documented in DESIGN.md: the camera-pose inverse is a
  * 2x2-sub-determinant fp32 inverse (not the 16-cofactor one, matrix_utils.h:958-1080); a voxel whose camera
- * z is exactly 0 is skipped (the reference divides by it).
+ * z is exactly 0 is skipped (the reference divides by it); a NaN depth pixel is ignored (the reference's allocation DDA
+ * never ends on one).
  */
 #include <math.h>
 #include <float.h>
@@ -215,7 +216,8 @@ static void allocate_from_depth(Tsdf* t, const float* depth, const float* T) { /
   long before = t->allocated;
   int n = o->height * o->width;
   for (int i = 0; i < n; ++i) {
-    if (depth[i] < o->min_sensor_depth || depth[i] > o->max_sensor_depth) continue;
+    /* documented deviation: NaN depth is rejected (the reference's `< min || > max` lets it into a DDA that never ends) */
+    if (!(depth[i] >= o->min_sensor_depth && depth[i] <= o->max_sensor_depth)) continue;
     f3 pu = get_point3d(o, i, depth[i]);
     f3 p = xform(T, pu);
     if (p.x == 0 && p.y == 0 && p.z == 0) continue;
@@ -281,9 +283,7 @@ static void integrate(Tsdf* t, const unsigned char* bgr, const float* depth, con
           if (!(px >= 0 && py >= 0 && px < o->width && py < o->height)) continue;
           int idx = py * o->width + px;
           float dz = depth[idx];
-          if (dz <= 0) continue;
-          if (dz < o->min_sensor_depth) continue;
-          if (dz > o->max_sensor_depth) continue;
+          if (!(dz > 0 && dz >= o->min_sensor_depth && dz <= o->max_sensor_depth)) continue; /* NaN fails it */
           f3 p3 = get_point3d(o, idx, dz);
           float sd = norm3(p3), vd = norm3(vc);
           float nsdf;

@@ -168,6 +168,7 @@ def _declare(l):
         "tdm_fusion_stream": (i, [vp, P(vp)]),
         "tdm_debug_mesh_axis_table": (i, [f, f, f, ip, fp, ip, ip, i]),
         "tdm_debug_hash_slot": (i, [i, i, i, i, ip]),
+        "tdm_debug_fast_div_eligible": (i, [f, f, f]),
         "tdm_fusion_set_option": (i, [vp, cp, i]),
         "tdm_fusion_last_alloc_ms": (i, [vp, fp]),
         "tdm_fusion_get_stats": (i, [vp, P(FusionStats)]),

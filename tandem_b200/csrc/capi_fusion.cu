@@ -152,6 +152,11 @@ int tdm_debug_hash_slot(int x, int y, int z, int num_buckets, int* reference_exp
   return tdm::hash_slot_host(x, y, z, num_buckets, reference_expression);
   TDM_API_END
 }
+int tdm_debug_fast_div_eligible(float voxel_size, float fx, float fy) {
+  TDM_API_BEGIN
+  return tdm::fast_div_eligible_host(voxel_size, fx, fy);
+  TDM_API_END
+}
 int tdm_fusion_set_option(tdm_fusion* h, const char* name, int value) {
   TDM_API_BEGIN
   TDM_CHECK(h && name, "null argument");

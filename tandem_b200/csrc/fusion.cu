@@ -217,7 +217,9 @@ __global__ void __launch_bounds__(128) k_allocate(FusionDev d, const float* __re
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float dz = depth[i];
-  if (dz < o.min_sensor_depth || dz > o.max_sensor_depth) return;
+  // written so that NaN fails it (the reference's `dz < min || dz > max` lets NaN through: its DDA then gets step 0 and never
+  // ends; DESIGN.md, "TSDF options").  +-inf fall outside the range either way.
+  if (!(dz >= o.min_sensor_depth && dz <= o.max_sensor_depth)) return;
   const float bs = mul_((float)o.block_size, o.voxel_size);
   const float3 start = make_float3(T.m[3], T.m[7], T.m[11]);
   const float3 p = xform(T, get_point3d(o, i, dz));
@@ -338,7 +340,7 @@ k_integrate_list(FusionDev d, const unsigned char* __restrict__ bgr, const float
       if (!(px.x >= 0 && px.y >= 0 && px.x < o.width && px.y < o.height)) continue;
       const int idx = px.y * o.width + px.x;
       const float dz = depth[idx];
-      if (dz <= 0 || dz < o.min_sensor_depth || dz > o.max_sensor_depth) continue;
+      if (!(dz > 0 && dz >= o.min_sensor_depth && dz <= o.max_sensor_depth)) continue;   // NaN fails it, as in K5
       const float sd = norm3(get_point3d(o, idx, dz)), vd = norm3(vc);
       float nsdf;
       if (vd > sub_(sd, tau) && vd < add_(sd, tau) && dz < o.max_sensor_depth) nsdf = sub_(sd, vd);
@@ -766,12 +768,39 @@ MeshAxisHost build_mesh_axis(float lower, float upper, float s) {
   return A;
 }
 
+// cdiv_ is correctly rounded for d (Markstein) unless d's significand is all ones or an intermediate can under- / overflow
+bool fast_div_divisor_ok(float d) {
+  unsigned u;
+  std::memcpy(&u, &d, 4);
+  const unsigned ex = (u >> 23) & 0xFF, man = u & 0x7FFFFF;
+  return d > 0.f && ex > 40 && ex < 214 && man != 0x7FFFFF;   // 2^-87 < d < 2^87, significand not all ones
+}
+bool fast_div_eligible(float voxel_size, float fx, float fy) {
+  return fast_div_divisor_ok(voxel_size) && fast_div_divisor_ok(fx) && fast_div_divisor_ok(fy);
+}
+
+// The ray-casts stop a ray after 100000 steps (the guard of tsdf_volume.cu's march as the oracle restates it).  The production
+// kernel advances over the clipped prefix of a ray without counting those steps, so once a ray can take that many steps it
+// would end differently from the comparator and the oracle.  Every step that does not end a ray adds at least
+// min(truncation_distance, voxel_size) to it (an empty sample adds tau, a weighted one with sdf >= voxel_size adds sdf), so
+// max_sensor_depth / min(tau, voxel_size) <= 50000 keeps every ray under half the guard, fp32 rounding of the sums included.
+constexpr float kMaxMarchSteps = 50000.f;
+void check_march_options(const tdm_fusion_options& o) {
+  TDM_CHECK(std::isfinite(o.voxel_size) && o.voxel_size > 0.f, "voxel_size must be positive and finite");
+  TDM_CHECK(std::isfinite(o.truncation_distance) && o.truncation_distance > 0.f, "truncation_distance must be positive and finite");
+  TDM_CHECK(std::isfinite(o.max_sensor_depth) && std::isfinite(o.min_sensor_depth), "sensor depth limits must be finite");
+  TDM_CHECK(o.max_sensor_depth / std::min(o.voxel_size, o.truncation_distance) <= kMaxMarchSteps,
+            "max_sensor_depth / min(voxel_size, truncation_distance) must not exceed 50000 (a ray would reach the ray-cast's "
+            "100000-step guard)");
+}
+
 }  // namespace
 
 // ================================================================================================
 class FusionImpl final : public FusionIface {
  public:
   FusionImpl(const tdm_fusion_options& o, int device) : device_(device) {
+    check_march_options(o);
     int nd = 0;
     if (cudaGetDeviceCount(&nd) != cudaSuccess || nd == 0)
       throw Error("tandem_b200: no CUDA device visible - this library has no CPU fallback");
@@ -791,13 +820,7 @@ class FusionImpl final : public FusionIface {
       d_.r_vs = one / o.voxel_size; d_.r_fx = one / o.fx; d_.r_fy = one / o.fy;
       volatile float two = 2.0f;
       d_.half_vs = o.voxel_size / two;
-      auto ok = [](float d) {
-        unsigned u;
-        std::memcpy(&u, &d, 4);
-        const unsigned ex = (u >> 23) & 0xFF, man = u & 0x7FFFFF;
-        return d > 0.f && ex > 40 && ex < 214 && man != 0x7FFFFF;   // 2^-87 < d < 2^87, significand not all ones
-      };
-      fast_div_ok_ = ok(o.voxel_size) && ok(o.fx) && ok(o.fy);
+      fast_div_ok_ = fast_div_eligible(o.voxel_size, o.fx, o.fy);
       // div.rn.f32's fast path is already ~8 instructions and the ray-cast is latency-, not issue-bound.  Kept as an A/B option
       // (bit-identical), off by default; DESIGN.md ("TSDF variants removed") records its timings.
       const char* e = getenv("TDM_FAST_DIV");
@@ -1374,6 +1397,9 @@ int hash_slot_host(int x, int y, int z, int num_buckets, int* reference_expressi
   }
   return hash_slot(x, y, z, num_buckets, magic, c32);
 }
+
+// host-only view of whether fast_div may be turned on for these divisors
+int fast_div_eligible_host(float voxel_size, float fx, float fy) { return fast_div_eligible(voxel_size, fx, fy) ? 1 : 0; }
 
 // host-only view of the mesh extractor's per-axis table (no GPU involved; used by the CPU test-suite)
 int mesh_axis_table(float lower, float upper, float voxel_size, int* ints5, float* floats4, int* ranges2, int* bmin, int cap) {

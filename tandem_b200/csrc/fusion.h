@@ -43,6 +43,7 @@ class FusionIface {
 
 FusionIface* make_fusion(const tdm_fusion_options& o, int device);
 int hash_slot_host(int x, int y, int z, int num_buckets, int* reference_expression);
+int fast_div_eligible_host(float voxel_size, float fx, float fy);
 int mesh_axis_table(float lower, float upper, float voxel_size, int* ints5, float* floats4, int* ranges2, int* bmin, int cap);
 
 }  // namespace tdm

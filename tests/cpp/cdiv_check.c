@@ -26,6 +26,21 @@ long cdiv_check_exhaustive(float d, float lo, float hi) {
   }
   return bad;
 }
+/* n random x against the fixed divisor d: random sign and significand, exponent uniform in 2^[-40, 40); returns mismatches */
+long cdiv_check_random_x(float d, uint64_t seed, long n) {
+  uint64_t s = seed * 0x9E3779B97F4A7C15ull + 1;
+  volatile float one = 1.0f;
+  const float r = one / d;
+  long bad = 0;
+  for (long i = 0; i < n; ++i) {
+    s ^= s << 13; s ^= s >> 7; s ^= s << 17;
+    const uint32_t a = (uint32_t)s;
+    const uint32_t xe = 127 - 40 + (uint32_t)(s >> 32) % 80;
+    const float x = from_bits((a & 0x80000000u) | (xe << 23) | (a & 0x7FFFFF));
+    if (bits(cdiv(x, d, r)) != bits(x / d)) ++bad;
+  }
+  return bad;
+}
 /* n random (x, d) pairs: x log-uniform in [1e-6, 1e6] with random sign, d log-uniform in [1e-4, 1e4]; returns mismatches */
 long cdiv_check_random(uint64_t seed, long n) {
   uint64_t s = seed * 0x9E3779B97F4A7C15ull + 1;
