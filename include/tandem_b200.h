@@ -550,9 +550,10 @@ int tdm_immature_activate(tdm_immature* s, int n_frames, const int* frame_slots,
  *     (:78-141), select (:295-438) and makeMaps (:142-291) - on a tdm_pyramid's levels 0..2, and FullSystem::makeNewTraces
  *     (FullSystem.cpp:1623-1647) into a set slot.  Every float operation is the reference's, correctly rounded and in its
  *     order; the random pattern is glibc's rand() & 0xFF after srand(3141592), as the constructor makes it (:43-45), computed
- *     without touching the process's rand state.  The selection reads absSquaredGrad without gamma weights: the reference's
- *     setting_gammaWeightsPixelSelect 1 multiplies it by gw * gw (HessianBlocks.cpp:184-188), which is exactly 1 for a linear
- *     response (B[i] = i, no photometric calibration), the contract here.
+ *     without touching the process's rand state.  The selection reads the pyramid's absSquaredGrad as it is: the reference's
+ *     setting_gammaWeightsPixelSelect 1 multiplies it by gw * gw (HessianBlocks.cpp:184-188), which tdm_undistort_frame (n11)
+ *     does, so the selection is exact for any B when the pyramid comes from there; tdm_pyramid_build applies no weights, which
+ *     is exact for a linear response (B[i] = i, no photometric calibration).
  *     The two definitional differences, reads of memory the reference never writes:
  *     - select reads level 2's last row at yf == h - 4 for every h; makeImages writes only rows 1..h2-2
  *       (HessianBlocks.cpp:169).  The pyramid holds 0 there, and that 0 is read.
@@ -605,6 +606,66 @@ int tdm_selector_make_maps(tdm_selector* s, tdm_pyramid* pyramid, float density,
  *     unchanged. */
 int tdm_immature_make_new_traces(tdm_immature* set, int host_slot, tdm_selector* sel, tdm_pyramid* pyramid, float density,
                                  tdm_select_result* out, int* n_added, int* u, int* v, float* type);
+
+/* n11  DSO's per-frame input on the device: the raw 8-bit frame goes through PhotometricUndistorter::processFrame
+ *     (tandem/src/util/Undistort.cpp:213-252), Undistort::undistort's bilinear remap (:393-490) and FrameHessian::makeImages
+ *     with its gamma weights (HessianBlocks.cpp:128-191) into a tdm_pyramid, and the colour frame through the dataset reader's
+ *     BGR remap (DatasetReader.h:354-400), in one launch plus the pyramid's.  Every float operation is the reference's,
+ *     correctly rounded and in its order.  The benchmark-only noise of undistort (benchmark_varNoise, applyBlurNoise; both off
+ *     by default) is not applied.
+ *     A remap entry (xx, yy) is outside the frame, and gives 0 (grey and BGR), when xx < 0, yy < 0, (int)xx + 1 > w_org - 1
+ *     or (int)yy + 1 > h_org - 1 (NaN too).  The reference tests xx < 0 alone and reads the four taps otherwise; its table
+ *     builder (Undistort.cpp:953-972) compares iy with wOrg - 1 and assigns ix where it means iy, so on landscape frames its
+ *     tables can hold rows at or below hOrg - 1, whose taps lie past its buffer.  Wherever the reference reads inside its
+ *     buffer the two agree. */
+typedef struct tdm_undistort tdm_undistort;
+typedef struct tdm_undistort_settings {
+  int w_org, h_org;                 /* raw frame (Undistort::wOrg, hOrg) */
+  int w, h;                         /* rectified frame = pyramid level 0 (Undistort::w, h) */
+  const float* remap_x;             /* w*h, Undistort::get_remapX(); -1 marks "outside" */
+  const float* remap_y;             /* w*h, Undistort::get_remapY(); both NULL = passthrough (needs w == w_org, h == h_org) */
+  const float* response;            /* first line of the photometric calibration file (G before normalisation), or NULL */
+  int n_response;                   /* 256..65536 when given */
+  const unsigned short* vignette;   /* w_org*h_org pixels of the vignette image (8- or 16-bit, widened), or NULL */
+  int photometric_calibration;      /* setting_photometricCalibration: 0, 1, 2 */
+  int use_exposure;                 /* setting_useExposure */
+  int gamma_weights;                /* setting_gammaWeightsPixelSelect */
+} tdm_undistort_settings;
+/* PhotometricUndistorter's constructor (Undistort.cpp:50-179) on the arrays the caller read from the calibration files:
+ *     G must be strictly increasing and is normalised to 255.0 * (G[i] - min) / (max - min) in double, stored as float;
+ *     photometric_calibration 0 makes it 255.0f * i / (float)(n_response - 1); the vignette is divided by its maximum and
+ *     inverted (1.0f / map).  The calibration is valid only when both response and vignette are given and G increases; an
+ *     invalid one is not an error, the frame then takes the factor path.  The camera's B (CalibHessian::B) starts as the
+ *     identity.  The remap tables are copied.  Invalid input (sizes not positive, one remap table without the other,
+ *     passthrough with w != w_org or h != h_org, n_response outside 256..65536 with a response, photometric_calibration
+ *     outside 0..2) is an error. */
+int tdm_undistort_create(const tdm_undistort_settings* s, int device, tdm_undistort** out);
+/* Waits for the undistorter's pending work. */
+void tdm_undistort_destroy(tdm_undistort* u);
+/* PhotometricUndistorter::getG(): *valid receives the reference's `valid`; G[0..255] the normalised G when valid, and is not
+ *     written otherwise (getG returns NULL then). */
+int tdm_undistort_get_gamma(tdm_undistort* u, float G[256], int* valid);
+/* FullSystem::setGammaFunction (FullSystem.cpp:232-253) on this camera's B: for i in 1..254 the first s in 1..254 with
+ *     Binv[s] <= i <= Binv[s+1] gives B[i] = s + (i - Binv[s]) / (Binv[s+1] - Binv[s]); an i without such an s keeps its
+ *     previous value (from the identity or an earlier call); B[0] = 0, B[255] = 255.  Binv NULL is a no-op, as there.  Waits
+ *     for the undistorter's pending frames. */
+int tdm_undistort_set_gamma(tdm_undistort* u, const float* Binv);
+/* processFrame + remap + makeImages into `out` (level 0 w x h, same device).  Photometric step: data = factor * raw when the
+ *     calibration is not valid, exposure <= 0 or photometric_calibration == 0; otherwise data = G[raw], times
+ *     vignetteMapInv with photometric_calibration 2 (a vignette 0 gives inf, and inf or NaN reach the image).  Passthrough
+ *     copies it.  Every level of `out` is then built as tdm_pyramid_build builds it; with gamma_weights, absSquaredGrad of
+ *     rows 1..h_l-2 is multiplied by gw * gw, gw = B[c+1] - B[c], c = (int)(I + 0.5f) clamped to [5, 250] - exactly 1 for the
+ *     identity B, so the result is then bit for bit tdm_pyramid_build's.  (int)(I + 0.5f) of a non-finite or out-of-range
+ *     I is INT_MIN (c = 5), as the reference's x86 build computes it.  *exposure_time (may be NULL) receives exposure, or 1
+ *     without use_exposure.  With bgr (w_org*h_org*3) and bgr_out (w*h*3) the colour frame is remapped too
+ *     (static_cast<unsigned char> of the bilinear value; passthrough copies it).
+ *     Ordering is tdm_pyramid_build's: asynchronous on the pyramid's stream, which records the pyramid's ready event, so
+ *     trackers, traces, activation and selection order themselves after it; it waits for the pyramid's readers.  The call
+ *     returns once gray and bgr have been read (page-locked buffers are DMA'd from directly, pageable ones staged) and, with
+ *     bgr_out, once bgr_out has landed (one host wait).  Invalid input (null handles or gray, only one of bgr / bgr_out, a
+ *     pyramid of another level-0 size or device) is an error and launches nothing. */
+int tdm_undistort_frame(tdm_undistort* u, const unsigned char* gray, float exposure, float factor, tdm_pyramid* out,
+                        float* exposure_time, const unsigned char* bgr, unsigned char* bgr_out);
 
 #ifdef __cplusplus
 }

@@ -6,5 +6,6 @@ from .mvsnet import DrMvsnet, DrMvsnetOutput, default_weights  # noqa: F401
 from .fusion import DrFusion, DrFusionOptions  # noqa: F401
 from .immature import ImmaturePoints, TRACE_DEFAULTS  # noqa: F401
 from .pixel_selector import PixelSelector, SELECT_DEFAULTS  # noqa: F401
+from .undistort import Undistorter  # noqa: F401
 from .tracker import (CudaCoarseTracker, ImagePyramid, set_coarse_tracking_ref, set_coarse_tracking_ref_nodia,  # noqa: F401
                       track_new_coarse, track_pyramid)

@@ -55,6 +55,15 @@ class SelectSettings(ctypes.Structure):
                 ("grad_downweight_per_level", ctypes.c_float), ("select_direction_distribution", ctypes.c_int)]
 
 
+class UndistortSettings(ctypes.Structure):
+    """tdm_undistort_settings (include/tandem_b200.h): the camera's remap tables and photometric calibration."""
+    _fields_ = [("w_org", ctypes.c_int), ("h_org", ctypes.c_int), ("w", ctypes.c_int), ("h", ctypes.c_int),
+                ("remap_x", ctypes.POINTER(ctypes.c_float)), ("remap_y", ctypes.POINTER(ctypes.c_float)),
+                ("response", ctypes.POINTER(ctypes.c_float)), ("n_response", ctypes.c_int),
+                ("vignette", ctypes.POINTER(ctypes.c_ushort)), ("photometric_calibration", ctypes.c_int),
+                ("use_exposure", ctypes.c_int), ("gamma_weights", ctypes.c_int)]
+
+
 class SelectResult(ctypes.Structure):
     """tdm_select_result (include/tandem_b200.h)."""
     _fields_ = [(k, ctypes.c_int) for k in ("num_selected", "n2", "n3", "n4", "potential_used", "potential_after", "reselected",
@@ -215,6 +224,11 @@ def _declare(l):
         "tdm_selector_set_potential": (i, [vp, i]),
         "tdm_selector_make_maps": (i, [vp, vp, f, i, f, fp, P(SelectResult)]),
         "tdm_immature_make_new_traces": (i, [vp, i, vp, vp, f, P(SelectResult), ip, ip, ip, fp]),
+        "tdm_undistort_create": (i, [P(UndistortSettings), i, P(vp)]),
+        "tdm_undistort_destroy": (None, [vp]),
+        "tdm_undistort_get_gamma": (i, [vp, fp, ip]),
+        "tdm_undistort_set_gamma": (i, [vp, fp]),
+        "tdm_undistort_frame": (i, [vp, vp, f, f, vp, fp, vp, vp]),
     }
     missing = []
     for name, (res, args) in sigs.items():

@@ -24,6 +24,9 @@ struct tdm_immature {
 struct tdm_selector {
   tdm::SelectorIface* impl;
 };
+struct tdm_undistort {
+  tdm::UndistortIface* impl;
+};
 struct tdm_fusion {   // same layout as in capi_fusion.cu (one pointer)
   tdm::FusionIface* impl;
 };
@@ -514,6 +517,43 @@ int tdm_immature_make_new_traces(tdm_immature* set, int host_slot, tdm_selector*
   const int n = set->impl->make_new_traces(host_slot, *sel->impl, *pyramid->impl, density,
                                            reinterpret_cast<tdm::SelectResult*>(out), u, v, type);
   if (n_added) *n_added = n;
+  return TDM_OK;
+  TDM_API_END
+}
+
+/* ---- n11: processFrame, the remap and makeImages' gamma weights on the device ---- */
+int tdm_undistort_create(const tdm_undistort_settings* s, int device, tdm_undistort** out) {
+  TDM_API_BEGIN
+  TDM_CHECK(s && out, "null argument");
+  *out = new tdm_undistort{tdm::make_undistort(*s, device)};
+  return TDM_OK;
+  TDM_API_END
+}
+void tdm_undistort_destroy(tdm_undistort* u) {
+  if (!u) return;
+  try { delete u->impl; } catch (...) {}
+  delete u;
+}
+int tdm_undistort_get_gamma(tdm_undistort* u, float G[256], int* valid) {
+  TDM_API_BEGIN
+  TDM_CHECK(u && G && valid, "null argument");
+  u->impl->get_gamma(G, valid);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_undistort_set_gamma(tdm_undistort* u, const float* Binv) {
+  TDM_API_BEGIN
+  TDM_CHECK(u, "null handle");
+  u->impl->set_gamma(Binv);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_undistort_frame(tdm_undistort* u, const unsigned char* gray, float exposure, float factor, tdm_pyramid* out,
+                        float* exposure_time, const unsigned char* bgr, unsigned char* bgr_out) {
+  TDM_API_BEGIN
+  TDM_CHECK(u && gray && out, "null argument");
+  const float t = u->impl->frame(gray, exposure, factor, *out->impl, bgr, bgr_out);
+  if (exposure_time) *exposure_time = t;
   return TDM_OK;
   TDM_API_END
 }

@@ -10,6 +10,7 @@
 // shuffles and one shared-memory pass, each CTA writes its partial vector, and the last CTA to finish (atomic
 // ticket) adds the partials in a fixed order and writes the result straight into mapped pinned host memory:
 // deterministic (the reference's float atomics are not), one launch, no memset, no D2H copy.
+#include <climits>
 #include <cmath>
 #include <cstring>
 #include <string>
@@ -328,20 +329,38 @@ __global__ void k_pyr_level(const float* __restrict__ src /*grey w*h (lvl 0) or 
   const float* q = src + 3 * (size_t)(2 * x + 2 * y * wprev);
   gray[i] = __fmul_rn(0.25f, __fadd_rn(__fadd_rn(__fadd_rn(q[0], q[3]), q[3 * wprev]), q[3 * wprev + 3]));
 }
-__global__ void k_pyr_grad(const float* __restrict__ gray, float* __restrict__ dI, float* __restrict__ absgrad, int wl, int hl) {
+// kGamma (n11): absSquaredGrad of [w, w*(h-1)) times gw * gw, gw = CalibHessian::getBGradOnly(I) (HessianBlocks.h:446-452)
+// on the camera's B (256 floats) - makeImages' setting_gammaWeightsPixelSelect branch (HessianBlocks.cpp:184-188).
+// (int)(I + 0.5f) is undefined in C for NaN, +-inf and values beyond int; the reference's x86 build converts with cvttss2si,
+// which gives INT_MIN there (clamped to 5).  That is reproduced; CUDA's own conversion would give 0 or INT_MAX.
+template <bool kGamma>
+__global__ void k_pyr_grad(const float* __restrict__ gray, float* __restrict__ dI, float* __restrict__ absgrad, int wl, int hl,
+                           const float* __restrict__ B) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= wl * hl) return;
   float dx = 0.f, dy = 0.f;
-  if (i >= wl && i < wl * (hl - 1)) {
+  const bool inner = i >= wl && i < wl * (hl - 1);
+  if (inner) {
     dx = __fmul_rn(0.5f, __fsub_rn(gray[i + 1], gray[i - 1]));
     dy = __fmul_rn(0.5f, __fsub_rn(gray[i + wl], gray[i - wl]));
     if (!isfinite(dx)) dx = 0.f;
     if (!isfinite(dy)) dy = 0.f;
   }
-  dI[3 * (size_t)i] = gray[i];
+  const float g = gray[i];
+  dI[3 * (size_t)i] = g;
   dI[3 * (size_t)i + 1] = dx;
   dI[3 * (size_t)i + 2] = dy;
-  absgrad[i] = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
+  float a = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
+  if constexpr (kGamma) {
+    if (inner) {
+      const float v = __fadd_rn(g, 0.5f);
+      int c = (v >= -2147483648.f && v < 2147483648.f) ? __float2int_rz(v) : INT_MIN;
+      c = c < 5 ? 5 : (c > 250 ? 250 : c);
+      const float gw = __fsub_rn(__ldg(B + c + 1), __ldg(B + c));
+      a = __fmul_rn(a, __fmul_rn(gw, gw));
+    }
+  }
+  absgrad[i] = a;
 }
 
 // ================================================================================================
@@ -1790,7 +1809,26 @@ class PyramidImpl final : public PyramidIface {
       const int wl = w_ >> l, hl = h_ >> l, n = wl * hl;
       const float* src = l == 0 ? d_in_.get() : d_dI_.get() + 3 * off_[l - 1];
       k_pyr_level<<<(n + 255) / 256, 256, 0, stream_.get()>>>(src, l > 0, l > 0 ? (w_ >> (l - 1)) : 0, d_gray_.get(), wl, hl);
-      k_pyr_grad<<<(n + 255) / 256, 256, 0, stream_.get()>>>(d_gray_.get(), d_dI_.get() + 3 * off_[l], d_abs_.get() + off_[l], wl, hl);
+      k_pyr_grad<false><<<(n + 255) / 256, 256, 0, stream_.get()>>>(d_gray_.get(), d_dI_.get() + 3 * off_[l], d_abs_.get() + off_[l],
+                                                                    wl, hl, nullptr);
+    }
+    TDM_CUDA(cudaGetLastError());
+    TDM_CUDA(cudaEventRecord(ready_.get(), stream_.get()));
+  }
+  float* device_input() override { return d_gray_.get(); }
+  void* stream() const override { return (void*)stream_.get(); }
+  void build_device(const float* d_B) override {
+    TDM_CUDA(cudaSetDevice(device_));
+    for (int l = 0; l < levels_; ++l) {
+      const int wl = w_ >> l, hl = h_ >> l, n = wl * hl;
+      if (l > 0)
+        k_pyr_level<<<(n + 255) / 256, 256, 0, stream_.get()>>>(d_dI_.get() + 3 * off_[l - 1], 1, w_ >> (l - 1), d_gray_.get(), wl, hl);
+      float* dI = d_dI_.get() + 3 * off_[l];
+      float* ag = d_abs_.get() + off_[l];
+      if (d_B)
+        k_pyr_grad<true><<<(n + 255) / 256, 256, 0, stream_.get()>>>(d_gray_.get(), dI, ag, wl, hl, d_B);
+      else
+        k_pyr_grad<false><<<(n + 255) / 256, 256, 0, stream_.get()>>>(d_gray_.get(), dI, ag, wl, hl, nullptr);
     }
     TDM_CUDA(cudaGetLastError());
     TDM_CUDA(cudaEventRecord(ready_.get(), stream_.get()));

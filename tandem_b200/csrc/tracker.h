@@ -2,6 +2,8 @@
 #pragma once
 #include "common.cuh"
 
+struct tdm_undistort_settings;
+
 namespace tdm {
 
 class PyramidIface;
@@ -151,8 +153,28 @@ class PyramidIface {
   virtual int height(int lvl) const = 0;
   virtual int levels() const = 0;
   virtual int device() const = 0;
+  // n11: build() from level 0's grey already on the device.  A producer writes it into device_input() (w*h floats) with work
+  // enqueued on stream() (a cudaStream_t) and then calls build_device, which records ready_event() as build() does.  d_B
+  // (256 floats on the device, or null): the camera's B; absSquaredGrad then carries makeImages' gamma weights.
+  virtual float* device_input() = 0;
+  virtual void* stream() const = 0;
+  virtual void build_device(const float* d_B) = 0;
 };
 PyramidIface* make_pyramid(int w, int h, int levels, int device);
+
+// n11 (undistort.cu): DSO's per-frame input - PhotometricUndistorter::processFrame, Undistort::undistort's bilinear remap,
+// the BGR remap of the dataset reader - into a pyramid (tdm_undistort_frame).
+class UndistortIface {
+ public:
+  virtual ~UndistortIface() = default;
+  virtual void get_gamma(float G[256], int* valid) const = 0;
+  virtual void set_gamma(const float* Binv) = 0;
+  // returns exposure_time; bgr / bgr_out both null or both given
+  virtual float frame(const unsigned char* gray, float exposure, float factor, PyramidIface& out, const unsigned char* bgr,
+                      unsigned char* bgr_out) = 0;
+  virtual int device() const = 0;
+};
+UndistortIface* make_undistort(const tdm_undistort_settings& s, int device);
 
 // n10 (pixsel.cu): PixelSelector::makeMaps on a pyramid's levels 0..2 (tdm_select_result's layout)
 struct SelectResult {

@@ -25,3 +25,4 @@ leg feature_cache_race $T2 racecheck tests/test_mvsnet_feature_cache_gpu.py -k "
 leg trace_mem $T1 memcheck tests/test_trace_gpu.py -k "not shim and not random and not 2560"
 leg activate_mem $T1 memcheck tests/test_activate_gpu.py -k "not shim and not random"
 leg pixsel_mem $T1 memcheck tests/test_pixsel_gpu.py -k "not shim and not sequences"
+leg undistort_mem $T1 memcheck tests/test_undistort_gpu.py -k "not shim and not tracker and not trace"
