@@ -667,6 +667,68 @@ int tdm_undistort_set_gamma(tdm_undistort* u, const float* Binv);
 int tdm_undistort_frame(tdm_undistort* u, const unsigned char* gray, float exposure, float factor, tdm_pyramid* out,
                         float* exposure_time, const unsigned char* bgr, unsigned char* bgr_out);
 
+/* n12  The per-residual part of DSO's windowed bundle adjustment on the device: FullSystem::linearizeAll
+ *     (tandem/src/FullSystem/FullSystemOptimize.cpp:142-210) - PointFrameResidual::linearize (Residuals.cpp:78-274) of every
+ *     active residual, setNewFrameEnergyTH (:93-141), and with fixLinearization applyRes (Residuals.cpp:306-328) and the
+ *     reductor's maxRelBaseline / numGoodResiduals update (:52-85) - plus applyRes_Reductor (:87-92).  A set holds the
+ *     window's active residuals for one FullSystem::optimize (activeResiduals, :422-439).  Every float operation is the
+ *     reference's, correctly rounded and in its order; relBS's 0.01 * norm is evaluated in double.  lastEnergyP is the double
+ *     sum of every residual's return (an OOB residual returns its state_energy), summed by a fixed tree: the same bits on
+ *     every call, within 1e-12 relative of the sequential sum (the reference's own order depends on its thread schedule). */
+typedef struct tdm_linearize_settings {
+  float huber_th;                     /* setting_huberTH, 9 */
+  float outlier_th_sum_component;     /* setting_outlierTHSumComponent, 2500 */
+  float affine_opt_mode_a;            /* setting_affineOptModeA, 1e12 (< 0: JabF[0] is 0) */
+  float affine_opt_mode_b;            /* setting_affineOptModeB, 1e8 (< 0: JabF[1] is 0) */
+  float frame_energy_th_n;            /* setting_frameEnergyTHN, 0.7 (in [0, 1)) */
+  float frame_energy_th_const_weight; /* setting_frameEnergyTHConstWeight, 0.5 */
+  float frame_energy_th_fac_median;   /* setting_frameEnergyTHFacMedian, 1.5 */
+  float overall_energy_th_weight;     /* setting_overallEnergyTHWeight, 1 */
+} tdm_linearize_settings;
+/* RawResidualJacobian's 74 floats in declaration order: resF[8], Jpdxi[2][6], Jpdc[2][4], Jpdd[2], JIdx[2][8], JabF[2][8],
+ *     JIdx2, JabJIdx, Jab2 (2x2, column-major) */
+enum { TDM_JACOBIAN_FLOATS = 74 };
+typedef struct tdm_active tdm_active;
+/* A set for up to capacity_points points and 8 residuals per point of a w x h camera.  settings NULL: the defaults above. */
+int tdm_active_create(int w, int h, int capacity_points, const tdm_linearize_settings* settings, int device, tdm_active** out);
+/* Waits for the set's pending work. */
+void tdm_active_destroy(tdm_active* s);
+/* Loads the window: a blocking upload on the set's stream, after the set's pending work, through page-locked staging; it has
+ *     landed when the call returns.  n_frames (2..8) frames in frameHessians order; per point its host frame, u, v,
+ *     color[8], weights[8] (n_points x 8), maxRelBaseline and numGoodResiduals; per residual, in activeResiduals order, its
+ *     point and target frame.  Every residual is reset as resetOOB does: state IN, state_energy 0, state_NewState OUTLIER,
+ *     state_NewEnergy 0.  Invalid input (null handles or needed arrays, n_frames outside 2..8, more points or residuals than
+ *     the capacity, a host, point or target index out of range, a target equal to its point's host) is an error and changes
+ *     nothing. */
+int tdm_active_load(tdm_active* s, int n_frames, int n_points, const int* point_host, const float* point_u, const float* point_v,
+                    const float* color, const float* weights, const float* max_rel_baseline, const int* num_good_residuals,
+                    int n_residuals, const int* res_point, const int* res_target);
+/* linearizeAll(fix_linearization) over the loaded residuals.  Inputs: frame_pyramids[f] (level 0 is target->dI); precalc
+ *     n_frames x n_frames x 27 floats, [host][target] = PRE_KRKiTll (row-major), PRE_KtTll, PRE_RTll_0 (row-major),
+ *     PRE_tTll_0, PRE_aff_mode, PRE_b0_mode (the diagonal is not read); frame_energy_th[f]; calib4 = fxl, fyl, cxl, cyl
+ *     (fxli = 1.0f / fxl); every point's idepth_scaled and idepth_zero_scaled.
+ *     Outputs (any may be NULL): *energy lastEnergyP; *new_frame_energy_th the newest frame's frameEnergyTH after
+ *     setNewFrameEnergyTH (12*12*8 when no residual to it has state_NewEnergyWithOutlier >= 0); per residual new_state
+ *     (state_NewState: IN 0, OOB 1, OUTLIER 2), new_energy (state_NewEnergy; the previous value where linearize returns
+ *     before setting it), new_energy_with_outlier (-1 on OOB returns), center_projected_to (3 floats; NaN where the reference
+ *     keeps its previous value: state OOB on entry or a failed centre projection) and jacobians (TDM_JACOBIAN_FLOATS floats,
+ *     defined where new_state is not OOB; they also stay in device memory).  With fix_linearization, also state (the applied
+ *     state_state), removed (1 where the final state is not IN: the residual goes to toRemove) and every point's updated
+ *     max_rel_baseline and num_good_residuals (isNew is always true in the reference).
+ *     Blocking (one host wait), on the set's stream after the build of every pyramid given; a later tdm_pyramid_build or
+ *     tdm_pyramid_destroy of any of them waits for it.  Invalid input (null handles or needed arrays, no load, a pyramid of
+ *     another level-0 size or device) is an error and launches nothing. */
+int tdm_active_linearize(tdm_active* s, tdm_pyramid* const* frame_pyramids, const float* precalc, const float* frame_energy_th,
+                         const float calib4[4], const float* idepth_scaled, const float* idepth_zero_scaled, int fix_linearization,
+                         double* energy, float* new_frame_energy_th, signed char* new_state, float* new_energy,
+                         float* new_energy_with_outlier, float* center_projected_to, float* jacobians, signed char* state,
+                         unsigned char* removed, float* max_rel_baseline, int* num_good_residuals);
+/* applyRes_Reductor: state_state = state_NewState and state_energy = state_NewEnergy for every residual not already OOB.
+ *     Asynchronous on the set's stream. */
+int tdm_active_apply_res(tdm_active* s);
+/* Every residual's state_state and state_energy (tests; synchronises); either may be NULL. */
+int tdm_active_get_state(tdm_active* s, signed char* state, float* energy);
+
 #ifdef __cplusplus
 }
 #endif

@@ -49,6 +49,13 @@ class ActivateSettings(ctypes.Structure):
     _fields_ = [("min_idepth_h_act", ctypes.c_float), ("gn_iterations", ctypes.c_int), ("min_obs", ctypes.c_int)]
 
 
+class LinearizeSettings(ctypes.Structure):
+    """tdm_linearize_settings (include/tandem_b200.h): the reference's constants of linearizeAll."""
+    _fields_ = [(k, ctypes.c_float) for k in ("huber_th", "outlier_th_sum_component", "affine_opt_mode_a", "affine_opt_mode_b",
+                                              "frame_energy_th_n", "frame_energy_th_const_weight", "frame_energy_th_fac_median",
+                                              "overall_energy_th_weight")]
+
+
 class SelectSettings(ctypes.Structure):
     """tdm_select_settings (include/tandem_b200.h): the reference's constants of PixelSelector."""
     _fields_ = [("min_grad_hist_cut", ctypes.c_float), ("min_grad_hist_add", ctypes.c_float),
@@ -229,6 +236,13 @@ def _declare(l):
         "tdm_undistort_get_gamma": (i, [vp, fp, ip]),
         "tdm_undistort_set_gamma": (i, [vp, fp]),
         "tdm_undistort_frame": (i, [vp, vp, f, f, vp, fp, vp, vp]),
+        "tdm_active_create": (i, [i, i, i, P(LinearizeSettings), i, P(vp)]),
+        "tdm_active_destroy": (None, [vp]),
+        "tdm_active_load": (i, [vp, i, i, ip, fp, fp, fp, fp, fp, ip, i, ip, ip]),
+        "tdm_active_linearize": (i, [vp, P(vp), fp, fp, fp, fp, fp, i, dp, fp, P(c.c_byte), fp, fp, fp, fp, P(c.c_byte),
+                                     P(c.c_ubyte), fp, ip]),
+        "tdm_active_apply_res": (i, [vp]),
+        "tdm_active_get_state": (i, [vp, P(c.c_byte), fp]),
     }
     missing = []
     for name, (res, args) in sigs.items():

@@ -11,6 +11,7 @@
 
 static_assert(sizeof(tdm_select_result) == sizeof(tdm::SelectResult), "tdm_select_result layout");
 static_assert(sizeof(tdm_select_settings) == 16, "tdm_select_settings layout");
+static_assert(sizeof(tdm_linearize_settings) == 32, "tdm_linearize_settings layout");
 
 struct tdm_tracker {
   tdm::TrackerIface* impl;
@@ -26,6 +27,9 @@ struct tdm_selector {
 };
 struct tdm_undistort {
   tdm::UndistortIface* impl;
+};
+struct tdm_active {
+  tdm::ActiveIface* impl;
 };
 struct tdm_fusion {   // same layout as in capi_fusion.cu (one pointer)
   tdm::FusionIface* impl;
@@ -554,6 +558,67 @@ int tdm_undistort_frame(tdm_undistort* u, const unsigned char* gray, float expos
   TDM_CHECK(u && gray && out, "null argument");
   const float t = u->impl->frame(gray, exposure, factor, *out->impl, bgr, bgr_out);
   if (exposure_time) *exposure_time = t;
+  return TDM_OK;
+  TDM_API_END
+}
+
+/* ---- n12: linearizeAll on the device ---- */
+int tdm_active_create(int w, int h, int capacity_points, const tdm_linearize_settings* settings, int device, tdm_active** out) {
+  TDM_API_BEGIN
+  TDM_CHECK(out, "null argument");
+  static const tdm_linearize_settings defaults = {9.f, 2500.f, 1e12f, 1e8f, 0.7f, 0.5f, 1.5f, 1.f};
+  *out = new tdm_active{tdm::make_active(w, h, capacity_points, (const float*)(settings ? settings : &defaults), device)};
+  return TDM_OK;
+  TDM_API_END
+}
+void tdm_active_destroy(tdm_active* s) {
+  if (!s) return;
+  try { delete s->impl; } catch (...) {}
+  delete s;
+}
+int tdm_active_load(tdm_active* s, int n_frames, int n_points, const int* point_host, const float* point_u, const float* point_v,
+                    const float* color, const float* weights, const float* max_rel_baseline, const int* num_good_residuals,
+                    int n_residuals, const int* res_point, const int* res_target) {
+  TDM_API_BEGIN
+  TDM_CHECK(s, "null handle");
+  s->impl->load(n_frames, n_points, point_host, point_u, point_v, color, weights, max_rel_baseline, num_good_residuals, n_residuals,
+                res_point, res_target);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_active_linearize(tdm_active* s, tdm_pyramid* const* frame_pyramids, const float* precalc, const float* frame_energy_th,
+                         const float calib4[4], const float* idepth_scaled, const float* idepth_zero_scaled, int fix_linearization,
+                         double* energy, float* new_frame_energy_th, signed char* new_state, float* new_energy,
+                         float* new_energy_with_outlier, float* center_projected_to, float* jacobians, signed char* state,
+                         unsigned char* removed, float* max_rel_baseline, int* num_good_residuals) {
+  TDM_API_BEGIN
+  TDM_CHECK(s && frame_pyramids, "null argument");
+  const tdm::PyramidIface* fp[8] = {};
+  const int n = s->impl->n_frames();
+  TDM_CHECK(n >= 2, "linearize before load");
+  for (int f = 0; f < n; ++f) {
+    TDM_CHECK(frame_pyramids[f], "null argument");
+    fp[f] = frame_pyramids[f]->impl;
+  }
+  tdm::ActiveIface::Outputs o;
+  o.energy = energy; o.new_frame_energy_th = new_frame_energy_th; o.new_state = new_state; o.new_energy = new_energy;
+  o.new_energy_with_outlier = new_energy_with_outlier; o.center_projected_to = center_projected_to; o.jacobians = jacobians;
+  o.state = state; o.removed = removed; o.max_rel_baseline = max_rel_baseline; o.num_good_residuals = num_good_residuals;
+  s->impl->linearize(fp, precalc, frame_energy_th, calib4, idepth_scaled, idepth_zero_scaled, fix_linearization, o);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_active_apply_res(tdm_active* s) {
+  TDM_API_BEGIN
+  TDM_CHECK(s, "null handle");
+  s->impl->apply_res();
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_active_get_state(tdm_active* s, signed char* state, float* energy) {
+  TDM_API_BEGIN
+  TDM_CHECK(s, "null handle");
+  s->impl->get_state(state, energy);
   return TDM_OK;
   TDM_API_END
 }

@@ -16,6 +16,7 @@
 
 #include <cub/block/block_scan.cuh>
 
+#include "dso_sample.cuh"
 #include "tracker.h"
 
 namespace tdm {
@@ -26,13 +27,6 @@ enum { IPS_GOOD = 0, IPS_OOB, IPS_OUTLIER, IPS_SKIPPED, IPS_BADCONDITION, IPS_UN
 // one row of 8 * cap 32-bit words per field (ImmatureRow, tracker.h); point i of slot s is word s * cap + i of every row
 constexpr int kRows = IM_ROWS, kSlots = 8;
 constexpr int kMaxSteps = 99;   // `if(numSteps >= 100) numSteps = 99;`
-
-__constant__ int c_pattern[8][2] = {{0, -2}, {-1, -1}, {1, -1}, {-2, 0}, {0, 0}, {2, 0}, {-1, 1}, {0, 2}};   // staticPattern[8]
-
-__device__ __forceinline__ float fm(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ float fa(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ float fs(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ float fd(float a, float b) { return __fdiv_rn(a, b); }
 
 struct Settings {   // tdm_trace_settings
   float max_pix_search, stepsize, gn_threshold, extra_slack_on_th, slack_interval, min_improvement_factor, huber, outlier_th,
@@ -49,24 +43,6 @@ struct TraceLaunch {
   int n_hosts, w, h, cap;
   Settings s;
 };
-
-// (int)x in 0..w-2 and (int)y in 0..h-2: the 2x2 footprint lies in the image.  Outside it a sample is a non-finite hit.
-__device__ __forceinline__ bool inside(float x, float y, int w, int h) {
-  return x > -1.f && y > -1.f && x < (float)(w - 1) && y < (float)(h - 1);
-}
-
-// getInterpolatedElement33 (globalFuncs.h:75-89), components 0..C-1 (C = 1: getInterpolatedElement31, :126-140)
-template <int C>
-__device__ __forceinline__ void interp(const float* __restrict__ dI, float x, float y, int w, float* out) {
-  const int ix = (int)x, iy = (int)y;
-  const float dx = fs(x, (float)ix), dy = fs(y, (float)iy), dxdy = fm(dx, dy);
-  const float* bp = dI + 3 * ((long long)ix + (long long)iy * w);
-  const float w0 = dxdy, w1 = fs(dy, dxdy), w2 = fs(dx, dxdy), w3 = fa(fs(fs(1.f, dx), dy), dxdy);
-#pragma unroll
-  for (int k = 0; k < C; ++k)
-    out[k] = fa(fa(fa(fm(w0, __ldg(bp + 3 * (1 + w) + k)), fm(w1, __ldg(bp + 3 * w + k))), fm(w2, __ldg(bp + 3 + k))),
-                fm(w3, __ldg(bp + k)));
-}
 
 __device__ __forceinline__ float huber_weight(float residual, float huber) {
   return fabsf(residual) < huber ? 1.f : fd(huber, fabsf(residual));

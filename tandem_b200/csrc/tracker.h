@@ -243,6 +243,36 @@ class ImmatureIface {
 };
 ImmatureIface* make_immature(int w, int h, int capacity_per_host, const float* settings /* tdm_trace_settings */, int device);
 
+// n12 (linearize.cu): the active residuals of one FullSystem::optimize and their linearisation (tdm_active_*)
+class ActiveIface {
+ public:
+  virtual ~ActiveIface() = default;
+  // blocking upload; every residual is reset as resetOOB does
+  virtual void load(int n_frames, int n_points, const int* host, const float* u, const float* v, const float* color,
+                    const float* weights, const float* max_rel_baseline, const int* num_good, int n_res, const int* res_point,
+                    const int* res_target) = 0;
+  struct Outputs {   // host memory; every pointer may be null
+    double* energy = nullptr;
+    float* new_frame_energy_th = nullptr;
+    signed char* new_state = nullptr;
+    float *new_energy = nullptr, *new_energy_with_outlier = nullptr, *center_projected_to = nullptr, *jacobians = nullptr;
+    signed char* state = nullptr;       // fix only
+    unsigned char* removed = nullptr;   // fix only
+    float* max_rel_baseline = nullptr;  // fix only
+    int* num_good_residuals = nullptr;  // fix only
+  };
+  // linearizeAll(fix) over frames[0..n_frames-1]'s level 0 (blocking, one host wait)
+  virtual void linearize(const PyramidIface* const* frames, const float* precalc, const float* frame_energy_th, const float* calib4,
+                         const float* idepth_scaled, const float* idepth_zero_scaled, int fix, Outputs& o) = 0;
+  virtual void apply_res() = 0;   // asynchronous
+  virtual void get_state(signed char* state, float* energy) = 0;   // synchronises
+  virtual const float* device_jacobians() const = 0;   // n_residuals() x 74 floats
+  virtual int n_frames() const = 0;
+  virtual int n_residuals() const = 0;
+  virtual int device() const = 0;
+};
+ActiveIface* make_active(int w, int h, int capacity_points, const float* settings /* tdm_linearize_settings */, int device);
+
 TrackerIface* make_tracker(int w, int h, float huber, float cutoff, int n_max, int device);
 
 }  // namespace tdm

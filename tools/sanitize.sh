@@ -26,3 +26,4 @@ leg trace_mem $T1 memcheck tests/test_trace_gpu.py -k "not shim and not random a
 leg activate_mem $T1 memcheck tests/test_activate_gpu.py -k "not shim and not random"
 leg pixsel_mem $T1 memcheck tests/test_pixsel_gpu.py -k "not shim and not sequences"
 leg undistort_mem $T1 memcheck tests/test_undistort_gpu.py -k "not shim and not tracker and not trace"
+leg linearize_mem $T1 memcheck tests/test_linearize_gpu.py -k "not shim and not seeded"
