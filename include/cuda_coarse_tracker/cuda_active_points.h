@@ -64,6 +64,29 @@ class CudaActivePoints {
   // applyRes_Reductor (asynchronous)
   void applyRes();
 
+  // n13: solveSystemF's accumulators over the data the last applyRes / linearize(fixLinearization) took (takeDataF).
+  // The inputs setAdjointsF and setDeltaF leave: adHost / adTarget [h + n * t], each frame's prior and delta_prior, cPrior,
+  // cDeltaF, each loaded point's priorF and deltaF.  Dense outputs are row-major with dim = 8 * n_frames + 4, ready for
+  // Eigen::Map<MatXX> / Eigen::Map<VecX> (the matrices are returned as std::vector so that this header needs no dynamic
+  // Eigen types).
+  struct SystemInputs {
+    std::vector<Eigen::Matrix<double, 8, 8>> adHost, adTarget;   // n_frames * n_frames each
+    std::vector<Eigen::Matrix<double, 8, 1>> prior, delta_prior;   // per frame
+    Eigen::Matrix<double, 4, 1> cPrior;
+    Eigen::Matrix<float, 4, 1> cDeltaF;
+    std::vector<float> priorF, deltaF;   // per loaded point
+  };
+  struct System {
+    int dim = 0;
+    std::vector<double> H_top, b_top, H_sc, b_sc;   // HA_top + HL_top, bA_top + bL_top, H_sc, b_sc
+    int resInA = 0;
+    std::vector<float> HdiF, idepth_hessian;     // per loaded point; 0 where no residual is active
+  };
+  // accumulateAF_MT + accumulateLF_MT + accumulateSCF_MT (blocking)
+  void accumulate(SystemInputs const &in, System *out);
+  // resubstituteF_MT's per-point step for the solved x (dim entries) with the last accumulate's adjoints (blocking)
+  void resubstitute(std::vector<double> const &x, std::vector<float> *step);
+
  private:
   tdm_active *handle_ = nullptr;
   int n_frames_ = 0, n_points_ = 0, n_res_ = 0;

@@ -729,6 +729,45 @@ int tdm_active_apply_res(tdm_active* s);
 /* Every residual's state_state and state_energy (tests; synchronises); either may be NULL. */
 int tdm_active_get_state(tdm_active* s, signed char* state, float* energy);
 
+/* ---- n13: solveSystemF's accumulators on the device (EnergyFunctional.cpp:775-913) ----
+ * The set keeps what DSO's applyRes(true) hands to the back-end (takeDataF, EnergyFunctionalStructs.cpp:39-50): at every
+ * tdm_active_apply_res and at the applied states of tdm_active_linearize(fix), each residual whose new state is IN keeps a
+ * copy of its Jacobian record and its JpJdF and becomes active; a residual whose new state is not IN becomes inactive; a
+ * residual already OOB is left as it is.  Loading clears every active flag.  The reference's takeDataF swaps the Jacobian
+ * pointers rather than copying; the two agree in optimize(), where a linearize precedes every apply, but two applies with no
+ * linearize between them hand the reference the older record and this set the latest one.  The copies and the accumulators' per-residual
+ * values add 350 bytes per residual slot to n12's 359, about 5.7 KB per capacity point (12 GB at the largest capacity, 2^21
+ * points), plus 6 MB for the accumulators' partial sums.  tdm_active_linearize's outputs are unchanged.
+ *
+ * n is the loaded n_frames, dim = 8 n + 4; records [host][target] are indexed host + n * target. */
+/* accumulateAF_MT + accumulateLF_MT + accumulateSCF_MT (blocking, one host wait) over the taken data, not over the last
+ * linearize's Jacobians.
+ *     ad_host, ad_target: n x n records, 8x8 row-major doubles (EnergyFunctional::adHost / adTarget; their float casts are
+ *       adHostF / adTargetF).  frame_prior, frame_delta_prior: n x 8 doubles (EFFrame::prior, delta_prior).  c_prior: 4
+ *       doubles (cPrior); c_delta: 4 floats (cDeltaF).  point_prior, point_delta: per loaded point, EFPoint::priorF, deltaF.
+ *     Outputs (each may be NULL): H_top = HA_top + HL_top (dim x dim, row-major) and b_top = bA_top + bL_top (dim); H_sc, b_sc;
+ *       n_active (resInA); per point hdi (HdiF) and idepth_hessian, 0 for a point with no active residual.  The host forms
+ *       either solver mode's HFinal from them.
+ *     The device's own maxRelBaseline of a point with no active residual becomes 0, as the reference's SC addPoint sets it.
+ *     Per-residual and per-point values are the reference's float expressions bit for bit; the accumulator sums are in
+ *     double, in a fixed order (the same bits on every call), and the stitch follows the reference's loop and product order.
+ *     Errors (nothing launched): a null handle or input, no load, no apply since the load, more than one residual of a point
+ *     to one target frame. */
+int tdm_active_accumulate(tdm_active* s, const double* ad_host, const double* ad_target, const double* frame_prior,
+                          const double* frame_delta_prior, const double c_prior[4], const float c_delta[4], const float* point_prior,
+                          const float* point_delta, double* H_top, double* b_top, double* H_sc, double* b_sc, int* n_active,
+                          float* hdi, float* idepth_hessian);
+/* resubstituteFPt for every loaded point (blocking): x (dim doubles) is the solved step, the adjoints are the last
+ * accumulate's; step gets one float per point (0 for a point with no active residual).  Error without an accumulate since
+ * the last apply or load. */
+int tdm_active_resubstitute(tdm_active* s, const double* x, float* step);
+/* The last accumulate's raw sums before the stitch (tests; synchronises); any pointer may be NULL.  top: n x n records of
+ * AccumulatorApprox's 91 terms (55 of update, 30 of updateTopRight, 6 of updateBotRight, in their order) and top_num their
+ * update counts; acc_e: n x n records 8x4 row-major; acc_eb: n x n records of 8; acc_d: n^3 records [host + n t1 + n^2 t2]
+ * 8x8 row-major and d_num their counts; hcc 4x4; bc 4. */
+int tdm_active_get_accumulators(tdm_active* s, double* top, int* top_num, double* acc_e, double* acc_eb, double* acc_d, int* d_num,
+                                double* hcc, double* bc);
+
 #ifdef __cplusplus
 }
 #endif

@@ -70,3 +70,34 @@ void CudaActivePoints::linearize(std::vector<tdm_pyramid *> const &frames, std::
 }
 
 void CudaActivePoints::applyRes() { chk(tdm_active_apply_res(handle_), "CudaActivePoints::applyRes"); }
+
+void CudaActivePoints::accumulate(SystemInputs const &in, System *out) {
+  const int n = n_frames_, dim = 8 * n + 4;
+  if ((int)in.adHost.size() != n * n || (int)in.adTarget.size() != n * n || (int)in.prior.size() != n ||
+      (int)in.delta_prior.size() != n || (int)in.priorF.size() != n_points_ || (int)in.deltaF.size() != n_points_)
+    throw std::runtime_error("CudaActivePoints::accumulate: sizes differ from the loaded window");
+  // the C ABI's 8x8 records are row-major; Eigen's fixed matrices are column-major
+  std::vector<double> aH(64 * n * n), aT(64 * n * n), pr(8 * n), dp(8 * n);
+  for (int k = 0; k < n * n; ++k)
+    for (int r = 0; r < 8; ++r)
+      for (int c = 0; c < 8; ++c) {
+        aH[64 * k + 8 * r + c] = in.adHost[k](r, c);
+        aT[64 * k + 8 * r + c] = in.adTarget[k](r, c);
+      }
+  for (int f = 0; f < n; ++f)
+    for (int i = 0; i < 8; ++i) { pr[8 * f + i] = in.prior[f][i]; dp[8 * f + i] = in.delta_prior[f][i]; }
+  out->dim = dim;
+  out->H_top.resize((size_t)dim * dim); out->H_sc.resize((size_t)dim * dim);
+  out->b_top.resize(dim); out->b_sc.resize(dim);
+  out->HdiF.resize(n_points_); out->idepth_hessian.resize(n_points_);
+  chk(tdm_active_accumulate(handle_, aH.data(), aT.data(), pr.data(), dp.data(), in.cPrior.data(), in.cDeltaF.data(), in.priorF.data(),
+                            in.deltaF.data(), out->H_top.data(), out->b_top.data(), out->H_sc.data(), out->b_sc.data(), &out->resInA,
+                            out->HdiF.data(), out->idepth_hessian.data()),
+      "CudaActivePoints::accumulate");
+}
+
+void CudaActivePoints::resubstitute(std::vector<double> const &x, std::vector<float> *step) {
+  if ((int)x.size() != 8 * n_frames_ + 4) throw std::runtime_error("CudaActivePoints::resubstitute: x needs 8 n_frames + 4 entries");
+  step->resize(n_points_);
+  chk(tdm_active_resubstitute(handle_, x.data(), step->data()), "CudaActivePoints::resubstitute");
+}

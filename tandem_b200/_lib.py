@@ -243,6 +243,9 @@ def _declare(l):
                                      P(c.c_ubyte), fp, ip]),
         "tdm_active_apply_res": (i, [vp]),
         "tdm_active_get_state": (i, [vp, P(c.c_byte), fp]),
+        "tdm_active_accumulate": (i, [vp, dp, dp, dp, dp, dp, fp, fp, fp, dp, dp, dp, dp, ip, fp, fp]),
+        "tdm_active_resubstitute": (i, [vp, dp, fp]),
+        "tdm_active_get_accumulators": (i, [vp, dp, ip, dp, dp, dp, ip, dp, dp]),
     }
     missing = []
     for name, (res, args) in sigs.items():

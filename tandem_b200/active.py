@@ -1,4 +1,4 @@
-"""n12: the active residuals of DSO's window for one FullSystem::optimize, kept in device memory, and their linearisation
+"""n12 / n13: the active residuals of DSO's window for one FullSystem::optimize, kept in device memory, and their linearisation
 (FullSystem::linearizeAll, FullSystemOptimize.cpp:142-210: PointFrameResidual::linearize for every residual,
 setNewFrameEnergyTH, and with fixLinearization applyRes and the maxRelBaseline / numGoodResiduals update) over the C ABI
 (include/tandem_b200.h, block n12)."""
@@ -8,6 +8,7 @@ import numpy as np
 
 from ._lib import LinearizeSettings, check, lib
 
+_dp = ctypes.POINTER(ctypes.c_double)
 _fp = ctypes.POINTER(ctypes.c_float)
 _ip = ctypes.POINTER(ctypes.c_int)
 _bp = ctypes.POINTER(ctypes.c_byte)
@@ -21,6 +22,8 @@ JACOBIAN_FLOATS = 74
 #: the array outputs of ActivePoints.linearize
 OUTPUTS = ("new_state", "new_energy", "new_energy_with_outlier", "center_projected_to", "jacobians", "state", "removed",
            "max_rel_baseline", "num_good_residuals")
+#: the array outputs of ActivePoints.accumulate
+ACC_OUTPUTS = ("H_top", "b_top", "H_sc", "b_sc", "hdi", "idepth_hessian")
 #: ResState
 IN, OOB, OUTLIER = 0, 1, 2
 
@@ -134,3 +137,76 @@ class ActivePoints:
         s, e = np.empty(self.n_residuals, np.int8), np.empty(self.n_residuals, np.float32)
         check(lib().tdm_active_get_state(self._h, _p(s, _bp), _p(e)))
         return dict(state=s, energy=e)
+
+    def accumulate(self, ad_host, ad_target, frame_prior, frame_delta_prior, c_prior, c_delta, point_prior, point_delta, out=None):
+        """accumulateAF_MT + accumulateLF_MT + accumulateSCF_MT over the data the last apply took (blocking).  ad_host,
+        ad_target (n, n, 8, 8) [host][target]; frame_prior, frame_delta_prior (n, 8); c_prior (4,) doubles; c_delta (4,)
+        floats; point_prior, point_delta one float per point.  Returns dict(H_top, b_top, H_sc, b_sc, n_active, hdi,
+        idepth_hessian) with H (8n+4, 8n+4) and b (8n+4,) doubles.  `out` may hold preallocated arrays (such as page-locked
+        ones) for the array keys, each of the exact shape and dtype the call returns."""
+        n, npt = self.n_frames, self.n_points
+        dim = 8 * n + 4
+        f64 = lambda a: np.ascontiguousarray(a, np.float64)
+        f32 = lambda a: np.ascontiguousarray(a, np.float32).ravel()
+        # [host][target] -> the C layout's record index host + n * target
+        aH, aT = (f64(np.swapaxes(np.asarray(a, np.float64).reshape(n, n, 8, 8), 0, 1)) for a in (ad_host, ad_target))
+        fpr, fdp, cp, cd = f64(frame_prior), f64(frame_delta_prior), f64(c_prior).ravel(), f32(c_delta)
+        pp, pd = f32(point_prior), f32(point_delta)
+        if aH.size != n * n * 64 or aT.size != n * n * 64:
+            raise ValueError("ad_host and ad_target need n_frames x n_frames 8x8 records")
+        if fpr.size != 8 * n or fdp.size != 8 * n or cp.size != 4 or cd.size != 4:
+            raise ValueError("frame_prior / frame_delta_prior need n_frames x 8 entries, c_prior and c_delta 4")
+        if pp.size != npt or pd.size != npt:
+            raise ValueError("one point_prior and point_delta per point")
+        shapes = dict(H_top=((dim, dim), np.float64), b_top=((dim,), np.float64), H_sc=((dim, dim), np.float64),
+                      b_sc=((dim,), np.float64), hdi=((npt,), np.float32), idepth_hessian=((npt,), np.float32))
+        o = self._outputs(shapes, out, ACC_OUTPUTS)
+        na = ctypes.c_int()
+        check(lib().tdm_active_accumulate(self._h, _p(aH, _dp), _p(aT, _dp), _p(fpr, _dp), _p(fdp, _dp), _p(cp, _dp), _p(cd), _p(pp),
+                                          _p(pd), _p(o["H_top"], _dp), _p(o["b_top"], _dp), _p(o["H_sc"], _dp), _p(o["b_sc"], _dp),
+                                          ctypes.byref(na), _p(o["hdi"]), _p(o["idepth_hessian"])))
+        return dict(o, n_active=na.value)
+
+    def resubstitute(self, x, out=None):
+        """resubstituteF_MT's per-point step for the solved x (8n+4 doubles) with the last accumulate's adjoints (blocking).
+        Returns one float per point; `out` may be a preallocated float32 array of that shape."""
+        x = np.ascontiguousarray(x, np.float64).ravel()
+        if x.size != 8 * self.n_frames + 4:
+            raise ValueError("x needs 8 n_frames + 4 entries")
+        o = self._outputs(dict(step=((self.n_points,), np.float32)), None if out is None else dict(step=out), ("step",))
+        check(lib().tdm_active_resubstitute(self._h, _p(x, _dp), _p(o["step"])))
+        return o["step"]
+
+    def get_accumulators(self):
+        """The last accumulate's raw sums before the stitch (synchronises): dict(top (n, n, 91) [host][target], top_num
+        (n, n), acc_e (n, n, 8, 4), acc_eb (n, n, 8), acc_d (n, n, n, 8, 8) [host][t1][t2], d_num (n, n, n), hcc (4, 4),
+        bc (4,))."""
+        n = self.n_frames
+        # the C layout is [target][host] (index host + n * target); returned transposed to [host][target]
+        r = dict(top=np.empty((n, n, 91)), top_num=np.empty((n, n), np.int32), acc_e=np.empty((n, n, 8, 4)),
+                 acc_eb=np.empty((n, n, 8)), acc_d=np.empty((n, n, n, 8, 8)), d_num=np.empty((n, n, n), np.int32),
+                 hcc=np.empty((4, 4)), bc=np.empty(4))
+        check(lib().tdm_active_get_accumulators(self._h, _p(r["top"], _dp), _p(r["top_num"], _ip), _p(r["acc_e"], _dp),
+                                                _p(r["acc_eb"], _dp), _p(r["acc_d"], _dp), _p(r["d_num"], _ip), _p(r["hcc"], _dp),
+                                                _p(r["bc"], _dp)))
+        for k in ("top", "top_num", "acc_e", "acc_eb"):
+            r[k] = np.ascontiguousarray(np.swapaxes(r[k], 0, 1))
+        for k in ("acc_d", "d_num"):
+            r[k] = np.ascontiguousarray(np.swapaxes(r[k], 0, 2))
+        return r
+
+    @staticmethod
+    def _outputs(shapes, out, allowed):
+        out = out or {}
+        unknown = set(out) - set(allowed)
+        if unknown:
+            raise TypeError(f"unknown outputs {sorted(unknown)}")
+        o = {}
+        for k, (s, t) in shapes.items():
+            a = out.get(k)
+            if a is None:
+                a = np.empty(s, t)
+            elif not (isinstance(a, np.ndarray) and a.shape == s and a.dtype == t and a.flags.c_contiguous and a.flags.writeable):
+                raise ValueError(f"out[{k!r}] must be a writeable C-contiguous {np.dtype(t).name} array of shape {s}")
+            o[k] = a
+        return o

@@ -623,4 +623,36 @@ int tdm_active_get_state(tdm_active* s, signed char* state, float* energy) {
   TDM_API_END
 }
 
+/* ---- n13: solveSystemF's accumulators on the device ---- */
+int tdm_active_accumulate(tdm_active* s, const double* ad_host, const double* ad_target, const double* frame_prior,
+                          const double* frame_delta_prior, const double c_prior[4], const float c_delta[4], const float* point_prior,
+                          const float* point_delta, double* H_top, double* b_top, double* H_sc, double* b_sc, int* n_active,
+                          float* hdi, float* idepth_hessian) {
+  TDM_API_BEGIN
+  TDM_CHECK(s, "null handle");
+  tdm::ActiveIface::AccInputs in;
+  in.ad_host = ad_host; in.ad_target = ad_target; in.frame_prior = frame_prior; in.frame_delta_prior = frame_delta_prior;
+  in.c_prior = c_prior; in.c_delta = c_delta; in.point_prior = point_prior; in.point_delta = point_delta;
+  tdm::ActiveIface::AccOutputs o;
+  o.H_top = H_top; o.b_top = b_top; o.H_sc = H_sc; o.b_sc = b_sc; o.n_active = n_active; o.hdi = hdi; o.idepth_hessian = idepth_hessian;
+  s->impl->accumulate(in, o);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_active_resubstitute(tdm_active* s, const double* x, float* step) {
+  TDM_API_BEGIN
+  TDM_CHECK(s, "null handle");
+  s->impl->resubstitute(x, step);
+  return TDM_OK;
+  TDM_API_END
+}
+int tdm_active_get_accumulators(tdm_active* s, double* top, int* top_num, double* acc_e, double* acc_eb, double* acc_d, int* d_num,
+                                double* hcc, double* bc) {
+  TDM_API_BEGIN
+  TDM_CHECK(s, "null handle");
+  s->impl->get_accumulators(top, top_num, acc_e, acc_eb, acc_d, d_num, hcc, bc);
+  return TDM_OK;
+  TDM_API_END
+}
+
 }  // extern "C"

@@ -47,7 +47,7 @@ struct Residuals {
   float *energy, *new_energy, *new_energy_wo, *center, *J, *relbs;
   double* ret;
   unsigned* key;
-  unsigned char* removed;
+  unsigned char *removed, *active, *took;   // active, took: the taken data's flags (accumulate.cu)
 };
 struct LinLaunch {
   const float* dI[kFrames];
@@ -208,7 +208,9 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize(LinLaunch L, Points P
       st = ns;
       R.state[r] = (signed char)ns;
       R.energy[r] = nE;
+      R.active[r] = ns == RS_IN;
     }
+    R.took[r] = st == RS_IN;
     float relBS = __int_as_float(0x7fc00000);
     if (st == RS_IN) {   // efResidual->isActive(); isNew is always true
       const float* K = pc + PC_KRKI;
@@ -227,13 +229,15 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize(LinLaunch L, Points P
   }
 }
 
-// applyRes_Reductor (FullSystemOptimize.cpp:87-92)
+// applyRes_Reductor (FullSystemOptimize.cpp:87-92); active / took: isActiveAndIsGoodNEW and whether takeDataF runs
 __global__ void k_apply(int n, signed char* __restrict__ state, float* __restrict__ energy, const signed char* __restrict__ new_state,
-                        const float* __restrict__ new_energy) {
+                        const float* __restrict__ new_energy, unsigned char* __restrict__ active, unsigned char* __restrict__ took) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= n || state[r] == RS_OOB) return;
+  if (r >= n) return;
+  if (state[r] == RS_OOB) { took[r] = 0; return; }
   state[r] = new_state[r];
   energy[r] = new_energy[r];
+  active[r] = took[r] = new_state[r] == RS_IN;
 }
 
 // the fix branch's per-point part: numGoodResiduals++ and the maxRelBaseline update for every residual whose final state is
@@ -310,6 +314,7 @@ class ActiveImpl final : public ActiveIface {
     TDM_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, (const unsigned*)nullptr, (unsigned*)nullptr, (int)rc, 0, 32, stream_.get()));
     sort_bytes_ = tb;
     d_sort_ = make_dev<char>(tb + 16);
+    acc_.reset(make_acc(cap));
   }
   ~ActiveImpl() override {
     cudaSetDevice(device_);
@@ -394,9 +399,19 @@ class ActiveImpl final : public ActiveIface {
       TDM_CUDA(cudaMemsetAsync(d_rf_.get(), 0, 4 * nr, st));
       TDM_CUDA(cudaMemsetAsync(d_rf_.get() + rc, 0, 4 * nr, st));
     }
+    n_frames_ = n_frames; n_points_ = n_points; n_res_ = n_res;
+    unique_targets_ = true;
+    for (int p = 0; p < n_points && unique_targets_; ++p) {
+      unsigned seen = 0;
+      for (int k = off[p]; k < off[p + 1]; ++k) {
+        const unsigned bit = 1u << res_target[list[k]];
+        if (seen & bit) unique_targets_ = false;
+        seen |= bit;
+      }
+    }
+    acc_->load(view(), host, st);
     // every later reader runs on the set's stream; the upload has landed when load returns
     TDM_CUDA(cudaStreamSynchronize(st));
-    n_frames_ = n_frames; n_points_ = n_points; n_res_ = n_res;
   }
 
   void linearize(const PyramidIface* const* frames, const float* precalc, const float* frame_energy_th, const float* calib4,
@@ -451,6 +466,7 @@ class ActiveImpl final : public ActiveIface {
         TDM_CUDA(cudaGetLastError());
       }
     }
+    if (fix) acc_->take(view(), stream_.get());   // applyRes(true) took the data of every residual now IN
     double* ds = d_small_.get();
     k_finish<<<1, kFinishThreads, 0, stream_.get()>>>(n_res_, R.ret, sorted, n_key, s_, ds, reinterpret_cast<float*>(ds + 1));
     TDM_CUDA(cudaGetLastError());
@@ -480,10 +496,26 @@ class ActiveImpl final : public ActiveIface {
 
   void apply_res() override {
     TDM_CUDA(cudaSetDevice(device_));
-    if (n_res_ == 0) return;
-    Residuals R = res_view();
-    k_apply<<<cdiv(n_res_, 256), 256, 0, stream_.get()>>>(n_res_, R.state, R.energy, R.new_state, R.new_energy);
-    TDM_CUDA(cudaGetLastError());
+    if (n_res_ > 0) {
+      Residuals R = res_view();
+      k_apply<<<cdiv(n_res_, 256), 256, 0, stream_.get()>>>(n_res_, R.state, R.energy, R.new_state, R.new_energy, R.active, R.took);
+      TDM_CUDA(cudaGetLastError());
+    }
+    if (n_frames_ >= 2) acc_->take(view(), stream_.get());
+  }
+
+  void accumulate(const AccInputs& in, AccOutputs& o) override {
+    TDM_CUDA(cudaSetDevice(device_));
+    acc_->accumulate(view(), stream_.get(), in, o);
+  }
+  void resubstitute(const double* x, float* step) override {
+    TDM_CUDA(cudaSetDevice(device_));
+    acc_->resubstitute(view(), stream_.get(), x, step);
+  }
+  void get_accumulators(double* top, int* top_num, double* acc_e, double* acc_eb, double* acc_d, int* d_num, double* hcc,
+                        double* bc) override {
+    TDM_CUDA(cudaSetDevice(device_));
+    acc_->get_accumulators(view(), stream_.get(), top, top_num, acc_e, acc_eb, acc_d, d_num, hcc, bc);
   }
 
   void get_state(signed char* state, float* energy) override {
@@ -511,11 +543,23 @@ class ActiveImpl final : public ActiveIface {
     R.center = f + 5 * rc; R.J = f + 8 * rc;
     R.ret = d_ret_.get();
     R.key = d_key_.get();
+    R.active = acc_->active();
+    R.took = acc_->took();
     return R;
+  }
+  ActiveView view() const {
+    const size_t cap = cap_, rc = 8ull * cap_;
+    ActiveView v;
+    v.n_frames = n_frames_; v.n_points = n_points_; v.n_res = n_res_; v.unique_targets = unique_targets_;
+    v.host = d_pint_.get(); v.off = d_pint_.get() + 2 * cap; v.res_of = d_rint_.get() + 2 * rc; v.res_target = d_rint_.get() + rc;
+    v.J = d_rf_.get() + 8 * rc;
+    v.max_rel_baseline = d_pf_.get() + 18 * cap;
+    return v;
   }
   int w_, h_, cap_, device_;
   Settings s_;
   int n_frames_ = 0, n_points_ = 0, n_res_ = 0;
+  bool unique_targets_ = true;
   size_t sort_bytes_ = 0;
   Stream stream_;
   Event done_;
@@ -528,6 +572,7 @@ class ActiveImpl final : public ActiveIface {
   HostPtr<float> h_in_;
   HostPtr<int> h_load_;
   HostPtr<double> h_small_;
+  std::unique_ptr<AccIface> acc_;   // after the buffers: destroyed first
 };
 
 }  // namespace

@@ -270,8 +270,48 @@ class ActiveIface {
   virtual int n_frames() const = 0;
   virtual int n_residuals() const = 0;
   virtual int device() const = 0;
+  // n13 (accumulate.cu): solveSystemF's accumulators over the data the last applyRes(true) took
+  struct AccInputs {   // host memory
+    const double *ad_host = nullptr, *ad_target = nullptr;                // n x n records [host][target], 8x8 row-major
+    const double *frame_prior = nullptr, *frame_delta_prior = nullptr;    // n x 8
+    const double* c_prior = nullptr;                                      // 4
+    const float* c_delta = nullptr;                                       // 4
+    const float *point_prior = nullptr, *point_delta = nullptr;           // per point
+  };
+  struct AccOutputs {   // host memory; every pointer may be null
+    double *H_top = nullptr, *b_top = nullptr, *H_sc = nullptr, *b_sc = nullptr;
+    int* n_active = nullptr;
+    float *hdi = nullptr, *idepth_hessian = nullptr;
+  };
+  virtual void accumulate(const AccInputs& in, AccOutputs& o) = 0;    // blocking
+  virtual void resubstitute(const double* x, float* step) = 0;        // blocking
+  virtual void get_accumulators(double* top, int* top_num, double* acc_e, double* acc_eb, double* acc_d, int* d_num, double* hcc,
+                                double* bc) = 0;                      // synchronises
 };
 ActiveIface* make_active(int w, int h, int capacity_points, const float* settings /* tdm_linearize_settings */, int device);
+
+// the device arrays of an ActiveImpl that the accumulators read
+struct ActiveView {
+  int n_frames, n_points, n_res;
+  bool unique_targets;   // at most one residual per (point, target)
+  const int *host, *off, *res_of, *res_target;   // per point; CSR offsets (n_points + 1) and list; per residual
+  const float* J;                                // the last linearize's Jacobians
+  float* max_rel_baseline;
+};
+// the taken data and accumulators of one active-residual set (accumulate.cu); every call runs on the set's stream
+class AccIface {
+ public:
+  virtual ~AccIface() = default;
+  virtual unsigned char* active() = 0;   // isActiveAndIsGoodNEW per residual
+  virtual unsigned char* took() = 0;     // set by each apply for the residuals it took
+  virtual void load(const ActiveView& v, const int* host, cudaStream_t st) = 0;   // host: host memory; asynchronous
+  virtual void take(const ActiveView& v, cudaStream_t st) = 0;                     // asynchronous, after an apply
+  virtual void accumulate(const ActiveView& v, cudaStream_t st, const ActiveIface::AccInputs& in, ActiveIface::AccOutputs& o) = 0;
+  virtual void resubstitute(const ActiveView& v, cudaStream_t st, const double* x, float* step) = 0;
+  virtual void get_accumulators(const ActiveView& v, cudaStream_t st, double* top, int* top_num, double* acc_e, double* acc_eb,
+                                double* acc_d, int* d_num, double* hcc, double* bc) = 0;
+};
+AccIface* make_acc(int capacity_points);
 
 TrackerIface* make_tracker(int w, int h, float huber, float cutoff, int n_max, int device);
 

@@ -27,3 +27,4 @@ leg activate_mem $T1 memcheck tests/test_activate_gpu.py -k "not shim and not ra
 leg pixsel_mem $T1 memcheck tests/test_pixsel_gpu.py -k "not shim and not sequences"
 leg undistort_mem $T1 memcheck tests/test_undistort_gpu.py -k "not shim and not tracker and not trace"
 leg linearize_mem $T1 memcheck tests/test_linearize_gpu.py -k "not shim and not seeded"
+leg accumulate_mem $T1 memcheck tests/test_accumulate_gpu.py -k "room or invalid or zero"
