@@ -306,6 +306,39 @@ __device__ __forceinline__ bool frag_pixel(const Tile& t, const TileOrigin& o, i
   return hh < t.R && ww < t.TW && h < t.H && w < t.W;
 }
 
+// The tile (row, column) of a consumer thread's two fragment row halves, carried across its sub-chunks of a plane.  Sub-chunk
+// wg + (k + 1) * NWG lies STEP = 64 * NWG positions after wg + k * NWG, so each half advances by STEP / P rows and STEP % P
+// columns with one wrap: the two divisions of frag_pixel happen once per CTA, and no register depends on the chunk count.
+// in(i) is frag_pixel's test (pad columns and positions beyond the grid are out).
+template <int NWG>
+struct FragRows {
+  int hh[2], ww[2];
+  int dq, dr;             // STEP / P, STEP % P
+  int hlim, wlim;         // rows / columns of the tile inside the grid
+  __device__ __forceinline__ FragRows(const Tile& t, const TileOrigin& o, int wg, int wq, int lane) {
+    constexpr int STEP = 64 * NWG;
+    dq = STEP / t.P;
+    dr = STEP - dq * t.P;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int l = wg * 64 + wq * 16 + (lane >> 2) + 8 * i;
+      hh[i] = l / t.P;
+      ww[i] = l - hh[i] * t.P;
+    }
+    hlim = min(t.R, t.H - o.h0);
+    wlim = min(t.TW, t.W - o.w0);
+  }
+  __device__ __forceinline__ bool in(int i) const { return hh[i] < hlim && ww[i] < wlim; }
+  __device__ __forceinline__ void next(int P) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      hh[i] += dq;
+      ww[i] += dr;
+      if (ww[i] >= P) { ww[i] -= P; ++hh[i]; }
+    }
+  }
+};
+
 // This thread's bias values, loaded once per CTA: bv[j][e] is added to fragment column 8j + 2 * (lane % 4) + e, i.e.
 // output column n0 + 8j + 2 * (lane % 4) + e (for CLASS, parity class x cout + channel); zero beyond cout
 template <bool CLASS, int NB>
@@ -515,22 +548,15 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
   const uint32_t b_lbo16 = (uint32_t)(NMMA * 16 >> 4);
   const int nsub = 2 * g.nch;                      // 64-position sub-chunks per plane
   ring.wait_weights();
-  // P8 position and first channel of column block j of pixel (d, h, w); false for blocks beyond COUT
-  auto out_at = [&](int d, int h, int w, int j, long long& pos, int& co) -> bool {
-    const int n = ns * NPAD + 8 * j + 2 * (lane & 3);
-    if constexpr (MODE == 3) {
-      // N = 4 parity classes x COUT: class (ph,pw) of input position (d,h,w) is output (d, 2h+ph, 2w+pw)
-      const int cls = n / g.cout;
-      co = n % g.cout;
-      const int oh2 = 2 * h + ((cls >> 1) & 1), ow2 = 2 * w + (cls & 1);
-      pos = ((((long long)(d + g.opd)) * g.oHp + (oh2 + 1)) * g.oWp + (ow2 + 1)) * 8;
-    } else {
-      co = n;
-      if (ns * NPAD + 8 * j >= g.cout) return false;
-      pos = ((((long long)(d + g.pd)) * g.Hp + (h + 1)) * g.Wp + (w + 1)) * 8;
-    }
-    return true;
-  };
+  // 16-bit outputs of MODE 0 / 3: fragment row half i of a sub-chunk stores at element fr.hh[i] * orow + fr.ww[i] * OCOL
+  // of its plane's base pointer (ob below), i.e. at P8 position (h + 1, w + 1) of pixel (h, w) in MODE 0, and at output
+  // (2h + 1, 2w + 1), class (0, 0), in MODE 3.  MODE 3's N = 4 parity classes x 8 channels (cout = 8, nsplit = 1: the host
+  // checks both) make column block j class (ph, pw) = (j >> 1, j & 1), channels 2 * (lane % 4) + e, of output
+  // (d, 2h + ph, 2w + pw).
+  static_assert(MODE != 3 || NPAD == 32, "MODE 3 writes 4 parity classes of 8 channels");
+  constexpr int OCOL = MODE == 3 ? 16 : 8;
+  const int orow = MODE == 3 ? 16 * g.oWp : 8 * g.Wp;
+  const FragRows<NWG> fr0(g, o, wg, wq, lane);
   // bias in registers, except for N = 128, whose 32 more registers would spill: it loads them in the epilogue.  MODE 1
   // slice ns holds output channels ns * CPS .. + CPS - 1 of all 8 classes (build_b_image_deconv): column n is class
   // n / CPS, channel ns * CPS + n % CPS.
@@ -548,13 +574,6 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
   // 32-byte runs in full, where two 4-byte accesses per lane filled half of each sector apiece.
   constexpr bool PAIR_EPI = MODE == 3;
   const int pq = lane & 1;
-  // element offset of the 8 bytes this lane moves for block pair k of pixel (d, h, w), in a tensor of group stride gs
-  auto pair_at = [&](int d, int h, int w, int k, long long gs) -> long long {
-    long long pos;
-    int co;
-    out_at(d, h, w, 2 * k + pq, pos, co);
-    return pos + (co >> 3) * gs + 4 * ((lane & 3) >> 1);
-  };
   // MODE 1: box element offset of this lane's channels 2q, 2q + 1 of class 0 for fragment row half i of this
   // warpgroup's k-th sub-chunk (sub-chunk wg + k * NWG), -1 for pad columns and rows beyond the tile; decoded once per
   // CTA.  Class (pd, ph, pw) and channel group c of the slice add c * 2 * PD_STR + pd * PD_STR + ph * PH_STR + pw * 8.
@@ -579,10 +598,16 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
     const int d = o.d0 + od;
     TOut* const box = reinterpret_cast<TOut*>(obox0 + (size_t)(od & 1) * obox_bytes);
     if constexpr (MODE == 1) mbar_wait(obox_full + (od & 1), (od >> 1) & 1);
+    // this lane's first element of tile position (0, 0) in output plane d (MODE 0: + column block 0 of the N slice)
+    TOut* ob = nullptr;
+    if constexpr (MODE == 3)
+      ob = out + (((long long)(d + g.opd) * g.oHp + 2 * o.h0 + 1) * g.oWp + 2 * o.w0 + 1) * 8 + 8 * pq + 4 * ((lane & 3) >> 1);
+    else if constexpr (MODE == 0 && !OUT_PLAIN)
+      ob = out + (((long long)(d + g.pd) * g.Hp + o.h0 + 1) * g.Wp + o.w0 + 1) * 8 + (ns * NPAD / 8) * g.out_gs + 2 * (lane & 3);
+    FragRows<NWG> fr = fr0;
 #pragma unroll 1
     for (int k = 0; wg + k * NWG < nsub; ++k) {
       const int sc = wg + k * NWG;
-      const int l = sc * 64 + wq * 16 + (lane >> 2);
       float acc[NMMA / 2];
       mma_subchunk<NMMA, TIn, KD, NBLK>(acc, slot16, (uint32_t)sc * 64u, sB16, b_lbo16, aoff, alo);
       if constexpr (MODE == 1) {
@@ -618,9 +643,17 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
       }
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        int h, w;
-        const bool in = frag_pixel(g, o, l, i, h, w);
+        if constexpr (OUT_PLAIN) {
+          int h, w;
+          if (!frag_pixel(g, o, sc * 64 + wq * 16 + (lane >> 2), i, h, w) || (lane & 3) != 0) continue;
+          float x = acc[2 * i];
+          if constexpr (HILO) x += acc[4 * (NPAD / 8) + 2 * i];
+          plain_out[((long long)d * g.H + h) * g.W + w] = x + bv[0][0];
+          continue;
+        }
+        const bool in = fr.in(i);
         if (!in && !PAIR_EPI) continue;   // PAIR_EPI: every lane takes part in the word exchange
+        TOut* const op = ob + (fr.hh[i] * orow + fr.ww[i] * OCOL);
         if constexpr (PAIR_EPI) {
 #pragma unroll
           for (int k2 = 0; k2 < NPAD / 16; ++k2) {
@@ -639,37 +672,29 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmap /*P8 input: {8, Wp, Hp, group
               v[p] = pack2<TOut>(x[0], x[1]);
             }
             const uint32_t own = pq ? v[1] : v[0], other = __shfl_xor_sync(0xffffffffu, pq ? v[0] : v[1], 1);
-            if (in) *reinterpret_cast<uint2*>(out + pair_at(d, h, w, k2, g.out_gs)) = pq ? make_uint2(other, own) : make_uint2(own, other);
-          }
-        } else if constexpr (OUT_PLAIN) {
-          if ((lane & 3) == 0) {
-            float x = acc[2 * i];
-            if constexpr (HILO) x += acc[4 * (NPAD / 8) + 2 * i];
-            plain_out[((long long)d * g.H + h) * g.W + w] = x + bv[0][0];
+            if (in) *reinterpret_cast<uint2*>(op + k2 * 8 * g.oWp) = pq ? make_uint2(other, own) : make_uint2(own, other);
           }
         } else {
 #pragma unroll
           for (int j = 0; j < NPAD / 8; ++j) {
-            long long pos;
-            int co;
-            if (!out_at(d, h, w, j, pos, co)) continue;
+            if (ns * NPAD + 8 * j >= g.cout) continue;
             float x[2];
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               x[e] = acc[4 * j + 2 * i + e];
               if constexpr (HILO) x[e] += acc[4 * (j + NPAD / 8) + 2 * i + e];
             }
-            const long long e0 = pos + (co >> 3) * g.out_gs + (co & 7);
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               if constexpr (BIAS_REG) x[e] += bv[j][e];
-              else x[e] += bias ? bias[co + e] : 0.f;
+              else x[e] += bias ? bias[ns * NPAD + 8 * j + 2 * (lane & 3) + e] : 0.f;
               if (g.relu) x[e] = fmaxf(x[e], 0.f);
             }
-            store2<TOut>(out + e0, x[0], x[1]);
+            store2<TOut>(op + j * g.out_gs, x[0], x[1]);
           }
         }
       }
+      fr.next(P);
     }
     if constexpr (MODE == 1) {
       // this warp's outputs of plane od are in the box: hand it to the producer's TMA store

@@ -77,6 +77,7 @@ k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ b
   ring.wait_weights();
   float bv[NPAD / 8][2];
   load_bias<false>(bv, bias, ns * NPAD, g.cout, lane);
+  const FragRows<NWG> fr0(g, o, wg, wq, lane);
   for (int od = 0; od < o.ndo; ++od) {
     const int first = KD == 3 ? 2 * od : od;
     ring.wait(first + KD - 1);
@@ -84,28 +85,30 @@ k_conv_tc_s2(const __grid_constant__ CUtensorMap tmap, const TIn* __restrict__ b
 #pragma unroll
     for (int kd = 0; kd < KD; ++kd) slot16[kd] = ring.slot16(first + kd);
     const int d = o.d0 + od;
+    // this lane's first element of output pixel (h0, w0), column block 0 of the N slice, in plane d; fragment row half i
+    // adds its P8 offset (hh * oWp + ww) * 8
+    TOut* const ob = out + (((long long)(d + g.opd) * g.oHp + o.h0 + 1) * g.oWp + o.w0 + 1) * 8 + (ns * NPAD / 8) * g.out_gs + 2 * (lane & 3);
+    FragRows<NWG> fr = fr0;
     for (int sc = wg; sc < nsub; sc += NWG) {
       float acc[NPAD / 2];
       mma_subchunk<NPAD, TIn, KD, NBLK>(acc, slot16, (uint32_t)sc * 64u, sB16, b_lbo16, aoff, alo);
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        int h, w;
-        if (!frag_pixel(g, o, sc * 64 + wq * 16 + (lane >> 2), i, h, w)) continue;
-        const long long pos = ((((long long)(d + g.opd)) * g.oHp + (h + 1)) * g.oWp + (w + 1)) * 8;
+        if (!fr.in(i)) continue;
+        TOut* const op = ob + (fr.hh[i] * g.oWp + fr.ww[i]) * 8;
 #pragma unroll
         for (int j = 0; j < NPAD / 8; ++j) {
-          const int co = ns * NPAD + 8 * j;
-          if (co >= g.cout) continue;
-          const int c = co + 2 * (lane & 3);
+          if (ns * NPAD + 8 * j >= g.cout) continue;
           float x[2];
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             x[e] = acc[4 * j + 2 * i + e] + bv[j][e];
             if (g.relu) x[e] = fmaxf(x[e], 0.f);
           }
-          store2<TOut>(out + pos + (co >> 3) * g.out_gs + (c & 7), x[0], x[1]);
+          store2<TOut>(op + j * g.out_gs, x[0], x[1]);
         }
       }
+      fr.next(g.P);
     }
     ring.release(first);                   // KD = 3: input planes 2*od and 2*od+1 are dead after output plane od
     if (KD == 3) ring.release(first + 1);

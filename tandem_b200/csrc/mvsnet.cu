@@ -995,7 +995,7 @@ class MvsnetEngine final : public MvsnetIface {
     // MODE 1: each N slice of NPAD columns is 8 classes x NPAD / 8 channels, whole output channel groups of the box;
     // MODE 3: the epilogue pairs column blocks pw = 0 / 1 of cout = 8
     TDM_CHECK((MODE != 1 || (c.cout == CIN / 2 && c.cout == c.nsplit * NPAD / 8 && NPAD % 64 == 0 && (NPAD == 64 || c.nsplit == 1))) &&
-              (MODE != 3 || c.cout == 8), wkey + ": parity-class layer with an unexpected cout");
+              (MODE != 3 || (c.cout == 8 && c.nsplit == 1)), wkey + ": parity-class layer with an unexpected cout");
     TDM_CHECK(MODE != 1 || (out.pd == 1 && (!res || (res->D == out.D && res->H == out.H && res->W == out.W && res->C == out.C))),
               wkey + ": transposed conv skip / output shapes differ");
     launch_tc<tc::k_conv_tc<TIn, TOut, CIN, NPAD, KD, PLAIN, MODE, HILO, Tail, NWG>>(dim3(pl.grid, c.nsplit), pl.smem, tcx.tmap, tcx.tmap_res, tcx.tmap_out, (const TIn*)c.bimg.get(),
